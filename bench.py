@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py - participant-steps/s of the batched env.step() hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c3|c4|c5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c3|c4|c5] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the fused tick (physics -> pose -> collisions -> out-of-bound -> status) over one
@@ -11,12 +11,18 @@ participants, SingleTrackKinematics + OBB collision, synthetic grid map.  For N>
 all-gather per step.
 
 Timing rules followed: W >= 3 warm-up steps; inputs larger than L2 - the timed steps rotate over R
-independent world replicas whose state + actions + outputs exceed the 126 MB L2 (R x 14.2 MB), so every
-step streams its state from HBM; device timing with CUDA events on the launching stream, barrier +
-synchronize on both sides, max over ranks; SM clocks and throttle reasons sampled with nvidia-smi while
-the timed region is repeated.  The K-step timed region is captured in a CUDA graph (the kernels are a few
-microseconds each; a Python launch loop would measure the interpreter) and is repeated `reps` times, the
-median repetition is reported.
+independent world replicas whose state + actions + outputs together exceed 2.5 x the L2 (50 MB on an H100),
+so every step streams its state from HBM; device timing with CUDA events on the launching stream, barrier +
+synchronize on both sides, max over ranks; SM clocks and throttle reasons sampled with nvidia-smi during
+the timed region.  The timed region is exactly K = --steps steps (default: about a second of work on an H100), in
+chunks of 8 ticks per replica that each start from the restored replicas (restores outside the CUDA events, chunk
+times summed), so the timed world stays the configured scene however large K is; a chunk is one CUDA-graph replay
+(the kernels are a few microseconds each; a Python launch loop would measure the interpreter).  Each e2e figure
+times K steps of its own loop in the same chunks.
+
+`--dump-outputs DIR` writes what the last timed step handed its caller - the stepped world's new state and the
+step's result arrays - as DIR/<name>.npy (float32), so that two builds can be compared output for output: the
+inputs depend only on the arguments (fixed seeds).
 
 `--impl reference` times the reference's own execution model for this path - one Python call per
 participant with NumPy scalar float64 arithmetic and per-pose predicate loops (oracle/scalar_port.py, a
@@ -42,6 +48,7 @@ if ROOT not in sys.path:
 METRIC = "participant_steps_per_sec"
 UNIT = "participant-steps/s"
 N_SCN, M_PART = 4096, 64
+TICKS_PER_CHUNK = 8   # ticks each world replica takes from its configured state before the timed region restores it
 
 # algorithmic bytes per participant-step of the fused kernel (DESIGN.md "Roofline"): reads x, y, heading,
 # speed (16) + action (8) + type id (1); writes x, y, heading, speed, vx, vy (24) + event byte (1) +
@@ -82,7 +89,7 @@ def _peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def make_scene(config: str, seed: int, n=None, m=None):
@@ -110,10 +117,10 @@ def make_scene_name(config: str) -> str:
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons while the timed region runs (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons while the timed region runs."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index: int):
         self.lines = []
@@ -132,23 +139,27 @@ class ClockSampler:
 
     def stop(self, t0, t1):
         if self.proc is None:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": 0}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": [], "samples": 0}
         time.sleep(0.15)
         self.proc.terminate()
-        sm, smax, reasons = [], [], set()
+        sm, smax, plim, reasons = [], [], [], set()
         for ts, line in self.lines:
-            if not (t0 - 0.05 <= ts <= t1 + 0.15):
+            if not (t0 <= ts <= t1):
                 continue
             f = [x.strip() for x in line.split(",")]
             try:
                 sm.append(float(f[0])); smax.append(float(f[1]))
             except Exception:
                 continue
+            try:
+                plim.append(float(f[7]))
+            except Exception:
+                pass
             for name, val in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[3:7]):
                 if val.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(smax) if smax else None,
-                "reasons": sorted(reasons), "samples": len(sm)}
+                "power_limit_w": min(plim) if plim else None, "reasons": sorted(reasons), "samples": len(sm)}
 
 
 # ------------------------------------------------------------------------------------------ CPU arms
@@ -223,12 +234,7 @@ def run_reference(args):
     cores = usable_cores()
     scene = make_scene(args.config, seed=1, n=args.scenarios or None)
     n, m = scene.shape
-    steps, warmup = max(1, args.steps), max(0, args.warmup)
-    # bounded: the whole run must end within a few minutes - ~2 k participant-steps/s per core measured for the port
-    est = n * m / (1900.0 * max(1, cores)) * (steps + warmup)
-    if est > 150.0:
-        warmup = min(warmup, 1)
-        steps = max(1, min(steps, int(150.0 / max(1e-9, n * m / (1900.0 * cores))) - warmup))
+    steps, warmup = args.steps, max(0, args.warmup)
     value, t_step = cpu_port_throughput(scene, n, cores, steps=steps, warmup=warmup, per_job=32)
     sample = (f"the whole batch every step: {n} scenarios x {m} participants, {steps} timed steps after {warmup} warm-up, "
               f"{cores} worker processes x jobs of 32 scenarios (per-agent Python loop = the reference's execution model; "
@@ -249,6 +255,34 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------ GPU arm
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(dirname, world, result, seed=0, extra=None):
+    """The arrays a caller of BatchedWorld.step receives from one step - the world's new state and the StepResult - as
+    float32 .npy files (the integer outputs are exact in float32).  When they exceed DUMP_LIMIT bytes, a fixed seeded
+    sample of whole scenarios is written instead, and its scenario indices go to sampled_scenarios.npy.  `extra`: further
+    arrays written whole (small: the gathered done masks of a multi-GPU run)."""
+    arrays = {k: getattr(world, k) for k in ("x", "y", "heading", "speed", "vx", "vy")}
+    arrays.update((k, getattr(result, k)) for k in ("flags", "hit_index", "hit_segment", "status", "done"))
+    extra = extra or {}
+    n = world.N
+    per_scenario = 4 * sum(t[0].numel() if t.dim() > 1 else 1 for t in arrays.values())
+    budget = DUMP_LIMIT - 4 * sum(t.numel() for t in extra.values())
+    keep = None
+    if per_scenario * n > budget:
+        k = (budget - (1 << 20)) // (per_scenario + 8)   # room for the index file and the .npy headers
+        keep = np.sort(np.random.default_rng(seed).choice(n, size=k, replace=False))
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy().astype(np.float32)
+        np.save(os.path.join(dirname, name + ".npy"), a if keep is None else a[keep])
+    for name, t in extra.items():
+        np.save(os.path.join(dirname, name + ".npy"), t.detach().cpu().numpy().astype(np.float32))
+    if keep is not None:
+        np.save(os.path.join(dirname, "sampled_scenarios.npy"), keep.astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -380,9 +414,38 @@ def run_ours(args):
         restore()
         barrier()
 
-    # capture the K-step timed region in a CUDA graph ----------------------------------------------
+    # The timed region: exactly K steps, in chunks of C = TICKS_PER_CHUNK x R steps that each start from the restored replicas
+    # (the restore and its barriers stay outside the CUDA events; the chunks' event times are summed).  So every replica takes
+    # at most TICKS_PER_CHUNK ticks from its configured state, whatever K: with a fixed action per replica, a long run would
+    # otherwise drive the participants to their speed bounds and time a saturated world instead of the configured scene.
+    # Step i of a chunk runs on replica i % R; a chunk is one CUDA-graph replay (the last one holds the K % C left over).
+    C = TICKS_PER_CHUNK * R
+    n_chunks, tail = K // C, K % C
+    chunks = [C] * n_chunks + ([tail] if tail else [])
+
+    def timed_chunks(run_steps, reset=None):
+        """(ms, our launches) of exactly K steps: run_steps(k) runs steps 0 .. k-1 of a chunk after reset() (default:
+        restore the replicas); max over ranks of each rank's sum."""
+        total, launches = 0.0, 0
+        for steps in chunks:
+            (reset or restore)()
+            barrier()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            l0 = lib.t2d_launch_count()
+            e0.record()
+            run_steps(steps)
+            e1.record()
+            launches += int(lib.t2d_launch_count() - l0)
+            barrier()
+            total += e0.elapsed_time(e1)
+        t = torch.tensor([total], dtype=torch.float64, device=device)
+        if world_size > 1:
+            dist.all_reduce(t, op=dist.ReduceOp.MAX)
+        return float(t.item()), launches
+
     def capture():
-        """(graph, our launches recorded in it), or (None, K) when capture is off or fails: the eager loop is timed then."""
+        """({steps: graph of that many steps}, our launches in the timed region), or (None, K) when capture is off or fails:
+        the eager loop is timed then."""
         if args.no_graph:
             return None, K
         try:
@@ -394,13 +457,17 @@ def run_ours(args):
                 join_comm()
             torch.cuda.current_stream(device).wait_stream(side)
             barrier()
-            g = torch.cuda.CUDAGraph()
-            l_cap = lib.t2d_launch_count()
-            with torch.cuda.graph(g):
-                for i in range(K):
-                    one_step(i)
-                join_comm()
-            return g, int(lib.t2d_launch_count() - l_cap)   # our kernels recorded in the graph (tick, done exchange)
+            graphs, per_graph = {}, {}
+            for steps in sorted(set(chunks)):
+                g = torch.cuda.CUDAGraph()
+                l_cap = lib.t2d_launch_count()
+                with torch.cuda.graph(g):
+                    for i in range(steps):
+                        one_step(i)
+                    join_comm()
+                graphs[steps] = g
+                per_graph[steps] = int(lib.t2d_launch_count() - l_cap)   # our kernels recorded (tick, done exchange)
+            return graphs, sum(per_graph[k] for k in chunks)
         except Exception as e:   # e.g. NCCL capture unsupported: fall back to the eager loop
             if rank == 0:
                 print(f"[bench] CUDA-graph capture failed ({type(e).__name__}: {e}); timing the eager loop", file=sys.stderr)
@@ -409,25 +476,16 @@ def run_ours(args):
 
     graph, graph_launches = capture()
 
+    def eager_steps(steps):
+        for i in range(steps):
+            one_step(i)
+        join_comm()
+
     def timed_region():
-        restore()
-        barrier()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        l0 = lib.t2d_launch_count()
-        e0.record()
         if graph is not None:
-            graph.replay()
-        else:
-            for i in range(K):
-                one_step(i)
-            join_comm()
-        e1.record()
-        barrier()
-        ms = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=device)
-        if world_size > 1:
-            dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-        launches = graph_launches if graph is not None else int(lib.t2d_launch_count() - l0)
-        return float(ms.item()), launches
+            ms, _ = timed_chunks(lambda steps: graph[steps].replay())
+            return ms, graph_launches
+        return timed_chunks(eager_steps)
 
     timed_region()  # one untimed pass through the exact timed path
 
@@ -454,53 +512,37 @@ def run_ours(args):
         timed_region()
     sampler = ClockSampler(local_rank) if rank == 0 else None
     t_wall0 = time.time()
-    reps_ms, launches = [], K
-    budget_s, t_begin = args.min_seconds, time.time()
-    while True:
-        ms, launches = timed_region()
-        reps_ms.append(ms)
-        more = len(reps_ms) < args.min_reps or (time.time() - t_begin < budget_s and len(reps_ms) < args.max_reps)
-        if world_size > 1:
-            # every repetition holds collectives (barrier, max over ranks), so all ranks must run the same number of them:
-            # rank 0's wall clock decides for everybody (each rank reading its own clock can disagree on the last one
-            # and leave a rank waiting in a barrier nobody else enters)
-            flag = torch.tensor([1 if more else 0], dtype=torch.int32, device=device)
-            dist.broadcast(flag, src=0)
-            more = bool(flag.item())
-        if not more:
-            break
+    ms_total, launches = timed_region()
     t_wall1 = time.time()
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
-    ms_total = float(np.median(reps_ms))
     ms_per_step = ms_total / K
     value = world_size * n * m * K / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        last = (K - 1) % R
+        extra = None
+        if done_all is not None:
+            # the gathered done masks rank 0 received in the last timed step (peer rows are padded); with the peer exchange
+            # at lag L they are the masks of step K - 1 - L, and the file name says so
+            lag = args.lag if peer is not None else 0
+            extra = {f"done_all_lag{lag}": done_all.view(world_size, row)[:, :n]}
+        dump_outputs(args.dump_outputs, worlds[last], worlds[last].result, extra=extra)
 
     # e2e: public API with HOST buffers, host<->device copies and a stream sync inside every timed step ----------------
     e2e = None
     if not args.no_e2e:
         from tactics2d_b200.controller import IDMController
 
-        def timed_loop(step_fn, reps):
-            restore()
+        def timed_loop(step_fn, reset=None):
+            """ms per step over K timed steps of step_fn, in the same chunks as the timed region."""
+            (reset or restore)()
             for i in range(max(W, R)):   # every world replica once: first calls build per-world state (staging buffers, graphs)
                 step_fn(i)
-            ms = []
-            for _ in range(reps):
-                restore()
-                barrier()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for i in range(K):
-                    step_fn(i)
-                e1.record()
-                barrier()
-                t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=device)
-                if world_size > 1:
-                    dist.all_reduce(t, op=dist.ReduceOp.MAX)
-                ms.append(float(t.item()))
-            return float(np.median(ms)) / K
 
-        reps_e2e = max(3, min(args.min_reps, 10))
+            def run(steps):
+                for i in range(steps):
+                    step_fn(i)
+            return timed_chunks(run, reset)[0] / K
+
         # (1) the headline: the reference env's contract - the caller's policy drives the EGO, one (steering, accel) per
         # scenario (envs/parking.py:219-239); the other 63 participants are driven by on-device IDM controllers
         # (t2d_control), so 8 N bytes go up and 2 N come back per step (t2d_step_host_ego)
@@ -524,7 +566,7 @@ def run_ours(args):
                     peer(worlds[r].result.done, done_all)
                 else:
                     dist.all_gather_into_tensor(done_all, worlds[r].result.done)
-        t_ego = timed_loop(ego_step, reps_e2e)
+        t_ego = timed_loop(ego_step)
         e2e = {"value": world_size * n * m / (t_ego * 1e-3), "unit": UNIT, "h2d_bytes_per_step": n * 2 * 4 + (n if world_size > 1 else 0),
                "d2h_bytes_per_step": 2 * n,
                "ms_per_step": t_ego,
@@ -537,7 +579,7 @@ def run_ours(args):
         if world_size == 1:
             # (2) every participant's action from the host (the round-1 figure): 8 N M bytes up per step
             host_act = [torch.from_numpy(synthetic.random_actions(500 + r, (n, m))).pin_memory() for r in range(min(R, 8))]
-            t_all = timed_loop(lambda i: worlds[i % R].step_host(host_act[i % len(host_act)]), reps_e2e)
+            t_all = timed_loop(lambda i: worlds[i % R].step_host(host_act[i % len(host_act)]))
             e2e["all_actions_from_host"] = {"value": n * m / (t_all * 1e-3), "unit": UNIT, "ms_per_step": t_all, "h2d_bytes_per_step": n * m * 2 * 4,
                                             "d2h_bytes_per_step": 2 * n, "api": "BatchedWorld.step_host(action [N, M, 2]) = t2d_step_host"}
             # (3) the Gym surface: BatchedTrafficEnv.step(ego action) -> observation views, reward, terminated, truncated, info,
@@ -561,7 +603,7 @@ def run_ours(args):
             l0 = lib.t2d_launch_count()
             env_step(0)
             per_call = int(lib.t2d_launch_count() - l0)
-            t_env = timed_loop(env_step, reps_e2e)
+            t_env = timed_loop(env_step, reset=env.reset)
             e2e["env_step"] = {"value": n * m / (t_env * 1e-3), "unit": UNIT, "ms_per_step": t_env, "h2d_bytes_per_step": n * 2 * 4,
                                "d2h_bytes_per_step": 6 * n, "our_launches_per_step": per_call,
                                "api": "BatchedTrafficEnv.step(ego action) with auto-reset: ego action H2D, reward + terminated + truncated D2H, sync"}
@@ -570,13 +612,6 @@ def run_ours(args):
     if rank == 0:
         peak, peak_src = _peaks()
         achieved = bytes_per_launch / (ms_per_step * 1e-3) / 1e9
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath):
-            try:
-                traffic = json.load(open(tpath)).get(args.config)
-            except Exception:
-                traffic = None
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world_size, "steps": K, "warmup": W,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong" if args.sharded else "weak", "vs_baseline": None,
@@ -584,15 +619,15 @@ def run_ours(args):
             "config": {"workload": scene0.name, "scenarios_per_gpu": n, "participants": m, "model": "SingleTrackKinematics" if args.config in ("c2", "c5") else args.config,
                        "interval_ms": 100, "delta_t_ms": 5, "map_segments": 0 if scene0.segments is None else int(len(scene0.segments)),
                        "l2_policy": f"inputs larger than L2: {R} world replicas x {bytes_per_launch / 1e6:.1f} MB rotate through the timed steps ({R * bytes_per_launch / 1e6:.0f} MB > {l2_bytes / 1e6:.0f} MB L2)",
-                       "timed_region": "CUDA graph of K steps" if graph is not None else "eager launch loop of K steps",
-                       "reps": len(reps_ms), "rep_ms_min": min(reps_ms), "rep_ms_max": max(reps_ms),
+                       "timed_region": (f"{len(chunks)} chunks of at most {C} steps ({TICKS_PER_CHUNK} ticks per replica), each from the "
+                                        "restored replicas: " + ("one CUDA-graph replay per chunk" if graph is not None else "eager launch loop")),
                        "collective": ("none (1 GPU)" if world_size == 1 else
                                       f"all-gather(done) per step by our own peer-memory kernel (t2d_exchange_allgather_lagged: put + signal per peer, wait, copy; lag {args.lag}: call k delivers the masks of step k - {args.lag}), side stream, overlaps the next tick" if peer is not None else
                                       "all_gather(done) per step (NCCL, side stream, overlaps the next tick)"),
                        "exchange_selfcheck": exchange_check, "prefetch_calibration": prefetch_cal},
-            "e2e": e2e, "gpu_launches": launches, "clocks": clocks,
+            "e2e": e2e, "gpu_launches": launches, "gpu": torch.cuda.get_device_name(device), "clocks": clocks,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src, "kernel": "t2d_step_kernel",
+                         "peak_source": peak_src, "kernel": "t2d_step_kernel",
                          "bytes_per_launch": bytes_per_launch,
                          "duration_us": ms_per_step * 1e3,
                          "note": "achieved = algorithmic bytes per launch / mean launch duration inside the timed CUDA-graph region"},
@@ -637,7 +672,9 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--exchange", choices=("peer", "nccl"), default="peer", help="N > 1: how the done masks are exchanged")
     ap.add_argument("--lag", type=int, default=2, help="peer exchange: deliver the gathered masks this many steps late (0 = synchronous)")
-    ap.add_argument("--steps", type=int, default=96)
+    ap.add_argument("--steps", type=int, default=None,
+                    help="timed steps, exactly (default: a window of about a second on an H100 - c2 40000, c3 / c4 10000, c5 500 - "
+                         "and 3 for --impl reference)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="c2", choices=["c2", "c3", "c4", "c5"])
@@ -645,14 +682,20 @@ def main():
     ap.add_argument("--scenarios", type=int, default=0, help="scenarios per GPU (with --sharded: of the whole job) instead of the configuration's")
     ap.add_argument("--sharded", action="store_true", help="strong scaling: the configuration's scenarios are split across the ranks")
     ap.add_argument("--no-prefetch-cal", action="store_true", help="N > 1: keep the library's prefetch policy instead of timing both settings")
-    ap.add_argument("--prefetch-cal-reps", type=int, default=15)
-    ap.add_argument("--min-reps", type=int, default=5)
-    ap.add_argument("--max-reps", type=int, default=400)
-    ap.add_argument("--min-seconds", type=float, default=2.0)
+    ap.add_argument("--prefetch-cal-reps", type=int, default=5)
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="--impl ours: write what the last timed step computed as DIR/<name>.npy (float32, at most 64 MB in all): "
+                         "the stepped world's state and step result (at N > 1: rank 0's shard) and, at N > 1, the gathered done masks")
     args = ap.parse_args()
+    if args.steps is None:
+        args.steps = 3 if args.impl == "reference" else {"c2": 40000, "c3": 10000, "c4": 10000, "c5": 500}[args.config]
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the GPU path's outputs: it needs --impl ours")
     if args.impl == "reference":
         run_reference(args)
     else:

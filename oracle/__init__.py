@@ -25,7 +25,7 @@ Parity pinning
 --------------
 * Physics (all four models, SingleTrackDrift included): PINNED.
   ``oracle/make_golden.py`` imports the *unmodified* reference
-  (``/root/reference/tactics2d/physics``) in the build container and writes
+  (``tactics2d/physics`` of a reference checkout) and writes
   ``tests/golden/physics_*.npz``; ``tests/test_oracle_golden.py`` holds the
   oracle to those vectors (<=1e-12 relative) and to the survey's KATs.
 * Controllers and lidar: PINNED to outputs of the unmodified reference classes

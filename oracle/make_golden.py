@@ -1,14 +1,13 @@
-"""Generate golden physics vectors from the UNMODIFIED reference (build container only).
+"""Generate golden physics vectors from the UNMODIFIED reference.
 
-TEST INFRASTRUCTURE ONLY.  Run here, where ``/root/reference`` exists:
+TEST INFRASTRUCTURE ONLY.  Run where a checkout of the reference (WoodOxen/tactics2d @ d7095aa) exists:
 
-    python oracle/make_golden.py            # writes tests/golden/physics_*.npz
+    T2D_REFERENCE=<reference checkout> python oracle/make_golden.py     # writes tests/golden/*.npz
 
 The reference's ``tactics2d.physics`` and ``tactics2d.participant.trajectory`` import
 with NumPy alone (SURVEY.md section 8c); nothing else of the reference is importable in
-this image (shapely / gymnasium absent).  The vectors are committed so that the GPU
-box (which has no ``/root/reference``) can hold both the oracle and the CUDA path to
-the reference's own numbers.  Action scripts replayed below are the reference test
+an environment without shapely / gymnasium.  The vectors are committed so that the tests
+hold both the oracle and the CUDA path to the reference's own numbers without the reference.  Action scripts replayed below are the reference test
 suite's ``VEHICLE_ACTION_LIST`` / ``PEDESTRIAN_ACTION_LIST`` (tests/test_physics.py:52-73).
 """
 
@@ -19,7 +18,7 @@ import sys
 
 import numpy as np
 
-REF = os.environ.get("T2D_REFERENCE", "/root/reference")
+REF = os.environ.get("T2D_REFERENCE")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 # medium_car, participant_template.py:78-95 ; ranges as Vehicle.load_from_template sets them
@@ -36,6 +35,8 @@ PEDESTRIAN_ACTION_LIST = [((0, 0), 100), ((1, 0), 500), ((-1, 0), 500), ((1, 0),
 
 
 def main():
+    if not REF or not os.path.isdir(os.path.join(REF, "tactics2d")):
+        sys.exit("set T2D_REFERENCE to a checkout of the reference (the directory that holds tactics2d/)")
     sys.path.insert(0, REF)
     from tactics2d.participant.trajectory import State
     from tactics2d.physics import PointMass, SingleTrackDynamics, SingleTrackKinematics

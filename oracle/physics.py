@@ -3,7 +3,7 @@
 Every function is vectorised over an arbitrary batch shape but performs, element
 by element, exactly the float64 operations of the reference in the reference's
 order; the reference lines are cited next to each block (paths relative to
-``/root/reference``).  Ranges that the reference stores as ``None`` (no
+a checkout of the reference).  Ranges that the reference stores as ``None`` (no
 constraint) are passed here as ``(-inf, +inf)``: ``np.clip`` with infinite
 bounds is the identity, which is what the reference's ``if range is not None``
 guard does.

@@ -1,6 +1,6 @@
-"""tactics2d_b200 - a B200-native batched ``env.step()`` for tactics2d.
+"""tactics2d_b200 - a GPU-native (H100, sm_90a) batched ``env.step()`` for tactics2d.
 
-One hot path, built from scratch for sm_100a behind the reference's class surface:
+One hot path, built from scratch for sm_90a behind the reference's class surface:
 per-participant physics (``tactics2d.physics``), pose (``tactics2d.participant``), collision /
 out-of-bound / time-limit events (``tactics2d.traffic``) and the Gym-style batched step/reset
 (``tactics2d.envs``), for N scenarios x M participants per call.  Host code is Python over a

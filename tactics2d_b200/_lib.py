@@ -1,6 +1,6 @@
 """ctypes binding of ``libt2d_b200.so`` (C ABI: ``include/t2d_b200.h``).
 
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is no
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is no
 CPU fallback: if the shared object is missing, loading fails loudly, and every compute entry
 point needs a CUDA device.
 """
@@ -94,7 +94,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a).  tactics2d_b200 has no CPU fallback.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a).  tactics2d_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SYMBOLS.items():
         fn = getattr(lib, name)

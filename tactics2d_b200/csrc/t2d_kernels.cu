@@ -1,4 +1,4 @@
-// t2d_kernels.cu - sm_100a kernels and the C ABI (include/t2d_b200.h) of the batched tick.
+// t2d_kernels.cu - sm_90a kernels and the C ABI (include/t2d_b200.h) of the batched tick.
 //
 // K1  t2d_step_kernel      fused physics -> pose -> dynamic collision (broadphase + filtered
 //                          narrowphase) -> static collision against the map tile in shared
@@ -295,14 +295,10 @@ __device__ __noinline__ void pair_resolve(int ti, int tj, int mp_shift, int psh,
   }
 }
 
-// Packed fp32 pair operations of the partner loop (T2D_SCALAR_PAIR: measurement builds fall back to two scalar operations).
-#if defined(T2D_SCALAR_PAIR)
+// Pair operations of the partner loop on two partners at once (sm_90 has no packed fp32 instructions: two scalar
+// operations each, the same roundings).
 __device__ __forceinline__ float2 pk_add(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 pk_fma(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-#else
-__device__ __forceinline__ float2 pk_add(float2 a, float2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ float2 pk_fma(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-#endif
 
 // One word of the partner loop = IPW iterations x PPL own participants x 2 partners.  X / Y: the partner positions of
 // the word's iterations (two per float2); nx2 / ny2: the lane's own positions, negated; nthr2: minus the squared
@@ -671,11 +667,10 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
   bool staged = false;
   // L2 prefetch of the first tile's state / action lines while the previous grid drains (its CTAs retire over a
   // microsecond or two; ours take their places one by one and would otherwise just sit in griddepcontrol.wait): L2 is the
-  // coherence point of the GPU, so a line fetched early can never be stale when it is loaded after the wait.  Measured
-  // at 4096 x 64 with cold inputs: 13.7 -> 12.65 us per tick on one GPU.  With a peer-memory done exchange running under
-  // the tick (8 GPUs) the same build measured SLOWER than without the prefetch (16.9 vs 14.25 us per step: the burst of
-  // prefetches competes with the exchange kernel's peer stores and system-scope fence, and the exchange chain then sets
-  // the pace), so the host leaves it off while an exchange object is alive in the process (T2D_PREFETCH=0 / 1 overrides).
+  // coherence point of the GPU, so a line fetched early can never be stale when it is loaded after the wait.  With a
+  // peer-memory done exchange running under the tick the burst of prefetches competes with the exchange kernel's peer
+  // stores and system-scope fence, and the exchange chain then sets the pace, so the host leaves it off while an
+  // exchange object is alive in the process (T2D_PREFETCH=0 / 1 overrides).
   {
     const long long n_ = ((long long)blockIdx.x * wpc + warp) * (32 >> A.g_shift) + (lane >> A.g_shift);
     const int m_ = (lane & (A.G - 1)) * PPL;
@@ -713,7 +708,7 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
     if (nvalid < 0) nvalid = 0;
     const long long idx0 = n * M + m0;
 
-#if defined(T2D_DEBUG_CLOCK)   // phase time stamps: measurement builds only (profiles/phase_clocks.py)
+#if defined(T2D_DEBUG_CLOCK)   // phase time stamps: measurement builds only
     // `dep`: a late result of the phase that ends here.  The (never taken) branch on it cannot be resolved before the value
     // has arrived, so the stamp charges a phase with the latency it creates instead of leaking it into the next one.
     #define T2D_STAMP(k, dep) do { if (A.dbg_clock) { if (__float_as_int((float)(dep)) == 0x7fbfffff) asm volatile("trap;"); \
@@ -813,7 +808,7 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
     T2D_STAMP(1, sx[0] + sy[PPL - 1] + shd[0] + sv[PPL - 1] + a0[0] + a1[PPL - 1] + (float)tidv[0]);
     // ------------------------------------------------------------------ physics
     if (A.do_physics) {
-      // Kinematic participants of the whole warp advance together in the packed 4-chain loop; slots holding another
+      // Kinematic participants of the whole warp advance together in the 4-chain loop; slots holding another
       // model (or nothing) ride along on a neutral row (zero speed / action, unbounded ranges) and are discarded.
       if (__any_sync(0xffffffffu, lane_any_kin)) {
         const Params* const null_row = &s_table[A.n_types];
@@ -949,8 +944,8 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
     int hit[PPL];
     {
       // hot loop: every lane runs it (idle slots hold NaN and never pass); branch-free; two partners per
-      // iteration in packed fp32 (FADD2 / FFMA2).  Per pair the margin d^2 - thr is formed by two fused multiply-adds
-      // and folded into a running minimum over the 32 tests of a word (one 3-input FMNMX per partner pair); only a
+      // iteration.  Per pair the margin d^2 - thr is formed by two fused multiply-adds
+      // and folded into a running minimum over the 32 tests of a word; only a
       // word whose minimum is <= 0 (rare) recomputes its verdict bits and goes to the out-of-line enqueue.
       float2 nx2[PPL], ny2[PPL], nthr2[PPL];
 #pragma unroll
@@ -1775,7 +1770,7 @@ struct t2d_ctx {
   float *x = nullptr, *y = nullptr, *h = nullptr, *v = nullptr, *vx = nullptr, *vy = nullptr;
   const uint8_t* type_id = nullptr;
   int32_t* step_count = nullptr;
-  int sm_count = 148;
+  int sm_count = 0;                // set by t2d_create from the device
   int max_smem_optin = 0;
   float rb_max = 0.0f;
   const float* ego_action = nullptr;   // t2d_set_ego_action
@@ -1843,7 +1838,7 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
   c->device = device;
   c->N = n_scenarios;
   c->M = m_participants;
-  // participants per lane: 4 (2 was measured on B200 at 4096 x 64 in both rounds: 55 % more instructions, 21.5 vs 13.9 us)
+  // participants per lane: 4 (2 per lane executes about 55 % more instructions per participant)
   const int ppl = 4;
   c->ppl = ppl;
   if (const char* e = getenv("T2D_PDL")) c->use_pdl = atoi(e) != 0;
@@ -1929,7 +1924,7 @@ int t2d_set_type_table(t2d_ctx* c, const t2d_type_params* table, int n_types) {
       rows[i] = derive_params(a);
     }
     {
-      // row n_types: the neutral kinematic row that K1's packed loop gives to slots holding another model or nothing
+      // row n_types: the neutral kinematic row that K1's 4-chain loop gives to slots holding another model or nothing
       // (zero speed and action in, unbounded ranges: every product stays finite and the result is discarded)
       AbiParams a{};
       a.lf = 1.0f; a.lr = 1.0f;
@@ -2217,9 +2212,11 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 // Warps per CTA of the tick.  One wave (the usual case: every warp tile is resident at once and the kernel's duration is
 // one tile's lifetime): the SM with the most warps sets the pace, and every CTA costs a launch + prologue (barrier
-// init, TMA staging) - measured on B200 at 4096 x 64: ~0.19 us per extra warp on the fullest SM, ~0.08 us per CTA on it
-// (2 x 7 warps: 16.4 us, 7 x 2: 16.8 us, 3 x 5: 16.7 us, 2 x 8: 17.0 us, 3 x 6 - a second wave at 128 registers - 23.9 us;
-// 1-warp CTAs are far worse and are not considered).  Several waves: persistent CTAs of the largest size.
+// init, TMA staging), weighed below as 0.42 of a warp on the fullest SM (1-warp CTAs are not considered: the prologue
+// is paid per warp there).  Several waves: persistent CTAs of the largest size.  On an H100 (132 SMs) 4096 x 64 is 2048 warp
+// tiles, more than the conservative 132 x 14, so it takes 8-warp CTAs; at the launch bounds' 2 CTAs per SM all 256 of them are
+// resident at once anyway (one wave).  On an H100 80GB HBM3 SXM at a 400 W power limit (T2D_WPC, 40000 timed steps) 8 and 4 warps
+// per CTA measured within 2 % of each other and 2 warps per CTA about 45 % slower.
 static int pick_wpc(long long tiles, int sm_count) {
   const int resident_warps = 14;   // per SM at the kernel's register budget, rounded down to what every variant reaches
   if (tiles > (long long)sm_count * resident_warps) return MAX_WARPS_PER_CTA;
@@ -2399,9 +2396,9 @@ int t2d_step_host(t2d_ctx* c, const float* action_host, uint8_t* flags, int16_t*
     for (cudaEvent_t& e : c->hs_chunk) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   }
   // Chunks of whole scenarios: the copy of chunk k + 1 (copy engine, own stream) runs under the kernel of chunk k.
-  // Measured on B200 (profiles/r01_e2e_probe.txt): at 4096 x 64 the 2 MiB upload is ~50 us against a 21 us kernel
-  // whose duration is one tile's lifetime whatever the batch, so splitting only adds ~3.5 us per chunk; it pays
-  // once a chunk alone fills the GPU, i.e. from ~1 M participants (8 MiB of actions) per chunk upwards.
+  // A kernel that does not fill the GPU lasts one tile's lifetime whatever the batch, so splitting a small upload only
+  // adds a fixed cost per chunk; it pays once a chunk alone fills the GPU, i.e. from ~1 M participants (8 MiB of
+  // actions) per chunk upwards.
   int chunks = c->host_chunks;
   if (chunks <= 0) chunks = (int)std::min<long long>(t2d_ctx::MAX_HOST_CHUNKS, std::max<long long>(1, (long long)N * M / (1 << 20)));
   int per = (N + chunks - 1) / chunks;
@@ -2761,7 +2758,9 @@ int t2d_physics_step(int device, const t2d_type_params* params, int interval_ms,
   A.dt_d = (double)delta_t / 1000.0;
   A.dt_rem_d = (double)(interval_ms % delta_t) / 1000.0;
   A.interval_d = (double)interval_ms / 1000.0;
-  const int grid = std::min((n + 255) / 256, 148 * 8);
+  int sms = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  const int grid = std::min((n + 255) / 256, sms * 8);
   t2d_physics_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(A);
   g_launches.fetch_add(1);
   CUDA_TRY(cudaGetLastError());

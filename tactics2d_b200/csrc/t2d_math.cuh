@@ -1,7 +1,7 @@
 // t2d_math.cuh - per-participant physics and per-pair predicates of the batched tick.
 //
 // Everything here is a pure function of its arguments so that the same source is
-//   * inlined into the sm_100a kernels (t2d_kernels.cu), and
+//   * inlined into the sm_90a kernels (t2d_kernels.cu), and
 //   * compiled by g++ into tests/hostsim (a unit-test harness that checks this arithmetic
 //     against the float64 oracle without a GPU; it is NOT a product fallback).
 //
@@ -11,7 +11,7 @@
 //     with a short polynomial for the small increment, and the position / heading sums are
 //     accumulated separately and added to the state once (one rounding at |x| scale).
 //   * SingleTrackDynamics: fp64 (the yaw/slip ODE is stiff below ~0.4 m/s, explicit Euler
-//     amplifies rounding by up to (0.745/v - 1)^20 there; B200 issues DFMA at half FFMA rate).
+//     amplifies rounding by up to (0.745/v - 1)^20 there; H100 issues DFMA at half FFMA rate).
 //   * PointMass: fp64 arithmetic on the fp32 state (a few dozen flops).
 //   * Collision predicates: fp32 with a forward error bound ("filtered predicate"); a pair
 //     whose margin is inside the bound is re-evaluated exactly as the float64 oracle does
@@ -137,7 +137,7 @@ T2D_HD int float_bits(float f) {
 #endif
 
 // Round-to-nearest-integer without the conversion unit: adding 1.5 * 2^23 leaves rint(u) in the low mantissa bits
-// (|u| < 2^22).  On sm_100a FRND / F2I run on the quarter-rate XU pipe, the busiest pipe of the tick before this.
+// (|u| < 2^22): FRND / F2I would run on the quarter-rate conversion pipe.
 constexpr float RINT_MAGIC = 12582912.0f;
 
 // np.mod(phi, 2*pi) for an fp32 angle: result in [0, 2*pi) (Cody-Waite two-term reduction).  q = rint(phi / 2 pi - 1/2)
@@ -205,8 +205,7 @@ T2D_HD void sincos_fast(float x, float* sn, float* cs) {
 constexpr float SIN_C3 = -1.6666667e-1f, SIN_C5 = 8.3333333e-3f;
 constexpr float COS_C2 = -0.5f, COS_C4 = 4.1666667e-2f, COS_C6 = -1.3888889e-3f;
 
-// (c, s) <- (c, s) rotated by d, given d and nd = -d.  Written as the exact operation sequence the packed
-// (FFMA2) kernel path uses, so that the scalar and packed paths are bit-identical.
+// (c, s) <- (c, s) rotated by d, given d and nd = -d.
 T2D_HD void rotate_small(float& c, float& s, float d, float nd) {
   const float dd = d * d;
   const float ts = fmaf(dd, fmaf(dd, SIN_C5, SIN_C3), 1.0f);
@@ -324,8 +323,8 @@ T2D_HD void kinematics_step(KinIO<W>& io, const Params* const (&p)[W], int n_ste
   // angles d_i = k dt v_i form an arithmetic sequence with the tiny step e = k dt a dt (<= 1e-4).  Instead of
   // evaluating the sin / cos polynomials of d_i every sub-step, carry (cos d_i - 1, -sin d_i) along by rotating them
   // by e (two adds + two fmas; sin e = e and cos e - 1 = -e^2 / 2 to fp32 precision, products with e^2 dropped),
-  // and drop the speed clamp and the running speed sum (closed form).  12 packed operations per pair of participants
-  // and sub-step instead of 17 packed + 4 scalar.  The scalar and packed forms perform the same operations.
+  // and drop the speed clamp and the running speed sum (closed form).  12 operations per participant and sub-step
+  // instead of 19.
   // One loop per warp: lanes that could take the fast loop next to lanes that cannot would make the warp run both, so
   // the warp takes it only when every lane that is executing this function can (the general loop is valid for all).
 #if defined(__CUDA_ARCH__)
@@ -348,52 +347,6 @@ T2D_HD void kinematics_step(KinIO<W>& io, const Params* const (&p)[W], int n_ste
     float v[W];
 #pragma unroll
     for (int i = 0; i < W; ++i) v[i] = io.v[i];
-    // (The packed FFMA2 form of this loop - two participants per instruction, the same operations - is kept for measurement
-    //  builds, -DT2D_PACKED_KIN_LOOP: on B200 it is no faster than four scalar chains, 13.9 vs 13.7 us per tick at 4096 x 64:
-    //  FFMA2 occupies the FMA pipe for two cycles, and four independent scalar chains hide their latency better than two packed ones.)
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000) && defined(T2D_PACKED_KIN_LOOP)
-    if constexpr (W == 4) {
-      float2 C2[2], S2[2], V2[2], SX2[2], SY2[2], H2[2], NSN2[2], SE2[2], NSE2[2], HE2[2], ADT2[2], W12[2];
-#pragma unroll
-      for (int q = 0; q < 2; ++q) {
-        C2[q] = make_float2(c[2 * q], c[2 * q + 1]);
-        S2[q] = make_float2(s[2 * q], s[2 * q + 1]);
-        V2[q] = make_float2(v[2 * q], v[2 * q + 1]);
-        SX2[q] = make_float2(0.0f, 0.0f); SY2[q] = SX2[q];
-        H2[q] = make_float2(h[2 * q], h[2 * q + 1]);
-        NSN2[q] = make_float2(nsn[2 * q], nsn[2 * q + 1]);
-        SE2[q] = make_float2(se[2 * q], se[2 * q + 1]);
-        NSE2[q] = make_float2(nse[2 * q], nse[2 * q + 1]);
-        HE2[q] = make_float2(he[2 * q], he[2 * q + 1]);
-        ADT2[q] = make_float2(adt[2 * q], adt[2 * q + 1]);
-        W12[q] = make_float2(w1[2 * q], w1[2 * q + 1]);
-      }
-      float fi = -1.0f;
-#pragma unroll 2
-      for (int it = 0; it < n_steps; ++it) {
-        fi += 1.0f;
-        const float2 FI = make_float2(fi, fi);
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          SX2[q] = __ffma2_rn(V2[q], C2[q], SX2[q]);
-          SY2[q] = __ffma2_rn(V2[q], S2[q], SY2[q]);
-          const float2 sn = make_float2(-NSN2[q].x, -NSN2[q].y);   // folds into the FFMA2 operand's negate modifier
-          const float2 cn = __ffma2_rn(S2[q], NSN2[q], __ffma2_rn(C2[q], H2[q], C2[q]));
-          const float2 sm = __ffma2_rn(C2[q], sn, __ffma2_rn(S2[q], H2[q], S2[q]));
-          const float2 hn = __ffma2_rn(NSN2[q], SE2[q], __fadd2_rn(H2[q], HE2[q]));
-          const float2 nn = __ffma2_rn(H2[q], NSE2[q], __fadd2_rn(NSN2[q], NSE2[q]));
-          C2[q] = cn; S2[q] = sm; H2[q] = hn; NSN2[q] = nn;
-          V2[q] = __ffma2_rn(FI, ADT2[q], W12[q]);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 2; ++q) {
-        c[2 * q] = C2[q].x; c[2 * q + 1] = C2[q].y; s[2 * q] = S2[q].x; s[2 * q + 1] = S2[q].y;
-        v[2 * q] = V2[q].x; v[2 * q + 1] = V2[q].y;
-        Sx[2 * q] = SX2[q].x; Sx[2 * q + 1] = SX2[q].y; Sy[2 * q] = SY2[q].x; Sy[2 * q + 1] = SY2[q].y;
-      }
-    } else
-#endif
     {
       float fi = -1.0f;
       T2D_KIN_UNROLL_PRAGMA
@@ -424,62 +377,7 @@ T2D_HD void kinematics_step(KinIO<W>& io, const Params* const (&p)[W], int n_ste
 #pragma unroll
   for (int i = 0; i < W; ++i) v[i] = io.v[i];
   // main sub-steps :137-148 ; derivatives from the OLD (phi, v), then v clipped
-  bool looped = false;
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000)
-  // Blackwell packed fp32: two participants per FFMA2 / FMUL2 / FADD2 (SASS FFMA2 ...), the same operation
-  // sequence as rotate_small() lane by lane, so the results are bit-identical to the scalar path.
-  if constexpr (W == 4) {
-    if (small) {
-      float2 C2[2], S2[2], V2[2], SX2[2], SY2[2], SV2[2], KDT2[2], NKDT2[2], ADT2[2], W12[2];
-#pragma unroll
-      for (int q = 0; q < 2; ++q) {
-        C2[q] = make_float2(c[2 * q], c[2 * q + 1]);
-        S2[q] = make_float2(s[2 * q], s[2 * q + 1]);
-        V2[q] = make_float2(v[2 * q], v[2 * q + 1]);
-        SX2[q] = make_float2(0.0f, 0.0f); SY2[q] = SX2[q]; SV2[q] = SX2[q];
-        KDT2[q] = make_float2(kdt[2 * q], kdt[2 * q + 1]);
-        NKDT2[q] = make_float2(-kdt[2 * q], -kdt[2 * q + 1]);
-        ADT2[q] = make_float2(adt[2 * q], adt[2 * q + 1]);
-        W12[q] = make_float2(w1[2 * q], w1[2 * q + 1]);
-      }
-      const float2 K_S5 = make_float2(SIN_C5, SIN_C5), K_S3 = make_float2(SIN_C3, SIN_C3), K_ONE = make_float2(1.0f, 1.0f);
-      const float2 K_C6 = make_float2(COS_C6, COS_C6), K_C4 = make_float2(COS_C4, COS_C4), K_C2 = make_float2(COS_C2, COS_C2);
-      float fi = -1.0f;
-      for (int it = 0; it < n_steps; ++it) {
-        fi += 1.0f;
-        const float2 FI = make_float2(fi, fi);
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          SX2[q] = __ffma2_rn(V2[q], C2[q], SX2[q]);
-          SY2[q] = __ffma2_rn(V2[q], S2[q], SY2[q]);
-          SV2[q] = __fadd2_rn(SV2[q], V2[q]);
-          const float2 d = __fmul2_rn(KDT2[q], V2[q]), nd = __fmul2_rn(NKDT2[q], V2[q]);
-          const float2 dd = __fmul2_rn(d, d);
-          const float2 ts = __ffma2_rn(dd, __ffma2_rn(dd, K_S5, K_S3), K_ONE);
-          const float2 sn = __fmul2_rn(d, ts), nsn = __fmul2_rn(nd, ts);
-          const float2 nhv = __fmul2_rn(dd, __ffma2_rn(dd, __ffma2_rn(dd, K_C6, K_C4), K_C2));
-          const float2 cn = __ffma2_rn(S2[q], nsn, __ffma2_rn(C2[q], nhv, C2[q]));
-          const float2 sm = __ffma2_rn(C2[q], sn, __ffma2_rn(S2[q], nhv, S2[q]));
-          C2[q] = cn;
-          S2[q] = sm;
-          const float2 wn = __ffma2_rn(FI, ADT2[q], W12[q]);
-          V2[q].x = clampf(wn.x, vlo[2 * q], vhi[2 * q]);
-          V2[q].y = clampf(wn.y, vlo[2 * q + 1], vhi[2 * q + 1]);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < 2; ++q) {
-        c[2 * q] = C2[q].x; c[2 * q + 1] = C2[q].y; s[2 * q] = S2[q].x; s[2 * q + 1] = S2[q].y;
-        v[2 * q] = V2[q].x; v[2 * q + 1] = V2[q].y;
-        Sx[2 * q] = SX2[q].x; Sx[2 * q + 1] = SX2[q].y; Sy[2 * q] = SY2[q].x; Sy[2 * q + 1] = SY2[q].y;
-        Sv[2 * q] = SV2[q].x; Sv[2 * q + 1] = SV2[q].y;
-      }
-      looped = true;
-    }
-  }
-#endif
-  if (looped) {
-  } else if (small) {
+  if (small) {
     float fi = -1.0f;
     for (int it = 0; it < n_steps; ++it) {
       fi += 1.0f;
@@ -525,8 +423,8 @@ struct OneIO {
   float w0, w1;              // SingleTrackDrift only: front / rear wheel angular speed in / out
 };
 
-// Written over W participants side by side; the kernels use W = 1 (two at a time was measured on B200: the call's
-// register footprint cost more than the second fp64 chain gained - C3 58.7 -> 69.1 us).
+// Written over W participants side by side; the kernels use W = 1 (a second fp64 chain per call enlarges the call's
+// register footprint, which bounds the occupancy of K1).
 template <int W>
 T2D_HD void dynamics_step_n(OneIO* const (&io)[W], const Params* const (&pp)[W], int n_steps, double dt) {
   double x[W], y[W], phi[W], v[W], d_phi[W], beta[W], sn[W], cs[W];

@@ -17,8 +17,8 @@ on-disk format to that tile; it follows the reference's own parsing rules:
                                                               (parse_osm.py:461-510, chaining rule :37-60).
 
 The tiles of the reference's 13 bundled maps (``data/{highD,inD,rounD}_map/*.osm``) are compiled once in
-the build container (``python -m tactics2d_b200.map`` -> ``tactics2d_b200/map/tiles/*.npz``) because
-``/root/reference`` does not exist on the GPU box.
+advance (``python -m tactics2d_b200.map <reference>/data`` -> ``tactics2d_b200/map/tiles/*.npz``) and ship with the
+package, so that nothing at run time needs the reference's map files.
 """
 
 from __future__ import annotations

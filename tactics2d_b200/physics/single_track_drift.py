@@ -2,7 +2,7 @@
 
 Constructor, ``step(state, omega_wf, omega_wr, accel, delta, interval) -> (State, omega_wf, omega_wr, accel, delta)``
 and ``verify_state`` follow the reference's ``tactics2d/physics/single_track_drift.py`` (:98-183, :467-499, :501-556).
-The integration (:340-465, tyre forces :185-338) runs in the sm_100a kernels in fp64, with the reference's built-in
+The integration (:340-465, tyre forces :185-338) runs in the sm_90a kernels in fp64, with the reference's built-in
 ``Tire`` coefficients (:14-49; a custom tyre object is not supported - the coefficients are compile-time constants of
 the kernel).  Unlike ``SingleTrackDynamics`` this model takes the remainder sub-step (:352-355) and carries the two
 wheel speeds from call to call; the returned State has ``vx = vy = None`` (:457-464).

@@ -4,7 +4,7 @@ Constructor (extra ``mass, mass_height, mu=0.7, I_z=1500, cf=cr=20.89``), ``step
 follow the reference's ``tactics2d/physics/single_track_dynamics.py`` (:58-138, :231-251, :253-303).  The
 model carries no hidden state between calls (:159-160 re-derive the yaw rate and slip angle per call) and has
 no remainder sub-step (:143); the returned State has ``vx = vy = None`` as in the reference (:220-227).
-The integration (:140-229) runs in the sm_100a kernels in fp64.
+The integration (:140-229) runs in the sm_90a kernels in fp64.
 """
 
 from __future__ import annotations

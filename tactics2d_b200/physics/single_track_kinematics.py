@@ -3,7 +3,7 @@
 Constructor, ``step`` signature / return value and ``verify_state`` follow the reference's
 ``tactics2d/physics/single_track_kinematics.py`` (:62-124 constructor and range rules, :178-198 ``step`` ->
 ``(State, accel, delta)`` with the clipped action, :200-250 ``verify_state``).  The integration itself
-(:126-176) runs in the sm_100a kernels: a single ``State`` goes through a batch of one; ``step_batch``
+(:126-176) runs in the sm_90a kernels: a single ``State`` goes through a batch of one; ``step_batch``
 advances n participants per launch.
 """
 

@@ -2,7 +2,7 @@
 
 This is the object behind the reference-shaped facades (``physics``, ``traffic``, ``envs``): it
 owns the fp32 SoA tensors, the C-ABI context, and forwards ``step`` / ``check_events`` / ``reset``
-to the sm_100a kernels.  PyTorch is only the device-memory container (``tensor.data_ptr()``) and
+to the sm_90a kernels.  PyTorch is only the device-memory container (``tensor.data_ptr()``) and
 the stream provider; there is no eager/CPU implementation behind it.
 
 Replaces the per-object loop of the reference tick: ``ScenarioManager.update`` ->
@@ -59,7 +59,7 @@ class BatchedWorld:
                  interval: int = 100, delta_t: int = 5, max_step: Optional[int] = None,
                  any_participant: bool = False, steer_first: bool = False):
         if not torch.cuda.is_available():
-            raise RuntimeError("tactics2d_b200 needs a CUDA device: the batched tick only exists as sm_100a kernels")
+            raise RuntimeError("tactics2d_b200 needs a CUDA device: the batched tick only exists as sm_90a kernels")
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":

@@ -10,12 +10,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: run with -m gpu)")
 
 
 def pytest_sessionstart(session):
     """The CUDA library is built in-tree (git-ignored): build it when it is missing or stale so that a fresh
-    checkout can run the suite (nvcc cross-compiles sm_100a without a GPU)."""
+    checkout can run the suite (nvcc cross-compiles sm_90a without a GPU)."""
     import shutil
 
     if shutil.which("nvcc") or os.path.exists("/usr/local/cuda/bin/nvcc"):

@@ -326,7 +326,7 @@ def test_reset_pool(cuda_device):
 # ---------------------------------------------------------------------------- the reference's own map files
 def test_config3_dynamics_on_highD_tile(cuda_device):
     """BASELINE.json configs[2]: SingleTrackDynamics + map-polyline collision on the highD_1 tile (compiled from
-    /root/reference/data/highD_map/highD_1.osm by tactics2d_b200.map; solid lane markings = road edges)."""
+    data/highD_map/highD_1.osm of the reference checkout by tactics2d_b200.map; solid lane markings = road edges)."""
     from tactics2d_b200 import synthetic
     from tactics2d_b200.map import load_collidable_segments
 

@@ -1,5 +1,5 @@
 """The oracle is pinned to the UNMODIFIED reference: golden vectors written by
-oracle/make_golden.py (which imports /root/reference/tactics2d/physics) and the survey's
+oracle/make_golden.py (which imports the reference's tactics2d/physics) and the survey's
 known-answer table (SURVEY.md section 8c)."""
 
 import os
