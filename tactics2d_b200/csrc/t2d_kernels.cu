@@ -1973,9 +1973,13 @@ static int build_tile(const TileIn& t, float cell_size, float reach, std::vector
   for (int p = 0; p < t.n_poly; ++p) {
     const int s0 = t.poly_start[p], s1 = t.poly_start[p + 1];
     if (s0 < 0 || s1 > n_seg || s1 - s0 < 3 || (p > 0 && s0 < t.poly_start[p])) return fail(T2D_E_INVALID, "poly_start: rings must be ascending, inside the segment list and have >= 3 edges");
-    for (int i = s0; i < s1; ++i) {   // a ring: every edge ends where the next one starts, the last one at the first one's start
-      const int j = i + 1 < s1 ? i + 1 : s0;
-      if (segments[4 * i + 2] != segments[4 * j] || segments[4 * i + 3] != segments[4 * j + 1]) return fail(T2D_E_INVALID, "poly_start: a ring's edges must chain and close");
+    // one object = one or more closed rings back to back (an Area's exterior, then its holes): every edge ends where the
+    // next one starts, except the edge that returns to its ring's first vertex - the next edge starts the next ring
+    int r0 = s0;
+    for (int i = s0; i < s1; ++i) {
+      if (segments[4 * i + 2] == segments[4 * r0] && segments[4 * i + 3] == segments[4 * r0 + 1]) { r0 = i + 1; continue; }
+      if (i + 1 == s1 || segments[4 * i + 2] != segments[4 * (i + 1)] || segments[4 * i + 3] != segments[4 * (i + 1) + 1])
+        return fail(T2D_E_INVALID, "poly_start: a ring's edges must chain and close");
     }
   }
   MapHeader mh{};

@@ -137,6 +137,14 @@ class BatchedWorld:
         cfg = _lib.Config(self.interval, self.delta_t, self.max_step, self.flags_cfg)
         _lib.check(self.lib.t2d_set_config(self._ctx, C.byref(cfg)))
 
+    def set_type_table(self, type_table: TypeTable):
+        """Replace the type table.  The map stays as it was built: its dilated cell lists cover the reach of the table
+        that was current at ``set_map``, and a participant whose type reaches further takes the slower exhaustive walk."""
+        if any(r.model == MODEL_DRIFT for r in type_table.rows) and self.omega_front is None:
+            raise ValueError("a SingleTrackDrift row needs a world created with one (its wheel speeds are allocated there)")
+        _lib.check(self.lib.t2d_set_type_table(self._ctx, type_table.to_c_array(), len(type_table)))
+        self.type_table = type_table
+
     def set_map(self, segments=None, bounds: Optional[Sequence[float]] = None, cell_size: float = 0.0, poly_start=None):
         """Static geometry of the scenario (shared by all N scenarios).
 

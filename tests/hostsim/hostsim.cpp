@@ -57,12 +57,13 @@ void hs_kinematics4(int n, const AbiParams* ap, int n_steps, double dt, double d
   }
 }
 
-// pose rows: x, y, heading, l, w  (w < 0: disc of radius l).  out_f32: -1/0/1 filter verdict; out_exact: 0/1
+// pose rows: x, y, heading, l, w  (w < 0: disc of radius l).  out_f32: -1/0/1 filter verdict; out_exact: 0/1.
+// The filters take (cos, sin) of the heading from sincos_fast, as K1's poses do.
 void hs_pairs(int n, const float* a, const float* b, int32_t* out_f32, int32_t* out_exact) {
   for (int i = 0; i < n; ++i) {
     const float* pa = a + 5 * i; const float* pb = b + 5 * i;
     float sa, ca, sb, cb;
-    sincosf(pa[2], &sa, &ca); sincosf(pb[2], &sb, &cb);
+    sincos_fast(pa[2], &sa, &ca); sincos_fast(pb[2], &sb, &cb);
     const bool ka = pa[4] < 0, kb = pb[4] < 0;
     int r; bool e;
     if (!ka && !kb) { r = obb_obb_f32(pa[0], pa[1], ca, sa, pa[3], pa[4], pb[0], pb[1], cb, sb, pb[3], pb[4]);
@@ -81,7 +82,7 @@ void hs_segments(int n, const float* a, const float* seg, int32_t* out_f32, int3
   for (int i = 0; i < n; ++i) {
     const float* pa = a + 5 * i; const float* s = seg + 4 * i;
     float sa, ca;
-    sincosf(pa[2], &sa, &ca);
+    sincos_fast(pa[2], &sa, &ca);
     if (pa[4] < 0) { out_f32[i] = circle_segment_f32(pa[0], pa[1], pa[3], s[0], s[1], s[2], s[3]);
                      out_exact[i] = circle_segment_f64(pa[0], pa[1], pa[3], s[0], s[1], s[2], s[3]); }
     else { out_f32[i] = obb_segment_f32(pa[0], pa[1], ca, sa, pa[3], pa[4], s[0], s[1], s[2], s[3]);
@@ -93,7 +94,7 @@ void hs_outbound(int n, const float* a, const float* bounds, int32_t* out_f32, i
   for (int i = 0; i < n; ++i) {
     const float* pa = a + 5 * i;
     float sa, ca;
-    sincosf(pa[2], &sa, &ca);
+    sincos_fast(pa[2], &sa, &ca);
     out_f32[i] = out_of_bound_f32(pa[0], pa[1], ca, sa, pa[3], pa[4], pa[4] < 0, bounds[0], bounds[1], bounds[2], bounds[3]);
     out_exact[i] = out_of_bound_f64(pa[0], pa[1], pa[2], pa[3], pa[4], pa[4] < 0, bounds[0], bounds[1], bounds[2], bounds[3]);
   }
