@@ -333,12 +333,6 @@ int t2d_physics_step(int device, const t2d_type_params* params /*host*/, int int
                      float* x, float* y, float* heading, float* speed, float* vx, float* vy, float* omega_front,
                      float* omega_rear, const float* action, float* applied, void* stream);
 
-/* Diagnostics for ad-hoc profiling of a library built with -DT2D_DEBUG_CLOCK (a normal build ignores the buffer): device
- * buffer int64[ceil(N / scenarios_per_warp)][10] that receives clock64() at the eight phase boundaries of every warp tile of
- * t2d_step (load, physics, pose, pair loop, pair drain, static, out-of-bound, end), the SM id and the warp's kernel-entry
- * clock.  NULL (default) disables it. */
-int t2d_debug_set_clock_buffer(t2d_ctx* ctx, long long* device_buffer);
-
 /* Tuning knob of t2d_step, no effect on results: the tick can ask L2 for its first input lines while the previous grid is
  * still draining (and for the next tile inside its persistent loop).  mode 1: on, 0: off, -1 (default): on unless a
  * peer-memory done exchange is alive in the process (on one GPU it saves ~1 us per tick at 4096 x 64; next to the

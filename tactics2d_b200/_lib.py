@@ -78,7 +78,6 @@ SYMBOLS = {
     "t2d_physics_step": (C.c_int, [C.c_int, C.POINTER(TypeParamsC), C.c_int, C.c_int, C.c_int] + [_P] * 11),
     "t2d_bind_wheel_state": (C.c_int, [_P, _P, _P]),
     "t2d_bind_reset_wheel_pool": (C.c_int, [_P, _P, _P]),
-    "t2d_debug_set_clock_buffer": (C.c_int, [_P, _P]),
     "t2d_set_prefetch": (C.c_int, [_P, C.c_int]),
     "t2d_launch_count": (C.c_int64, []),
 }

@@ -35,12 +35,10 @@
 
 namespace t2d {
 
-#ifndef T2D_K1_MAX_WARPS
-#define T2D_K1_MAX_WARPS 8
-#endif
-constexpr int MAX_WARPS_PER_CTA = T2D_K1_MAX_WARPS;
+constexpr int MAX_WARPS_PER_CTA = 8;
 constexpr int CTA_THREADS = MAX_WARPS_PER_CTA * 32;   // upper bound; the host picks the warps per CTA (pick_wpc)
-constexpr int POSE_PER_WARP = 128;      // 32 lanes x 4 participants per lane (PPL, template parameter of K1: 2 or 4)
+constexpr int PPL = 4;                  // participants per lane of K1
+constexpr int POSE_PER_WARP = 32 * PPL;
 constexpr int MAP_SMEM_LIMIT = 120 * 1024;
 
 struct MapHeader {   // 128 bytes, start of a tile's blob
@@ -103,7 +101,6 @@ struct StepArgs {
   int32_t* goal_noact_count;       // [N]
   float goal_threshold;
   int goal_noact_max;
-  long long* dbg_clock;            // optional [n_tiles][8] phase time stamps (T2D_DEBUG_CLOCK); nullptr in production
   float *wheel_f, *wheel_r;        // [N][M] wheel angular speeds of the SingleTrackDrift participants, or nullptr
 };
 
@@ -219,7 +216,7 @@ __device__ __noinline__ void other_model_step(OneIO& io, const Params& p, int n_
 
 // Static broadphase, level 1: the clearance field.  One shared-memory load tells whether the pose's
 // bounding circle can reach any segment at all (most participants are nowhere near a wall).
-// near_segments split in two so that the global byte load can be issued early and consumed late:
+// The test is split in two so that the global byte load can be issued early and consumed late:
 // near_fetch returns the quantised clearance under the participant (0 = treat as near: outside the grid but within
 // reach of it; 255 = far), near_decide compares it with the bounding radius.
 __device__ __forceinline__ unsigned near_fetch(const float ax, const float ay, const float rbound, const MapHeader& mh, const uint8_t* fine,
@@ -251,30 +248,16 @@ __device__ __forceinline__ bool near_decide(unsigned q, unsigned alt, const floa
   return (float)v * CLEAR_QUANT <= rbound * 1.0001f + 1e-3f;
 }
 
-__device__ __forceinline__ bool near_segments(const float ax, const float ay, const float rbound, const MapHeader& mh,
-                                              const uint8_t* fine) {
-  const float r = rbound * 1.0001f + 1e-3f;
-  const float fx = (ax - mh.x0) * mh.inv_cell, fy = (ay - mh.y0) * mh.inv_cell;
-  const int gx = mh.gx, gy = mh.gy;
-  if (!(fx >= 0.0f && fy >= 0.0f && fx < (float)gx && fy < (float)gy)) {
-    // outside the grid: reachable only within r of its box
-    const float ox = fmaxf(fmaxf(-fx, fx - (float)gx), 0.0f), oy = fmaxf(fmaxf(-fy, fy - (float)gy), 0.0f);
-    return fmaxf(ox, oy) * mh.cell <= r;
-  }
-  const int k = mh.fine;
-  const int ix = min((int)(fx * (float)k), gx * k - 1), iy = min((int)(fy * (float)k), gy * k - 1);
-  return (float)__ldg(fine + (size_t)iy * (gx * k) + ix) * CLEAR_QUANT <= r;
-}
-
 // Own pose of participant `idx` back from the warp's shared-memory tile (the hot loops keep only x, y
 // and the bounding radius in registers; the rare exact paths re-read the rest).
 // The warp's pose tile is addressed by participant slot (scenario slot x padded participants + participant), but laid
 // out lane-minor: slot = lane * PPL + i lives at word i * 32 + lane, so that the lanes' stores of their own PPL
-// participants are conflict-free (consecutive lanes, consecutive 16-byte words).  psh = log2(PPL).
-__device__ __forceinline__ int pslot(int slot, int psh) { return ((slot & ((1 << psh) - 1)) << 5) | (slot >> psh); }
+// participants are conflict-free (consecutive lanes, consecutive 16-byte words).
+static_assert(PPL == 4, "pslot's masks and shifts are those of 4 participants per lane");
+__device__ __forceinline__ int pslot(int slot) { return ((slot & 3) << 5) | (slot >> 2); }
 
-__device__ __forceinline__ Pose load_pose(const float4* poseA, const float4* poseB, int slot, int psh) {
-  const int idx = pslot(slot, psh);
+__device__ __forceinline__ Pose load_pose(const float4* poseA, const float4* poseB, int slot) {
+  const int idx = pslot(slot);
   const float4 a = poseA[idx], b = poseB[idx];
   Pose p;
   p.x = a.x; p.y = a.y; p.h = a.w; p.c = b.x; p.s = b.y; p.l = b.z; p.w = b.w;
@@ -286,60 +269,69 @@ constexpr int POS_EXT_PER_WARP = 768;   // circularly extended x / y arrays: (32
 
 // Exact test of one candidate pair (tile indices ti, tj of the same scenario); a hit is recorded for both
 // ends as the minimum partner index (scenario-local), which is what "first hit in list order" means.
-__device__ __noinline__ void pair_resolve(int ti, int tj, int mp_shift, int psh, const float4* poseA, const float4* poseB, int* hitmin) {
-  const Pose a = load_pose(poseA, poseB, ti, psh), b = load_pose(poseA, poseB, tj, psh);
+__device__ __noinline__ void pair_resolve(int ti, int tj, int mp_shift, const float4* poseA, const float4* poseB, int* hitmin) {
+  const Pose a = load_pose(poseA, poseB, ti), b = load_pose(poseA, poseB, tj);
   if (pair_hit(a, b)) {
     const int mask = (1 << mp_shift) - 1;
-    atomicMin(&hitmin[pslot(ti, psh)], tj & mask);
-    atomicMin(&hitmin[pslot(tj, psh)], ti & mask);
+    atomicMin(&hitmin[pslot(ti)], tj & mask);
+    atomicMin(&hitmin[pslot(tj)], ti & mask);
   }
 }
 
-// Pair operations of the partner loop on two partners at once (sm_90 has no packed fp32 instructions: two scalar
-// operations each, the same roundings).
-__device__ __forceinline__ float2 pk_add(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 pk_fma(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+// One word of the partner loop = IPW iterations x PPL own participants x 2 partners.  X / Y: the word's 2 * IPW partner
+// positions; nx / ny: the lane's own positions, negated; nthr: minus the squared broadphase reach.  The margin of a
+// pair, d^2 - thr, is <= 0 for a candidate; a NaN position (empty slot) gives a NaN margin, which neither the minimum nor
+// the comparison picks up.  FIRST: word 0, where the combinations with partner offset <= 0 (the lane's own participants
+// and pairs owned by the other end) are left out at compile time.
+constexpr int IPW = 16 / PPL;   // iterations per 32-bit word (2 * PPL bits each)
 
-// One word of the partner loop = IPW iterations x PPL own participants x 2 partners.  X / Y: the partner positions of
-// the word's iterations (two per float2); nx2 / ny2: the lane's own positions, negated; nthr2: minus the squared
-// broadphase reach.  The margin of a pair, d^2 - thr, is <= 0 for a candidate; a NaN position (empty slot) gives a NaN
-// margin, which neither the minimum nor the comparison picks up.  FIRST: word 0, where the combinations with partner
-// offset <= 0 (the lane's own participants and pairs owned by the other end) are left out at compile time.
-template <int PPL, bool FIRST>
-__device__ __forceinline__ float pair_word_min(const float2 (&X)[16 / PPL], const float2 (&Y)[16 / PPL], const float2 (&nx2)[PPL],
-                                               const float2 (&ny2)[PPL], const float2 (&nthr2)[PPL]) {
+// The margins of one own participant against the partners of iteration uu (2 uu and 2 uu + 1): two adds and two fused
+// multiply-adds each.  The two chains are interleaved step by step; written one margin after the other, the same
+// operations get a different schedule from ptxas.
+__device__ __forceinline__ void pair_margins(const float (&X)[2 * IPW], const float (&Y)[2 * IPW], int uu, float nx, float ny,
+                                             float nthr, float& d0, float& d1) {
+  const float dx0 = X[2 * uu] + nx, dx1 = X[2 * uu + 1] + nx;
+  const float dy0 = Y[2 * uu] + ny, dy1 = Y[2 * uu + 1] + ny;
+  const float e0 = fmaf(dy0, dy0, nthr), e1 = fmaf(dy1, dy1, nthr);
+  d0 = fmaf(dx0, dx0, e0);
+  d1 = fmaf(dx1, dx1, e1);
+}
+
+template <bool FIRST>
+__device__ __forceinline__ float pair_word_min(const float (&X)[2 * IPW], const float (&Y)[2 * IPW], const float (&nx)[PPL],
+                                               const float (&ny)[PPL], const float (&nthr)[PPL]) {
   float m = INFINITY;
 #pragma unroll
-  for (int uu = 0; uu < 16 / PPL; ++uu) {
+  for (int uu = 0; uu < IPW; ++uu) {
 #pragma unroll
     for (int i = 0; i < PPL; ++i) {
       const bool v0 = !FIRST || (2 * uu - i >= 1), v1 = !FIRST || (2 * uu + 1 - i >= 1);
       if (!v0 && !v1) continue;
-      const float2 dx = pk_add(X[uu], nx2[i]), dy = pk_add(Y[uu], ny2[i]);
-      const float2 d2 = pk_fma(dx, dx, pk_fma(dy, dy, nthr2[i]));
-      if (v0 && v1) m = fminf(m, fminf(d2.x, d2.y));
-      else if (v0) m = fminf(m, d2.x);
-      else m = fminf(m, d2.y);
+      float d0, d1;
+      pair_margins(X, Y, uu, nx[i], ny[i], nthr[i], d0, d1);
+      if (v0 && v1) m = fminf(m, fminf(d0, d1));
+      else if (v0) m = fminf(m, d0);
+      else m = fminf(m, d1);
     }
   }
   return m;
 }
 
 // The verdict bits of a word whose minimum margin was <= 0: bit ((uu * PPL + i) * 2 + e), the same margins recomputed.
-template <int PPL, bool FIRST>
-__device__ __forceinline__ unsigned pair_word_bits(const float2 (&X)[16 / PPL], const float2 (&Y)[16 / PPL], const float2 (&nx2)[PPL],
-                                                   const float2 (&ny2)[PPL], const float2 (&nthr2)[PPL]) {
+template <bool FIRST>
+__device__ __forceinline__ unsigned pair_word_bits(const float (&X)[2 * IPW], const float (&Y)[2 * IPW], const float (&nx)[PPL],
+                                                   const float (&ny)[PPL], const float (&nthr)[PPL]) {
   unsigned bits = 0;
 #pragma unroll
-  for (int uu = 0; uu < 16 / PPL; ++uu) {
+  for (int uu = 0; uu < IPW; ++uu) {
 #pragma unroll
     for (int i = 0; i < PPL; ++i) {
       const bool v0 = !FIRST || (2 * uu - i >= 1), v1 = !FIRST || (2 * uu + 1 - i >= 1);
       if (!v0 && !v1) continue;
-      const float2 dx = pk_add(X[uu], nx2[i]), dy = pk_add(Y[uu], ny2[i]);
-      const float2 d2 = pk_fma(dx, dx, pk_fma(dy, dy, nthr2[i]));
-      if (v0 && d2.x <= 0.0f) bits |= 1u << ((uu * PPL + i) * 2);
-      if (v1 && d2.y <= 0.0f) bits |= 2u << ((uu * PPL + i) * 2);
+      float d0, d1;
+      pair_margins(X, Y, uu, nx[i], ny[i], nthr[i], d0, d1);
+      if (v0 && d0 <= 0.0f) bits |= 1u << ((uu * PPL + i) * 2);
+      if (v1 && d1 <= 0.0f) bits |= 2u << ((uu * PPL + i) * 2);
     }
   }
   return bits;
@@ -349,7 +341,6 @@ __device__ __forceinline__ unsigned pair_word_bits(const float2 (&X)[16 / PPL], 
 // bit ((uu * PPL + i) * 2 + e) = own participant m0 + i against extended slot m0 + 2 (u_base + uu) + e.  Keep the
 // combinations whose partner offset q is 1..Mh (every unordered pair once; q <= 0 are the lane's own participants
 // or pairs owned by the other end) and push them on the warp's queue.
-template <int PPL>
 __device__ __forceinline__ void pair_enqueue_bits(unsigned bits, int u_base, int t0, int tb, int m0, int M, int Mh,
                                                   unsigned* queue, int* qcount) {
   while (bits) {
@@ -373,19 +364,17 @@ __device__ __forceinline__ void pair_enqueue_bits(unsigned bits, int u_base, int
 
 // Dense-scene fallback (the candidate queue overflowed): every lane resolves all pairs of its own participants
 // against all partners of the scenario directly.  Correct for any density, slow, and never on the hot path.
-template <int PPL>
 __device__ __noinline__ void pair_exhaustive(int t0, int tb, int m0, int M, int mp_shift, float rb_max, const float4* poseA,
                                              const float4* poseB, int* hitmin) {
-  constexpr int psh = PPL == 4 ? 2 : 1;
   for (int i = 0; i < PPL; ++i) {
     if (m0 + i >= M) break;
-    const float4 a = poseA[pslot(t0 + i, psh)];
+    const float4 a = poseA[pslot(t0 + i)];
     if (!(a.x == a.x)) continue;
     const float rr = a.z + rb_max;
     for (int j = m0 + i + 1; j < M; ++j) {
-      const float4 b = poseA[pslot(tb + j, psh)];
+      const float4 b = poseA[pslot(tb + j)];
       const float dx = b.x - a.x, dy = b.y - a.y;
-      if (fmaf(dx, dx, dy * dy) <= fmaf(rr * rr, 1.00001f, 1e-12f)) pair_resolve(t0 + i, tb + j, mp_shift, psh, poseA, poseB, hitmin);
+      if (fmaf(dx, dx, dy * dy) <= fmaf(rr * rr, 1.00001f, 1e-12f)) pair_resolve(t0 + i, tb + j, mp_shift, poseA, poseB, hitmin);
     }
   }
 }
@@ -508,7 +497,7 @@ struct TileRef {
   const unsigned char* blob;   // the blob in global memory (fine field, polygon data)
 };
 
-template <int PPL, bool MAP_TABLE>
+template <bool MAP_TABLE>
 __device__ __forceinline__ void static_phase(unsigned near_bits, int t0, int lane, int tile_first_scn, int mp_shift, const StepArgs& A,
                                              const unsigned char* s_map, const float4* poseA, const float4* poseB, int* segmin,
                                              unsigned* queue, int* qcount) {
@@ -520,7 +509,6 @@ __device__ __forceinline__ void static_phase(unsigned near_bits, int t0, int lan
     if (near) queue[base + __popc(m & ((1u << lane) - 1u))] = (unsigned)(t0 + i);
     base += __popc(m);
   }
-  constexpr int psh = PPL == 4 ? 2 : 1;
   // the tile of participant slot ti (its scenario = the warp tile's first scenario + ti / padded participants)
   auto tile_of = [&](int ti) {
     TileRef t;
@@ -537,41 +525,40 @@ __device__ __forceinline__ void static_phase(unsigned near_bits, int t0, int lan
   for (int k = lane; k < base; k += 32) {
     const int ti = (int)queue[k];
     const TileRef t = tile_of(ti);
-    const Pose a = load_pose(poseA, poseB, ti, psh);
-    const int best = t.mh->n_seg > 0 ? static_walk(ti, a, poseA[pslot(ti, psh)].z, *t.mh, map_view(t.sec, *t.mh), queue, qcount) : 0x7fffffff;
-    segmin[pslot(ti, psh)] = best;   // one lane per participant: plain store (-2 = needs the exact walk)
+    const Pose a = load_pose(poseA, poseB, ti);
+    const int best = t.mh->n_seg > 0 ? static_walk(ti, a, poseA[pslot(ti)].z, *t.mh, map_view(t.sec, *t.mh), queue, qcount) : 0x7fffffff;
+    segmin[pslot(ti)] = best;   // one lane per participant: plain store (-2 = needs the exact walk)
   }
   __syncwarp();
   const int n_x = min(*qcount, QCAP - QX0);
   for (int k = lane; k < n_x; k += 32) {   // undecided (participant, segment) pairs: exact test
     const unsigned e = queue[QX0 + k];
     const int ti = (int)(e >> 16), sidx = (int)(e & 0xffffu);
-    int* sm = &segmin[pslot(ti, psh)];
+    int* sm = &segmin[pslot(ti)];
     if (*sm != -2 && sidx < *sm) {
       const TileRef t = tile_of(ti);
-      if (seg_exact(load_pose(poseA, poseB, ti, psh), reinterpret_cast<const float4*>(t.sec + t.mh->off_seg)[sidx])) atomicMin(sm, sidx);
+      if (seg_exact(load_pose(poseA, poseB, ti), reinterpret_cast<const float4*>(t.sec + t.mh->off_seg)[sidx])) atomicMin(sm, sidx);
     }
   }
   __syncwarp();
   for (int k = lane; k < base; k += 32) {   // the out-of-line walk where needed; then edges -> objects, polygon containment
     const int ti = (int)queue[k];
-    int* sm = &segmin[pslot(ti, psh)];
+    int* sm = &segmin[pslot(ti)];
     const TileRef t = tile_of(ti);
     if (*sm == -2) {
       const MapView mv = map_view(t.sec, *t.mh);
-      *sm = static_walk_exact(load_pose(poseA, poseB, ti, psh), poseA[pslot(ti, psh)].z, *t.mh, mv.seg, mv.cell_start, mv.items);
+      *sm = static_walk_exact(load_pose(poseA, poseB, ti), poseA[pslot(ti)].z, *t.mh, mv.seg, mv.cell_start, mv.items);
     }
     if (t.mh->n_poly > 0) {
-      const float4 pa = poseA[pslot(ti, psh)];
+      const float4 pa = poseA[pslot(ti)];
       *sm = static_objects(*sm, pa.x, pa.y, *t.mh, t.blob);
     }
   }
   __syncwarp();
 }
 
-__device__ __noinline__ bool oob_slow(const float4* poseA, const float4* poseB, int idx, int psh, float xmin, float xmax, float ymin,
-                                      float ymax) {
-  const Pose a = load_pose(poseA, poseB, idx, psh);
+__device__ __noinline__ bool oob_slow(const float4* poseA, const float4* poseB, int idx, float xmin, float xmax, float ymin, float ymax) {
+  const Pose a = load_pose(poseA, poseB, idx);
   int r = out_of_bound_f32(a.x, a.y, a.c, a.s, a.l, a.w, a.w < 0.0f, xmin, xmax, ymin, ymax);
   if (r < 0) r = out_of_bound_f64(a.x, a.y, a.h, a.l, a.w, a.w < 0.0f, xmin, xmax, ymin, ymax) ? 1 : 0;
   return r != 0;
@@ -616,16 +603,11 @@ __device__ __forceinline__ void prefetch_tile_l2(const StepArgs& A, long long i)
 // ---------------------------------------------------------------------------- K1
 // KIN_ONLY: every type in the table is SingleTrackKinematics or static - the fp64 models are compiled out
 // (their register footprint would otherwise bound the occupancy of the whole kernel).
-#if defined(T2D_K1_MAXNREG)   // experiments: an explicit register budget instead of the launch bounds
-#define T2D_K1_BOUNDS __maxnreg__(T2D_K1_MAXNREG)
-#else
-#define T2D_K1_BOUNDS __launch_bounds__(CTA_THREADS, (PPL == 4 ? 2 : 3))
-#endif
 // MAP_TABLE: every scenario names its own static-geometry tile (t2d_set_map_table); the tiles are then read from global
 // memory, header included.  Otherwise one tile serves all scenarios: header in the constant bank, sections staged into
 // shared memory once per CTA.
-template <int PPL, bool KIN_ONLY, bool MAP_TABLE>
-__global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A) {
+template <bool KIN_ONLY, bool MAP_TABLE>
+__global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_constant__ StepArgs A) {
   extern __shared__ __align__(128) unsigned char smem[];
   // carve: [map blob | 16B aligned] [type table] [pose tiles, hit mins, queues, positions] [mbarrier]; every
   // offset, shift and count that depends only on the launch shape comes precomputed from the host
@@ -645,9 +627,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem + A.off_bar);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-#if defined(T2D_DEBUG_CLOCK)
-  const long long t_entry = A.dbg_clock ? clock64() : 0;
-#endif
   // Programmatic dependent launch: let the next tick's grid start launching now (its prologue - shared-memory
   // carve, mbarrier, TMA staging of the static table / map - overlaps this grid's tail) ...
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -708,15 +687,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
     if (nvalid < 0) nvalid = 0;
     const long long idx0 = n * M + m0;
 
-#if defined(T2D_DEBUG_CLOCK)   // phase time stamps: measurement builds only
-    // `dep`: a late result of the phase that ends here.  The (never taken) branch on it cannot be resolved before the value
-    // has arrived, so the stamp charges a phase with the latency it creates instead of leaking it into the next one.
-    #define T2D_STAMP(k, dep) do { if (A.dbg_clock) { if (__float_as_int((float)(dep)) == 0x7fbfffff) asm volatile("trap;"); \
-      if (lane == 0) A.dbg_clock[(long long)tile * 10 + (k)] = clock64(); } } while (0)
-#else
-    #define T2D_STAMP(k, dep) do { } while (0)
-#endif
-    T2D_STAMP(0, 0.0f);
     // ------------------------------------------------------------------ load
     float sx[PPL], sy[PPL], shd[PPL], sv[PPL], svx[PPL], svy[PPL], a0[PPL], a1[PPL];
     int tidv[PPL];
@@ -736,18 +706,11 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       for (int i = 0; i < PPL; ++i) tidv[i] = tb8[i];
       if (A.do_physics) {
         float2 act[PPL];
-        if constexpr (PPL == 4) {
-          float lo[4], hi[4];
-          ld_vec<float, 4>(A.action + 2 * idx0, lo);
-          ld_vec<float, 4>(A.action + 2 * idx0 + 4, hi);
-          act[0] = make_float2(lo[0], lo[1]); act[1] = make_float2(lo[2], lo[3]);
-          act[2] = make_float2(hi[0], hi[1]); act[3] = make_float2(hi[2], hi[3]);
-        } else {
-          float raw[2 * PPL];
-          ld_vec<float, 2 * PPL>(A.action + 2 * idx0, raw);
-#pragma unroll
-          for (int i = 0; i < PPL; ++i) act[i] = make_float2(raw[2 * i], raw[2 * i + 1]);
-        }
+        float lo[4], hi[4];
+        ld_vec<float, 4>(A.action + 2 * idx0, lo);
+        ld_vec<float, 4>(A.action + 2 * idx0 + 4, hi);
+        act[0] = make_float2(lo[0], lo[1]); act[1] = make_float2(lo[2], lo[3]);
+        act[2] = make_float2(hi[0], hi[1]); act[3] = make_float2(hi[2], hi[3]);
 #pragma unroll
         for (int i = 0; i < PPL; ++i) { a0[i] = act[i].x; a1[i] = act[i].y; }
         if (A.needs_vel_in) {
@@ -783,7 +746,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       staged = true;
     }
     // the participant's type row; its third 16-byte group holds the collision shape and the model / shape ids
-    constexpr int psh = PPL == 4 ? 2 : 1;
     float ch[PPL], sh[PPL];
     bool active[PPL], kin[PPL];
     const Params* pp[PPL];
@@ -805,7 +767,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
         if (model[i] <= MODEL_DYNAMICS || model[i] == MODEL_DRIFT) { float t = a0[i]; a0[i] = a1[i]; a1[i] = t; }
     }
 
-    T2D_STAMP(1, sx[0] + sy[PPL - 1] + shd[0] + sv[PPL - 1] + a0[0] + a1[PPL - 1] + (float)tidv[0]);
     // ------------------------------------------------------------------ physics
     if (A.do_physics) {
       // Kinematic participants of the whole warp advance together in the 4-chain loop; slots holding another
@@ -873,7 +834,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       for (int i = 0; i < PPL; ++i) sincos_fast(shd[i], &sh[i], &ch[i]);
     }
 
-    T2D_STAMP(2, sx[0] + sy[PPL - 1] + ch[0] + sh[PPL - 1] + svx[PPL - 1]);
     // ------------------------------------------------------------------ poses -> shared
     // Only (x, y, bounding radius) stay in registers; the full pose lives in the warp's smem tile.
     float px[PPL], py[PPL], rb[PPL];
@@ -935,7 +895,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       }
     }
 
-    T2D_STAMP(3, 0.0f);
     // ------------------------------------------------------------------ dynamic collision
     // Every unordered pair once: participant i tests partners (i+1 .. i+M/2) mod M.  A lane walks the
     // partners of its PPL participants together (one 128-bit pose load per partner, PPL distance tests);
@@ -947,63 +906,55 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       // iteration.  Per pair the margin d^2 - thr is formed by two fused multiply-adds
       // and folded into a running minimum over the 32 tests of a word; only a
       // word whose minimum is <= 0 (rare) recomputes its verdict bits and goes to the out-of-line enqueue.
-      float2 nx2[PPL], ny2[PPL], nthr2[PPL];
+      float nx[PPL], ny[PPL], nthr[PPL];
 #pragma unroll
       for (int i = 0; i < PPL; ++i) {
         const float rr = rb[i] + A.rb_max;
         const float thr = fmaf(rr * rr, 1.00001f, 1e-12f);   // conservative: any partner's bounding radius <= rb_max
-        nx2[i] = make_float2(-px[i], -px[i]);
-        ny2[i] = make_float2(-py[i], -py[i]);
-        nthr2[i] = make_float2(-thr, -thr);
+        nx[i] = -px[i];
+        ny[i] = -py[i];
+        nthr[i] = -thr;
       }
       // partner pairs u = 0 .. U-1 cover offsets -(PPL-1) .. >= Mh; U is rounded up to whole words (the extended
       // arrays are long enough), so the word body has no bounds test and its loads can be issued back to back
-      constexpr int IPW = 16 / PPL;                        // iterations per 32-bit word (2 * PPL bits each)
       const int n_words = Mh > 0 ? (((Mh + PPL + 1) >> 1) + IPW - 1) / IPW : 0;
-      const float2* bx = reinterpret_cast<const float2*>(posx + m0);
-      const float2* by = reinterpret_cast<const float2*>(posy + m0);
-      // one word = 2 * IPW consecutive partners: 128-bit loads when the lane's window is 16-byte aligned (PPL = 4)
-      auto load_word = [&](int uw, float2 (&X)[IPW], float2 (&Y)[IPW]) {
-        if constexpr (PPL == 4) {
+      // one word = 2 * IPW consecutive partners: 128-bit loads (every scenario's window and m0 are 16-byte aligned)
+      const float4* bx = reinterpret_cast<const float4*>(posx + m0);
+      const float4* by = reinterpret_cast<const float4*>(posy + m0);
+      auto load_word = [&](int uw, float (&X)[2 * IPW], float (&Y)[2 * IPW]) {
 #pragma unroll
-          for (int q = 0; q < IPW / 2; ++q) {
-            const float4 xv = reinterpret_cast<const float4*>(bx)[uw * (IPW / 2) + q];
-            const float4 yv = reinterpret_cast<const float4*>(by)[uw * (IPW / 2) + q];
-            X[2 * q] = make_float2(xv.x, xv.y); X[2 * q + 1] = make_float2(xv.z, xv.w);
-            Y[2 * q] = make_float2(yv.x, yv.y); Y[2 * q + 1] = make_float2(yv.z, yv.w);
-          }
-        } else {
-#pragma unroll
-          for (int uu = 0; uu < IPW; ++uu) { X[uu] = bx[uw * IPW + uu]; Y[uu] = by[uw * IPW + uu]; }
+        for (int q = 0; q < IPW / 2; ++q) {
+          const float4 xv = bx[uw * (IPW / 2) + q], yv = by[uw * (IPW / 2) + q];
+          X[4 * q] = xv.x; X[4 * q + 1] = xv.y; X[4 * q + 2] = xv.z; X[4 * q + 3] = xv.w;
+          Y[4 * q] = yv.x; Y[4 * q + 1] = yv.y; Y[4 * q + 2] = yv.z; Y[4 * q + 3] = yv.w;
         }
       };
       if (n_words > 0) {   // word 0 also meets the lane's own participants (offset <= 0): those tests are compiled out
-        float2 X[IPW], Y[IPW];
+        float X[2 * IPW], Y[2 * IPW];
         load_word(0, X, Y);
-        if (pair_word_min<PPL, true>(X, Y, nx2, ny2, nthr2) <= 0.0f) {
-          const unsigned bits = pair_word_bits<PPL, true>(X, Y, nx2, ny2, nthr2);
-          if (bits) pair_enqueue_bits<PPL>(bits, 0, t0, tb, m0, M, Mh, queue, qcount);
+        if (pair_word_min<true>(X, Y, nx, ny, nthr) <= 0.0f) {
+          const unsigned bits = pair_word_bits<true>(X, Y, nx, ny, nthr);
+          if (bits) pair_enqueue_bits(bits, 0, t0, tb, m0, M, Mh, queue, qcount);
         }
       }
       for (int uw = 1; uw < n_words; ++uw) {
-        float2 X[IPW], Y[IPW];
+        float X[2 * IPW], Y[2 * IPW];
         load_word(uw, X, Y);
-        if (pair_word_min<PPL, false>(X, Y, nx2, ny2, nthr2) <= 0.0f) {
-          const unsigned bits = pair_word_bits<PPL, false>(X, Y, nx2, ny2, nthr2);
-          if (bits) pair_enqueue_bits<PPL>(bits, uw * IPW, t0, tb, m0, M, Mh, queue, qcount);
+        if (pair_word_min<false>(X, Y, nx, ny, nthr) <= 0.0f) {
+          const unsigned bits = pair_word_bits<false>(X, Y, nx, ny, nthr);
+          if (bits) pair_enqueue_bits(bits, uw * IPW, t0, tb, m0, M, Mh, queue, qcount);
         }
       }
       __syncwarp();
-      T2D_STAMP(4, *qcount);
       // narrowphase: the queued candidate pairs, one per lane (or the exhaustive pass if the queue overflowed)
       const int n_q = *qcount;
       if (n_q <= QCAP) {
         for (int k = lane; k < n_q; k += 32) {
           const unsigned e = queue[k];
-          pair_resolve((int)(e >> 16), (int)(e & 0xffffu), mp_shift, psh, poseA, poseB, hitmin);
+          pair_resolve((int)(e >> 16), (int)(e & 0xffffu), mp_shift, poseA, poseB, hitmin);
         }
       } else {
-        pair_exhaustive<PPL>(t0, tb, m0, M, mp_shift, A.rb_max, poseA, poseB, hitmin);
+        pair_exhaustive(t0, tb, m0, M, mp_shift, A.rb_max, poseA, poseB, hitmin);
       }
       __syncwarp();
 #pragma unroll
@@ -1016,7 +967,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       __syncwarp();
     }
 
-    T2D_STAMP(5, hit[0] + hit[PPL - 1]);
     // ------------------------------------------------------------------ static collision
     int hseg[PPL];
 #pragma unroll
@@ -1027,7 +977,7 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       for (int i = 0; i < PPL; ++i)
         if (((solid_bits >> i) & 1u) && near_decide(near_q[i], near_alt[i], rb[i])) near_bits |= 1u << i;
       if (__any_sync(0xffffffffu, near_bits != 0)) {
-        static_phase<PPL, MAP_TABLE>(near_bits, t0, lane, tile * spw, mp_shift, A, s_map, poseA, poseB, hitmin, queue, qcount);
+        static_phase<MAP_TABLE>(near_bits, t0, lane, tile * spw, mp_shift, A, s_map, poseA, poseB, hitmin, queue, qcount);
 #pragma unroll
         for (int i = 0; i < PPL; ++i) {
           const int h = hitmin[i * 32 + lane];
@@ -1036,7 +986,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
       }
     }
 
-    T2D_STAMP(6, hseg[0] + hseg[PPL - 1]);
     // ------------------------------------------------------------------ out of bound + flags
     // the boundary box of this lane's scenario (Map.boundary of its tile)
     float bxmin = A.bxmin, bxmax = A.bxmax, bymin = A.bymin, bymax = A.bymax;
@@ -1061,7 +1010,7 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
     if (oob_check) {
 #pragma unroll
       for (int i = 0; i < PPL; ++i)
-        if (((oob_check >> i) & 1u) && oob_slow(poseA, poseB, t0 + i, psh, bxmin, bxmax, bymin, bymax)) fl[i] |= T2D_F_OUTBOUND;
+        if (((oob_check >> i) & 1u) && oob_slow(poseA, poseB, t0 + i, bxmin, bxmax, bymin, bymax)) fl[i] |= T2D_F_OUTBOUND;
     }
     if (nvalid == PPL && A.vec_ok) {
       int16_t h16[PPL], s16[PPL];
@@ -1098,7 +1047,7 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
         uint8_t st = T2D_STATUS_NORMAL;
         unsigned goal = 0;
         if (A.goal_target != nullptr) {   // the ego is participant 0 = this lane's first slot
-          const float4 ea = poseA[pslot(t0, psh)], eb = poseB[pslot(t0, psh)];
+          const float4 ea = poseA[pslot(t0)], eb = poseB[pslot(t0)];
           if (ea.x == ea.x && eb.w >= 0.0f) goal = ego_goal_events(A, n, ea.x, ea.y, ea.w, eb.z, eb.w);
         }
         if (goal & 1u) st = T2D_STATUS_COMPLETED;                    // parking.py:387-390 (lowest priority)
@@ -1111,15 +1060,6 @@ __global__ void T2D_K1_BOUNDS t2d_step_kernel(const __grid_constant__ StepArgs A
         if (A.done) A.done[n] = st != T2D_STATUS_NORMAL;             // parking.py:243-248
       }
     }
-    T2D_STAMP(7, fl[0] + fl[PPL - 1]);
-#if defined(T2D_DEBUG_CLOCK)
-    if (A.dbg_clock && lane == 0) {
-      unsigned smid;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      A.dbg_clock[(long long)tile * 10 + 8] = smid;
-      A.dbg_clock[(long long)tile * 10 + 9] = t_entry;
-    }
-#endif
     __syncwarp();   // pose tile is reused by the next tile
   }
   if (!staged) mbar_wait(s_bar, 0);   // never leave a bulk copy in flight at exit
@@ -1749,7 +1689,7 @@ struct t2d_exchange {
 };
 
 struct t2d_ctx {
-  int device = 0, N = 0, M = 0, G = 0, ppl = 4;
+  int device = 0, N = 0, M = 0, G = 0;
   t2d_config cfg{};
   int n_types = 0;
   bool has_pointmass = false;
@@ -1784,7 +1724,6 @@ struct t2d_ctx {
   int prefetch_override = -1;      // T2D_PREFETCH=0 / 1 (experiments; -1 = on unless a done exchange is alive)
   int wpc_override = 0;            // T2D_WPC=w: warps per CTA of the tick (experiments; 0 = pick from the batch size)
   int grid_limit = 0;              // T2D_GRID_LIMIT=k: at most k CTAs of the persistent tick grid per SM (experiments; 0 = occupancy)
-  long long* dbg_clock = nullptr;
   int occ_smem[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};   // per warps-per-CTA: smem the cached occupancy was computed for
   int occ_val[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   int occ_variant[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -1838,9 +1777,6 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
   c->device = device;
   c->N = n_scenarios;
   c->M = m_participants;
-  // participants per lane: 4 (2 per lane executes about 55 % more instructions per participant)
-  const int ppl = 4;
-  c->ppl = ppl;
   if (const char* e = getenv("T2D_PDL")) c->use_pdl = atoi(e) != 0;
   if (const char* e = getenv("T2D_GRID_LIMIT")) c->grid_limit = std::max(0, atoi(e));
   if (const char* e = getenv("T2D_PREFETCH")) c->prefetch_override = atoi(e) != 0 ? 1 : 0;
@@ -1850,7 +1786,7 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
   }
   if (const char* e = getenv("T2D_HOST_CHUNKS")) c->host_chunks = std::max(0, std::min(atoi(e), (int)t2d_ctx::MAX_HOST_CHUNKS));
   int g = 1;
-  while (g * ppl < m_participants) g <<= 1;
+  while (g * PPL < m_participants) g <<= 1;
   c->G = g;
   c->cfg = *cfg;
   cudaDeviceProp prop;
@@ -2273,14 +2209,13 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
   A.bxmin = c->bounds[0]; A.bxmax = c->bounds[1]; A.bymin = c->bounds[2]; A.bymax = c->bounds[3];
   A.prefetch = c->prefetch_override >= 0 ? c->prefetch_override : (g_exchanges_alive.load() == 0 ? 1 : 0);
   A.needs_vel_in = (c->has_pointmass || c->has_drift) ? 1 : 0;   // (drift: K1 passes the pre-pass's vx, vy through)
-  bool vec = (c->M % c->ppl == 0) && aligned16(A.x) && aligned16(A.y) && aligned16(A.h) && aligned16(A.v) && aligned16(A.vx) &&
+  bool vec = (c->M % PPL == 0) && aligned16(A.x) && aligned16(A.y) && aligned16(A.h) && aligned16(A.v) && aligned16(A.vx) &&
              aligned16(A.vy) && (reinterpret_cast<uintptr_t>(A.type_id) % 4 == 0) && (!action || aligned16(action)) &&
              (!flags || reinterpret_cast<uintptr_t>(flags) % 4 == 0) && (!hit_index || reinterpret_cast<uintptr_t>(hit_index) % 8 == 0) &&
              (!hit_segment || reinterpret_cast<uintptr_t>(hit_segment) % 8 == 0);
   A.vec_ok = vec ? 1 : 0;
 
   A.rb_max = c->rb_max;
-  A.dbg_clock = c->dbg_clock;
   A.goal_target = c->goal_target ? c->goal_target + 5 * (size_t)first : nullptr;
   A.goal_iou = c->goal_iou ? c->goal_iou + first : nullptr;
   A.goal_last_pose = c->goal_last_pose ? c->goal_last_pose + 4 * (size_t)first : nullptr;
@@ -2305,7 +2240,7 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
     A.n_tiles = (int)tiles;
     A.g_shift = 0;
     while ((1 << A.g_shift) < c->G) ++A.g_shift;
-    const int MP = c->G * c->ppl;
+    const int MP = c->G * PPL;
     A.mp_shift = 0;
     while ((1 << A.mp_shift) < MP) ++A.mp_shift;
     A.ext = ((3 * MP) / 2 + 16 + 3) & ~3;   // a multiple of 4 floats: every scenario's window starts 16-byte aligned
@@ -2314,8 +2249,8 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
   if (smem > c->max_smem_optin) return fail(T2D_E_UNSUPPORTED, "shared memory budget exceeded");
   using kernel_t = void (*)(StepArgs);
   kernel_t kern;
-  if (c->kin_only) kern = map_table ? (kernel_t)t2d_step_kernel<4, true, true> : (kernel_t)t2d_step_kernel<4, true, false>;
-  else kern = map_table ? (kernel_t)t2d_step_kernel<4, false, true> : (kernel_t)t2d_step_kernel<4, false, false>;
+  if (c->kin_only) kern = map_table ? (kernel_t)t2d_step_kernel<true, true> : (kernel_t)t2d_step_kernel<true, false>;
+  else kern = map_table ? (kernel_t)t2d_step_kernel<false, true> : (kernel_t)t2d_step_kernel<false, false>;
   {
     // cudaFuncSetAttribute applies to the kernel function for the whole process and SETS the value: worlds of
     // different sizes share it, so the opt-in is tracked per (device, kernel variant) and only ever raised.
@@ -2371,12 +2306,6 @@ int t2d_set_goal(t2d_ctx* c, const float* target, float arrival_threshold, int n
   if (target && !(arrival_threshold > 0.0f && arrival_threshold <= 1.0f)) return fail(T2D_E_INVALID, "arrival_threshold must be in (0, 1]");
   c->goal_target = target; c->goal_iou = iou_out; c->goal_last_pose = last_pose; c->goal_noact_count = no_action_count;
   c->goal_threshold = arrival_threshold; c->goal_noact_max = no_action_max_step;
-  return T2D_OK;
-}
-
-int t2d_debug_set_clock_buffer(t2d_ctx* c, long long* device_buffer) {
-  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  c->dbg_clock = device_buffer;
   return T2D_OK;
 }
 

@@ -36,14 +36,6 @@
 #define T2D_RSQRTF(x) (1.0f / sqrtf(x))
 #endif
 
-#define T2D_PRAGMA_(x) _Pragma(#x)
-#define T2D_PRAGMA(x) T2D_PRAGMA_(x)
-#if defined(T2D_KIN_UNROLL)   // measurement builds: unroll factor of the kinematic sub-step loop
-#define T2D_KIN_UNROLL_PRAGMA T2D_PRAGMA(unroll T2D_KIN_UNROLL)
-#else
-#define T2D_KIN_UNROLL_PRAGMA
-#endif
-
 namespace t2d {
 
 constexpr int MODEL_KINEMATICS = 0;
@@ -265,15 +257,11 @@ T2D_HD void kinematics_step(KinIO<W>& io, const Params* const (&p)[W], int n_ste
   // term instead of an accumulated sum.
   float c[W], s[W], w1[W], Sx[W], Sy[W], Sv[W], kdt[W], adt[W], vlo[W], vhi[W], k[W], a[W];
   bool small = true;
-#if defined(T2D_NO_FAST_KIN)   // (measurement builds only: always take the general loop)
-  bool lin = false;
-#else
   // fast loop: no participant of this group touches a speed bound during the tick, and the tick has at most 24
   // sub-steps - the carried rotation accumulates rounding quadratically in the sub-step count (measured against float64
   // at v <= 69 m/s: 4e-6 at 20 sub-steps, 9e-6 at 100, 2e-5 at 40 sub-steps of a 200 ms tick; the general loop stays
   // below 7e-6 there), so longer ticks keep the general loop
   bool lin = n_steps >= 2 && n_steps <= 24;
-#endif
   // Trigonometry of the steering angle and the heading first, for all W participants in one basic block; the arguments
   // the short forms cannot take (a steering range beyond +-pi/4, a heading beyond +-512) are re-done afterwards, once.
   float sd[W], cd[W], sp[W], cp[W];
@@ -349,7 +337,6 @@ T2D_HD void kinematics_step(KinIO<W>& io, const Params* const (&p)[W], int n_ste
     for (int i = 0; i < W; ++i) v[i] = io.v[i];
     {
       float fi = -1.0f;
-      T2D_KIN_UNROLL_PRAGMA
       for (int it = 0; it < n_steps; ++it) {
         fi += 1.0f;
 #pragma unroll
