@@ -28,6 +28,11 @@
  *                        TimeExceed.update                tactics2d/traffic/event_detection/time_exceed.py:26-33
  *   t2d_set_goal         Arrival.update / NoAction.update  tactics2d/traffic/event_detection/arrival.py:32-47, no_action.py:32-53
  *   t2d_lidar_scan       SingleLineLidar._scan_obstacles   tactics2d/sensor/lidar.py:128-221
+ *   t2d_set_bev_styles   the colour / z-order tables of MatplotlibRenderer   tactics2d/renderer/matplotlib_config.py,
+ *                                                         sensor/camera.py:56-87 (style key of an element)
+ *   t2d_bev_render       BEVCamera.update + MatplotlibRenderer.update / save_single_frame(return_array=True)
+ *                                                         tactics2d/sensor/camera.py:333-386,
+ *                                                         renderer/matplotlib_renderer.py:542-768
  *   t2d_set_controllers  IDMController / AccelerationController / PurePursuitController objects
  *                                                         tactics2d/controller/idm_controller.py:33-58,
  *                                                         acceleration_controller.py:33-80, pure_pursuit_controller.py:26-49
@@ -232,6 +237,38 @@ int t2d_bind_reset_wheel_pool(t2d_ctx* ctx, const float* pool_omega_front, const
  * (lidar.py:160); scan: DEVICE float [N][n_beams], +inf where nothing is hit within the range.  Obstacles are the map
  * segments given to t2d_set_map and the pose rings of the other box-shaped participants. */
 int t2d_lidar_scan(t2d_ctx* ctx, int n_beams, float max_range, const double* beam_cos_sin, float* scan, void* stream);
+
+/* ---- bird's-eye-view observation of the ego of every scenario ------------------------------------------------------
+ * t2d_set_bev_styles + t2d_bev_render replace BEVCamera.update (tactics2d/sensor/camera.py:333-386) followed by
+ * MatplotlibRenderer.update / save_single_frame(return_array=True) (renderer/matplotlib_renderer.py:542-768): the
+ * 200 x 200 x 3 uint8 observation of ParkingEnv / RacingEnv (envs/parking.py:130, racing.py:102).  The contract, and
+ * where it deliberately differs from the reference's renderer, is DESIGN.md section 1 "BEV observation".
+ * A style is a colour, a z order (larger is drawn on top; equal z keeps the draw order) and the stroke width in points
+ * that open map segments of that style are drawn with (the renderer's 200 dpi: w = line_width_pt * 200 / 72 pixels).
+ * Rows with a fixed meaning: */
+#define T2D_MAX_BEV_STYLES 64
+#define T2D_BEV_STYLE_BACKGROUND 0 /* pixels no primitive covers */
+#define T2D_BEV_STYLE_ARROW 1      /* the heading triangle of every drawn box participant */
+#define T2D_BEV_STYLE_RING 2       /* a map ring object without a per-segment style */
+#define T2D_BEV_STYLE_OPEN 3       /* an open map segment without a per-segment style */
+#define T2D_BEV_NOT_DRAWN 255
+typedef struct t2d_bev_style {
+  uint8_t r, g, b;
+  int8_t z;
+  float line_width_pt;
+} t2d_bev_style;
+/* HOST arrays, copied.  table: n_styles rows (4..T2D_MAX_BEV_STYLES); type_style [n_types]: the style of every
+ * participant type (T2D_BEV_NOT_DRAWN: not drawn; box types are drawn as their pose ring plus the heading triangle, disc
+ * types as their disc, SHAPE_NONE types never); seg_style [n_seg_total]: the style of every map segment of the current
+ * map, tiles back to back in tile order (a ring object takes the style of its first segment), or NULL for the defaults
+ * T2D_BEV_STYLE_RING / T2D_BEV_STYLE_OPEN; target_style: the style of the t2d_set_goal rectangle (T2D_BEV_NOT_DRAWN: not
+ * drawn).  t2d_set_map / t2d_set_map_polygons / t2d_set_map_table drop the per-segment styles back to the defaults. */
+int t2d_set_bev_styles(t2d_ctx* ctx, const t2d_bev_style* table, int n_styles, const uint8_t* type_style,
+                       const uint8_t* seg_style, int n_seg_total, int target_style);
+/* Renders every scenario's view into out: DEVICE uint8 [N][height][width][3] RGB when rgb != 0, else [N][height][width]
+ * style indices (RGB = the style's colour).  range: HOST float [4] = (left, right, front, back) in metres, each in
+ * (0, 1e5]; width, height in 1..1024.  One launch, no allocation, no synchronisation: capturable in a CUDA graph. */
+int t2d_bev_render(t2d_ctx* ctx, int width, int height, const float* range, int rgb, uint8_t* out, void* stream);
 
 /* On-device NPC controllers (tactics2d/controller).  A controller row is one configured controller object; the fields
  * are the reference's attribute names.  kind selects the law:

@@ -44,6 +44,11 @@ class ControllerParamsC(C.Structure):
         "min_pre_aiming_distance", "pp_interval", "wheel_base")]
 
 
+class BevStyleC(C.Structure):
+    """``t2d_bev_style``: colour, z order and stroke width (points) of one BEV style row."""
+    _fields_ = [("r", C.c_uint8), ("g", C.c_uint8), ("b", C.c_uint8), ("z", C.c_int8), ("line_width_pt", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol include/t2d_b200.h declares
 _P = C.c_void_p
 SYMBOLS = {
@@ -66,6 +71,8 @@ SYMBOLS = {
     "t2d_set_goal": (C.c_int, [_P, _P, C.c_float, C.c_int, _P, _P, _P]),
     "t2d_reset": (C.c_int, [_P, _P, _P, C.c_int] + [_P] * 7),
     "t2d_lidar_scan": (C.c_int, [_P, C.c_int, C.c_float, _P, _P, _P]),
+    "t2d_set_bev_styles": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int]),
+    "t2d_bev_render": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "t2d_set_controllers": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P]),
     "t2d_set_paths": (C.c_int, [_P, _P, _P, C.c_int]),
     "t2d_control": (C.c_int, [_P, _P, _P]),

@@ -1654,6 +1654,8 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
 
 }  // namespace t2d
 
+#include "t2d_bev.cuh"
+
 // =============================================================================================
 // C ABI
 // =============================================================================================
@@ -1747,6 +1749,14 @@ struct t2d_ctx {
   cudaStream_t hs_copy = nullptr;
   cudaEvent_t hs_begin = nullptr, hs_chunk[MAX_HOST_CHUNKS] = {};
   int host_chunks = 0;                 // 0 = pick from the batch size
+  // BEV observation (t2d_set_bev_styles / t2d_bev_render)
+  std::vector<int> tile_nseg;          // segments of every tile of the current map, in tile order
+  int n_bev_styles = 0;                // 0: styles not set
+  t2d_bev_style bev_style[bev::MAX_STYLES] = {};
+  uint8_t bev_type_style[T2D_MAX_TYPES] = {};
+  int bev_target_style = bev::NO_STYLE;
+  uint8_t* d_seg_style = nullptr;      // per segment, tiles back to back; nullptr: the default ring / open styles
+  uint32_t* d_seg_base = nullptr;      // [n_tiles] first entry of every tile in d_seg_style
 };
 
 extern "C" {
@@ -1806,6 +1816,8 @@ int t2d_destroy(t2d_ctx* c) {
   if (c->d_ctab) cudaFree(c->d_ctab);
   if (c->d_path_v) cudaFree(c->d_path_v);
   if (c->d_path_off) cudaFree(c->d_path_off);
+  if (c->d_seg_style) cudaFree(c->d_seg_style);
+  if (c->d_seg_base) cudaFree(c->d_seg_base);
   if (c->hs_action) cudaFree(c->hs_action);
   if (c->hs_ego_pinned) cudaFreeHost(c->hs_ego_pinned);
   if (c->hs_out) cudaFree(c->hs_out);
@@ -2083,6 +2095,9 @@ int t2d_set_map_table(t2d_ctx* c, const t2d_map_tile* tiles, int n_tiles, const 
   CUDA_TRY(cudaSetDevice(c->device));
   if (c->d_map) { cudaFree(c->d_map); c->d_map = nullptr; }
   if (c->d_tile_off) { cudaFree(c->d_tile_off); c->d_tile_off = nullptr; }
+  if (c->d_seg_style) { cudaFree(c->d_seg_style); c->d_seg_style = nullptr; }   // a new map: default segment styles
+  if (c->d_seg_base) { cudaFree(c->d_seg_base); c->d_seg_base = nullptr; }
+  c->tile_nseg.clear();
   c->map_bytes = 0; c->n_tiles = 0; c->tile_id = nullptr; c->has_bounds = false; c->has_segments = false;
   c->mh = MapHeader{};
   if (n_tiles == 0) return T2D_OK;
@@ -2105,6 +2120,7 @@ int t2d_set_map_table(t2d_ctx* c, const t2d_map_tile* tiles, int n_tiles, const 
   CUDA_TRY(cudaMalloc(&c->d_tile_off, sizeof(uint32_t) * (size_t)n_tiles));
   CUDA_TRY(cudaMemcpy(c->d_tile_off, offs.data(), sizeof(uint32_t) * (size_t)n_tiles, cudaMemcpyHostToDevice));
   c->n_tiles = n_tiles;
+  for (int i = 0; i < n_tiles; ++i) c->tile_nseg.push_back(tiles[i].n_seg);
   c->tile_id = n_tiles > 1 ? tile_id : nullptr;
   c->map_bytes = (int)c->mh.smem_bytes;     // what a single tile stages into shared memory
   c->has_bounds = any_bounds; c->has_segments = any_seg;
@@ -2480,6 +2496,92 @@ int t2d_lidar_scan(t2d_ctx* c, int n_beams, float max_range, const double* beam_
   A.N = c->N; A.M = c->M; A.n_beams = n_beams; A.range = (double)max_range;
   const int grid = (c->N + LIDAR_WARPS - 1) / LIDAR_WARPS;
   t2d_lidar_kernel<<<grid, LIDAR_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  g_launches.fetch_add(1);
+  CUDA_TRY(cudaGetLastError());
+  return T2D_OK;
+}
+
+int t2d_set_bev_styles(t2d_ctx* c, const t2d_bev_style* table, int n_styles, const uint8_t* type_style, const uint8_t* seg_style,
+                       int n_seg_total, int target_style) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (!table || n_styles < 4 || n_styles > T2D_MAX_BEV_STYLES) return fail(T2D_E_INVALID, "n_styles must be in 4..64");
+  if (!type_style) return fail(T2D_E_INVALID, "type_style is NULL");
+  for (int i = 0; i < n_styles; ++i)
+    if (!(table[i].line_width_pt >= 0.0f && table[i].line_width_pt <= 100.0f))
+      return fail(T2D_E_INVALID, "style line width must be in [0, 100] pt");
+  auto ok = [&](int s) { return s == bev::NO_STYLE || (s >= 0 && s < n_styles); };
+  for (int t = 0; t < c->n_types; ++t)
+    if (!ok(type_style[t])) return fail(T2D_E_INVALID, "type_style: no such style");
+  if (!ok(target_style)) return fail(T2D_E_INVALID, "target_style: no such style");
+  long long total = 0;
+  for (int k : c->tile_nseg) total += k;
+  if (seg_style) {
+    if (n_seg_total != total) return fail(T2D_E_INVALID, "n_seg_total differs from the segments of the map's tiles");
+    for (long long s = 0; s < total; ++s)
+      if (!ok(seg_style[s])) return fail(T2D_E_INVALID, "seg_style: no such style");
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  if (c->d_seg_style) { cudaFree(c->d_seg_style); c->d_seg_style = nullptr; }
+  if (c->d_seg_base) { cudaFree(c->d_seg_base); c->d_seg_base = nullptr; }
+  if (seg_style && total > 0) {
+    std::vector<uint32_t> base(c->tile_nseg.size());
+    uint32_t acc = 0;
+    for (size_t i = 0; i < base.size(); ++i) { base[i] = acc; acc += (uint32_t)c->tile_nseg[i]; }
+    CUDA_TRY(cudaMalloc(&c->d_seg_style, (size_t)total));
+    CUDA_TRY(cudaMemcpy(c->d_seg_style, seg_style, (size_t)total, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMalloc(&c->d_seg_base, sizeof(uint32_t) * base.size()));
+    CUDA_TRY(cudaMemcpy(c->d_seg_base, base.data(), sizeof(uint32_t) * base.size(), cudaMemcpyHostToDevice));
+  }
+  memcpy(c->bev_style, table, sizeof(t2d_bev_style) * (size_t)n_styles);
+  memset(c->bev_type_style, bev::NO_STYLE, sizeof(c->bev_type_style));
+  memcpy(c->bev_type_style, type_style, (size_t)c->n_types);
+  c->bev_target_style = target_style;
+  c->n_bev_styles = n_styles;
+  // opt in to the kernel's shared memory here: t2d_bev_render must stay free of anything a graph capture rejects
+  CUDA_TRY(cudaFuncSetAttribute(bev::t2d_bev_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(bev::Smem)));
+  return T2D_OK;
+}
+
+int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rgb, uint8_t* out, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (c->n_bev_styles == 0) return fail(T2D_E_STATE, "BEV styles not set: call t2d_set_bev_styles first");
+  if (!range || !out) return fail(T2D_E_INVALID, "t2d_bev_render: range / out is NULL");
+  if (width < 1 || height < 1 || width > bev::MAX_SIDE || height > bev::MAX_SIDE)
+    return fail(T2D_E_INVALID, "t2d_bev_render: width and height must be in 1..1024");
+  for (int k = 0; k < 4; ++k)
+    if (!(range[k] > 0.0f && range[k] <= 1.0e5f)) return fail(T2D_E_INVALID, "t2d_bev_render: every range must be in (0, 1e5] m");
+  // the window (matplotlib_renderer.py:152-164, auto_scale :200-224), in the float64 oracle's operation order
+  const double L = range[0], R = range[1], F = range[2], B = range[3];
+  const double x_min = -L, x_max = R, y_min = -B, y_max = F;
+  const double ww = x_max - x_min, wh = y_max - y_min;
+  const double cx = (x_min + x_max) / 2, cy = (y_min + y_max) / 2;
+  const double aspect = (double)height / (double)width;
+  double nw, nh;
+  if (wh / ww > aspect) { nw = wh / aspect; nh = wh; }
+  else { nw = ww; nh = ww * aspect; }
+  const double nx0 = cx - nw / 2, nx1 = cx + nw / 2, ny0 = cy - nh / 2, ny1 = cy + nh / 2;
+  bev::Args A{};
+  A.win.xmin = nx0; A.win.ymax = ny1;
+  A.win.px = (nx1 - nx0) / width; A.win.py = (ny1 - ny0) / height;
+  for (int s = 0; s < c->n_bev_styles; ++s) {
+    const t2d_bev_style& st = c->bev_style[s];
+    const double hw = (double)st.line_width_pt * 200.0 / 72.0 / 2.0 * A.win.px;   // points at the renderer's 200 dpi
+    A.hw2[s] = hw * hw;
+    A.style_rgb[s][0] = st.r; A.style_rgb[s][1] = st.g; A.style_rgb[s][2] = st.b;
+    A.style_z[s] = st.z;
+  }
+  memcpy(A.type_style, c->bev_type_style, sizeof(A.type_style));
+  A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table; A.n_types = c->n_types;
+  A.N = c->N; A.M = c->M;
+  A.map_blob = c->d_map; A.tile_off = c->d_tile_off; A.tile_id = c->n_tiles > 1 ? c->tile_id : nullptr;
+  A.seg_style = c->d_seg_style; A.seg_base = c->d_seg_base;
+  A.target = c->goal_target; A.target_style = c->bev_target_style;
+  A.ring_style = T2D_BEV_STYLE_RING; A.open_style = T2D_BEV_STYLE_OPEN;
+  A.W = width; A.H = height; A.rgb = rgb ? 1 : 0; A.out = out;
+  CUDA_TRY(cudaSetDevice(c->device));
+  bev::t2d_bev_kernel<<<c->N, bev::CTA, sizeof(bev::Smem), (cudaStream_t)stream>>>(A);
   g_launches.fetch_add(1);
   CUDA_TRY(cudaGetLastError());
   return T2D_OK;

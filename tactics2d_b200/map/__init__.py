@@ -269,3 +269,25 @@ def polygons_to_segments(polygons, polylines=()):
             segs.append(np.concatenate([v[:-1], v[1:]], 1))
     seg = np.concatenate(segs, 0).astype(np.float32) if segs else np.zeros((0, 4), np.float32)
     return np.ascontiguousarray(seg), np.asarray(starts, dtype=np.int32)
+
+
+def area_style_key(area: Area) -> str:
+    """The BEV style key of an Area as ``BEVCamera._get_type`` picks it (sensor/camera.py:56-87): its subtype, else its
+    type, else ``"area"``.  A key without a row in ``sensor.camera.BEV_STYLES`` draws as ``"area"``."""
+    from ..sensor.camera import BEV_STYLES
+
+    key = area.subtype or area.type_ or "area"
+    return key if key in BEV_STYLES else "area"
+
+
+def segment_style_keys(polygons, polylines=(), polyline_key: str = "road_border"):
+    """Per-segment BEV style keys in the layout :func:`polygons_to_segments` returns for the same arguments: every
+    edge of an Area gets :func:`area_style_key` (a bare vertex array: ``"obstacle"``), every polyline piece
+    ``polyline_key``.  Pass the result as the ``"style"`` of a tile (``BatchedWorld.set_map`` / ``set_map_table``)."""
+    seg, ps = polygons_to_segments(polygons, polylines)
+    keys = []
+    for p, poly in enumerate(polygons):
+        k = area_style_key(poly) if isinstance(poly, Area) else "obstacle"
+        keys += [k] * int(ps[p + 1] - ps[p])
+    keys += [polyline_key] * (len(seg) - len(keys))
+    return keys

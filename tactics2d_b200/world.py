@@ -106,6 +106,8 @@ class BatchedWorld:
         self.tiles, self.tile_id = None, None
         self.bounds = None
         self._goal = None
+        self._seg_style_keys = []
+        self._bev_cfg = None
 
     # ------------------------------------------------------------------ plumbing
     def _bind(self):
@@ -145,7 +147,8 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_set_type_table(self._ctx, type_table.to_c_array(), len(type_table)))
         self.type_table = type_table
 
-    def set_map(self, segments=None, bounds: Optional[Sequence[float]] = None, cell_size: float = 0.0, poly_start=None):
+    def set_map(self, segments=None, bounds: Optional[Sequence[float]] = None, cell_size: float = 0.0, poly_start=None,
+                style=None):
         """Static geometry of the scenario (shared by all N scenarios).
 
         ``segments``: array [S, 4] of (x1, y1, x2, y2) collidable pieces in list order - what
@@ -154,7 +157,9 @@ class BatchedWorld:
         (out_bound.py:50-65), or None;
         ``poly_start``: int array [P + 1] marking the segments that close up to ``Area`` polygons (ring p = segments
         [poly_start[p], poly_start[p + 1])): a pose inside a polygon collides with it even when it touches no edge, and
-        ``hit_segment`` then names the first object hit by its first segment (see :func:`polygons_to_segments`)."""
+        ``hit_segment`` then names the first object hit by its first segment (see :func:`polygons_to_segments`);
+        ``style``: optional BEV style key of every segment (a ring object is drawn in the style of its first segment;
+        :func:`tactics2d_b200.map.segment_style_keys`), default ``obstacle`` for rings and ``road_border`` otherwise."""
         seg = None if segments is None else np.ascontiguousarray(np.asarray(segments, dtype=np.float32).reshape(-1, 4))
         n_seg = 0 if seg is None else seg.shape[0]
         b = None if bounds is None else np.ascontiguousarray(np.asarray(bounds, dtype=np.float32))
@@ -167,10 +172,12 @@ class BatchedWorld:
         self.poly_start = ps
         self.bounds = None if b is None else tuple(float(v) for v in b)
         self.tiles, self.tile_id = None, None
+        self._seg_style_keys = [self._check_style_keys(style, n_seg)]
+        self._push_bev_styles()
 
     def set_map_table(self, tiles, tile_id, cell_size: float = 0.0):
         """A different map per scenario: ``tiles`` is a list of dicts ``{"segments": [S, 4], "bounds": (4,) or None,
-        "poly_start": [P + 1] or None}`` (what ``_ParkingScenarioManager.reset`` builds per episode - the lot's wall and
+        "poly_start": [P + 1] or None, "style": [S] BEV style keys or None}`` (what ``_ParkingScenarioManager.reset`` builds per episode - the lot's wall and
         obstacle Areas and ``map_.boundary``, envs/parking.py:397-441 - or the reference's ``data/*_map`` files, one tile
         each: ``map.polygons_to_segments(map.load_areas(name, subtypes), [lines])``), ``tile_id`` an integer array [N]: the tile of every scenario.  The ids live in ``self.tile_id`` (uint16
         device tensor) and may be rewritten between ticks."""
@@ -195,6 +202,9 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_set_map_table(self._ctx, rows, len(tiles), _ptr(self.tile_id), float(cell_size)))
         self.tiles = [dict(segments=k[0], bounds=None if k[1] is None else tuple(float(v) for v in k[1]), poly_start=k[2]) for k in keep]
         self.segments, self.poly_start, self.bounds = None, None, None
+        self._seg_style_keys = [self._check_style_keys(t.get("style"), 0 if k[0] is None else k[0].shape[0])
+                                for t, k in zip(tiles, keep)]
+        self._push_bev_styles()
 
     def set_goal(self, target=None, arrival_threshold: float = 0.95, no_action_max_step: int = 100):
         """Target area per scenario for the ego (participant 0): array [N, 5] = (cx, cy, heading, half_len, half_wid),
@@ -436,6 +446,99 @@ class BatchedWorld:
             self._lidar = cache = (key, cs.contiguous(), scan)
         _lib.check(self.lib.t2d_lidar_scan(self._ctx, int(n_beams), float(max_range), _ptr(cache[1]), _ptr(cache[2]), self._stream()))
         return cache[2]
+
+    # ------------------------------------------------------------------ BEV observation
+    @staticmethod
+    def _check_style_keys(keys, n_seg):
+        from .sensor.camera import BEV_STYLES
+
+        if keys is None:
+            return None
+        keys = list(keys)
+        if len(keys) != n_seg:
+            raise ValueError(f"style needs one key per segment ({n_seg}), got {len(keys)}")
+        bad = [k for k in keys if k is not None and k not in BEV_STYLES]
+        if bad:
+            raise ValueError(f"unknown BEV style keys {sorted(set(bad))}")
+        return keys
+
+    def set_bev_styles(self, type_styles=None, target: Optional[str] = "target_area"):
+        """Choose how ``bev`` draws each participant type and the goal rectangle, by style key of
+        :data:`tactics2d_b200.sensor.camera.BEV_STYLES`.  ``type_styles``: one key (or None = not drawn) per type-table
+        row, default from each row's template name (:func:`~tactics2d_b200.sensor.camera.default_type_style`);
+        ``target``: the style of the ``set_goal`` rectangle, None = not drawn.  Map segments take the ``style`` given to
+        ``set_map`` / ``set_map_table``."""
+        from .sensor.camera import BEV_STYLES, default_type_style
+
+        if type_styles is None:
+            type_styles = [default_type_style(r) for r in self.type_table.rows]
+        type_styles = list(type_styles)
+        if len(type_styles) != len(self.type_table):
+            raise ValueError(f"type_styles needs one key per type-table row ({len(self.type_table)})")
+        for k in type_styles + [target]:
+            if k is not None and k not in BEV_STYLES:
+                raise ValueError(f"unknown BEV style key {k!r}")
+        self._bev_cfg = (type_styles, target)
+        self._push_bev_styles()
+
+    def _push_bev_styles(self):
+        from .sensor.camera import BEV_STYLES, NOT_DRAWN, STYLE_KEYS, style_rgb
+
+        if self._bev_cfg is None:
+            return
+        type_styles, target = self._bev_cfg
+        idx = {k: i for i, k in enumerate(STYLE_KEYS)}
+        table = (_lib.BevStyleC * len(STYLE_KEYS))()
+        for i, k in enumerate(STYLE_KEYS):
+            r, g, b = style_rgb(k)
+            table[i] = _lib.BevStyleC(r, g, b, BEV_STYLES[k][1], BEV_STYLES[k][2])
+        ts = np.asarray([NOT_DRAWN if k is None else idx[k] for k in type_styles], dtype=np.uint8)
+        seg = None
+        if any(keys is not None for keys in self._seg_style_keys):
+            parts = []
+            polys = [self.poly_start] if self.tiles is None else [t["poly_start"] for t in self.tiles]
+            for keys, ps in zip(self._seg_style_keys, polys):
+                if keys is None:   # this tile keeps the defaults
+                    ring = np.zeros(self._tile_nseg(len(parts)), bool)
+                    if ps is not None and len(ps) >= 2:
+                        ring[ps[0]:ps[-1]] = True
+                    parts.append(np.where(ring, idx["obstacle"], idx["road_border"]).astype(np.uint8))
+                else:
+                    parts.append(np.asarray([NOT_DRAWN if k is None else idx[k] for k in keys], dtype=np.uint8))
+            seg = np.ascontiguousarray(np.concatenate(parts)) if parts else None
+        n_seg_total = 0 if seg is None else len(seg)
+        _lib.check(self.lib.t2d_set_bev_styles(
+            self._ctx, table, len(STYLE_KEYS), C.c_void_p(ts.ctypes.data),
+            C.c_void_p(0 if seg is None or n_seg_total == 0 else seg.ctypes.data), n_seg_total,
+            NOT_DRAWN if target is None else idx[target]))
+
+    def _tile_nseg(self, i):
+        if self.tiles is None:
+            return 0 if self.segments is None else self.segments.shape[0]
+        s = self.tiles[i]["segments"]
+        return 0 if s is None else s.shape[0]
+
+    def bev(self, resolution=(200, 200), perception_range=(20.0, 20.0, 20.0, 20.0), rgb: bool = True) -> torch.Tensor:
+        """Bird's-eye view of every scenario's ego (``BEVCamera.update`` + ``MatplotlibRenderer``, sensor/camera.py:333-386,
+        renderer/matplotlib_renderer.py:542-768) in one launch: ``uint8 [N, H, W, 3]`` RGB, or with ``rgb=False`` the
+        style indices ``uint8 [N, H, W]`` (RGB = ``sensor.camera.palette()[index]``).  ``resolution`` = (width, height);
+        ``perception_range`` = R or (left, right, front, back) in metres.  The returned tensor is a buffer the world
+        reuses on the next call with the same shape.  Uses the default styles until ``set_bev_styles`` is called."""
+        if self._bev_cfg is None:
+            self.set_bev_styles()
+        w, h = int(resolution[0]), int(resolution[1])
+        pr = perception_range
+        rng = np.ascontiguousarray(np.asarray([pr] * 4 if np.ndim(pr) == 0 else pr, dtype=np.float32).reshape(4))
+        key = (w, h, bool(rgb))
+        cache = getattr(self, "_bev_out", None)
+        if cache is None or cache[0] != key:
+            if not (1 <= w <= 1024 and 1 <= h <= 1024):
+                raise ValueError("resolution: width and height must be in 1..1024")
+            shape = (self.N, h, w, 3) if rgb else (self.N, h, w)
+            self._bev_out = cache = (key, torch.empty(shape, dtype=torch.uint8, device=self.device))
+        _lib.check(self.lib.t2d_bev_render(self._ctx, w, h, C.c_void_p(rng.ctypes.data), 1 if rgb else 0, _ptr(cache[1]),
+                                           self._stream()))
+        return cache[1]
 
     def reset(self, mask: torch.Tensor, pool: dict, pool_index: Optional[torch.Tensor] = None):
         """Re-initialise the scenarios with ``mask[n] != 0`` from row ``pool_index[n]`` (default n)
