@@ -337,6 +337,31 @@ __device__ __forceinline__ unsigned pair_word_bits(const float (&X)[2 * IPW], co
   return bits;
 }
 
+// Minus the squared broadphase reach of an own participant of bounding radius rb: conservative, since any partner's
+// bounding radius is <= rb_max.  The per-lane sweep and the compacted sweep form it from the same floats.
+__device__ __forceinline__ float neg_reach2(float rb, float rb_max) {
+  const float rr = rb + rb_max;
+  return -fmaf(rr * rr, 1.00001f, 1e-12f);
+}
+
+// Box (xmin, xmax, ymin, ymax) of the 8 extended slots x[0..7], y[0..7] (16-byte aligned) a partner word reads.  A slot
+// whose x is NaN (non-solid, empty) is left out, its y too; an all-NaN window gives the empty box (+inf, -inf, +inf, -inf).
+__device__ __forceinline__ float4 window_box(const float* x, const float* y) {
+  float4 b = make_float4(INFINITY, -INFINITY, INFINITY, -INFINITY);
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    const float4 xv = reinterpret_cast<const float4*>(x)[q], yv = reinterpret_cast<const float4*>(y)[q];
+    const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, ys[4] = {yv.x, yv.y, yv.z, yv.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float yk = xs[k] == xs[k] ? ys[k] : __int_as_float(0x7fc00000);
+      b.x = fminf(b.x, xs[k]); b.y = fmaxf(b.y, xs[k]);   // (fminf / fmaxf return the other operand for a NaN)
+      b.z = fminf(b.z, yk); b.w = fmaxf(b.w, yk);
+    }
+  }
+  return b;
+}
+
 // Broadphase slow path.  `bits` holds the distance-test verdicts of four partner-loop iterations of this lane:
 // bit ((uu * PPL + i) * 2 + e) = own participant m0 + i against extended slot m0 + 2 (u_base + uu) + e.  Keep the
 // combinations whose partner offset q is 1..Mh (every unordered pair once; q <= 0 are the lane's own participants
@@ -849,7 +874,6 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       // (lane-minor layout, see pslot: these stores are conflict-free)
       poseA[i * 32 + lane] = make_float4(px[i], py[i], rb[i], shd[i]);
       poseB[i * 32 + lane] = make_float4(ch[i], sh[i], g2.x, g2.y);
-      hitmin[i * 32 + lane] = 0x7fffffff;
     }
     // circularly extended positions: slot k holds participant k mod M, i.e. this lane's PPL participants go to
     // m0 .. m0 + PPL - 1 and to the copies M and 2 M further on that still fit
@@ -909,42 +933,119 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       float nx[PPL], ny[PPL], nthr[PPL];
 #pragma unroll
       for (int i = 0; i < PPL; ++i) {
-        const float rr = rb[i] + A.rb_max;
-        const float thr = fmaf(rr * rr, 1.00001f, 1e-12f);   // conservative: any partner's bounding radius <= rb_max
         nx[i] = -px[i];
         ny[i] = -py[i];
-        nthr[i] = -thr;
+        nthr[i] = neg_reach2(rb[i], A.rb_max);
       }
       // partner pairs u = 0 .. U-1 cover offsets -(PPL-1) .. >= Mh; U is rounded up to whole words (the extended
       // arrays are long enough), so the word body has no bounds test and its loads can be issued back to back
       const int n_words = Mh > 0 ? (((Mh + PPL + 1) >> 1) + IPW - 1) / IPW : 0;
       // one word = 2 * IPW consecutive partners: 128-bit loads (every scenario's window and m0 are 16-byte aligned)
-      const float4* bx = reinterpret_cast<const float4*>(posx + m0);
-      const float4* by = reinterpret_cast<const float4*>(posy + m0);
-      auto load_word = [&](int uw, float (&X)[2 * IPW], float (&Y)[2 * IPW]) {
+      auto load_word = [&](const float* wx, const float* wy, float (&X)[2 * IPW], float (&Y)[2 * IPW]) {
 #pragma unroll
         for (int q = 0; q < IPW / 2; ++q) {
-          const float4 xv = bx[uw * (IPW / 2) + q], yv = by[uw * (IPW / 2) + q];
+          const float4 xv = reinterpret_cast<const float4*>(wx)[q], yv = reinterpret_cast<const float4*>(wy)[q];
           X[4 * q] = xv.x; X[4 * q + 1] = xv.y; X[4 * q + 2] = xv.z; X[4 * q + 3] = xv.w;
           Y[4 * q] = yv.x; Y[4 * q + 1] = yv.y; Y[4 * q + 2] = yv.z; Y[4 * q + 3] = yv.w;
         }
       };
+      // Box cull of words 1 .. n_words-1.  In an ordered scene most of them hold no partner within reach of any of the
+      // lane's participants, but nearly every warp has SOME lane that needs each word, so skipping words per warp never
+      // fires.  Instead every lane tests its own box against the box of each word's 8 partner slots, and the (lane, word)
+      // items that survive are compacted into a per-warp list that all 32 lanes sweep together.
+      //
+      // Why a culled word holds no candidate.  Let own participant i and partner j have the margin
+      // d = fma(dx, dx, fma(dy, dy, -thr)) <= 0, dx = fl(Xj - px_i), dy = fl(Yj - py_i), as the sweep computes it.  A NaN
+      // operand makes d NaN and an infinite dx or dy makes it +inf or NaN, so everything below is finite.  (a) Rounding is
+      // monotone and every v >= 2^-149 rounds to >= 2^-149 > 0, so d <= 0 means dx^2 + e < 2^-149 for e = fl(dy^2 - thr)
+      // >= -thr (thr is a float); likewise e < 2^-149 means dy^2 - thr < 2^-149.  Hence |dx|, |dy| < sqrt(thr) + 2^-74.
+      // (b) dx rounds the exact Xj - px_i with relative error 2^-24 (absolute 2^-150 among subnormals), so
+      // |Xj - px_i| < (sqrt(thr) + 2^-74)(1 + 2^-23) + 2^-149, and the same for y.  (c) thr = fl(fl(rr^2) * 1.00001f +
+      // 1e-12f), rr = fl(rb_i + rb_max), so sqrt(thr) <= rr * 1.0000051 * (1 + 2^-24) + 1.0000001e-6 and the bound of (b)
+      // is below D = rr * 1.0000054 + 1.1e-6.  (d) The lane box [lx0, lx1] x [ly0, ly1] is the exact min / max of the
+      // lane's positions whose x is not NaN, and the window box that of the word's 8 slots (window_box), so
+      // px_i - Xj >= lx0 - wx1 exactly.  The test rounds that difference once: g = fl(lx0 - wx1) > T with T a float
+      // implies lx0 - wx1 > T exactly (monotone rounding again), so no coordinate-dependent slack enters - at |x| = 1e4
+      // as at the origin - and T = fl(fma(max_i rr_i, 1.0001f, 1e-5f)) >= rr * 1.0000999 + 0.99e-5 > D.  So a word culled
+      // by any of the four sides has |Xj - px_i| > D or |Yj - py_i| > D for each of its 32 pairs: no candidate.  A NaN
+      // or infinite operand of the test (empty boxes against each other, inf - inf) makes a comparison false, i.e. keeps
+      // the word, which is always allowed; an empty lane or window box (+inf - finite) culls it, correctly.
+      //
+      // The window boxes live in the warp's queue area and the item list in its hit-minimum area: nothing is queued
+      // before the sweep (the table is dead once the list is built, and a __syncwarp separates the two), and the hit
+      // minima are first written after the sweep.
+      int n_items = 0;
+      uint8_t* items = reinterpret_cast<uint8_t*>(hitmin);   // (uw - 1) << 5 | lane: at most 32 x 8 bytes (M <= 128)
+      if (n_words > 1) {   // (M is uniform: so is n_words)
+        // window j of a scenario = extended slots 4 j .. 4 j + 7: lane gl, word uw reads window gl + 2 uw.  With M <= 4 G,
+        // n_words - 1 <= G / 4, so the 32 / G scenarios of a warp hold at most 32 / G x 1.5 G = 48 boxes = QCAP words.
+        const int wstride = G + 2 * (n_words - 1);
+        float4* wbox = reinterpret_cast<float4*>(queue) + sub * wstride;
+        for (int j = gl; j < wstride; j += G) wbox[j] = window_box(posx + 4 * j, posy + 4 * j);
+        float lx0 = INFINITY, lx1 = -INFINITY, ly0 = INFINITY, ly1 = -INFINITY, rr_max = 0.0f;
+#pragma unroll
+        for (int i = 0; i < PPL; ++i) {
+          const float yk = px[i] == px[i] ? py[i] : __int_as_float(0x7fc00000);
+          lx0 = fminf(lx0, px[i]); lx1 = fmaxf(lx1, px[i]); ly0 = fminf(ly0, yk); ly1 = fmaxf(ly1, yk);
+          rr_max = fmaxf(rr_max, rb[i] + A.rb_max);
+        }
+        const float reach = fmaf(rr_max, 1.0001f, 1e-5f);
+        __syncwarp();
+        for (int uw = 1; uw < n_words; ++uw) {
+          const float4 b = wbox[gl + 2 * uw];
+          const bool need = !(lx0 - b.y > reach || b.x - lx1 > reach || ly0 - b.w > reach || b.z - ly1 > reach);
+          const unsigned m = __ballot_sync(0xffffffffu, need);
+          if (need) items[n_items + __popc(m & ((1u << lane) - 1u))] = (uint8_t)(((uw - 1) << 5) | lane);
+          n_items += __popc(m);
+        }
+        __syncwarp();
+      }
       if (n_words > 0) {   // word 0 also meets the lane's own participants (offset <= 0): those tests are compiled out
         float X[2 * IPW], Y[2 * IPW];
-        load_word(0, X, Y);
+        load_word(posx + m0, posy + m0, X, Y);
         if (pair_word_min<true>(X, Y, nx, ny, nthr) <= 0.0f) {
           const unsigned bits = pair_word_bits<true>(X, Y, nx, ny, nthr);
           if (bits) pair_enqueue_bits(bits, 0, t0, tb, m0, M, Mh, queue, qcount);
         }
       }
-      for (int uw = 1; uw < n_words; ++uw) {
-        float X[2 * IPW], Y[2 * IPW];
-        load_word(uw, X, Y);
-        if (pair_word_min<false>(X, Y, nx, ny, nthr) <= 0.0f) {
-          const unsigned bits = pair_word_bits<false>(X, Y, nx, ny, nthr);
-          if (bits) pair_enqueue_bits(bits, uw * IPW, t0, tb, m0, M, Mh, queue, qcount);
+      if ((n_items + 31) >> 5 < n_words - 1) {
+        // the list takes fewer warp passes than every lane sweeping all its words: an item reloads its owner's positions
+        // and reach from the pose tile; margins, verdict bits and queue entries are the per-lane sweep's, in another order
+        // (the narrowphase's atomicMin does not depend on it, and overflow is decided on the same count)
+        for (int k = lane; k < n_items; k += 32) {
+          const unsigned it = items[k];
+          const int ol = (int)(it & 31u), uw = (int)(it >> 5) + 1;
+          const int osub = ol >> A.g_shift, om0 = (ol & (G - 1)) * PPL, otb = osub * MP;
+          float onx[PPL], ony[PPL], onthr[PPL];
+#pragma unroll
+          for (int i = 0; i < PPL; ++i) {
+            const float4 a = poseA[i * 32 + ol];
+            onx[i] = -a.x;
+            ony[i] = -a.y;
+            onthr[i] = neg_reach2(a.z, A.rb_max);
+          }
+          const int off = osub * EXT + om0 + uw * 2 * IPW;
+          float X[2 * IPW], Y[2 * IPW];
+          load_word(s_posx + warp * POS_EXT_PER_WARP + off, s_posy + warp * POS_EXT_PER_WARP + off, X, Y);
+          if (pair_word_min<false>(X, Y, onx, ony, onthr) <= 0.0f) {
+            const unsigned bits = pair_word_bits<false>(X, Y, onx, ony, onthr);
+            if (bits) pair_enqueue_bits(bits, uw * IPW, otb + om0, otb, om0, M, Mh, queue, qcount);
+          }
+        }
+      } else {
+        // unordered scenes: nearly every word is needed, and the lanes sweep their own words from registers
+        for (int uw = 1; uw < n_words; ++uw) {
+          float X[2 * IPW], Y[2 * IPW];
+          load_word(posx + m0 + uw * 2 * IPW, posy + m0 + uw * 2 * IPW, X, Y);
+          if (pair_word_min<false>(X, Y, nx, ny, nthr) <= 0.0f) {
+            const unsigned bits = pair_word_bits<false>(X, Y, nx, ny, nthr);
+            if (bits) pair_enqueue_bits(bits, uw * IPW, t0, tb, m0, M, Mh, queue, qcount);
+          }
         }
       }
+      __syncwarp();   // the item list is dead: the hit minima take its place
+#pragma unroll
+      for (int i = 0; i < PPL; ++i) hitmin[i * 32 + lane] = 0x7fffffff;
       __syncwarp();
       // narrowphase: the queued candidate pairs, one per lane (or the exhaustive pass if the queue overflowed)
       const int n_q = *qcount;
