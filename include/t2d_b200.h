@@ -43,6 +43,8 @@
  *   t2d_check_events     the same detectors on caller-supplied poses (no physics)
  *   t2d_reset            ScenarioManager.reset / ParticipantBase.reset
  *                                                         tactics2d/envs/parking.py:397-441, participant_base.py:236-246
+ *   t2d_set_log          Trajectory.get_state / Vehicle.get_pose of logged participants at a frame
+ *                                                         participant/trajectory/trajectory.py:97-113, vehicle.py:263-281
  *
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types cross the ABI;
@@ -230,6 +232,38 @@ int t2d_reset(t2d_ctx* ctx, const uint8_t* mask, const int32_t* pool_index, int 
               const float* pool_vy, void* stream);
 /* Optional initial wheel speeds for t2d_reset: DEVICE arrays [n_pool][M] indexed like the other pool columns (NULL, NULL unbinds). */
 int t2d_bind_reset_wheel_pool(t2d_ctx* ctx, const float* pool_omega_front, const float* pool_omega_rear);
+
+/* ---- log replay: recorded tracks drive participants around a simulated ego ------------------------------------------
+ * Trajectory.get_state(frame) / Vehicle.get_pose(frame) (participant/trajectory/trajectory.py:97-113,
+ * participant/element/vehicle.py:263-281) for every replayed slot of every scenario, on the device.  The contract
+ * (sampling, interpolation between frames, absent tracks) is DESIGN.md section 1 "Log replay".
+ * A track k is present on [first_ms[k], first_ms[k] + (n_frames[k] - 1) * period_ms[k]] and holds n_frames[k] records
+ * (x, y, heading, vx, vy), fp32, in records starting at record sum(n_frames[0..k-1]).  Its type_row must be a
+ * T2D_MODEL_STATIC row of the type table: the tick then only builds the pose of a replayed slot and checks it like any
+ * other participant.  Episode row p starts at t0_ms[p] and binds slot m to track row_track[p * M + m] (-1: not
+ * replayed; a track at most once per row).  Before every tick, scenario n samples its row log_row[n] at
+ * t = t0_ms[row] + (step_count[n] + 1) * interval_ms, the time the tick produces: a replayed slot takes the track's
+ * state at t, and type_id T2D_TYPE_INACTIVE while the track is absent.  t2d_check_events does not replay.
+ * t2d_reset sets log_row[n] = pool_index[n] (n without pool_index) for the masked scenarios, needs n_pool == n_rows,
+ * and samples those scenarios at t0 at once.  While a log is bound the tick keeps every static slot's vx, vy. */
+typedef struct t2d_log {
+  int32_t n_tracks;           /* >= 1 */
+  const int32_t* first_ms;    /* HOST [n_tracks] time stamp of the first record */
+  const int32_t* n_frames;    /* HOST [n_tracks] >= 1 */
+  const int32_t* period_ms;   /* HOST [n_tracks] > 0 */
+  const uint8_t* type_row;    /* HOST [n_tracks] type-table row, model T2D_MODEL_STATIC */
+  const float* records;       /* HOST [sum n_frames][5] x, y, heading, vx, vy; finite */
+  int32_t n_rows;             /* >= 1 */
+  const int32_t* t0_ms;       /* HOST [n_rows] */
+  const int32_t* row_track;   /* HOST [n_rows][M] in [-1, n_tracks) */
+  int32_t* log_row;           /* DEVICE [N], caller-owned: the row each scenario runs */
+  uint8_t* type_id;           /* DEVICE [N][M]: the type_id array of t2d_bind_state - the replay writes it, so the
+                                 writable pointer is passed here and must equal the bound one */
+} t2d_log;
+/* Host arrays are copied.  NULL unbinds.  Rejected (the previous log stays bound): malformed tables, a non-static track
+ * row, a type_id other than the bound one.  A later t2d_set_type_table that makes a track's row non-static is
+ * rejected too. */
+int t2d_set_log(t2d_ctx* ctx, const t2d_log* log);
 
 /* Single-line lidar of the ego (participant 0) of every scenario: SingleLineLidar._scan_obstacles
  * (tactics2d/sensor/lidar.py:128-221).  n_beams = point_density (lidar.py:49), max_range = perception range;

@@ -49,6 +49,13 @@ class BevStyleC(C.Structure):
     _fields_ = [("r", C.c_uint8), ("g", C.c_uint8), ("b", C.c_uint8), ("z", C.c_int8), ("line_width_pt", C.c_float)]
 
 
+class LogC(C.Structure):
+    """``t2d_log``: a recording's tracks and episode rows (host pointers) + the log_row / type_id device arrays."""
+    _fields_ = [("n_tracks", C.c_int32), ("first_ms", C.c_void_p), ("n_frames", C.c_void_p), ("period_ms", C.c_void_p),
+                ("type_row", C.c_void_p), ("records", C.c_void_p), ("n_rows", C.c_int32), ("t0_ms", C.c_void_p),
+                ("row_track", C.c_void_p), ("log_row", C.c_void_p), ("type_id", C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/t2d_b200.h declares
 _P = C.c_void_p
 SYMBOLS = {
@@ -85,6 +92,7 @@ SYMBOLS = {
     "t2d_physics_step": (C.c_int, [C.c_int, C.POINTER(TypeParamsC), C.c_int, C.c_int, C.c_int] + [_P] * 11),
     "t2d_bind_wheel_state": (C.c_int, [_P, _P, _P]),
     "t2d_bind_reset_wheel_pool": (C.c_int, [_P, _P, _P]),
+    "t2d_set_log": (C.c_int, [_P, C.POINTER(LogC)]),
     "t2d_set_prefetch": (C.c_int, [_P, C.c_int]),
     "t2d_launch_count": (C.c_int64, []),
 }

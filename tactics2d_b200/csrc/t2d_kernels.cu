@@ -8,6 +8,7 @@
 // K3  t2d_physics_kernel   flat batch through one physics model (PhysicsModelBase.step).
 // K4  t2d_lidar_kernel     single-line lidar of every scenario's ego (per-edge beam windows).
 // K5  t2d_control_kernel   NPC controllers: IDM, cruise / adaptive cruise, pure pursuit.
+// K7  t2d_replay_kernel    log replay: recorded tracks pose the replayed slots before K1 / after K2.
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory.
 //
 // Work decomposition of K1: a scenario (M <= 128 participants) is owned by a group of G lanes of
@@ -1308,6 +1309,88 @@ __global__ void __launch_bounds__(128) t2d_drift_kernel(const __grid_constant__ 
   }
 }
 
+// ---------------------------------------------------------------------------- K7
+// Log replay (t2d_set_log): every replayed slot takes its track's state at the time the next tick produces (or, in
+// reset mode, at the row's t0), before K1, which then only builds the pose of these static-model slots.  One thread
+// per (scenario, slot), consecutive threads on consecutive slots: the [N, M] row_track reads and the state / type_id
+// stores coalesce; the track entry and its two frame records are gathers.  Interpolation in fp64 with explicit
+// round-to-nearest operations (no FMA contraction), in the order oracle/replay.py states.
+struct ReplayTrack { int32_t first_ms, period_ms, n_frames, rec_off; };
+
+struct ReplayArgs {
+  float *x, *y, *h, *v, *vx, *vy;
+  uint8_t* type_id;
+  const int32_t* step_count;       // [N]
+  const int32_t* log_row;          // [N] the row each scenario runs (tick mode)
+  const uint8_t* mask;             // reset mode: [N] the scenarios being reset; nullptr in tick mode
+  const int32_t* pool_index;       // reset mode: the new row of each masked scenario, nullptr = row n
+  int32_t* log_row_out;            // reset mode: log_row, written for the masked scenarios
+  const ReplayTrack* tracks;       // [n_tracks]
+  const uint8_t* track_type;       // [n_tracks]
+  const float* rec;                // [sum n_frames][5] x, y, heading, vx, vy
+  const int32_t* t0;               // [n_rows] ms
+  const int32_t* row_track;        // [n_rows][M], -1 = not replayed
+  int N, M, n_rows, offset, interval_ms;
+};
+
+__device__ __forceinline__ float replay_lerp(float a, float b, double w) {   // a + w (b - a)
+  return __double2float_rn(__dadd_rn((double)a, __dmul_rn(w, __dsub_rn((double)b, (double)a))));
+}
+
+__global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__ ReplayArgs A) {
+  constexpr double PI_D = 3.141592653589793, TWO_PI_D = 6.283185307179586;
+  const long long total = (long long)A.N * A.M;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int n = (int)(i / A.M), m = (int)(i - (long long)n * A.M);
+    int row;
+    if (A.mask != nullptr) {
+      if (!A.mask[n]) continue;
+      row = A.pool_index ? A.pool_index[n] : n;
+      row = min(max(row, 0), A.n_rows - 1);   // as K2 clamps its pool row (n_pool == n_rows)
+      if (m == 0) A.log_row_out[n] = row;
+    } else {
+      row = min(max(A.log_row[n], 0), A.n_rows - 1);
+    }
+    const int k = A.row_track[(long long)row * A.M + m];
+    if (k < 0) continue;
+    const int4 tr4 = __ldg(reinterpret_cast<const int4*>(A.tracks) + k);
+    const int first = tr4.x, period = tr4.y, n_frames = tr4.z, rec_off = tr4.w;
+    const long long t = (long long)A.t0[row] + ((long long)A.step_count[n] + A.offset) * A.interval_ms;
+    const long long d = t - first;
+    if (d < 0 || d > (long long)(n_frames - 1) * period) {   // the track is not in the scene at t
+      A.type_id[i] = T2D_TYPE_INACTIVE;
+      continue;
+    }
+    const long long j = d / period;
+    const int r = (int)(d - j * period);
+    const float* a = A.rec + 5 * ((long long)rec_off + j);
+    float x, y, h, vx, vy;
+    if (r == 0) {   // on a frame: the record, bit for bit
+      x = a[0]; y = a[1]; h = a[2]; vx = a[3]; vy = a[4];
+    } else {        // between frames j and j + 1 (an extension: the reference has no state there)
+      const float* b = a + 5;
+      const double w = __ddiv_rn((double)r, (double)period);
+      x = replay_lerp(a[0], b[0], w);
+      y = replay_lerp(a[1], b[1], w);
+      vx = replay_lerp(a[3], b[3], w);
+      vy = replay_lerp(a[4], b[4], w);
+      const double ha = (double)a[2];
+      double dh = __dsub_rn((double)b[2], ha);   // the shorter arc: fold once into [-pi, pi]
+      if (dh > PI_D) dh = __dsub_rn(dh, TWO_PI_D);
+      else if (dh < -PI_D) dh = __dadd_rn(dh, TWO_PI_D);
+      double hh = __dadd_rn(ha, __dmul_rn(w, dh));
+      if (hh < 0.0) hh = __dadd_rn(hh, TWO_PI_D);   // wrap once into [0, 2 pi)
+      else if (hh >= TWO_PI_D) hh = __dsub_rn(hh, TWO_PI_D);
+      h = __double2float_rn(hh);
+      if (h == (float)TWO_PI_D) h = 0.0f;   // just below 2 pi, rounded up to fp32(2 pi): the same direction as 0
+    }
+    // State.speed (state.py:143-146) from the fp32 velocity
+    const float v = __double2float_rn(__dsqrt_rn(__dadd_rn(__dmul_rn((double)vx, (double)vx), __dmul_rn((double)vy, (double)vy))));
+    A.x[i] = x; A.y[i] = y; A.h[i] = h; A.v[i] = v; A.vx[i] = vx; A.vy[i] = vy;
+    A.type_id[i] = A.track_type[k];
+  }
+}
+
 struct PhysArgs {
   Params p;
   float *x, *y, *h, *v, *vx, *vy;
@@ -1858,6 +1941,18 @@ struct t2d_ctx {
   int bev_target_style = bev::NO_STYLE;
   uint8_t* d_seg_style = nullptr;      // per segment, tiles back to back; nullptr: the default ring / open styles
   uint32_t* d_seg_base = nullptr;      // [n_tiles] first entry of every tile in d_seg_style
+  // log replay (t2d_set_log / K7)
+  bool has_log = false;
+  int log_tracks = 0, log_rows = 0;
+  ReplayTrack* d_log_tracks = nullptr;
+  uint8_t* d_log_track_type = nullptr;
+  float* d_log_rec = nullptr;
+  int32_t* d_log_t0 = nullptr;
+  int32_t* d_log_row_track = nullptr;
+  int32_t* log_row = nullptr;          // caller-owned DEVICE [N]
+  uint8_t* log_type_id = nullptr;      // writable alias of type_id, checked against the bound one before every launch
+  std::vector<uint8_t> log_track_type; // host copy: t2d_set_type_table keeps these rows static
+  std::vector<int> type_model;         // host copy of the current type table's model ids
 };
 
 extern "C" {
@@ -1908,6 +2003,18 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
   return T2D_OK;
 }
 
+static void free_log(t2d_ctx* c) {
+  if (c->d_log_tracks) cudaFree(c->d_log_tracks);
+  if (c->d_log_track_type) cudaFree(c->d_log_track_type);
+  if (c->d_log_rec) cudaFree(c->d_log_rec);
+  if (c->d_log_t0) cudaFree(c->d_log_t0);
+  if (c->d_log_row_track) cudaFree(c->d_log_row_track);
+  c->d_log_tracks = nullptr; c->d_log_track_type = nullptr; c->d_log_rec = nullptr; c->d_log_t0 = nullptr;
+  c->d_log_row_track = nullptr;
+  c->has_log = false; c->log_tracks = c->log_rows = 0; c->log_row = nullptr; c->log_type_id = nullptr;
+  c->log_track_type.clear();
+}
+
 int t2d_destroy(t2d_ctx* c) {
   if (!c) return T2D_OK;
   cudaSetDevice(c->device);
@@ -1919,6 +2026,7 @@ int t2d_destroy(t2d_ctx* c) {
   if (c->d_path_off) cudaFree(c->d_path_off);
   if (c->d_seg_style) cudaFree(c->d_seg_style);
   if (c->d_seg_base) cudaFree(c->d_seg_base);
+  free_log(c);
   if (c->hs_action) cudaFree(c->hs_action);
   if (c->hs_ego_pinned) cudaFreeHost(c->hs_ego_pinned);
   if (c->hs_out) cudaFree(c->hs_out);
@@ -1942,6 +2050,9 @@ int t2d_set_type_table(t2d_ctx* c, const t2d_type_params* table, int n_types) {
   if (!c || !table) return fail(T2D_E_INVALID, "ctx/table is NULL");
   if (n_types <= 0 || n_types > T2D_MAX_TYPES) return fail(T2D_E_INVALID, "n_types must be in 1..64");
   static_assert(sizeof(t2d_type_params) == sizeof(AbiParams), "type table layout");
+  for (uint8_t row : c->log_track_type)   // a bound log's tracks must stay static rows (K1 would integrate on the log)
+    if (row >= n_types || table[row].model != T2D_MODEL_STATIC)
+      return fail(T2D_E_INVALID, "type table: row " + std::to_string(row) + " of a replayed track must exist and be T2D_MODEL_STATIC");
   c->has_pointmass = false;
   bool has_drift = false;
   float rb_max = 0.0f;
@@ -1985,6 +2096,8 @@ int t2d_set_type_table(t2d_ctx* c, const t2d_type_params* table, int n_types) {
     CUDA_TRY(cudaMemcpy(c->d_table, rows.data(), (n_types + 1) * sizeof(Params), cudaMemcpyHostToDevice));
   }
   c->n_types = n_types;
+  c->type_model.resize(n_types);
+  for (int i = 0; i < n_types; ++i) c->type_model[i] = table[i].model;
   c->has_drift = has_drift;
   c->rb_max = rb_max;
   c->kin_only = true;
@@ -2265,6 +2378,89 @@ int t2d_bind_reset_wheel_pool(t2d_ctx* c, const float* pool_omega_front, const f
   return T2D_OK;
 }
 
+int t2d_set_log(t2d_ctx* c, const t2d_log* L) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!L) {
+    CUDA_TRY(cudaSetDevice(c->device));
+    free_log(c);
+    return T2D_OK;
+  }
+  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (L->n_tracks <= 0 || L->n_rows <= 0) return fail(T2D_E_INVALID, "t2d_set_log: n_tracks and n_rows must be >= 1");
+  if (!L->first_ms || !L->n_frames || !L->period_ms || !L->type_row || !L->records || !L->t0_ms || !L->row_track || !L->log_row ||
+      !L->type_id)
+    return fail(T2D_E_INVALID, "t2d_set_log: NULL array");
+  if (L->type_id != c->type_id)
+    return fail(T2D_E_INVALID, "t2d_set_log: type_id is not the array bound with t2d_bind_state");
+  const int K = L->n_tracks, M = c->M;
+  std::vector<ReplayTrack> tracks((size_t)K);
+  long long n_rec = 0;
+  for (int k = 0; k < K; ++k) {
+    if (L->period_ms[k] <= 0) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": period_ms must be > 0");
+    if (L->n_frames[k] < 1) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": no frames");
+    const int row = L->type_row[k];
+    if (row >= c->n_types) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": type_row outside the type table");
+    if (c->type_model[row] != T2D_MODEL_STATIC)
+      return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": type_row is not a T2D_MODEL_STATIC row");
+    tracks[k] = ReplayTrack{L->first_ms[k], L->period_ms[k], L->n_frames[k], (int32_t)n_rec};
+    n_rec += L->n_frames[k];
+    if (n_rec > INT32_MAX / 5) return fail(T2D_E_UNSUPPORTED, "t2d_set_log: too many records");
+  }
+  for (long long i = 0; i < 5 * n_rec; ++i)
+    if (!std::isfinite(L->records[i])) return fail(T2D_E_INVALID, "t2d_set_log: record " + std::to_string(i / 5) + " is not finite");
+  std::vector<int> seen((size_t)K, -1);
+  for (int p = 0; p < L->n_rows; ++p)
+    for (int m = 0; m < M; ++m) {
+      const int k = L->row_track[(size_t)p * M + m];
+      if (k < -1 || k >= K) return fail(T2D_E_INVALID, "t2d_set_log: row_track entry outside [-1, n_tracks)");
+      if (k < 0) continue;
+      if (seen[k] == p) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + " bound twice in row " + std::to_string(p));
+      seen[k] = p;
+    }
+  CUDA_TRY(cudaSetDevice(c->device));
+  free_log(c);
+  CUDA_TRY(cudaMalloc(&c->d_log_tracks, sizeof(ReplayTrack) * (size_t)K));
+  CUDA_TRY(cudaMalloc(&c->d_log_track_type, (size_t)K));
+  CUDA_TRY(cudaMalloc(&c->d_log_rec, sizeof(float) * 5 * (size_t)n_rec));
+  CUDA_TRY(cudaMalloc(&c->d_log_t0, sizeof(int32_t) * (size_t)L->n_rows));
+  CUDA_TRY(cudaMalloc(&c->d_log_row_track, sizeof(int32_t) * (size_t)L->n_rows * M));
+  CUDA_TRY(cudaMemcpy(c->d_log_tracks, tracks.data(), sizeof(ReplayTrack) * (size_t)K, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(c->d_log_track_type, L->type_row, (size_t)K, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(c->d_log_rec, L->records, sizeof(float) * 5 * (size_t)n_rec, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(c->d_log_t0, L->t0_ms, sizeof(int32_t) * (size_t)L->n_rows, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(c->d_log_row_track, L->row_track, sizeof(int32_t) * (size_t)L->n_rows * M, cudaMemcpyHostToDevice));
+  c->log_track_type.assign(L->type_row, L->type_row + K);
+  c->log_tracks = K; c->log_rows = L->n_rows;
+  c->log_row = L->log_row; c->log_type_id = L->type_id;
+  c->has_log = true;
+  return T2D_OK;
+}
+
+// K7 over the scenarios [first, first + count): tick mode (mask == nullptr, offset 1) or reset mode (the masked scenarios
+// take row pool_index[n] / n, offset 0).
+static int launch_replay(t2d_ctx* c, void* stream, int first, int count, int offset, const uint8_t* mask, const int32_t* pool_index) {
+  if (c->log_type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+  const size_t p0 = (size_t)first * c->M;
+  ReplayArgs R{};
+  R.x = c->x + p0; R.y = c->y + p0; R.h = c->h + p0; R.v = c->v + p0; R.vx = c->vx + p0; R.vy = c->vy + p0;
+  R.type_id = c->log_type_id + p0;
+  R.step_count = c->step_count + first;
+  R.log_row = c->log_row + first;
+  R.mask = mask ? mask + first : nullptr;
+  R.pool_index = pool_index ? pool_index + first : nullptr;
+  R.log_row_out = mask ? c->log_row + first : nullptr;
+  R.tracks = c->d_log_tracks; R.track_type = c->d_log_track_type; R.rec = c->d_log_rec;
+  R.t0 = c->d_log_t0; R.row_track = c->d_log_row_track;
+  R.N = count; R.M = c->M; R.n_rows = c->log_rows; R.offset = offset; R.interval_ms = c->cfg.interval_ms;
+  const long long total = (long long)count * c->M;
+  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)c->sm_count * 8);
+  t2d_replay_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(R);
+  g_launches.fetch_add(1);
+  CUDA_TRY(cudaGetLastError());
+  return T2D_OK;
+}
+
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // Warps per CTA of the tick.  One wave (the usual case: every warp tile is resident at once and the kernel's duration is
@@ -2298,6 +2494,8 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
   if (do_physics && !action) return fail(T2D_E_INVALID, "action is NULL");
   if (do_physics && c->has_drift && !(c->wheel_f && c->wheel_r))
     return fail(T2D_E_STATE, "the type table holds a SingleTrackDrift row: call t2d_bind_wheel_state first");
+  if (do_physics && c->has_log && c->log_type_id != c->type_id)
+    return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
   CUDA_TRY(cudaSetDevice(c->device));
   if (count < 0) count = c->N - first;
   if (first < 0 || count <= 0 || first + count > c->N) return fail(T2D_E_INVALID, "scenario range out of bounds");
@@ -2325,7 +2523,8 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
   A.do_physics = do_physics; A.has_bounds = c->has_bounds ? 1 : 0;
   A.bxmin = c->bounds[0]; A.bxmax = c->bounds[1]; A.bymin = c->bounds[2]; A.bymax = c->bounds[3];
   A.prefetch = c->prefetch_override >= 0 ? c->prefetch_override : (g_exchanges_alive.load() == 0 ? 1 : 0);
-  A.needs_vel_in = (c->has_pointmass || c->has_drift) ? 1 : 0;   // (drift: K1 passes the pre-pass's vx, vy through)
+  // (drift / replay: K1 passes the pre-pass's vx, vy through)
+  A.needs_vel_in = (c->has_pointmass || c->has_drift || (do_physics && c->has_log)) ? 1 : 0;
   bool vec = (c->M % PPL == 0) && aligned16(A.x) && aligned16(A.y) && aligned16(A.h) && aligned16(A.v) && aligned16(A.vx) &&
              aligned16(A.vy) && (reinterpret_cast<uintptr_t>(A.type_id) % 4 == 0) && (!action || aligned16(action)) &&
              (!flags || reinterpret_cast<uintptr_t>(flags) % 4 == 0) && (!hit_index || reinterpret_cast<uintptr_t>(hit_index) % 8 == 0) &&
@@ -2379,6 +2578,8 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
       configured = smem;
     }
   }
+  if (do_physics && c->has_log)
+    if (int r = launch_replay(c, stream, first, count, 1, nullptr, nullptr)) return r;
   if (do_physics && c->has_drift) {
     const long long total = (long long)count * c->M;
     const int dgrid = (int)std::min<long long>((total + 127) / 128, (long long)c->sm_count * 16);
@@ -2567,6 +2768,8 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
   if (!mask || !pool_x || !pool_y || !pool_heading || !pool_speed) return fail(T2D_E_INVALID, "t2d_reset: NULL array");
   if (n_pool <= 0) return fail(T2D_E_INVALID, "n_pool must be > 0");
+  if (c->has_log && n_pool != c->log_rows) return fail(T2D_E_INVALID, "t2d_reset: with a log bound, pool row p is episode row p (n_pool == n_rows)");
+  if (c->has_log && c->log_type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
   CUDA_TRY(cudaSetDevice(c->device));
   ResetArgs A{};
   A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy; A.step_count = c->step_count;
@@ -2581,6 +2784,7 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   t2d_reset_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(A);
   g_launches.fetch_add(1);
   CUDA_TRY(cudaGetLastError());
+  if (c->has_log) return launch_replay(c, stream, 0, c->N, 0, mask, pool_index);   // the new episode's traffic at t0
   return T2D_OK;
 }
 

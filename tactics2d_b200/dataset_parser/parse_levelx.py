@@ -137,6 +137,21 @@ class LevelXParser:
         return participants, actual
 
 
+def template_row(rows, cls, length: float, width: float) -> int:
+    """The type-table row of a LevelX road user: among the rows of its class (vehicle, cyclist = lf == lr and narrow,
+    pedestrian = disc), the one nearest to its logged length and width."""
+    kind = {Vehicle: 0, Cyclist: 1, Pedestrian: 2}[cls]
+    best, score = 0, np.inf
+    for i, r in enumerate(rows):
+        r_kind = 2 if r.shape == 1 else (1 if abs(r.lf - r.lr) < 1e-9 and r.half_wid < 0.6 else 0)
+        if r_kind != kind:
+            continue
+        s = abs(2 * (r.radius if r.shape == 1 else r.half_len) - length) + abs(2 * (r.radius if r.shape == 1 else r.half_wid) - width)
+        if s < score:
+            best, score = i, s
+    return best
+
+
 def initial_state_pool(parser: LevelXParser, file, folder: str, m_participants: int, stamps, type_table=None, ids=None):
     """Rows of initial states for ``BatchedWorld.reset``: row p holds the up-to-``m_participants`` road users present in the
     log at time ``stamps[p]`` (ms; lowest track ids first), the rest of the row is empty slots (type 255).
@@ -154,19 +169,7 @@ def initial_state_pool(parser: LevelXParser, file, folder: str, m_participants: 
     cls_of = {int(r[parser.id_key]): (parser._CLASS_MAPPING[r["class"]], float(r[parser.key_length]), float(r[parser.key_width]))
               for _, r in meta.iterrows()}
 
-    def row_for(cls, length, width):
-        kind = {Vehicle: 0, Cyclist: 1, Pedestrian: 2}[cls]
-        best, score = 0, np.inf
-        for i, r in enumerate(rows):
-            r_kind = 2 if r.shape == 1 else (1 if abs(r.lf - r.lr) < 1e-9 and r.half_wid < 0.6 else 0)
-            if r_kind != kind:
-                continue
-            s = abs(2 * (r.radius if r.shape == 1 else r.half_len) - length) + abs(2 * (r.radius if r.shape == 1 else r.half_wid) - width)
-            if s < score:
-                best, score = i, s
-        return best
-
-    type_of = {k: row_for(*v) for k, v in cls_of.items()}
+    type_of = {k: template_row(rows, *v) for k, v in cls_of.items()}
     P, M = len(stamps), int(m_participants)
     pool = {k: np.zeros((P, M), np.float32) for k in ("x", "y", "heading", "speed", "vx", "vy")}
     tid = np.full((P, M), TYPE_INACTIVE, np.uint8)

@@ -47,8 +47,12 @@ class BatchedTrafficEnv:
     def __init__(self, scene, device="cuda:0", max_step: int = 1000, step_size: int = 100, delta_t: int = 5,
                  any_participant: bool = False, auto_reset: bool = True, target=None, arrival_threshold: float = 0.95,
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
-                 bev_range=(20.0, 20.0, 20.0, 20.0)):
+                 bev_range=(20.0, 20.0, 20.0, 20.0), replay=None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
+        ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
+        ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
+        initial states and the type table then come from it and only the map and bounds from ``scene`` (which may be None);
+        an auto-reset restarts the scenario's row, ``reset(options={"shuffle": True})`` deals the rows out anew;
         ``target``: optional [N, 5] target areas (cx, cy, heading, half_len, half_wid) for the egos - enables the
         ``Arrival`` (-> COMPLETED / ``terminated``) and ``NoAction`` detectors and the IoU reward terms of
         ``ParkingEnv._get_reward`` (parking.py:148-190); ``observation``: ``"state"`` (the state tensors) or ``"bev"``
@@ -62,6 +66,9 @@ class BatchedTrafficEnv:
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
+        self.replay = replay
+        if replay is not None:
+            scene = replay.scene() if scene is None else replay.scene(scene.segments, scene.bounds, scene.name)
         self.scene = scene
         n, m = scene.shape
         self.num_envs, self.num_participants = n, m
@@ -75,6 +82,8 @@ class BatchedTrafficEnv:
         self._pool = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dev) for k, v in scene.state().items()}
         self._type_id = torch.from_numpy(scene.type_id).to(dev)
         self.scenario_manager.set_initial_state(self._pool)
+        if replay is not None:
+            self.world.set_log(replay.log, replay.t0, replay.row_track)
         self._action = torch.zeros((n, m, 2), dtype=torch.float32, device=dev)
         self._rng = np.random.default_rng(0)
         if target is not None:
@@ -105,7 +114,10 @@ class BatchedTrafficEnv:
         perm = None
         if options and options.get("shuffle"):
             perm = torch.from_numpy(self._rng.permutation(self.num_envs).astype(np.int32)).to(self.world.device)
-        self.world.type_id.copy_(self._type_id)
+        if self.replay is not None and perm is not None:   # the rows' own types (the replayed slots' are rewritten anyway)
+            self.world.type_id.copy_(self._type_id[perm.long()])
+        else:
+            self.world.type_id.copy_(self._type_id)
         self.scenario_manager.reset(pool_index=perm)
         self.world.reset_env_trackers()
         status = torch.full((self.num_envs,), int(ScenarioStatus.NORMAL), dtype=torch.uint8, device=self.world.device)
@@ -146,7 +158,7 @@ class BatchedTrafficEnv:
         if r.iou is not None:
             info["iou"] = r.iou
         if self.auto_reset:
-            self.scenario_manager.reset(mask=e.done)
+            self.scenario_manager.reset(mask=e.done, pool_index=w.log_row)   # (a log: restart the scenario's row)
         return self._obs(), e.reward, e.terminated, e.truncated, info
 
     def render(self):

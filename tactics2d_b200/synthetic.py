@@ -168,3 +168,58 @@ def with_inactive(scene: Scene, fraction: float, seed: int = 0) -> Scene:
     tid[rng.uniform(0, 1, tid.shape) < fraction] = TYPE_INACTIVE
     return Scene(scene.table, scene.x, scene.y, scene.heading, scene.speed, scene.vx, scene.vy, tid, scene.segments,
                  scene.bounds, scene.name + f" ({fraction:.0%} inactive)", dict(scene.meta))
+
+
+def replay_episodes(n_rows: int, m: int, n_tracks: int, seed: int = 0, table: Optional[TypeTable] = None, size: float = 200.0,
+                    duration_ms: int = 60000, period_ms: int = 40, max_frames: int = 250, horizon_ms: int = 6000):
+    """A seeded synthetic recording for log replay (``tactics2d_b200.dataset_parser.ReplayEpisodes``): ``n_tracks`` vehicle
+    tracks of 1..``max_frames`` records every ``period_ms`` (a quarter of them starting off the period grid), wandering
+    headings that cross 0 / 2 pi, spread over ``duration_ms``; ``n_rows`` episode rows starting on a 20 ms grid, each with a
+    random kinematic ego in slot 0 and up to m - 1 of the tracks present in [t0, t0 + horizon_ms] in slots 1.. (random
+    picks, -1 when fewer overlap).  Every track's type row is the static twin of a random vehicle row of ``table``
+    (default: the 9 vehicle templates)."""
+    from .dataset_parser.replay import ReplayEpisodes, ReplayLog
+    from .participant.element import Vehicle
+
+    rng = np.random.default_rng(seed)
+    base = table if table is not None else TypeTable.vehicles("kinematics")
+    veh = [i for i, r in enumerate(base.rows) if r.model == 0 and r.shape == 0]
+    table, twin = base.with_static_twins(veh)
+    K = int(n_tracks)
+    nfr = rng.integers(1, max_frames + 1, K).astype(np.int32)
+    first = (rng.integers(-max_frames // 2, duration_ms // period_ms, K) * period_ms).astype(np.int64)
+    first += np.where(rng.uniform(0, 1, K) < 0.25, rng.integers(1, period_ms, K), 0)
+    cls_row = rng.choice(veh, K)
+    recs = []
+    for k in range(K):
+        n = int(nfr[k])
+        h = rng.uniform(0, 2 * np.pi) + np.cumsum(rng.normal(0, 0.08, n))
+        v = np.abs(rng.uniform(0, 20) + np.cumsum(rng.normal(0, 0.3, n)))
+        vx, vy = v * np.cos(h), v * np.sin(h)
+        x = rng.uniform(0, size) + np.cumsum(vx) * period_ms / 1000
+        y = rng.uniform(0, size) + np.cumsum(vy) * period_ms / 1000
+        recs.append(np.stack([x, y, np.mod(h, 2 * np.pi), vx, vy], 1).astype(np.float32))
+    rows = table.rows
+    log = ReplayLog(ids=np.arange(K, dtype=np.int64), first_ms=first.astype(np.int32), n_frames=nfr,
+                    period_ms=np.full(K, period_ms, np.int32), records=np.ascontiguousarray(np.concatenate(recs)),
+                    type_row=np.asarray([twin[int(r)] for r in cls_row], np.uint8), cls=[Vehicle] * K,
+                    length=np.asarray([2 * rows[r].half_len for r in cls_row]), width=np.asarray([2 * rows[r].half_wid for r in cls_row]))
+    P = int(n_rows)
+    t0 = (rng.integers(0, duration_ms // 20, P) * 20).astype(np.int32)
+    last = log.last_ms
+    row_track = np.full((P, m), -1, np.int32)
+    tid = np.full((P, m), TYPE_INACTIVE, np.uint8)
+    for p in range(P):
+        cand = np.nonzero((last >= t0[p]) & (first <= t0[p] + horizon_ms))[0]
+        pick = rng.choice(cand, min(len(cand), m - 1), replace=False)
+        row_track[p, 1:1 + len(pick)] = pick
+        on = (first[pick] <= t0[p]) & (last[pick] >= t0[p])
+        tid[p, 1:1 + len(pick)] = np.where(on, log.type_row[pick], TYPE_INACTIVE)
+    x, y, h, v, ego = _arena(rng, P, 1, size, None, 15.0, table, veh)
+    z = lambda: np.zeros((P, m))
+    px, py, ph, pv = z(), z(), z(), z()
+    px[:, 0], py[:, 0], ph[:, 0], pv[:, 0] = x[:, 0], y[:, 0], h[:, 0], v[:, 0]
+    tid[:, 0] = ego[:, 0]
+    sc = _finish(table, px, py, ph, pv, tid, None, None, "replay")
+    pool = sc.state()
+    return ReplayEpisodes(log, table, pool, tid, row_track, t0, np.zeros(P, np.int64))

@@ -150,6 +150,23 @@ class TypeTable:
                 return i
         raise KeyError(name)
 
+    def with_static_twins(self, rows: Iterable[int]):
+        """This table plus one ``MODEL_STATIC`` copy of each of ``rows`` (same shape, extents and name, so BEV styles and the
+        lidar treat it like its class): the rows replayed participants take (``BatchedWorld.set_log``).  Returns
+        ``(table, twin)`` with ``twin[row]`` the index of row's twin; a row that is static already is its own twin."""
+        from dataclasses import replace
+
+        out, twin = list(self.rows), {}
+        for r in sorted({int(v) for v in rows}):
+            if self.rows[r].model == MODEL_STATIC:
+                twin[r] = r
+                continue
+            twin[r] = len(out)
+            out.append(replace(self.rows[r], model=MODEL_STATIC))
+        if len(out) > MAX_TYPES:
+            raise ValueError(f"static twins of {len(twin)} rows do not fit a {MAX_TYPES}-row table ({len(out)} rows)")
+        return TypeTable(out), twin
+
     def to_c_array(self):
         arr = (TypeParamsC * len(self.rows))()
         for i, r in enumerate(self.rows):

@@ -284,6 +284,50 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_control(self._ctx, _ptr(action), self._stream()))
         return action
 
+    # ------------------------------------------------------------------ log replay
+    def set_log(self, log, t0=None, row_track=None):
+        """Replay recorded tracks in the slots bound to them (``t2d_set_log``; DESIGN.md section 1 "Log replay").  ``log``:
+        a :class:`tactics2d_b200.dataset_parser.ReplayLog` (or any object with ``first_ms, n_frames, period_ms, type_row``
+        [K] and ``records`` [F, 5]) whose type rows are static rows of this world's table, or None to unbind; ``t0`` [P]:
+        the start time (ms) of every episode row; ``row_track`` [P, M]: the track each slot of a row replays, -1 for none.
+        Before every tick, scenario n's replayed slots take their tracks' state at ``t0[log_row[n]] + (step + 1) *
+        interval``; ``reset`` sets ``log_row`` from its ``pool_index`` (pool row p = episode row p) and shows the new row's
+        traffic at once.  Replayed slots are checked like any participant; an env over a log keeps the default ego-only
+        status (``any_participant=False``)."""
+        if log is None:
+            _lib.check(self.lib.t2d_set_log(self._ctx, None))
+            self._log = None
+            return
+        i32 = lambda a: np.ascontiguousarray(np.asarray(a), dtype=np.int32)
+        keep = dict(first=i32(log.first_ms), n_frames=i32(log.n_frames), period=i32(log.period_ms),
+                    type_row=np.ascontiguousarray(np.asarray(log.type_row), dtype=np.uint8),
+                    records=np.ascontiguousarray(np.asarray(log.records), dtype=np.float32).reshape(-1, 5),
+                    t0=i32(t0).reshape(-1), row_track=i32(row_track))
+        n_rows = keep["t0"].shape[0]
+        if keep["row_track"].shape != (n_rows, self.M):
+            raise ValueError(f"row_track must be [{n_rows}, {self.M}] (one row per t0)")
+        k = keep["first"].shape[0]
+        if not (keep["n_frames"].shape == keep["period"].shape == keep["type_row"].shape == (k,)):
+            raise ValueError("first_ms, n_frames, period_ms and type_row need one entry per track")
+        if keep["records"].shape[0] != int(keep["n_frames"].astype(np.int64).sum()):
+            raise ValueError("records must hold sum(n_frames) rows")
+        log_row = torch.arange(self.N, dtype=torch.int32, device=self.device)
+        c = self._log_struct(keep, log_row, self.type_id)
+        _lib.check(self.lib.t2d_set_log(self._ctx, C.byref(c)))
+        self._log = dict(keep, log_row=log_row)
+
+    def _log_struct(self, keep, log_row, type_id):
+        p = lambda a: C.c_void_p(a.ctypes.data)
+        return _lib.LogC(keep["first"].shape[0], p(keep["first"]), p(keep["n_frames"]), p(keep["period"]), p(keep["type_row"]),
+                         p(keep["records"]), keep["t0"].shape[0], p(keep["t0"]), p(keep["row_track"]), _ptr(log_row), _ptr(type_id))
+
+    @property
+    def log_row(self) -> Optional[torch.Tensor]:
+        """int32 [N] device tensor: the episode row every scenario runs (None without a log).  ``reset`` writes it; it may
+        be rewritten between ticks."""
+        lg = getattr(self, "_log", None)
+        return None if lg is None else lg["log_row"]
+
     # ------------------------------------------------------------------ state
     def set_wheel_state(self, omega_front, omega_rear):
         """Wheel angular speeds [N, M] of the SingleTrackDrift participants (``omega_wf`` / ``omega_wr``)."""
