@@ -45,6 +45,7 @@
  *                                                         tactics2d/envs/parking.py:397-441, participant_base.py:236-246
  *   t2d_set_log          Trajectory.get_state / Vehicle.get_pose of logged participants at a frame
  *                                                         participant/trajectory/trajectory.py:97-113, vehicle.py:263-281
+ *   t2d_set_log_schedule the same, with several tracks replayed one after the other in a slot
  *
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types cross the ABI;
@@ -255,7 +256,7 @@ typedef struct t2d_log {
   const float* records;       /* HOST [sum n_frames][5] x, y, heading, vx, vy; finite */
   int32_t n_rows;             /* >= 1 */
   const int32_t* t0_ms;       /* HOST [n_rows] */
-  const int32_t* row_track;   /* HOST [n_rows][M] in [-1, n_tracks) */
+  const int32_t* row_track;   /* HOST [n_rows][M] in [-1, n_tracks); NULL for t2d_set_log_schedule */
   int32_t* log_row;           /* DEVICE [N], caller-owned: the row each scenario runs */
   uint8_t* type_id;           /* DEVICE [N][M]: the type_id array of t2d_bind_state - the replay writes it, so the
                                  writable pointer is passed here and must equal the bound one */
@@ -264,6 +265,19 @@ typedef struct t2d_log {
  * row, a type_id other than the bound one.  A later t2d_set_type_table that makes a track's row non-static is
  * rejected too. */
 int t2d_set_log(t2d_ctx* ctx, const t2d_log* log);
+/* Slot schedules (DESIGN.md section 1 "Log replay", "Slot schedules"): slot m of row p replays, one after the other,
+ * the tracks slot_track[slot_off[p * M + m] .. slot_off[p * M + m + 1]), whose presence intervals [first, last] must be
+ * strictly increasing and disjoint (last of an entry < first of the next).  At sample time t the slot shows the entry
+ * present at t, else T2D_TYPE_INACTIVE with its state untouched; t2d_set_log's row_track is the case of at most one
+ * entry per slot.  log->row_track must be NULL; every other field is checked as t2d_set_log checks it.
+ *   slot_off    HOST int32 [n_rows * M + 1], slot_off[0] == 0, monotone, slot_off[n_rows * M] == n_entries
+ *   slot_track  HOST int32 [n_entries] in [0, n_tracks); a track at most once per row, over all the row's slots;
+ *               every scheduled track's last stamp must fit int32 ms
+ *   track_out   optional caller-owned DEVICE int32 [N][M]: every replay launch (ticks, t2d_step_host chunks, t2d_reset)
+ *               writes the track each slot it samples shows, -1 while the slot shows none or is not replayed
+ * Host arrays are copied.  Rejected (the previous log stays bound): any malformed field. */
+int t2d_set_log_schedule(t2d_ctx* ctx, const t2d_log* log, const int32_t* slot_off, const int32_t* slot_track,
+                         int32_t n_entries, int32_t* track_out);
 
 /* Single-line lidar of the ego (participant 0) of every scenario: SingleLineLidar._scan_obstacles
  * (tactics2d/sensor/lidar.py:128-221).  n_beams = point_density (lidar.py:49), max_range = perception range;

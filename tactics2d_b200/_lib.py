@@ -93,6 +93,7 @@ SYMBOLS = {
     "t2d_bind_wheel_state": (C.c_int, [_P, _P, _P]),
     "t2d_bind_reset_wheel_pool": (C.c_int, [_P, _P, _P]),
     "t2d_set_log": (C.c_int, [_P, C.POINTER(LogC)]),
+    "t2d_set_log_schedule": (C.c_int, [_P, C.POINTER(LogC), _P, _P, C.c_int32, _P]),
     "t2d_set_prefetch": (C.c_int, [_P, C.c_int]),
     "t2d_launch_count": (C.c_int64, []),
 }

@@ -1312,10 +1312,16 @@ __global__ void __launch_bounds__(128) t2d_drift_kernel(const __grid_constant__ 
 // ---------------------------------------------------------------------------- K7
 // Log replay (t2d_set_log): every replayed slot takes its track's state at the time the next tick produces (or, in
 // reset mode, at the row's t0), before K1, which then only builds the pose of these static-model slots.  One thread
-// per (scenario, slot), consecutive threads on consecutive slots: the [N, M] row_track reads and the state / type_id
-// stores coalesce; the track entry and its two frame records are gathers.  Interpolation in fp64 with explicit
-// round-to-nearest operations (no FMA contraction), in the order oracle/replay.py states.
+// per (scenario, slot), consecutive threads on consecutive slots: the [N, M] slot offset reads and the state / type_id
+// stores coalesce; the schedule entries, the track entry and its two frame records are gathers.  A slot's schedule is
+// a run of entries with strictly increasing, disjoint presence intervals; the thread takes the first entry whose last
+// stamp is >= t (the slot's final entry if none is), so a schedule of L entries costs ceil(log2 L) dependent probes.
+// When no schedule of the log holds more than one entry (t2d_set_log's row_track, and any such schedule), the host
+// uploads the slots' tracks as one [n_rows][M] array instead and the offsets and the entry gather drop out of the
+// dependent chain.  Whether the chosen track is present at t is then decided exactly as for a single track.  Interpolation in fp64 with explicit round-to-nearest operations (no FMA
+// contraction), in the order oracle/replay.py states.
 struct ReplayTrack { int32_t first_ms, period_ms, n_frames, rec_off; };
+struct ReplayEntry { int32_t last_ms, track; };   // one 8-byte load per probe
 
 struct ReplayArgs {
   float *x, *y, *h, *v, *vx, *vy;
@@ -1329,7 +1335,11 @@ struct ReplayArgs {
   const uint8_t* track_type;       // [n_tracks]
   const float* rec;                // [sum n_frames][5] x, y, heading, vx, vy
   const int32_t* t0;               // [n_rows] ms
-  const int32_t* row_track;        // [n_rows][M], -1 = not replayed
+  const int32_t* slot_off;         // [n_rows * M + 1] schedule of (row, m): entries [slot_off[row M + m], slot_off[row M + m + 1])
+  const ReplayEntry* entries;      // [E]
+  const int32_t* slot_track1;      // when no schedule has more than one entry: [n_rows * M] its track, -1 for none
+                                   // (slot_off / entries then unused); nullptr otherwise
+  int32_t* track_out;              // [N][M] the track each slot shows, -1 for none; nullptr: not written
   int N, M, n_rows, offset, interval_ms;
 };
 
@@ -1351,16 +1361,39 @@ __global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__
     } else {
       row = min(max(A.log_row[n], 0), A.n_rows - 1);
     }
-    const int k = A.row_track[(long long)row * A.M + m];
-    if (k < 0) continue;
+    const long long s = (long long)row * A.M + m;
+    int k;
+    long long t;
+    if (A.slot_track1 != nullptr) {   // at most one entry per slot: the track itself, no offsets
+      k = __ldg(A.slot_track1 + s);
+      if (k < 0) {
+        if (A.track_out) A.track_out[i] = -1;
+        continue;
+      }
+      t = (long long)A.t0[row] + ((long long)A.step_count[n] + A.offset) * A.interval_ms;
+    } else {
+      int lo = __ldg(A.slot_off + s), hi = __ldg(A.slot_off + s + 1) - 1;
+      if (hi < lo) {   // an empty schedule: the slot is not replayed
+        if (A.track_out) A.track_out[i] = -1;
+        continue;
+      }
+      t = (long long)A.t0[row] + ((long long)A.step_count[n] + A.offset) * A.interval_ms;
+      while (lo < hi) {   // the first entry with last_ms >= t; the final one stands for "after every entry"
+        const int mid = (lo + hi) >> 1;
+        if ((long long)__ldg(&A.entries[mid].last_ms) >= t) hi = mid;
+        else lo = mid + 1;
+      }
+      k = __ldg(&A.entries[lo].track);
+    }
     const int4 tr4 = __ldg(reinterpret_cast<const int4*>(A.tracks) + k);
     const int first = tr4.x, period = tr4.y, n_frames = tr4.z, rec_off = tr4.w;
-    const long long t = (long long)A.t0[row] + ((long long)A.step_count[n] + A.offset) * A.interval_ms;
     const long long d = t - first;
     if (d < 0 || d > (long long)(n_frames - 1) * period) {   // the track is not in the scene at t
       A.type_id[i] = T2D_TYPE_INACTIVE;
+      if (A.track_out) A.track_out[i] = -1;
       continue;
     }
+    if (A.track_out) A.track_out[i] = k;
     const long long j = d / period;
     const int r = (int)(d - j * period);
     const float* a = A.rec + 5 * ((long long)rec_off + j);
@@ -1948,8 +1981,11 @@ struct t2d_ctx {
   uint8_t* d_log_track_type = nullptr;
   float* d_log_rec = nullptr;
   int32_t* d_log_t0 = nullptr;
-  int32_t* d_log_row_track = nullptr;
+  int32_t* d_log_slot_off = nullptr;   // [n_rows * M + 1] schedule offsets
+  ReplayEntry* d_log_entries = nullptr;
+  int32_t* d_log_slot_track1 = nullptr; // [n_rows * M] instead of the two above when no schedule has two entries
   int32_t* log_row = nullptr;          // caller-owned DEVICE [N]
+  int32_t* log_track_out = nullptr;    // caller-owned DEVICE [N][M] or nullptr
   uint8_t* log_type_id = nullptr;      // writable alias of type_id, checked against the bound one before every launch
   std::vector<uint8_t> log_track_type; // host copy: t2d_set_type_table keeps these rows static
   std::vector<int> type_model;         // host copy of the current type table's model ids
@@ -2008,10 +2044,13 @@ static void free_log(t2d_ctx* c) {
   if (c->d_log_track_type) cudaFree(c->d_log_track_type);
   if (c->d_log_rec) cudaFree(c->d_log_rec);
   if (c->d_log_t0) cudaFree(c->d_log_t0);
-  if (c->d_log_row_track) cudaFree(c->d_log_row_track);
+  if (c->d_log_slot_off) cudaFree(c->d_log_slot_off);
+  if (c->d_log_entries) cudaFree(c->d_log_entries);
+  if (c->d_log_slot_track1) cudaFree(c->d_log_slot_track1);
   c->d_log_tracks = nullptr; c->d_log_track_type = nullptr; c->d_log_rec = nullptr; c->d_log_t0 = nullptr;
-  c->d_log_row_track = nullptr;
+  c->d_log_slot_off = nullptr; c->d_log_entries = nullptr; c->d_log_slot_track1 = nullptr;
   c->has_log = false; c->log_tracks = c->log_rows = 0; c->log_row = nullptr; c->log_type_id = nullptr;
+  c->log_track_out = nullptr;
   c->log_track_type.clear();
 }
 
@@ -2378,6 +2417,116 @@ int t2d_bind_reset_wheel_pool(t2d_ctx* c, const float* pool_omega_front, const f
   return T2D_OK;
 }
 
+// t2d_set_log (row_track, slot_off == nullptr) and t2d_set_log_schedule: validate everything, then replace the bound log.
+// A row_track binding becomes a schedule of at most one entry per slot.
+static int set_log(t2d_ctx* c, const t2d_log* L, const char* who, const int32_t* slot_off, const int32_t* slot_track,
+                   int n_entries, int32_t* track_out) {
+  const std::string fn = who;
+  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (L->n_tracks <= 0 || L->n_rows <= 0) return fail(T2D_E_INVALID, fn + ": n_tracks and n_rows must be >= 1");
+  if (!L->first_ms || !L->n_frames || !L->period_ms || !L->type_row || !L->records || !L->t0_ms || !L->log_row || !L->type_id)
+    return fail(T2D_E_INVALID, fn + ": NULL array");
+  if (slot_off == nullptr && !L->row_track) return fail(T2D_E_INVALID, fn + ": NULL array");
+  if (slot_off != nullptr && L->row_track) return fail(T2D_E_INVALID, fn + ": row_track must be NULL (the schedule binds the slots)");
+  if (L->type_id != c->type_id)
+    return fail(T2D_E_INVALID, fn + ": type_id is not the array bound with t2d_bind_state");
+  const int K = L->n_tracks, M = c->M;
+  const long long PM = (long long)L->n_rows * M;
+  std::vector<ReplayTrack> tracks((size_t)K);
+  std::vector<long long> last((size_t)K);
+  long long n_rec = 0;
+  for (int k = 0; k < K; ++k) {
+    if (L->period_ms[k] <= 0) return fail(T2D_E_INVALID, fn + ": track " + std::to_string(k) + ": period_ms must be > 0");
+    if (L->n_frames[k] < 1) return fail(T2D_E_INVALID, fn + ": track " + std::to_string(k) + ": no frames");
+    const int row = L->type_row[k];
+    if (row >= c->n_types) return fail(T2D_E_INVALID, fn + ": track " + std::to_string(k) + ": type_row outside the type table");
+    if (c->type_model[row] != T2D_MODEL_STATIC)
+      return fail(T2D_E_INVALID, fn + ": track " + std::to_string(k) + ": type_row is not a T2D_MODEL_STATIC row");
+    tracks[k] = ReplayTrack{L->first_ms[k], L->period_ms[k], L->n_frames[k], (int32_t)n_rec};
+    last[k] = (long long)L->first_ms[k] + (long long)(L->n_frames[k] - 1) * L->period_ms[k];
+    n_rec += L->n_frames[k];
+    if (n_rec > INT32_MAX / 5) return fail(T2D_E_UNSUPPORTED, fn + ": too many records");
+  }
+  for (long long i = 0; i < 5 * n_rec; ++i)
+    if (!std::isfinite(L->records[i])) return fail(T2D_E_INVALID, fn + ": record " + std::to_string(i / 5) + " is not finite");
+  std::vector<int32_t> off((size_t)PM + 1, 0);
+  std::vector<ReplayEntry> entries;
+  std::vector<int> seen((size_t)K, -1);
+  if (slot_off == nullptr) {
+    for (int p = 0; p < L->n_rows; ++p)
+      for (int m = 0; m < M; ++m) {
+        const long long s = (long long)p * M + m;
+        const int k = L->row_track[s];
+        if (k < -1 || k >= K) return fail(T2D_E_INVALID, fn + ": row_track entry outside [-1, n_tracks)");
+        if (k >= 0) {
+          if (seen[k] == p) return fail(T2D_E_INVALID, fn + ": track " + std::to_string(k) + " bound twice in row " + std::to_string(p));
+          seen[k] = p;
+          // a slot's final entry is never probed: its last stamp only has to be an int32, not exact
+          entries.push_back(ReplayEntry{(int32_t)std::min<long long>(last[k], INT32_MAX), k});
+        }
+        off[s + 1] = (int32_t)entries.size();
+      }
+  } else {
+    if (!slot_track && n_entries > 0) return fail(T2D_E_INVALID, fn + ": NULL array");
+    if (n_entries < 0) return fail(T2D_E_INVALID, fn + ": n_entries must be >= 0");
+    if (slot_off[0] != 0 || slot_off[PM] != n_entries)
+      return fail(T2D_E_INVALID, fn + ": slot_off must run from 0 to n_entries");
+    for (long long s = 0; s < PM; ++s)
+      if (slot_off[s + 1] < slot_off[s]) return fail(T2D_E_INVALID, fn + ": slot_off is not monotone at slot " + std::to_string(s));
+    entries.resize((size_t)n_entries);
+    for (int p = 0; p < L->n_rows; ++p)
+      for (int m = 0; m < M; ++m) {
+        const long long s = (long long)p * M + m;
+        for (int e = slot_off[s]; e < slot_off[s + 1]; ++e) {
+          const int k = slot_track[e];
+          const std::string at = fn + ": row " + std::to_string(p) + " slot " + std::to_string(m) + ": ";
+          if (k < 0 || k >= K) return fail(T2D_E_INVALID, at + "slot_track entry outside [0, n_tracks)");
+          if (seen[k] == p) return fail(T2D_E_INVALID, at + "track " + std::to_string(k) + " scheduled twice in the row");
+          seen[k] = p;
+          if (e > slot_off[s] && (long long)L->first_ms[k] <= last[slot_track[e - 1]])
+            return fail(T2D_E_INVALID, at + "track " + std::to_string(k) + " does not start after the previous entry ends");
+          if (last[k] > INT32_MAX) return fail(T2D_E_UNSUPPORTED, at + "track " + std::to_string(k) + ": last stamp exceeds int32 ms");
+          entries[e] = ReplayEntry{(int32_t)last[k], k};
+        }
+      }
+    std::copy(slot_off, slot_off + PM + 1, off.begin());
+  }
+  // at most one entry per slot (every row_track binding): the slots' tracks as one array, no search
+  std::vector<int32_t> one;
+  bool single = true;
+  for (long long s = 0; s < PM && single; ++s) single = off[s + 1] - off[s] <= 1;
+  if (single) {
+    one.assign((size_t)PM, -1);
+    for (long long s = 0; s < PM; ++s)
+      if (off[s + 1] > off[s]) one[s] = entries[off[s]].track;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  free_log(c);
+  CUDA_TRY(cudaMalloc(&c->d_log_tracks, sizeof(ReplayTrack) * (size_t)K));
+  CUDA_TRY(cudaMalloc(&c->d_log_track_type, (size_t)K));
+  CUDA_TRY(cudaMalloc(&c->d_log_rec, sizeof(float) * 5 * (size_t)n_rec));
+  CUDA_TRY(cudaMalloc(&c->d_log_t0, sizeof(int32_t) * (size_t)L->n_rows));
+  if (single) {
+    CUDA_TRY(cudaMalloc(&c->d_log_slot_track1, sizeof(int32_t) * one.size()));
+    CUDA_TRY(cudaMemcpy(c->d_log_slot_track1, one.data(), sizeof(int32_t) * one.size(), cudaMemcpyHostToDevice));
+  } else {
+    CUDA_TRY(cudaMalloc(&c->d_log_slot_off, sizeof(int32_t) * off.size()));
+    CUDA_TRY(cudaMalloc(&c->d_log_entries, sizeof(ReplayEntry) * entries.size()));
+    CUDA_TRY(cudaMemcpy(c->d_log_slot_off, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(c->d_log_entries, entries.data(), sizeof(ReplayEntry) * entries.size(), cudaMemcpyHostToDevice));
+  }
+  CUDA_TRY(cudaMemcpy(c->d_log_tracks, tracks.data(), sizeof(ReplayTrack) * (size_t)K, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(c->d_log_track_type, L->type_row, (size_t)K, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(c->d_log_rec, L->records, sizeof(float) * 5 * (size_t)n_rec, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(c->d_log_t0, L->t0_ms, sizeof(int32_t) * (size_t)L->n_rows, cudaMemcpyHostToDevice));
+  c->log_track_type.assign(L->type_row, L->type_row + K);
+  c->log_tracks = K; c->log_rows = L->n_rows;
+  c->log_row = L->log_row; c->log_type_id = L->type_id; c->log_track_out = track_out;
+  c->has_log = true;
+  return T2D_OK;
+}
+
 int t2d_set_log(t2d_ctx* c, const t2d_log* L) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (!L) {
@@ -2385,56 +2534,14 @@ int t2d_set_log(t2d_ctx* c, const t2d_log* L) {
     free_log(c);
     return T2D_OK;
   }
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
-  if (L->n_tracks <= 0 || L->n_rows <= 0) return fail(T2D_E_INVALID, "t2d_set_log: n_tracks and n_rows must be >= 1");
-  if (!L->first_ms || !L->n_frames || !L->period_ms || !L->type_row || !L->records || !L->t0_ms || !L->row_track || !L->log_row ||
-      !L->type_id)
-    return fail(T2D_E_INVALID, "t2d_set_log: NULL array");
-  if (L->type_id != c->type_id)
-    return fail(T2D_E_INVALID, "t2d_set_log: type_id is not the array bound with t2d_bind_state");
-  const int K = L->n_tracks, M = c->M;
-  std::vector<ReplayTrack> tracks((size_t)K);
-  long long n_rec = 0;
-  for (int k = 0; k < K; ++k) {
-    if (L->period_ms[k] <= 0) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": period_ms must be > 0");
-    if (L->n_frames[k] < 1) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": no frames");
-    const int row = L->type_row[k];
-    if (row >= c->n_types) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": type_row outside the type table");
-    if (c->type_model[row] != T2D_MODEL_STATIC)
-      return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + ": type_row is not a T2D_MODEL_STATIC row");
-    tracks[k] = ReplayTrack{L->first_ms[k], L->period_ms[k], L->n_frames[k], (int32_t)n_rec};
-    n_rec += L->n_frames[k];
-    if (n_rec > INT32_MAX / 5) return fail(T2D_E_UNSUPPORTED, "t2d_set_log: too many records");
-  }
-  for (long long i = 0; i < 5 * n_rec; ++i)
-    if (!std::isfinite(L->records[i])) return fail(T2D_E_INVALID, "t2d_set_log: record " + std::to_string(i / 5) + " is not finite");
-  std::vector<int> seen((size_t)K, -1);
-  for (int p = 0; p < L->n_rows; ++p)
-    for (int m = 0; m < M; ++m) {
-      const int k = L->row_track[(size_t)p * M + m];
-      if (k < -1 || k >= K) return fail(T2D_E_INVALID, "t2d_set_log: row_track entry outside [-1, n_tracks)");
-      if (k < 0) continue;
-      if (seen[k] == p) return fail(T2D_E_INVALID, "t2d_set_log: track " + std::to_string(k) + " bound twice in row " + std::to_string(p));
-      seen[k] = p;
-    }
-  CUDA_TRY(cudaSetDevice(c->device));
-  free_log(c);
-  CUDA_TRY(cudaMalloc(&c->d_log_tracks, sizeof(ReplayTrack) * (size_t)K));
-  CUDA_TRY(cudaMalloc(&c->d_log_track_type, (size_t)K));
-  CUDA_TRY(cudaMalloc(&c->d_log_rec, sizeof(float) * 5 * (size_t)n_rec));
-  CUDA_TRY(cudaMalloc(&c->d_log_t0, sizeof(int32_t) * (size_t)L->n_rows));
-  CUDA_TRY(cudaMalloc(&c->d_log_row_track, sizeof(int32_t) * (size_t)L->n_rows * M));
-  CUDA_TRY(cudaMemcpy(c->d_log_tracks, tracks.data(), sizeof(ReplayTrack) * (size_t)K, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(c->d_log_track_type, L->type_row, (size_t)K, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(c->d_log_rec, L->records, sizeof(float) * 5 * (size_t)n_rec, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(c->d_log_t0, L->t0_ms, sizeof(int32_t) * (size_t)L->n_rows, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(c->d_log_row_track, L->row_track, sizeof(int32_t) * (size_t)L->n_rows * M, cudaMemcpyHostToDevice));
-  c->log_track_type.assign(L->type_row, L->type_row + K);
-  c->log_tracks = K; c->log_rows = L->n_rows;
-  c->log_row = L->log_row; c->log_type_id = L->type_id;
-  c->has_log = true;
-  return T2D_OK;
+  return set_log(c, L, "t2d_set_log", nullptr, nullptr, 0, nullptr);
+}
+
+int t2d_set_log_schedule(t2d_ctx* c, const t2d_log* L, const int32_t* slot_off, const int32_t* slot_track, int32_t n_entries,
+                         int32_t* track_out) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!L || !slot_off) return fail(T2D_E_INVALID, "t2d_set_log_schedule: log / slot_off is NULL (t2d_set_log(ctx, NULL) unbinds)");
+  return set_log(c, L, "t2d_set_log_schedule", slot_off, slot_track, n_entries, track_out);
 }
 
 // K7 over the scenarios [first, first + count): tick mode (mask == nullptr, offset 1) or reset mode (the masked scenarios
@@ -2451,7 +2558,8 @@ static int launch_replay(t2d_ctx* c, void* stream, int first, int count, int off
   R.pool_index = pool_index ? pool_index + first : nullptr;
   R.log_row_out = mask ? c->log_row + first : nullptr;
   R.tracks = c->d_log_tracks; R.track_type = c->d_log_track_type; R.rec = c->d_log_rec;
-  R.t0 = c->d_log_t0; R.row_track = c->d_log_row_track;
+  R.t0 = c->d_log_t0; R.slot_off = c->d_log_slot_off; R.entries = c->d_log_entries; R.slot_track1 = c->d_log_slot_track1;
+  R.track_out = c->log_track_out ? c->log_track_out + p0 : nullptr;
   R.N = count; R.M = c->M; R.n_rows = c->log_rows; R.offset = offset; R.interval_ms = c->cfg.interval_ms;
   const long long total = (long long)count * c->M;
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)c->sm_count * 8);

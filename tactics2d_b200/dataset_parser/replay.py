@@ -8,7 +8,7 @@ The contract is DESIGN.md section 1 "Log replay"."""
 from __future__ import annotations
 
 from dataclasses import dataclass, replace
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -96,15 +96,22 @@ class ReplayEpisodes:
     ``BatchedTrafficEnv(..., replay=episodes)``): row p starts at ``t0[p]``; ``pool`` / ``type_id`` [P, M] are the initial
     states (slot 0 the ego's logged state at t0, bit for bit, with its class's kinematic row; the replayed slots are
     written by the replay at the reset itself), ``row_track`` [P, M] binds slots to tracks (-1: not replayed),
-    ``dropped[p]``: tracks of row p's window that did not fit its M - 1 slots."""
+    ``dropped[p]``: tracks of row p's window that did not fit its M - 1 slots.  Episodes built with slot reuse bind their
+    slots with ``schedule = (slot_off [P * M + 1], slot_track [E])`` instead (``BatchedWorld.set_log``) and have no
+    ``row_track``."""
 
     log: ReplayLog
     table: TypeTable
     pool: dict
     type_id: np.ndarray
-    row_track: np.ndarray
+    row_track: Optional[np.ndarray]
     t0: np.ndarray
     dropped: np.ndarray
+    schedule: Optional[Tuple[np.ndarray, np.ndarray]] = None
+
+    def binding(self) -> dict:
+        """The slot binding as ``BatchedWorld.set_log`` keywords: ``row_track=`` or ``schedule=``."""
+        return dict(row_track=self.row_track) if self.schedule is None else dict(schedule=self.schedule)
 
     def scene(self, segments=None, bounds=None, name: str = "replay"):
         """A :class:`tactics2d_b200.synthetic.Scene` of the P rows (one scenario per row) on the given map."""
@@ -122,12 +129,19 @@ def _speed(vx, vy):
 
 
 def build_replay_episodes(log: ReplayLog, m_participants: int, t0s: Sequence[int], ego_tracks: Sequence[int],
-                          type_table: Optional[TypeTable] = None, horizon_ms: Optional[int] = None) -> ReplayEpisodes:
+                          type_table: Optional[TypeTable] = None, horizon_ms: Optional[int] = None,
+                          reuse_slots: bool = False) -> ReplayEpisodes:
     """Row p: the ego is track ``ego_tracks[p]`` (a track id), simulated from its record at ``t0s[p]`` (which must be one of
     its frames); slots 1..M-1 replay the other tracks present somewhere in the window [t0, t0 + horizon_ms] (to the end
     of the log without a horizon), ordered by (first time stamp, id); the ego's own track is never replayed.
     ``type_table`` (default ``TypeTable.from_templates("kinematics")``) gets one static twin per class row the log uses
-    (``TypeTable.with_static_twins``): every track's ``type_row`` is the twin of its class row."""
+    (``TypeTable.with_static_twins``): every track's ``type_row`` is the twin of its class row.
+
+    ``reuse_slots``: instead of one track per slot, each slot gets a schedule (``ReplayEpisodes.schedule``): in that same
+    order, every track goes to the lowest slot in 1..M-1 whose last track ends strictly before the track's first stamp
+    (greedy interval partitioning, so a row uses exactly as many slots as the most tracks of its window present at one
+    time), and ``dropped[p]`` counts the tracks that found no such slot.  A slot's initial type is that of its track
+    present at t0 (255 if none)."""
     table = type_table if type_table is not None else TypeTable.from_templates("kinematics")
     M = int(m_participants)
     t0s = [int(v) for v in t0s]
@@ -145,6 +159,7 @@ def build_replay_episodes(log: ReplayLog, m_participants: int, t0s: Sequence[int
     pool = {k: np.zeros((P, M), np.float32) for k in ("x", "y", "heading", "speed", "vx", "vy")}
     tid = np.full((P, M), TYPE_INACTIVE, np.uint8)
     row_track = np.full((P, M), -1, np.int32)
+    slots = [[[] for _ in range(M)] for _ in range(P)] if reuse_slots else None
     dropped = np.zeros(P, np.int64)
     for p, (t0, ego_id) in enumerate(zip(t0s, ego_tracks)):
         if not lo <= t0 <= hi:
@@ -159,9 +174,28 @@ def build_replay_episodes(log: ReplayLog, m_participants: int, t0s: Sequence[int
         tid[p, 0] = class_row[e]
         end = np.inf if horizon_ms is None else t0 + int(horizon_ms)
         others = [int(k) for k in order if k != e and last[k] >= t0 and first[k] <= end]
+        if reuse_slots:
+            free_after = np.full(M, np.iinfo(np.int64).min, np.int64)   # slot m takes a track starting after this
+            free_after[0] = np.iinfo(np.int64).max                       # (slot 0 is the ego's)
+            for k in others:
+                m = int(np.argmax(free_after < first[k]))
+                if not free_after[m] < first[k]:
+                    dropped[p] += 1
+                    continue
+                slots[p][m].append(k)
+                free_after[m] = last[k]
+                if first[k] <= t0 <= last[k]:
+                    tid[p, m] = type_row[k]
+            continue
         dropped[p] = max(0, len(others) - (M - 1))
         for m, k in enumerate(others[:M - 1], start=1):
             row_track[p, m] = k
             if first[k] <= t0 <= last[k]:
                 tid[p, m] = type_row[k]
-    return ReplayEpisodes(replace(log, type_row=type_row), table, pool, tid, row_track, np.asarray(t0s, np.int32), dropped)
+    t0_arr = np.asarray(t0s, np.int32)
+    if not reuse_slots:
+        return ReplayEpisodes(replace(log, type_row=type_row), table, pool, tid, row_track, t0_arr, dropped)
+    flat = [s for row in slots for s in row]
+    slot_off = np.concatenate([[0], np.cumsum([len(s) for s in flat])]).astype(np.int32)
+    slot_track = np.asarray([k for s in flat for k in s], np.int32)
+    return ReplayEpisodes(replace(log, type_row=type_row), table, pool, tid, None, t0_arr, dropped, (slot_off, slot_track))

@@ -52,7 +52,9 @@ class BatchedTrafficEnv:
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
         initial states and the type table then come from it and only the map and bounds from ``scene`` (which may be None);
-        an auto-reset restarts the scenario's row, ``reset(options={"shuffle": True})`` deals the rows out anew;
+        an auto-reset restarts the scenario's row, ``reset(options={"shuffle": True})`` deals the rows out anew; episodes
+        with slot schedules (``build_replay_episodes(..., reuse_slots=True)``) add ``info["track"]``, the int32 [N, M]
+        track each slot shows after the step's auto-reset (``BatchedWorld.replay_track``);
         ``target``: optional [N, 5] target areas (cx, cy, heading, half_len, half_wid) for the egos - enables the
         ``Arrival`` (-> COMPLETED / ``terminated``) and ``NoAction`` detectors and the IoU reward terms of
         ``ParkingEnv._get_reward`` (parking.py:148-190); ``observation``: ``"state"`` (the state tensors) or ``"bev"``
@@ -83,7 +85,7 @@ class BatchedTrafficEnv:
         self._type_id = torch.from_numpy(scene.type_id).to(dev)
         self.scenario_manager.set_initial_state(self._pool)
         if replay is not None:
-            self.world.set_log(replay.log, replay.t0, replay.row_track)
+            self.world.set_log(replay.log, replay.t0, **replay.binding())
         self._action = torch.zeros((n, m, 2), dtype=torch.float32, device=dev)
         self._rng = np.random.default_rng(0)
         if target is not None:
@@ -102,8 +104,11 @@ class BatchedTrafficEnv:
         return self.scenario_manager.get_observation()
 
     def _info(self, status, traffic, flags, hit_index, hit_segment):
-        return {"scenario_status": status, "traffic_status": traffic, "flags": flags, "hit_index": hit_index,
+        info = {"scenario_status": status, "traffic_status": traffic, "flags": flags, "hit_index": hit_index,
                 "hit_segment": hit_segment, "step_count": self.world.step_count}
+        if self.world.replay_track is not None:   # scheduled replay: the track each slot shows (-1: none)
+            info["track"] = self.world.replay_track
+        return info
 
     # ------------------------------------------------------------------ gym surface
     def reset(self, seed: int = None, options: dict = None):

@@ -223,3 +223,58 @@ def replay_episodes(n_rows: int, m: int, n_tracks: int, seed: int = 0, table: Op
     sc = _finish(table, px, py, ph, pv, tid, None, None, "replay")
     pool = sc.state()
     return ReplayEpisodes(log, table, pool, tid, row_track, t0, np.zeros(P, np.int64))
+
+
+def highway_log(duration_ms: int = 200000, seed: int = 0, rate_per_s: float = 1.85, length_m: float = 420.0,
+                speed=(25.0, 38.0), lanes_per_side: int = 3, lane_width: float = 3.75, period_ms: int = 40):
+    """A seeded highway-like recording (a :class:`tactics2d_b200.dataset_parser.ReplayLog`, type rows unassigned), modelled
+    on highD's traffic (no LevelX data ships with this repository): road users arrive as a Poisson process of
+    ``rate_per_s`` per second over ``duration_ms``, each on a random lane of either carriageway (``lanes_per_side`` lanes
+    of ``lane_width`` m each side of y = 0; +x above, -x below), and drive straight through the ``length_m`` stretch at
+    their own constant speed drawn from ``speed`` (m/s), one record every ``period_ms`` from their arrival (on the period
+    grid) until they leave it.  One in eight is a truck (16 m x 2.5 m), the others cars (4.5 m x 1.9 m)."""
+    from .dataset_parser.replay import ReplayLog
+    from .participant.element import Vehicle
+
+    rng = np.random.default_rng(seed)
+    arrivals = []
+    t = rng.exponential(1000.0 / rate_per_s)
+    while t < duration_ms:
+        arrivals.append(t)
+        t += rng.exponential(1000.0 / rate_per_s)
+    K = len(arrivals)
+    first = (np.floor(np.asarray(arrivals) / period_ms) * period_ms).astype(np.int64)
+    v = rng.uniform(speed[0], speed[1], K)
+    lane = rng.integers(0, 2 * lanes_per_side, K)
+    fwd = lane < lanes_per_side
+    y = np.where(fwd, -(lane + 0.5), (lane - lanes_per_side + 0.5)) * lane_width
+    truck = rng.uniform(0, 1, K) < 0.125
+    nfr = (np.floor(length_m / (v * period_ms / 1000.0)) + 1).astype(np.int32)
+    recs = []
+    for k in range(K):
+        s = v[k] * np.arange(nfr[k]) * (period_ms / 1000.0)
+        x = s if fwd[k] else length_m - s
+        vx = np.full(nfr[k], v[k] if fwd[k] else -v[k])
+        h = np.full(nfr[k], 0.0 if fwd[k] else np.pi)
+        recs.append(np.stack([x, np.full(nfr[k], y[k]), h, vx, np.zeros(nfr[k])], 1).astype(np.float32))
+    return ReplayLog(ids=np.arange(K, dtype=np.int64), first_ms=first.astype(np.int32), n_frames=nfr,
+                     period_ms=np.full(K, period_ms, np.int32), records=np.ascontiguousarray(np.concatenate(recs)),
+                     type_row=np.full(K, TYPE_INACTIVE, np.uint8), cls=[Vehicle] * K,
+                     length=np.where(truck, 16.0, 4.5), width=np.where(truck, 2.5, 1.9))
+
+
+def highway_episodes(n_rows: int, m: int, seed: int = 0, duration_ms: int = 200000, horizon_ms: Optional[int] = 100000,
+                     reuse_slots: bool = True, log=None, **log_kw):
+    """Episode rows over :func:`highway_log` (``build_replay_episodes``): row p's ego is a random road user, starting at a
+    random frame of the first half of its pass, with ``t0`` in the first ``duration_ms - horizon_ms`` of the log so that
+    the window lies inside the recording; the other slots replay the window's tracks, one after the other when
+    ``reuse_slots``."""
+    from .dataset_parser.replay import build_replay_episodes
+
+    log = highway_log(duration_ms, seed, **log_kw) if log is None else log
+    rng = np.random.default_rng(seed + 1)
+    span = duration_ms - (horizon_ms or 0)
+    ok = np.nonzero(log.first_ms < span)[0]
+    ego = rng.choice(ok, int(n_rows))
+    t0 = log.first_ms[ego] + rng.integers(0, (log.n_frames[ego] + 1) // 2) * log.period_ms[ego]
+    return build_replay_episodes(log, m, t0.tolist(), log.ids[ego].tolist(), horizon_ms=horizon_ms, reuse_slots=reuse_slots)

@@ -285,11 +285,14 @@ class BatchedWorld:
         return action
 
     # ------------------------------------------------------------------ log replay
-    def set_log(self, log, t0=None, row_track=None):
+    def set_log(self, log, t0=None, row_track=None, schedule=None):
         """Replay recorded tracks in the slots bound to them (``t2d_set_log``; DESIGN.md section 1 "Log replay").  ``log``:
         a :class:`tactics2d_b200.dataset_parser.ReplayLog` (or any object with ``first_ms, n_frames, period_ms, type_row``
         [K] and ``records`` [F, 5]) whose type rows are static rows of this world's table, or None to unbind; ``t0`` [P]:
-        the start time (ms) of every episode row; ``row_track`` [P, M]: the track each slot of a row replays, -1 for none.
+        the start time (ms) of every episode row; exactly one of ``row_track`` [P, M]: the track each slot of a row
+        replays, -1 for none, and ``schedule = (slot_off, slot_track)``: slot m of row p replays the tracks
+        ``slot_track[slot_off[p * M + m] : slot_off[p * M + m + 1]]`` one after the other (``t2d_set_log_schedule``; their
+        presence intervals strictly increasing and disjoint), and :attr:`replay_track` then shows which one each slot holds.
         Before every tick, scenario n's replayed slots take their tracks' state at ``t0[log_row[n]] + (step + 1) *
         interval``; ``reset`` sets ``log_row`` from its ``pool_index`` (pool row p = episode row p) and shows the new row's
         traffic at once.  Replayed slots are checked like any participant; an env over a log keeps the default ego-only
@@ -298,14 +301,20 @@ class BatchedWorld:
             _lib.check(self.lib.t2d_set_log(self._ctx, None))
             self._log = None
             return
+        if (row_track is None) == (schedule is None):
+            raise ValueError("give exactly one of row_track and schedule")
         i32 = lambda a: np.ascontiguousarray(np.asarray(a), dtype=np.int32)
         keep = dict(first=i32(log.first_ms), n_frames=i32(log.n_frames), period=i32(log.period_ms),
                     type_row=np.ascontiguousarray(np.asarray(log.type_row), dtype=np.uint8),
                     records=np.ascontiguousarray(np.asarray(log.records), dtype=np.float32).reshape(-1, 5),
-                    t0=i32(t0).reshape(-1), row_track=i32(row_track))
+                    t0=i32(t0).reshape(-1), row_track=None if row_track is None else i32(row_track))
         n_rows = keep["t0"].shape[0]
-        if keep["row_track"].shape != (n_rows, self.M):
+        if row_track is not None and keep["row_track"].shape != (n_rows, self.M):
             raise ValueError(f"row_track must be [{n_rows}, {self.M}] (one row per t0)")
+        if schedule is not None:
+            keep["slot_off"], keep["slot_track"] = i32(schedule[0]).reshape(-1), i32(schedule[1]).reshape(-1)
+            if keep["slot_off"].shape[0] != n_rows * self.M + 1:
+                raise ValueError(f"slot_off must hold n_rows * M + 1 = {n_rows * self.M + 1} offsets")
         k = keep["first"].shape[0]
         if not (keep["n_frames"].shape == keep["period"].shape == keep["type_row"].shape == (k,)):
             raise ValueError("first_ms, n_frames, period_ms and type_row need one entry per track")
@@ -313,13 +322,29 @@ class BatchedWorld:
             raise ValueError("records must hold sum(n_frames) rows")
         log_row = torch.arange(self.N, dtype=torch.int32, device=self.device)
         c = self._log_struct(keep, log_row, self.type_id)
-        _lib.check(self.lib.t2d_set_log(self._ctx, C.byref(c)))
-        self._log = dict(keep, log_row=log_row)
+        if schedule is None:
+            _lib.check(self.lib.t2d_set_log(self._ctx, C.byref(c)))
+            track = None
+        else:
+            track = torch.full((self.N, self.M), -1, dtype=torch.int32, device=self.device)
+            p = lambda a: C.c_void_p(a.ctypes.data)
+            _lib.check(self.lib.t2d_set_log_schedule(self._ctx, C.byref(c), p(keep["slot_off"]), p(keep["slot_track"]),
+                                                     int(keep["slot_track"].shape[0]), _ptr(track)))
+        self._log = dict(keep, log_row=log_row, track=track)
 
     def _log_struct(self, keep, log_row, type_id):
         p = lambda a: C.c_void_p(a.ctypes.data)
+        rt = keep.get("row_track")
         return _lib.LogC(keep["first"].shape[0], p(keep["first"]), p(keep["n_frames"]), p(keep["period"]), p(keep["type_row"]),
-                         p(keep["records"]), keep["t0"].shape[0], p(keep["t0"]), p(keep["row_track"]), _ptr(log_row), _ptr(type_id))
+                         p(keep["records"]), keep["t0"].shape[0], p(keep["t0"]), None if rt is None else p(rt), _ptr(log_row),
+                         _ptr(type_id))
+
+    @property
+    def replay_track(self) -> Optional[torch.Tensor]:
+        """int32 [N, M] device tensor: the track each slot shows, -1 while it shows none or is not replayed (None unless a
+        log is bound with a ``schedule``).  Every replay - each tick and each reset of a scenario - rewrites its slots."""
+        lg = getattr(self, "_log", None)
+        return None if lg is None else lg["track"]
 
     @property
     def log_row(self) -> Optional[torch.Tensor]:
