@@ -46,6 +46,8 @@
  *   t2d_set_log          Trajectory.get_state / Vehicle.get_pose of logged participants at a frame
  *                                                         participant/trajectory/trajectory.py:97-113, vehicle.py:263-281
  *   t2d_set_log_schedule the same, with several tracks replayed one after the other in a slot
+ *   t2d_observe          (no reference counterpart) the ego-frame vector observation: ego motion, goal, nearest
+ *                        participants and nearest map segments of every scenario's ego
  *
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types cross the ABI;
@@ -317,6 +319,32 @@ int t2d_set_bev_styles(t2d_ctx* ctx, const t2d_bev_style* table, int n_styles, c
  * style indices (RGB = the style's colour).  range: HOST float [4] = (left, right, front, back) in metres, each in
  * (0, 1e5]; width, height in 1..1024.  One launch, no allocation, no synchronisation: capturable in a CUDA graph. */
 int t2d_bev_render(t2d_ctx* ctx, int width, int height, const float* range, int rgb, uint8_t* out, void* stream);
+
+/* ---- vector observation of the ego of every scenario -----------------------------------------------------------------
+ * One fp32 row of F = 16 + 11 k_agents + 9 k_segments values per scenario, everything in the frame of participant 0 (origin
+ * at its centre, +x along its heading).  The contract is DESIGN.md section 1 "Vector observation".  Blocks in this order:
+ *   ego      [8]  valid, speed, v_long, v_lat, half_len, half_wid, is_disc, t_frac (= step_count / max_step, 0 without one)
+ *   goal     [8]  valid, ex, ey, cos dh, sin dh, half_len, half_wid, dist   (the t2d_set_goal target; zeros without one)
+ *   agents   [K][11] valid, ex, ey, cos dh, sin dh, v_x, v_y, half_len, half_wid, is_disc, dist: the K nearest other
+ *                 participants (slots >= 1, active, shape not NONE) whose centre lies within agent_range, by (d^2, slot)
+ *   segments [S][9]  valid, ex1, ey1, ex2, ey2, ecx, ecy, dist, in_ring: the S nearest segments of the scenario's map tile
+ *                 within segment_range of the ego centre, by (d^2, segment index); (ecx, ecy) is the closest point
+ * Absent and padding rows are zeros with index -1; with the ego slot empty the whole row is zeros. */
+#define T2D_OBS_MAX_AGENTS 127
+#define T2D_OBS_MAX_SEGMENTS 256
+typedef struct t2d_obs_config {
+  int32_t k_agents;    /* 0..T2D_OBS_MAX_AGENTS */
+  int32_t k_segments;  /* 0..T2D_OBS_MAX_SEGMENTS */
+  float agent_range;   /* metres, (0, 1e5]; closed: d^2 <= r^2 in fp64 */
+  float segment_range; /* metres, (0, 1e5] */
+} t2d_obs_config;
+/* out: DEVICE float [N][F]; agent_index: DEVICE int16 [N][k_agents] (the slot of each agent row) or NULL; segment_index:
+ * DEVICE int16 [N][k_segments] (the segment's index in its tile) or NULL.  Reads the goal target when one is bound and the
+ * map tile(s) when set.  Rejected without a launch: k_agents / k_segments out of bounds, a range that is not finite or not
+ * in (0, 1e5], out == NULL (T2D_E_INVALID), state not bound (T2D_E_STATE).  One launch, no allocation, no
+ * synchronisation: capturable in a CUDA graph. */
+int t2d_observe(t2d_ctx* ctx, const t2d_obs_config* cfg, float* out, int16_t* agent_index, int16_t* segment_index,
+                void* stream);
 
 /* On-device NPC controllers (tactics2d/controller).  A controller row is one configured controller object; the fields
  * are the reference's attribute names.  kind selects the law:

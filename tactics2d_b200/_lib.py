@@ -56,6 +56,11 @@ class LogC(C.Structure):
                 ("row_track", C.c_void_p), ("log_row", C.c_void_p), ("type_id", C.c_void_p)]
 
 
+class ObsConfigC(C.Structure):
+    """``t2d_obs_config``: rows and ranges of the vector observation."""
+    _fields_ = [("k_agents", C.c_int32), ("k_segments", C.c_int32), ("agent_range", C.c_float), ("segment_range", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol include/t2d_b200.h declares
 _P = C.c_void_p
 SYMBOLS = {
@@ -80,6 +85,7 @@ SYMBOLS = {
     "t2d_lidar_scan": (C.c_int, [_P, C.c_int, C.c_float, _P, _P, _P]),
     "t2d_set_bev_styles": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int]),
     "t2d_bev_render": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
+    "t2d_observe": (C.c_int, [_P, C.POINTER(ObsConfigC), _P, _P, _P, _P]),
     "t2d_set_controllers": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P]),
     "t2d_set_paths": (C.c_int, [_P, _P, _P, C.c_int]),
     "t2d_control": (C.c_int, [_P, _P, _P]),

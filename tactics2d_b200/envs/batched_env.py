@@ -20,8 +20,9 @@ Keeps the contract of the reference's single-ego envs (``tactics2d/envs/parking.
 
 What differs, deliberately: the environment is *vectorised* (every quantity has a leading N axis and lives on
 the GPU), all M participants are simulated (the ego is participant 0; the others take ``npc_action`` or zeros),
-the observation is the state tensors themselves by default, or with ``observation="bev"`` the reference's bird's-eye
-view image of every ego rendered on the device (``BatchedWorld.bev``), and scenarios are drawn from a pool of initial states instead of the reference's map generators.
+the observation is the state tensors themselves by default, with ``observation="bev"`` the reference's bird's-eye
+view image of every ego rendered on the device (``BatchedWorld.bev``), or with ``observation="vector"`` the ego-frame vector
+of its motion, goal, nearest participants and nearest map segments (``BatchedWorld.observe``), and scenarios are drawn from a pool of initial states instead of the reference's map generators.
 The reference envs construct a ``render_manager`` that is commented out at this commit and crash on the
 first ``update`` (SURVEY.md section 3.4); this class follows their documented contract, not the crash.
 """
@@ -47,7 +48,7 @@ class BatchedTrafficEnv:
     def __init__(self, scene, device="cuda:0", max_step: int = 1000, step_size: int = 100, delta_t: int = 5,
                  any_participant: bool = False, auto_reset: bool = True, target=None, arrival_threshold: float = 0.95,
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
-                 bev_range=(20.0, 20.0, 20.0, 20.0), replay=None):
+                 bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -59,12 +60,18 @@ class BatchedTrafficEnv:
         ``Arrival`` (-> COMPLETED / ``terminated``) and ``NoAction`` detectors and the IoU reward terms of
         ``ParkingEnv._get_reward`` (parking.py:148-190); ``observation``: ``"state"`` (the state tensors) or ``"bev"``
         (``uint8 [N, H, W, 3]``, the view of ``BatchedWorld.bev(bev_resolution, bev_range)``, rendered after the
-        auto-reset so that a finished scenario shows its new episode; one more launch per step)."""
+        auto-reset so that a finished scenario shows its new episode; one more launch per step) or ``"vector"`` (fp32 [N, F], the
+        ``flat`` row of ``BatchedWorld.observe(**vector_obs)``, also computed after the auto-reset; ``vector_obs`` takes its
+        keyword arguments ``k_agents``, ``k_segments``, ``agent_range``, ``segment_range``)."""
         import torch
 
-        if observation not in ("state", "bev"):
-            raise ValueError(f"observation must be 'state' or 'bev', got {observation!r}")
+        if observation not in ("state", "bev", "vector"):
+            raise ValueError(f"observation must be 'state', 'bev' or 'vector', got {observation!r}")
         self.observation = observation
+        self.vector_obs = dict(vector_obs or {})
+        unknown = set(self.vector_obs) - {"k_agents", "k_segments", "agent_range", "segment_range"}
+        if unknown:
+            raise ValueError(f"vector_obs: unknown keys {sorted(unknown)}")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -93,6 +100,8 @@ class BatchedTrafficEnv:
         if observation == "bev":
             w, h = self.bev_resolution
             self.observation_space = {"shape": (n, h, w, 3), "dtype": "uint8", "low": 0, "high": 255}
+        elif observation == "vector":
+            self.observation_space = {"shape": (n, self.world.observe(**self.vector_obs).flat.shape[1]), "dtype": "float32"}
         else:
             self.observation_space = {"shape": (n, m, 6), "dtype": "float32"}
         self.action_space = {"shape": (n, 2), "low": (-np.inf, -np.inf), "high": (np.inf, np.inf)}
@@ -101,6 +110,8 @@ class BatchedTrafficEnv:
     def _obs(self):
         if self.observation == "bev":
             return self.world.bev(self.bev_resolution, self.bev_range, rgb=True)
+        if self.observation == "vector":
+            return self.world.observe(**self.vector_obs).flat
         return self.scenario_manager.get_observation()
 
     def _info(self, status, traffic, flags, hit_index, hit_segment):

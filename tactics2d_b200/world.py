@@ -50,6 +50,32 @@ class EnvResult:
     traffic_status: torch.Tensor  # uint8 [N, M] TrafficStatus codes
 
 
+# Columns of the blocks of the vector observation (``BatchedWorld.observe``; DESIGN.md section 1 "Vector observation").
+# Positions and velocities are in the ego frame: origin at the ego's centre, +x along its heading; dh = heading - ego heading.
+EGO_FIELDS = ("valid", "speed", "v_long", "v_lat", "half_len", "half_wid", "is_disc", "t_frac")
+GOAL_FIELDS = ("valid", "ex", "ey", "cos_dh", "sin_dh", "half_len", "half_wid", "dist")
+AGENT_FIELDS = ("valid", "ex", "ey", "cos_dh", "sin_dh", "v_x", "v_y", "half_len", "half_wid", "is_disc", "dist")
+SEGMENT_FIELDS = ("valid", "ex1", "ey1", "ex2", "ey2", "ecx", "ecy", "dist", "in_ring")
+
+
+def vector_obs_width(k_agents: int, k_segments: int) -> int:
+    """F, the length of one scenario's row of the vector observation."""
+    return len(EGO_FIELDS) + len(GOAL_FIELDS) + len(AGENT_FIELDS) * int(k_agents) + len(SEGMENT_FIELDS) * int(k_segments)
+
+
+@dataclass
+class VectorObservation:
+    """Views of one device buffer written by ``BatchedWorld.observe`` (overwritten by its next call with the same config)."""
+
+    flat: torch.Tensor           # fp32 [N, F]: ego, goal, agents, segments back to back
+    ego: torch.Tensor            # fp32 [N, 8]   (EGO_FIELDS)
+    goal: torch.Tensor           # fp32 [N, 8]   (GOAL_FIELDS; zeros without a goal)
+    agents: torch.Tensor         # fp32 [N, K, 11] (AGENT_FIELDS), nearest first
+    segments: torch.Tensor       # fp32 [N, S, 9]  (SEGMENT_FIELDS), nearest first
+    agent_index: torch.Tensor    # int16 [N, K]: the participant slot of each agent row, -1 for padding
+    segment_index: torch.Tensor  # int16 [N, S]: the segment's index in its tile, -1 for padding
+
+
 def _ptr(t: Optional[torch.Tensor]):
     return C.c_void_p(0 if t is None else t.data_ptr())
 
@@ -608,6 +634,34 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_bev_render(self._ctx, w, h, C.c_void_p(rng.ctypes.data), 1 if rgb else 0, _ptr(cache[1]),
                                            self._stream()))
         return cache[1]
+
+    # ------------------------------------------------------------------ vector observation
+    def observe(self, k_agents: int = 16, k_segments: int = 32, agent_range: float = 50.0,
+                segment_range: float = 30.0) -> VectorObservation:
+        """The ego-frame vector observation of every scenario's ego (participant 0) in one launch (``t2d_observe``): its
+        motion, the ``set_goal`` target, the ``k_agents`` nearest other participants whose centre lies within
+        ``agent_range`` metres and the ``k_segments`` nearest segments of its map tile within ``segment_range``, nearest
+        first, ties to the lower index; absent rows are zeros with index -1 (DESIGN.md section 1 "Vector observation").
+        The tensors are views of one buffer per ``(k_agents, k_segments)`` that the next call with those counts reuses."""
+        K, S = int(k_agents), int(k_segments)
+        cache = self.__dict__.setdefault("_obs_out", {})
+        obs = cache.get((K, S))
+        if obs is None:
+            if not (0 <= K <= 127 and 0 <= S <= 256):
+                raise ValueError("k_agents must be in 0..127 and k_segments in 0..256")
+            flat = torch.empty((self.N, vector_obs_width(K, S)), dtype=torch.float32, device=self.device)
+            a0 = len(EGO_FIELDS) + len(GOAL_FIELDS)
+            s0 = a0 + len(AGENT_FIELDS) * K
+            obs = cache[(K, S)] = VectorObservation(
+                flat=flat, ego=flat[:, :len(EGO_FIELDS)], goal=flat[:, len(EGO_FIELDS):a0],
+                agents=flat[:, a0:s0].view(self.N, K, len(AGENT_FIELDS)),
+                segments=flat[:, s0:].view(self.N, S, len(SEGMENT_FIELDS)),
+                agent_index=torch.empty((self.N, K), dtype=torch.int16, device=self.device),
+                segment_index=torch.empty((self.N, S), dtype=torch.int16, device=self.device))
+        cfg = _lib.ObsConfigC(K, S, float(agent_range), float(segment_range))
+        _lib.check(self.lib.t2d_observe(self._ctx, C.byref(cfg), _ptr(obs.flat), _ptr(obs.agent_index),
+                                        _ptr(obs.segment_index), self._stream()))
+        return obs
 
     def reset(self, mask: torch.Tensor, pool: dict, pool_index: Optional[torch.Tensor] = None):
         """Re-initialise the scenarios with ``mask[n] != 0`` from row ``pool_index[n]`` (default n)
