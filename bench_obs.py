@@ -8,6 +8,11 @@ agent rows and 32 segment rows within 50 m / 30 m.  A call is timed with CUDA ev
 bytes (the state of every slot, the tile ids, the segments of each scenario's tile, the row and indices written) and their
 share of the H100 SXM data sheet's 3.35 TB/s.  Then ``BatchedTrafficEnv.step`` at C2 with ``observation="state"`` and
 ``"vector"``, alternating, in wall-clock microseconds per step (the env's step ends in host work, not in a graph).
+
+``--agents`` times the per-agent observation instead (K9, ``BatchedWorld.observe_agents``) on the same three scenes: every
+slot observing (Q = M) and the ego alone (Q = 1, observer 0), each alternated with K8's ``observe`` on the same world for
+``--rounds`` rounds; its bytes add the rows and indices of every observer (the state, tile ids and segments are counted once
+per scenario, as for K8).
 """
 
 from __future__ import annotations
@@ -61,19 +66,21 @@ def _world(scene):
     return w, len(s.segments), scene == "c4"
 
 
-def _time_observe(w, seconds):
+def _time_observe(w, seconds, call=None):
     import torch
 
     args = (K_AGENTS, K_SEGMENTS, AGENT_RANGE, SEGMENT_RANGE)
+    if call is None:
+        call = lambda: w.observe(*args)
     st = torch.cuda.Stream()
     st.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(st):
         for _ in range(3):
-            w.observe(*args)
+            call()
     torch.cuda.current_stream().wait_stream(st)
     g = torch.cuda.CUDAGraph()
     with torch.cuda.graph(g):
-        w.observe(*args)
+        call()
     for _ in range(20):
         g.replay()
     torch.cuda.synchronize()
@@ -99,6 +106,30 @@ def _bytes(w, n_seg, map_table):
     read = w.N * (w.M * 21 + 4 + (2 if map_table else 0) + 16 * n_seg)
     write = w.N * (4 * F + 2 * (K_AGENTS + K_SEGMENTS))
     return read, write
+
+
+def _agents(a, gpu, power):
+    """K9 with every slot and with observer 0 alone, each alternated with K8 on the same world."""
+    import torch
+
+    args = (K_AGENTS, K_SEGMENTS, AGENT_RANGE, SEGMENT_RANGE)
+    for scene in a.scenes.split(","):
+        w, n_seg, map_table = _world(scene)
+        ego = torch.zeros((w.N, 1), dtype=torch.int16, device=w.device)
+        k8_rd, k8_wr = _bytes(w, n_seg, map_table)
+        for r in range(a.rounds):
+            for kernel, q, call in (("k9", w.M, lambda: w.observe_agents(*args)), ("k8", 1, None),
+                                    ("k9", 1, lambda: w.observe_agents(*args, observers=ego)), ("k8", 1, None)):
+                us, reps = _time_observe(w, a.seconds, call)
+                rd = k8_rd + (2 * w.N * q if call is not None and q == 1 else 0)   # the observer list
+                wr = k8_wr * q
+                print(json.dumps(dict(metric="observe_agents" if kernel == "k9" else "observe", kernel=kernel, scene=scene,
+                                      round=r, n=w.N, m=w.M, q=q, segments_per_tile=n_seg, k_agents=K_AGENTS,
+                                      k_segments=K_SEGMENTS, agent_range=AGENT_RANGE, segment_range=SEGMENT_RANGE, gpu=gpu,
+                                      power_limit=power, us_per_call=round(us, 2), replays=reps, bytes_read=rd,
+                                      bytes_written=wr, achieved_gb_s=round((rd + wr) / (us * 1e-6) / 1e9, 1),
+                                      share_of_hbm=round((rd + wr) / (us * 1e-6) / PEAK_BYTES_PER_S, 3))), flush=True)
+        w.close()
 
 
 def _time_env(observation, steps, warmup):
@@ -128,12 +159,17 @@ def main(argv=None):
     ap.add_argument("--scenes", default="c2,c4,round")
     ap.add_argument("--env-steps", type=int, default=2000)
     ap.add_argument("--env-rounds", type=int, default=3)
+    ap.add_argument("--agents", action="store_true", help="time observe_agents (K9) against observe (K8) instead")
+    ap.add_argument("--rounds", type=int, default=3, help="with --agents: alternating rounds per scene")
     a = ap.parse_args(argv)
     import torch
 
     if not torch.cuda.is_available():
         sys.exit("bench_obs.py needs a CUDA device")
     gpu, power = _gpu_info()
+    if a.agents:
+        _agents(a, gpu, power)
+        return
     for scene in a.scenes.split(","):
         w, n_seg, map_table = _world(scene)
         us, reps = _time_observe(w, a.seconds)

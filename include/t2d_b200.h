@@ -48,6 +48,8 @@
  *   t2d_set_log_schedule the same, with several tracks replayed one after the other in a slot
  *   t2d_observe          (no reference counterpart) the ego-frame vector observation: ego motion, goal, nearest
  *                        participants and nearest map segments of every scenario's ego
+ *   t2d_observe_agents   (no reference counterpart) the same observation seen from a list of observer slots per scenario,
+ *                        for multi-agent control
  *
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types cross the ABI;
@@ -345,6 +347,26 @@ typedef struct t2d_obs_config {
  * synchronisation: capturable in a CUDA graph. */
 int t2d_observe(t2d_ctx* ctx, const t2d_obs_config* cfg, float* out, int16_t* agent_index, int16_t* segment_index,
                 void* stream);
+
+/* ---- per-agent vector observation: the same row seen from any list of observer slots ---------------------------------
+ * DESIGN.md section 1 "Per-agent vector observation".  Row (n, q), q < Q = n_observers (1..T2D_OBS_MAX_OBSERVERS), is
+ * t2d_observe's row with slot j = observers[n][q] in the place of participant 0: the frame and the ego block are j's, the
+ * agent candidates are every other slot (slot 0 included) that is active, has a shape and lies within agent_range, by
+ * (d^2, slot), and the segments are measured from j's centre.  observers: DEVICE int16 [N][Q], or NULL for slot q in row q
+ * of every scenario (needs Q <= M).  A value outside [0, M) or an empty slot (type_id >= n_types) gives an absent row
+ * (zeros, every index -1); duplicates are allowed; the kernel applies this to the device data, nothing is checked on the host.
+ * Goal block: goals == NULL - the rows observed by slot 0 take the t2d_set_goal target, every other row zeros; else goals is
+ * DEVICE float [N][Q][5] (cx, cy, heading, half_len, half_wid) per row, a row whose cx is NaN gets zeros.  t_frac is the
+ * scenario's.  With observers [n] = {0} and goals == NULL a row is bit-identical to t2d_observe's.
+ * out: DEVICE float [N][Q][F] (F as t2d_observe, 64-bit offsets: N·Q·F may exceed 2^31); agent_index: DEVICE int16 [N][Q][K]
+ * or NULL; segment_index: DEVICE int16 [N][Q][S] or NULL.  Rejected without a launch: everything t2d_observe rejects,
+ * n_observers outside 1..128, observers == NULL with n_observers > M (T2D_E_INVALID), state not bound (T2D_E_STATE).
+ * One launch, no allocation, no synchronisation: capturable in a CUDA graph. */
+#define T2D_OBS_MAX_OBSERVERS 128
+int t2d_observe_agents(t2d_ctx* ctx, const t2d_obs_config* cfg, const int16_t* observers /* DEVICE [N][Q] or NULL */,
+                       int32_t n_observers /* Q */, const float* goals /* DEVICE [N][Q][5] or NULL */,
+                       float* out /* DEVICE [N][Q][F] */, int16_t* agent_index /* [N][Q][K] or NULL */,
+                       int16_t* segment_index /* [N][Q][S] or NULL */, void* stream);
 
 /* On-device NPC controllers (tactics2d/controller).  A controller row is one configured controller object; the fields
  * are the reference's attribute names.  kind selects the law:

@@ -10,6 +10,7 @@
 // K5  t2d_control_kernel   NPC controllers: IDM, cruise / adaptive cruise, pure pursuit.
 // K7  t2d_replay_kernel    log replay: recorded tracks pose the replayed slots before K1 / after K2.
 // K8  t2d_obs_kernel       the ego-frame vector observation (t2d_obs.cuh).
+// K9  t2d_obs_agents_kernel the same observation from a list of observer slots per scenario (t2d_obs.cuh).
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory.
 //
 // Work decomposition of K1: a scenario (M <= 128 participants) is owned by a group of G lanes of
@@ -3028,6 +3029,45 @@ int t2d_observe(t2d_ctx* c, const t2d_obs_config* cfg, float* out, int16_t* agen
   CUDA_TRY(cudaSetDevice(c->device));
   const int grid = (c->N + obs::WARPS - 1) / obs::WARPS;
   obs::t2d_obs_kernel<<<grid, obs::WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  g_launches.fetch_add(1);
+  CUDA_TRY(cudaGetLastError());
+  return T2D_OK;
+}
+
+int t2d_observe_agents(t2d_ctx* c, const t2d_obs_config* cfg, const int16_t* observers, int32_t n_observers,
+                       const float* goals, float* out, int16_t* agent_index, int16_t* segment_index, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!cfg) return fail(T2D_E_INVALID, "t2d_observe_agents: cfg is NULL");
+  if (cfg->k_agents < 0 || cfg->k_agents > T2D_OBS_MAX_AGENTS)
+    return fail(T2D_E_INVALID, "t2d_observe_agents: k_agents must be in 0..127");
+  if (cfg->k_segments < 0 || cfg->k_segments > T2D_OBS_MAX_SEGMENTS)
+    return fail(T2D_E_INVALID, "t2d_observe_agents: k_segments must be in 0..256");
+  if (!(cfg->agent_range > 0.0f && cfg->agent_range <= 1.0e5f) || !(cfg->segment_range > 0.0f && cfg->segment_range <= 1.0e5f))
+    return fail(T2D_E_INVALID, "t2d_observe_agents: agent_range and segment_range must be in (0, 1e5] m");
+  if (!out) return fail(T2D_E_INVALID, "t2d_observe_agents: out is NULL");
+  if (n_observers < 1 || n_observers > T2D_OBS_MAX_OBSERVERS)
+    return fail(T2D_E_INVALID, "t2d_observe_agents: n_observers must be in 1..128");
+  if (!observers && n_observers > c->M)
+    return fail(T2D_E_INVALID, "t2d_observe_agents: without an observer list n_observers must not exceed the slots per scenario");
+  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  obs::AgentArgs G{};
+  obs::Args& A = G.a;
+  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy;
+  A.type_id = c->type_id; A.step_count = c->step_count; A.table = c->d_table; A.n_types = c->n_types;
+  A.N = c->N; A.M = c->M; A.max_step = c->cfg.max_step;
+  A.map_blob = c->d_map; A.tile_off = c->d_tile_off; A.tile_id = c->n_tiles > 1 ? c->tile_id : nullptr;
+  A.target = c->goal_target;
+  A.K = cfg->k_agents; A.S = cfg->k_segments;
+  A.F = obs::EGO_F + obs::GOAL_F + obs::AGENT_F * A.K + obs::SEG_F * A.S;
+  const double ra = cfg->agent_range, rs = cfg->segment_range;
+  A.ra2 = ra * ra; A.rs2 = rs * rs;
+  A.out = out; A.agent_index = agent_index; A.segment_index = segment_index;
+  G.observers = observers; G.goals = goals; G.Q = n_observers;
+  CUDA_TRY(cudaSetDevice(c->device));
+  const long long rows = (long long)c->N * n_observers;
+  const int grid = (int)std::min<long long>((rows + obs::WARPS - 1) / obs::WARPS, 1ll << 30);   // the kernel strides past 2^32 rows
+  obs::t2d_obs_agents_kernel<<<grid, obs::WARPS * 32, 0, (cudaStream_t)stream>>>(G);
   g_launches.fetch_add(1);
   CUDA_TRY(cudaGetLastError());
   return T2D_OK;

@@ -10,6 +10,9 @@
 // the lanes take the tile's segments 32 at a time; each chunk's in-range candidates are sorted by (d2, index) and merged into a
 // running best-S list in shared memory.  Ties in d2 go to the lower index everywhere, so the result does not depend on the
 // chunking or on lane order.  The row is assembled in shared memory 32 entries at a time and stored by consecutive lanes.
+//
+// K9 (t2d_obs_agents_kernel, DESIGN.md section 1 "Per-agent vector observation") is the same row seen from any slot: one warp
+// per (scenario, observer) row runs the row routine K8 runs, so a row observed by slot 0 without per-row goals is K8's row.
 #pragma once
 
 #include <stdint.h>
@@ -116,25 +119,32 @@ __device__ __forceinline__ void flush(float* dst, const float* stage, int n, int
   __syncwarp();
 }
 
-__global__ void __launch_bounds__(WARPS * 32) t2d_obs_kernel(const __grid_constant__ Args A) {
-  __shared__ Smem s_all[WARPS];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long n = (long long)blockIdx.x * WARPS + warp;
-  if (n >= A.N) return;
-  Smem& sm = s_all[warp];
+// An absent row (no observer): F zeros, every index -1.  rid: the row's number in out / agent_index / segment_index.
+__device__ __forceinline__ void absent_row(const Args& A, float* row, long long rid, int K, int S, int lane) {
+  for (int i = lane; i < A.F; i += 32) row[i] = 0.0f;
+  if (A.agent_index) for (int i = lane; i < K; i += 32) A.agent_index[rid * K + i] = -1;
+  if (A.segment_index) for (int i = lane; i < S; i += 32) A.segment_index[rid * S + i] = -1;
+}
+
+// The row of scenario n seen from its slot jo (0 <= jo < M), written by one warp to row rid of out / agent_index /
+// segment_index; the goal rectangle (cx, cy, heading, half_len, half_wid) is row grow of gtab, gtab == nullptr gives the zero
+// block.  K8 and K9 both run it; EGO (K8) fixes jo = 0, which keeps K8's candidate test as the slots j >= 1, and takes row n
+// of the t2d_set_goal target whatever gtab says.
+template <bool EGO>
+__device__ __forceinline__ void observe_row(const Args& A, Smem& sm, int lane, long long n, long long rid, int jo,
+                                            const float* gtab, long long grow) {
   const long long base = n * A.M;
-  float* row = A.out + n * (long long)A.F;
+  const long long po = base + jo;
+  float* row = A.out + rid * (long long)A.F;
   const int K = A.K, S = A.S;
-  const int t0 = A.type_id[base];
-  if (t0 >= A.n_types) {   // no ego: the whole row is zeros, every index -1
-    for (int i = lane; i < A.F; i += 32) row[i] = 0.0f;
-    if (A.agent_index) for (int i = lane; i < K; i += 32) A.agent_index[n * K + i] = -1;
-    if (A.segment_index) for (int i = lane; i < S; i += 32) A.segment_index[n * S + i] = -1;
+  const int t0 = A.type_id[po];
+  if (t0 >= A.n_types) {   // no observer: the whole row is zeros, every index -1
+    absent_row(A, row, rid, K, S, lane);
     return;
   }
   Frame f;
-  f.x0 = A.x[base]; f.y0 = A.y[base];
-  const double h0 = A.h[base];
+  f.x0 = A.x[po]; f.y0 = A.y[po];
+  const double h0 = A.h[po];
   sincos_angle(h0, &f.s, &f.c);
 
   // ---- the tile (as K4 finds it)
@@ -155,7 +165,7 @@ __global__ void __launch_bounds__(WARPS * 32) t2d_obs_kernel(const __grid_consta
       const int j = j0 + lane;
       bool in = false;
       unsigned long long key = NO_KEY;
-      if (j >= 1 && j < A.M) {
+      if ((EGO ? j >= 1 : j != jo) && j < A.M) {
         const int t = A.type_id[base + j];
         if (t < A.n_types && A.table[t].shape() != SHAPE_NONE) {
           const double dx = dsub(A.x[base + j], f.x0), dy = dsub(A.y[base + j], f.y0);
@@ -246,13 +256,14 @@ __global__ void __launch_bounds__(WARPS * 32) t2d_obs_kernel(const __grid_consta
     const Params& pe = A.table[t0];
     float hl, hw, disc;
     extents(pe, hl, hw, disc);
-    const double vx = A.vx[base], vy = A.vy[base];
-    o[0] = 1.0f; o[1] = A.v[base];
+    const double vx = A.vx[po], vy = A.vy[po];
+    o[0] = 1.0f; o[1] = A.v[po];
     o[2] = f32(f.ex(vx, vy)); o[3] = f32(f.ey(vx, vy));
     o[4] = hl; o[5] = hw; o[6] = disc;
     o[7] = A.max_step > 0 ? f32(__ddiv_rn((double)A.step_count[n], (double)A.max_step)) : 0.0f;
-    if (A.target) {
-      const float* g = A.target + n * 5;
+    const float* gt = EGO ? A.target : gtab;   // K8: the t2d_set_goal target of the scenario
+    if (gt) {
+      const float* g = gt + (EGO ? n : grow) * 5;
       const double dx = dsub(g[0], f.x0), dy = dsub(g[1], f.y0);
       double sd, cd;
       sincos_angle(dsub(g[2], h0), &sd, &cd);
@@ -285,7 +296,7 @@ __global__ void __launch_bounds__(WARPS * 32) t2d_obs_kernel(const __grid_consta
     } else if (r < K) {
       for (int k = 0; k < AGENT_F; ++k) o[k] = 0.0f;
     }
-    if (A.agent_index && r < K) A.agent_index[n * K + r] = (int16_t)j;
+    if (A.agent_index && r < K) A.agent_index[rid * K + r] = (int16_t)j;
     flush(row + EGO_F + GOAL_F + r0 * AGENT_F, sm.stage, nrow * AGENT_F, lane);
   }
 
@@ -308,8 +319,50 @@ __global__ void __launch_bounds__(WARPS * 32) t2d_obs_kernel(const __grid_consta
     } else if (r < S) {
       for (int k = 0; k < SEG_F; ++k) o[k] = 0.0f;
     }
-    if (A.segment_index && r < S) A.segment_index[n * S + r] = (int16_t)si;
+    if (A.segment_index && r < S) A.segment_index[rid * S + r] = (int16_t)si;
     flush(srow + r0 * SEG_F, sm.stage, nrow * SEG_F, lane);
+  }
+}
+
+// K8: the row of every scenario's ego (participant 0), one warp per scenario.
+__global__ void __launch_bounds__(WARPS * 32) t2d_obs_kernel(const __grid_constant__ Args A) {
+  __shared__ Smem s_all[WARPS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long n = (long long)blockIdx.x * WARPS + warp;
+  if (n >= A.N) return;
+  observe_row<true>(A, s_all[warp], lane, n, n, 0, nullptr, 0);
+}
+
+// K9: the rows of a list of observers per scenario, one warp per (scenario, observer) row.  The rows of one scenario are
+// consecutive, so the warps of a CTA share its slots and its tile's segments through L1.
+struct AgentArgs {
+  Args a;                     // out / agent_index / segment_index are indexed by the row n·Q + q
+  const int16_t* observers;   // [N][Q], or nullptr: observer q is slot q
+  const float* goals;         // [N][Q][5], or nullptr: slot 0's rows take the t2d_set_goal target, the others none
+  int Q;
+};
+
+__global__ void __launch_bounds__(WARPS * 32) t2d_obs_agents_kernel(const __grid_constant__ AgentArgs G) {
+  __shared__ Smem s_all[WARPS];
+  const Args& A = G.a;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long rows = (long long)A.N * G.Q;
+  for (long long rid = (long long)blockIdx.x * WARPS + warp; rid < rows; rid += (long long)gridDim.x * WARPS) {
+    const long long n = rid / G.Q;
+    const int q = (int)(rid - n * G.Q);
+    const int jo = G.observers ? G.observers[rid] : q;
+    if (jo < 0 || jo >= A.M) {   // not a slot: an absent row
+      absent_row(A, A.out + rid * (long long)A.F, rid, A.K, A.S, lane);
+      continue;
+    }
+    const float* gtab = nullptr;   // the goal: row grow of gtab
+    long long grow = 0;
+    if (G.goals) {
+      if (!isnan(G.goals[rid * 5])) { gtab = G.goals; grow = rid; }
+    } else if (jo == 0) {
+      gtab = A.target; grow = n;
+    }
+    observe_row<false>(A, s_all[warp], lane, n, rid, jo, gtab, grow);
   }
 }
 

@@ -62,14 +62,19 @@ class BatchedTrafficEnv:
         (``uint8 [N, H, W, 3]``, the view of ``BatchedWorld.bev(bev_resolution, bev_range)``, rendered after the
         auto-reset so that a finished scenario shows its new episode; one more launch per step) or ``"vector"`` (fp32 [N, F], the
         ``flat`` row of ``BatchedWorld.observe(**vector_obs)``, also computed after the auto-reset; ``vector_obs`` takes its
-        keyword arguments ``k_agents``, ``k_segments``, ``agent_range``, ``segment_range``)."""
+        keyword arguments ``k_agents``, ``k_segments``, ``agent_range``, ``segment_range``) or ``"agents"`` (fp32 [N, Q, F],
+        the ``flat`` rows of ``BatchedWorld.observe_agents(**vector_obs)``, one per observer slot, for multi-agent control,
+        also computed after the auto-reset; ``vector_obs`` may then also hold ``observers`` and ``goals``)."""
         import torch
 
-        if observation not in ("state", "bev", "vector"):
-            raise ValueError(f"observation must be 'state', 'bev' or 'vector', got {observation!r}")
+        if observation not in ("state", "bev", "vector", "agents"):
+            raise ValueError(f"observation must be 'state', 'bev', 'vector' or 'agents', got {observation!r}")
         self.observation = observation
         self.vector_obs = dict(vector_obs or {})
-        unknown = set(self.vector_obs) - {"k_agents", "k_segments", "agent_range", "segment_range"}
+        keys = {"k_agents", "k_segments", "agent_range", "segment_range"}
+        if observation == "agents":
+            keys |= {"observers", "goals"}
+        unknown = set(self.vector_obs) - keys
         if unknown:
             raise ValueError(f"vector_obs: unknown keys {sorted(unknown)}")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
@@ -102,6 +107,9 @@ class BatchedTrafficEnv:
             self.observation_space = {"shape": (n, h, w, 3), "dtype": "uint8", "low": 0, "high": 255}
         elif observation == "vector":
             self.observation_space = {"shape": (n, self.world.observe(**self.vector_obs).flat.shape[1]), "dtype": "float32"}
+        elif observation == "agents":
+            self.observation_space = {"shape": tuple(self.world.observe_agents(**self.vector_obs).flat.shape),
+                                      "dtype": "float32"}
         else:
             self.observation_space = {"shape": (n, m, 6), "dtype": "float32"}
         self.action_space = {"shape": (n, 2), "low": (-np.inf, -np.inf), "high": (np.inf, np.inf)}
@@ -112,6 +120,8 @@ class BatchedTrafficEnv:
             return self.world.bev(self.bev_resolution, self.bev_range, rgb=True)
         if self.observation == "vector":
             return self.world.observe(**self.vector_obs).flat
+        if self.observation == "agents":
+            return self.world.observe_agents(**self.vector_obs).flat
         return self.scenario_manager.get_observation()
 
     def _info(self, status, traffic, flags, hit_index, hit_segment):

@@ -76,6 +76,21 @@ class VectorObservation:
     segment_index: torch.Tensor  # int16 [N, S]: the segment's index in its tile, -1 for padding
 
 
+@dataclass
+class AgentObservation:
+    """Views of one device buffer written by ``BatchedWorld.observe_agents`` (overwritten by its next call with the same
+    counts): row (n, q) is the vector observation of scenario n seen from slot ``observers[n, q]``."""
+
+    flat: torch.Tensor           # fp32 [N, Q, F]
+    ego: torch.Tensor            # fp32 [N, Q, 8]      (EGO_FIELDS, of the observer)
+    goal: torch.Tensor           # fp32 [N, Q, 8]      (GOAL_FIELDS)
+    agents: torch.Tensor         # fp32 [N, Q, K, 11]  (AGENT_FIELDS), nearest first
+    segments: torch.Tensor       # fp32 [N, Q, S, 9]   (SEGMENT_FIELDS), nearest first
+    agent_index: torch.Tensor    # int16 [N, Q, K]: the participant slot of each agent row, -1 for padding
+    segment_index: torch.Tensor  # int16 [N, Q, S]: the segment's index in its tile, -1 for padding
+    observers: Optional[torch.Tensor]   # int16 [N, Q] as passed, or None: row q is slot q
+
+
 def _ptr(t: Optional[torch.Tensor]):
     return C.c_void_p(0 if t is None else t.data_ptr())
 
@@ -661,6 +676,52 @@ class BatchedWorld:
         cfg = _lib.ObsConfigC(K, S, float(agent_range), float(segment_range))
         _lib.check(self.lib.t2d_observe(self._ctx, C.byref(cfg), _ptr(obs.flat), _ptr(obs.agent_index),
                                         _ptr(obs.segment_index), self._stream()))
+        return obs
+
+    def observe_agents(self, k_agents: int = 16, k_segments: int = 32, agent_range: float = 50.0,
+                       segment_range: float = 30.0, observers: Optional[torch.Tensor] = None,
+                       goals: Optional[torch.Tensor] = None) -> AgentObservation:
+        """``observe`` from the point of view of a list of observer slots per scenario, in one launch
+        (``t2d_observe_agents``; DESIGN.md section 1 "Per-agent vector observation").  ``observers``: int16 ``[N, Q]``
+        device tensor of slots, Q in 1..128 (a value outside ``[0, M)`` or an empty slot gives an absent row; duplicates
+        are allowed), or None for every slot (Q = M).  The agents of a row are the nearest other slots, slot 0 included.
+        ``goals``: fp32 ``[N, Q, 5]`` (cx, cy, heading, half_len, half_wid) per row, a NaN cx for none; without it the rows
+        observed by slot 0 take the ``set_goal`` target and the others none.  A row observed by slot 0 without ``goals``
+        equals ``observe``'s row.  The tensors are views of one buffer per ``(k_agents, k_segments, Q)`` that the next call
+        with those counts reuses."""
+        K, S = int(k_agents), int(k_segments)
+        # observers / goals reach the kernel as raw pointers: a host tensor, a wrong dtype or shape would be read out of bounds
+        if observers is None:
+            Q = self.M
+        else:
+            if (not torch.is_tensor(observers) or observers.device != self.device or observers.dtype != torch.int16
+                    or observers.dim() != 2 or observers.shape[0] != self.N or not observers.is_contiguous()):
+                raise ValueError(f"observers must be a contiguous int16 [{self.N}, Q] tensor on {self.device}")
+            Q = int(observers.shape[1])
+        if not 1 <= Q <= 128:
+            raise ValueError("the number of observers per scenario must be in 1..128")
+        if goals is not None:
+            if (not torch.is_tensor(goals) or goals.device != self.device or goals.dtype != torch.float32
+                    or tuple(goals.shape) != (self.N, Q, 5) or not goals.is_contiguous()):
+                raise ValueError(f"goals must be a contiguous fp32 [{self.N}, {Q}, 5] tensor on {self.device}")
+        cache = self.__dict__.setdefault("_agent_obs_out", {})
+        obs = cache.get((K, S, Q))
+        if obs is None:
+            if not (0 <= K <= 127 and 0 <= S <= 256):
+                raise ValueError("k_agents must be in 0..127 and k_segments in 0..256")
+            flat = torch.empty((self.N, Q, vector_obs_width(K, S)), dtype=torch.float32, device=self.device)
+            a0 = len(EGO_FIELDS) + len(GOAL_FIELDS)
+            s0 = a0 + len(AGENT_FIELDS) * K
+            obs = cache[(K, S, Q)] = AgentObservation(
+                flat=flat, ego=flat[..., :len(EGO_FIELDS)], goal=flat[..., len(EGO_FIELDS):a0],
+                agents=flat[..., a0:s0].view(self.N, Q, K, len(AGENT_FIELDS)),
+                segments=flat[..., s0:].view(self.N, Q, S, len(SEGMENT_FIELDS)),
+                agent_index=torch.empty((self.N, Q, K), dtype=torch.int16, device=self.device),
+                segment_index=torch.empty((self.N, Q, S), dtype=torch.int16, device=self.device), observers=None)
+        obs.observers = observers
+        cfg = _lib.ObsConfigC(K, S, float(agent_range), float(segment_range))
+        _lib.check(self.lib.t2d_observe_agents(self._ctx, C.byref(cfg), _ptr(observers), Q, _ptr(goals), _ptr(obs.flat),
+                                               _ptr(obs.agent_index), _ptr(obs.segment_index), self._stream()))
         return obs
 
     def reset(self, mask: torch.Tensor, pool: dict, pool_index: Optional[torch.Tensor] = None):
