@@ -231,7 +231,8 @@ int t2d_set_goal(t2d_ctx* ctx, const float* target, float arrival_threshold, int
  * state and zero step_count[n]; pool_vx / pool_vy may be NULL (then speed x (cos, sin)(heading)).  Everything else the
  * world owns per participant starts fresh too: the NoAction detector state of t2d_set_goal, the controllers' last_accel
  * (0), and the SingleTrackDrift wheel speeds bound with t2d_bind_wheel_state - from the pool columns of
- * t2d_bind_reset_wheel_pool when bound, else free rolling (speed / wheel_radius). */
+ * t2d_bind_reset_wheel_pool when bound, else free rolling (speed / wheel_radius).  With agents bound (t2d_set_agents)
+ * the retired slots take their types back and the per-row NoAction state is cleared. */
 int t2d_reset(t2d_ctx* ctx, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x,
               const float* pool_y, const float* pool_heading, const float* pool_speed, const float* pool_vx,
               const float* pool_vy, void* stream);
@@ -432,6 +433,33 @@ int t2d_step_host_ego(t2d_ctx* ctx, const float* ego_action_host, float* action,
 int t2d_env_epilogue(t2d_ctx* ctx, const uint8_t* flags, const uint8_t* scn_status, float* reward, uint8_t* terminated,
                      uint8_t* truncated, uint8_t* traffic_status, uint8_t* done, float* max_iou, float* min_dist,
                      int reset_trackers_on_done, void* stream);
+
+/* ---- per-agent status, reward and retirement (no reference counterpart) ---------------------------------------------
+ * DESIGN.md section 1 "Per-agent status and reward".  The agents are the rows of an observer list, as in
+ * t2d_observe_agents: observers DEVICE int16 [N][Q], Q = n_observers in 1..T2D_OBS_MAX_OBSERVERS, or NULL for slot q in
+ * row q (Q <= M).  Row (n, q) is active when observers[n][q] is in [0, M) and that slot's type_id < n_types when the
+ * epilogue runs; an inactive row is absent (status 0, reward 0, terminated / truncated 0, iou 0).  Duplicates are allowed.
+ * goals: DEVICE float [N][Q][5] (cx, cy, heading, half_len, half_wid) or NULL; a NaN cx means the row has no goal.  A row
+ * with a goal whose slot is a box has the Arrival / NoAction detectors of t2d_set_goal (same threshold rule, same
+ * arithmetic), with per-row state last_pose [N][Q][4] and noact_count [N][Q] (zero them before the first step).
+ * retired_type DEVICE uint8 [N][M] (fill with 255 before the first step): a row that settles (status not NORMAL) retires
+ * its slot - the type goes into retired_type and type_id becomes 255, so the bound type_id must be writable.
+ * While agents are bound, t2d_reset also restores the retired types of the masked scenarios (before its log replay, which
+ * rewrites replayed slots as before) and clears their per-row NoAction state.  observers == NULL with n_observers == 0
+ * unbinds.  Rejected: n_observers outside 1..128, observers == NULL with n_observers > M, a NULL state array, a threshold
+ * outside (0, 1] with goals (T2D_E_INVALID).  The arrays are the caller's and must stay alive while bound. */
+int t2d_set_agents(t2d_ctx* ctx, const int16_t* observers, int32_t n_observers, const float* goals, float arrival_threshold,
+                   int no_action_max_step, float* last_pose, int32_t* noact_count, uint8_t* retired_type);
+/* K10: for every row, the status chain of t2d_step applied to its own slot (time exceeded, no action, out of bound,
+ * collision, completed, normal), terminated / truncated / reward by t2d_env_epilogue's rules, iou [N][Q] (0 without
+ * detectors), the per-episode extrema max_iou / min_dist [N][Q] (initialise to -inf / +inf), retirement, and
+ * done[n] = 1 when no row of scenario n is NORMAL (a scenario whose rows are all absent is done at every step).  With
+ * reset_trackers_on_done the extrema of the done scenarios restart.  traffic_status [N][M] may be NULL; every other array
+ * is required (T2D_E_INVALID).  State not bound or no agents bound: T2D_E_STATE.  All arrays DEVICE; one launch, no
+ * allocation, no synchronisation: capturable in a CUDA graph. */
+int t2d_agents_epilogue(t2d_ctx* ctx, const uint8_t* flags, float* reward, uint8_t* terminated, uint8_t* truncated,
+                        uint8_t* agent_status, float* iou, uint8_t* done, float* max_iou, float* min_dist,
+                        uint8_t* traffic_status, int reset_trackers_on_done, void* stream);
 
 /* ---- done-mask exchange across the GPUs of one node, over peer memory (NVLink / NVSwitch) -------------------------
  * Scenarios are sharded across ranks (one process per GPU); the one exchange of the path is "every rank learns every

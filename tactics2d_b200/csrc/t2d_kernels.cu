@@ -11,6 +11,7 @@
 // K7  t2d_replay_kernel    log replay: recorded tracks pose the replayed slots before K1 / after K2.
 // K8  t2d_obs_kernel       the ego-frame vector observation (t2d_obs.cuh).
 // K9  t2d_obs_agents_kernel the same observation from a list of observer slots per scenario (t2d_obs.cuh).
+// K10 t2d_agents_epilogue_kernel status, reward and retirement of every agent row of an observer list.
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory.
 //
 // Work decomposition of K1: a scenario (M <= 128 participants) is owned by a group of G lanes of
@@ -1187,6 +1188,12 @@ struct ResetArgs {
   const Params* table;
   int n_types;
   int N, M, n_pool;
+  // t2d_set_agents: the slots K10 retired take their types back, and the per-row NoAction state starts fresh
+  uint8_t* agent_type_id;              // writable alias of type_id, or nullptr: no agents bound
+  uint8_t* agent_retired;              // [N][M], 255 = not retired
+  float* agent_last_pose;              // [N][Q][4]
+  int32_t* agent_noact_count;          // [N][Q]
+  int agent_q;
 };
 
 __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
@@ -1200,6 +1207,14 @@ __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
     A.x[i] = A.px[s]; A.y[i] = A.py[s]; A.h[i] = A.ph[s]; A.v[i] = A.pv[s];
     A.vx[i] = A.pvx ? A.pvx[s] : A.pv[s] * cosf(A.ph[s]);
     A.vy[i] = A.pvy ? A.pvy[s] : A.pv[s] * sinf(A.ph[s]);
+    if (A.agent_type_id != nullptr) {
+      const uint8_t rt = A.agent_retired[i];
+      if (rt != 0xff) { A.agent_type_id[i] = rt; A.agent_retired[i] = 0xff; }
+      for (int q = m; q < A.agent_q; q += A.M) {   // NoAction.reset of every row
+        A.agent_last_pose[4 * ((long long)n * A.agent_q + q) + 3] = 0.0f;
+        A.agent_noact_count[(long long)n * A.agent_q + q] = 0;
+      }
+    }
     if (A.wheel_f != nullptr) {
       float wf = 0.0f, wr = 0.0f;
       if (A.pool_wf != nullptr) {
@@ -1241,6 +1256,37 @@ struct EnvArgs {
   int N, M, max_step, reset_trackers;
 };
 
+// The reward chain of _get_reward (parking.py:148-190) for one scored participant: st its ScenarioStatus, ts its
+// TrafficStatus as check_status leaves it (only the collision detector sets it), step_count its scenario's tick count.
+// max_iou == nullptr skips the IoU term, min_dist == nullptr the progress term (target = the goal centre, (x, y) the
+// participant's position).  Out of line: the env epilogue and K10 run this one compiled copy, so that their rewards agree
+// bit for bit whatever the compiler would contract in an inlined copy.
+__device__ __noinline__ float reward_chain(int st, int ts, int step_count, int max_step, float iou, float* max_iou,
+                                           const float* target, float* min_dist, float x, float y) {
+  float r;
+  if (ts == 3 || ts == 4) r = -5.0f;                                             // :151-152 (+ dynamic collision, an extension)
+  else if (st == T2D_STATUS_TIME_EXCEEDED || st == T2D_STATUS_NO_ACTION) r = -1.0f;   // :153-157
+  else if (st == T2D_STATUS_OUT_BOUND) r = -5.0f;                                // :158-159
+  else if (st == T2D_STATUS_COMPLETED) r = 5.0f;                                 // :160-161
+  else {
+    r = max_step > 0 ? -tanhf((float)step_count / (float)max_step) * 0.001f : 0.0f;   // :163
+    if (max_iou != nullptr) {
+      const float best = *max_iou;
+      r += (best == -INFINITY) ? iou : iou - best;                                 // :164-169
+      *max_iou = fmaxf(best, iou);                                                 // :170
+    }
+    if (min_dist != nullptr) {
+      const float dx = x - target[0], dy = y - target[1];
+      const float d = sqrtf(dx * dx + dy * dy), best = *min_dist;                  // :172-185
+      if (d < best) {                                                              // :186-188 (inf on the first step: the
+        if (best != INFINITY) r += (best - d) * 0.1f;                              //  reference adds inf there; we add nothing)
+        *min_dist = d;
+      }
+    }
+  }
+  return r;
+}
+
 __global__ void __launch_bounds__(256) t2d_env_epilogue_kernel(const __grid_constant__ EnvArgs A) {
   const long long total = (long long)A.N * A.M;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -1255,27 +1301,10 @@ __global__ void __launch_bounds__(256) t2d_env_epilogue_kernel(const __grid_cons
     const int ego_ts = st == T2D_STATUS_FAILED ? ts : 1;
     const bool term = st == T2D_STATUS_COMPLETED;                                  // :243-244
     const bool trunc = !term && (st != T2D_STATUS_NORMAL || ego_ts != 1);          // :245-248
-    float r;
-    if (ego_ts == 3 || ego_ts == 4) r = -5.0f;                                     // :151-152 (+ dynamic collision, an extension)
-    else if (st == T2D_STATUS_TIME_EXCEEDED || st == T2D_STATUS_NO_ACTION) r = -1.0f;   // :153-157
-    else if (st == T2D_STATUS_OUT_BOUND) r = -5.0f;                                // :158-159
-    else if (st == T2D_STATUS_COMPLETED) r = 5.0f;                                 // :160-161
-    else {
-      r = A.max_step > 0 ? -tanhf((float)A.step_count[n] / (float)A.max_step) * 0.001f : 0.0f;   // :163
-      if (A.iou != nullptr && A.max_iou != nullptr) {
-        const float iou = A.iou[n], best = A.max_iou[n];
-        r += (best == -INFINITY) ? iou : iou - best;                               // :164-169
-        A.max_iou[n] = fmaxf(best, iou);                                           // :170
-      }
-      if (A.target != nullptr && A.min_dist != nullptr) {
-        const float dx = A.x[i] - A.target[5 * (long long)n], dy = A.y[i] - A.target[5 * (long long)n + 1];
-        const float d = sqrtf(dx * dx + dy * dy), best = A.min_dist[n];            // :172-185
-        if (d < best) {                                                            // :186-188 (inf on the first step: the
-          if (best != INFINITY) r += (best - d) * 0.1f;                            //  reference adds inf there; we add nothing)
-          A.min_dist[n] = d;
-        }
-      }
-    }
+    const bool scored_iou = A.iou != nullptr && A.max_iou != nullptr;
+    const float r = reward_chain(st, ego_ts, A.step_count[n], A.max_step, scored_iou ? A.iou[n] : 0.0f,
+                                 scored_iou ? A.max_iou + n : nullptr, A.target ? A.target + 5 * (long long)n : nullptr,
+                                 (A.target && A.min_dist) ? A.min_dist + n : nullptr, A.x[i], A.y[i]);
     A.reward[n] = r;
     if (A.terminated) A.terminated[n] = term;
     if (A.truncated) A.truncated[n] = trunc;
@@ -1284,6 +1313,107 @@ __global__ void __launch_bounds__(256) t2d_env_epilogue_kernel(const __grid_cons
       if (A.max_iou) A.max_iou[n] = -INFINITY;
       if (A.min_dist) A.min_dist[n] = INFINITY;
     }
+  }
+}
+
+// ---------------------------------------------------------------------------- K10 per-agent epilogue
+// DESIGN.md section 1 "Per-agent status and reward": the status chain, terminated / truncated and the reward chain of the
+// env epilogue for every row (n, q) of an observer list, retirement of the slots whose rows settle, and the done mask
+// "no row of the scenario is NORMAL".  One warp per scenario; lane l takes rows l, l + 32, l + 64, l + 96.
+struct AgentArgs {
+  // Arrival / NoAction go through K1's ego_goal_events, which reads its arrays from a StepArgs and indexes them by its
+  // second argument: here only the goal_* fields are set, to the per-row arrays, and the index is the row n·Q + q.  K1
+  // and K10 so run one compiled copy of the detectors (bit-exact agreement) and K1's code is untouched.
+  StepArgs g;                   // goal_target = goals [N][Q][5] or nullptr, goal_iou = iou [N][Q], goal_last_pose [N][Q][4],
+                                // goal_noact_count [N][Q], goal_threshold, goal_noact_max
+  const uint8_t* flags;         // [N][M] event byte of the tick
+  const int16_t* observers;     // [N][Q] or nullptr: row q is slot q
+  const float *x, *y, *h;       // [N][M] state after the tick
+  uint8_t* type_id;             // [N][M]: a settled row's slot becomes 255 ...
+  uint8_t* retired;             // [N][M]: ... and keeps its type here (255: not retired)
+  const int32_t* step_count;    // [N]
+  const Params* table;
+  float *max_iou, *min_dist;    // [N][Q] per-episode extrema
+  float* reward;                // [N][Q]
+  uint8_t *terminated, *truncated, *status;   // [N][Q]
+  uint8_t* done;                // [N]
+  uint8_t* traffic_status;      // [N][M] or nullptr
+  int N, M, Q, n_types, max_step, reset_trackers;
+};
+
+constexpr int K10_WARPS = 8;
+constexpr int K10_ROWS_PER_LANE = T2D_OBS_MAX_OBSERVERS / 32;   // Q <= 128
+
+__global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(const __grid_constant__ AgentArgs A) {
+  const int lane = threadIdx.x & 31;
+  const long long n = (long long)blockIdx.x * K10_WARPS + (threadIdx.x >> 5);
+  if (n >= A.N) return;   // whole warps
+  const long long s0 = n * A.M, r0 = n * A.Q;
+  if (A.traffic_status) {
+    for (int m = lane; m < A.M; m += 32) {
+      const unsigned f = A.flags[s0 + m];
+      A.traffic_status[s0 + m] = (f & T2D_F_STATIC) ? 3 : ((f & T2D_F_DYNAMIC) ? 4 : 1);
+    }
+  }
+  const int cnt = A.step_count[n];
+  const bool time_up = A.max_step > 0 && cnt > A.max_step;                     // parking.py:366-369
+  bool any_normal = false;
+  unsigned settle = 0;                                                          // bit k: row lane + 32 k retires its slot
+#pragma unroll 1
+  for (int k = 0; k < K10_ROWS_PER_LANE; ++k) {
+    const int q = lane + 32 * k;
+    if (q >= A.Q) break;
+    const long long r = r0 + q;
+    const int j = A.observers ? A.observers[r] : q;
+    const int t = (j >= 0 && j < A.M) ? A.type_id[s0 + j] : 0xff;
+    if (t >= A.n_types) {   // absent row
+      A.status[r] = 0; A.reward[r] = 0.0f; A.terminated[r] = 0; A.truncated[r] = 0; A.g.goal_iou[r] = 0.0f;
+      continue;
+    }
+    const long long i = s0 + j;
+    const float x = A.x[i], y = A.y[i];
+    const float* goal = A.g.goal_target ? A.g.goal_target + 5 * r : nullptr;
+    const bool has_goal = goal != nullptr && goal[0] == goal[0];
+    unsigned ev = 0;
+    float iou = 0.0f;
+    const Vec4 g2 = params_group(A.table + t, 2);   // (pose_l, pose_w, rbound, model | shape << 8)
+    // K1's condition for the ego: a solid box (pose tile: x not NaN, pose_w >= 0)
+    if (has_goal && x == x && (__float_as_int(g2.w) >> 8) != SHAPE_NONE && g2.y >= 0.0f) {
+      ev = ego_goal_events(A.g, r, x, y, A.h[i], g2.x, g2.y);   // writes goal_iou[r]
+      iou = A.g.goal_iou[r];
+    } else {
+      A.g.goal_iou[r] = 0.0f;
+    }
+    const unsigned f = A.flags[i];
+    int st = T2D_STATUS_NORMAL;                                                 // parking.py:366-390, lowest priority first
+    if (ev & 1u) st = T2D_STATUS_COMPLETED;
+    if (f & T2D_F_DYNAMIC) st = T2D_STATUS_FAILED;
+    if (f & T2D_F_STATIC) st = T2D_STATUS_FAILED;
+    if (f & T2D_F_OUTBOUND) st = T2D_STATUS_OUT_BOUND;
+    if (ev & 2u) st = T2D_STATUS_NO_ACTION;
+    if (time_up) st = T2D_STATUS_TIME_EXCEEDED;
+    const int ts = st == T2D_STATUS_FAILED ? ((f & T2D_F_STATIC) ? 3 : 4) : 1;
+    const bool term = st == T2D_STATUS_COMPLETED;
+    const bool trunc = !term && st != T2D_STATUS_NORMAL;
+    A.reward[r] = reward_chain(st, ts, cnt, A.max_step, iou, has_goal ? A.max_iou + r : nullptr, goal,
+                               has_goal ? A.min_dist + r : nullptr, x, y);
+    A.status[r] = (uint8_t)st; A.terminated[r] = term; A.truncated[r] = trunc;
+    any_normal = any_normal || st == T2D_STATUS_NORMAL;
+    if (st != T2D_STATUS_NORMAL) {   // retire the slot (duplicate rows store the same type)
+      settle |= 1u << k;
+      A.retired[i] = (uint8_t)t;
+    }
+  }
+  // every row has read its slot's type before any slot leaves type_id
+  const bool done = !__any_sync(0xffffffffu, any_normal);
+  if (lane == 0) A.done[n] = done;
+  __syncwarp();
+#pragma unroll 1
+  for (int k = 0; k < K10_ROWS_PER_LANE; ++k) {
+    const int q = lane + 32 * k;
+    if (q >= A.Q) break;
+    if (A.reset_trackers && done) { A.max_iou[r0 + q] = -INFINITY; A.min_dist[r0 + q] = INFINITY; }
+    if ((settle >> k) & 1u) A.type_id[s0 + (A.observers ? A.observers[r0 + q] : q)] = 0xff;
   }
 }
 
@@ -1942,7 +2072,16 @@ struct t2d_ctx {
   int32_t* goal_noact_count = nullptr;
   float goal_threshold = 0.95f;
   int goal_noact_max = 0;
-  bool use_pdl = true;             // T2D_PDL=0 disables programmatic dependent launch
+  // per-agent status and reward (t2d_set_agents / K10); agent_q == 0: not bound
+  int agent_q = 0;
+  const int16_t* agent_observers = nullptr;
+  const float* agent_goals = nullptr;
+  float agent_threshold = 0.95f;
+  int agent_noact_max = 0;
+  float* agent_last_pose = nullptr;
+  int32_t* agent_noact_count = nullptr;
+  uint8_t* agent_retired = nullptr;
+  bool use_pdl = true;            // T2D_PDL=0 disables programmatic dependent launch
   int prefetch_override = -1;      // T2D_PREFETCH=0 / 1 (experiments; -1 = on unless a done exchange is alive)
   int wpc_override = 0;            // T2D_WPC=w: warps per CTA of the tick (experiments; 0 = pick from the batch size)
   int grid_limit = 0;              // T2D_GRID_LIMIT=k: at most k CTAs of the persistent tick grid per SM (experiments; 0 = occupancy)
@@ -2869,6 +3008,49 @@ int t2d_env_epilogue(t2d_ctx* c, const uint8_t* flags, const uint8_t* scn_status
   return T2D_OK;
 }
 
+int t2d_set_agents(t2d_ctx* c, const int16_t* observers, int32_t n_observers, const float* goals, float arrival_threshold,
+                   int no_action_max_step, float* last_pose, int32_t* noact_count, uint8_t* retired_type) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!observers && n_observers == 0) {   // unbind
+    c->agent_q = 0; c->agent_observers = nullptr; c->agent_goals = nullptr;
+    c->agent_last_pose = nullptr; c->agent_noact_count = nullptr; c->agent_retired = nullptr;
+    return T2D_OK;
+  }
+  if (n_observers < 1 || n_observers > T2D_OBS_MAX_OBSERVERS) return fail(T2D_E_INVALID, "t2d_set_agents: n_observers must be in 1..128");
+  if (!observers && n_observers > c->M) return fail(T2D_E_INVALID, "t2d_set_agents: without observers row q is slot q (n_observers <= M)");
+  if (!last_pose || !noact_count || !retired_type) return fail(T2D_E_INVALID, "t2d_set_agents: NULL state array");
+  if (goals && !(arrival_threshold > 0.0f && arrival_threshold <= 1.0f)) return fail(T2D_E_INVALID, "arrival_threshold must be in (0, 1]");
+  c->agent_q = n_observers; c->agent_observers = observers; c->agent_goals = goals;
+  c->agent_threshold = arrival_threshold; c->agent_noact_max = no_action_max_step;
+  c->agent_last_pose = last_pose; c->agent_noact_count = noact_count; c->agent_retired = retired_type;
+  return T2D_OK;
+}
+
+int t2d_agents_epilogue(t2d_ctx* c, const uint8_t* flags, float* reward, uint8_t* terminated, uint8_t* truncated,
+                        uint8_t* agent_status, float* iou, uint8_t* done, float* max_iou, float* min_dist, uint8_t* traffic_status,
+                        int reset_trackers_on_done, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (c->agent_q == 0) return fail(T2D_E_STATE, "t2d_agents_epilogue: no agents bound: call t2d_set_agents first");
+  if (!flags || !reward || !terminated || !truncated || !agent_status || !iou || !done || !max_iou || !min_dist)
+    return fail(T2D_E_INVALID, "t2d_agents_epilogue: NULL array");
+  CUDA_TRY(cudaSetDevice(c->device));
+  AgentArgs A{};
+  A.g.goal_target = c->agent_goals; A.g.goal_iou = iou; A.g.goal_last_pose = c->agent_last_pose;
+  A.g.goal_noact_count = c->agent_noact_count; A.g.goal_threshold = c->agent_threshold; A.g.goal_noact_max = c->agent_noact_max;
+  A.flags = flags; A.observers = c->agent_observers; A.x = c->x; A.y = c->y; A.h = c->h;
+  A.type_id = const_cast<uint8_t*>(c->type_id); A.retired = c->agent_retired; A.step_count = c->step_count; A.table = c->d_table;
+  A.max_iou = max_iou; A.min_dist = min_dist; A.reward = reward; A.terminated = terminated; A.truncated = truncated;
+  A.status = agent_status; A.done = done; A.traffic_status = traffic_status;
+  A.N = c->N; A.M = c->M; A.Q = c->agent_q; A.n_types = c->n_types; A.max_step = c->cfg.max_step;
+  A.reset_trackers = reset_trackers_on_done ? 1 : 0;
+  t2d_agents_epilogue_kernel<<<(c->N + K10_WARPS - 1) / K10_WARPS, K10_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  g_launches.fetch_add(1);
+  CUDA_TRY(cudaGetLastError());
+  return T2D_OK;
+}
+
 int t2d_check_events(t2d_ctx* c, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment, void* stream) {
   return launch_step(c, nullptr, flags, hit_index, hit_segment, nullptr, nullptr, stream, 0);
 }
@@ -2890,6 +3072,10 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   A.wheel_f = c->wheel_f; A.wheel_r = c->wheel_r; A.pool_wf = c->reset_pool_wf; A.pool_wr = c->reset_pool_wr;
   A.last_accel = c->ctrl_last_accel; A.type_id = c->type_id; A.table = c->d_table; A.n_types = c->n_types;
   A.N = c->N; A.M = c->M; A.n_pool = n_pool;
+  if (c->agent_q > 0) {   // the bound type_id is the caller's writable device array (K10 retires slots in it)
+    A.agent_type_id = const_cast<uint8_t*>(c->type_id); A.agent_retired = c->agent_retired;
+    A.agent_last_pose = c->agent_last_pose; A.agent_noact_count = c->agent_noact_count; A.agent_q = c->agent_q;
+  }
   const long long total = (long long)c->N * c->M;
   const int grid = (int)std::min<long long>((total + 255) / 256, (long long)c->sm_count * 8);
   t2d_reset_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(A);

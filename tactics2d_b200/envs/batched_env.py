@@ -48,7 +48,8 @@ class BatchedTrafficEnv:
     def __init__(self, scene, device="cuda:0", max_step: int = 1000, step_size: int = 100, delta_t: int = 5,
                  any_participant: bool = False, auto_reset: bool = True, target=None, arrival_threshold: float = 0.95,
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
-                 bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None):
+                 bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
+                 agent_rewards: bool = False):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -64,11 +65,21 @@ class BatchedTrafficEnv:
         ``flat`` row of ``BatchedWorld.observe(**vector_obs)``, also computed after the auto-reset; ``vector_obs`` takes its
         keyword arguments ``k_agents``, ``k_segments``, ``agent_range``, ``segment_range``) or ``"agents"`` (fp32 [N, Q, F],
         the ``flat`` rows of ``BatchedWorld.observe_agents(**vector_obs)``, one per observer slot, for multi-agent control,
-        also computed after the auto-reset; ``vector_obs`` may then also hold ``observers`` and ``goals``)."""
+        also computed after the auto-reset; ``vector_obs`` may then also hold ``observers`` and ``goals``);
+        ``agent_rewards``: with ``observation="agents"``, score every observer row as an agent (``BatchedWorld.set_agents``
+        with the same ``observers`` / ``goals``, ``arrival_threshold`` and ``no_action_max_step``): ``step`` returns
+        ``[N, Q]`` reward / terminated / truncated, ``info`` adds ``agent_status`` and ``agent_iou``, a settled agent's slot
+        leaves the world until its scenario resets, and a scenario auto-resets when none of its agents is NORMAL.  The
+        per-row goals replace ``target``, which is then rejected."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
             raise ValueError(f"observation must be 'state', 'bev', 'vector' or 'agents', got {observation!r}")
+        if agent_rewards and observation != "agents":
+            raise ValueError("agent_rewards needs observation='agents' (its observer list names the agents)")
+        if agent_rewards and target is not None:
+            raise ValueError("agent_rewards takes per-row goals in vector_obs['goals'], not target")
+        self.agent_rewards = bool(agent_rewards)
         self.observation = observation
         self.vector_obs = dict(vector_obs or {})
         keys = {"k_agents", "k_segments", "agent_range", "segment_range"}
@@ -102,6 +113,9 @@ class BatchedTrafficEnv:
         self._rng = np.random.default_rng(0)
         if target is not None:
             self.world.set_goal(target, arrival_threshold, no_action_max_step)
+        if self.agent_rewards:
+            self.world.set_agents(self.vector_obs.get("observers"), self.vector_obs.get("goals"), arrival_threshold,
+                                  no_action_max_step)
         if observation == "bev":
             w, h = self.bev_resolution
             self.observation_space = {"shape": (n, h, w, 3), "dtype": "uint8", "low": 0, "high": 255}
@@ -140,6 +154,9 @@ class BatchedTrafficEnv:
         perm = None
         if options and options.get("shuffle"):
             perm = torch.from_numpy(self._rng.permutation(self.num_envs).astype(np.int32)).to(self.world.device)
+        if self.agent_rewards:   # every slot takes its pool row's type below; no retired type of the old episodes survives
+            self.world.retired_type.fill_(255)
+            self.world.reset_agent_trackers()
         if self.replay is not None and perm is not None:   # the rows' own types (the replayed slots' are rewritten anyway)
             self.world.type_id.copy_(self._type_id[perm.long()])
         else:
@@ -177,6 +194,14 @@ class BatchedTrafficEnv:
         if w.last_accel is not None:
             w.control(full)
         self.scenario_manager.update(full)
+        if self.agent_rewards:   # one K10 launch instead of the ego's epilogue; retired slots ignore their action rows
+            a = w.agents_epilogue(reset_trackers_on_done=self.scenario_manager.reset_trackers_on_done)
+            r = w.result
+            info = self._info(r.status, a.traffic, r.flags, r.hit_index, r.hit_segment)
+            info["agent_status"], info["agent_iou"] = a.status, a.iou
+            if self.auto_reset:
+                self.scenario_manager.reset(mask=a.done, pool_index=w.log_row)
+            return self._obs(), a.reward, a.terminated, a.truncated, info
         status, traffic = self.scenario_manager.check_status()
         e = self.scenario_manager.env_result
         r = w.result

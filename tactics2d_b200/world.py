@@ -50,6 +50,20 @@ class EnvResult:
     traffic_status: torch.Tensor  # uint8 [N, M] TrafficStatus codes
 
 
+@dataclass
+class AgentEnvResult:
+    """Device tensors written by ``agents_epilogue`` (views of buffers owned by the world, overwritten by its next call):
+    row (n, q) is the agent observed by slot ``observers[n, q]`` (DESIGN.md section 1 "Per-agent status and reward")."""
+
+    reward: torch.Tensor          # fp32 [N, Q]
+    terminated: torch.Tensor      # bool [N, Q]: the row's status is COMPLETED
+    truncated: torch.Tensor       # bool [N, Q]: active, not terminated, not NORMAL
+    status: torch.Tensor          # uint8 [N, Q] ScenarioStatus codes of the rows, 0 for absent rows
+    iou: torch.Tensor             # fp32 [N, Q]: IoU(pose, goal), 0 without the detectors
+    done: torch.Tensor            # uint8 [N]: no row of the scenario is NORMAL (the mask ``reset`` takes)
+    traffic: torch.Tensor         # uint8 [N, M] TrafficStatus codes
+
+
 # Columns of the blocks of the vector observation (``BatchedWorld.observe``; DESIGN.md section 1 "Vector observation").
 # Positions and velocities are in the ego frame: origin at the ego's centre, +x along its heading; dh = heading - ego heading.
 EGO_FIELDS = ("valid", "speed", "v_long", "v_lat", "half_len", "half_wid", "is_disc", "t_frac")
@@ -537,6 +551,62 @@ class BatchedWorld:
             e["max_iou"].fill_(-float("inf"))
             e["min_dist"].fill_(float("inf"))
 
+    # ------------------------------------------------------------------ per-agent status and reward
+    def set_agents(self, observers: Optional[torch.Tensor] = None, goals: Optional[torch.Tensor] = None,
+                   arrival_threshold: float = 0.95, no_action_max_step: int = 100):
+        """Score every row of an observer list as an agent (``t2d_set_agents``; DESIGN.md section 1 "Per-agent status and
+        reward").  ``observers``: int16 ``[N, Q]`` device tensor of slots, Q in 1..128 (a value outside ``[0, M)`` or an
+        empty slot gives an absent row; duplicates are allowed), or None for every slot (Q = M); ``goals``: fp32
+        ``[N, Q, 5]`` (cx, cy, heading, half_len, half_wid) per row, a NaN cx for none.  A row with a goal whose slot is a
+        box gets ``set_goal``'s Arrival / NoAction detectors.  The world owns the detector state, the retired types and the
+        outputs of ``agents_epilogue``; a settled row retires its slot (type 255) until ``reset`` restores it."""
+        Q = self._agent_rows(observers, goals)
+        f32, dev = torch.float32, self.device
+        self._agents = dict(
+            observers=observers, goals=goals, Q=Q,
+            last_pose=torch.zeros((self.N, Q, 4), dtype=f32, device=dev),
+            noact_count=torch.zeros((self.N, Q), dtype=torch.int32, device=dev),
+            retired_type=torch.full((self.N, self.M), TYPE_INACTIVE, dtype=torch.uint8, device=dev),
+            reward=torch.zeros((self.N, Q), dtype=f32, device=dev),
+            terminated=torch.zeros((self.N, Q), dtype=torch.bool, device=dev),
+            truncated=torch.zeros((self.N, Q), dtype=torch.bool, device=dev),
+            status=torch.zeros((self.N, Q), dtype=torch.uint8, device=dev),
+            iou=torch.zeros((self.N, Q), dtype=f32, device=dev),
+            done=torch.zeros(self.N, dtype=torch.uint8, device=dev),
+            traffic=torch.ones((self.N, self.M), dtype=torch.uint8, device=dev),
+            max_iou=torch.full((self.N, Q), -float("inf"), dtype=f32, device=dev),
+            min_dist=torch.full((self.N, Q), float("inf"), dtype=f32, device=dev))
+        a = self._agents
+        _lib.check(self.lib.t2d_set_agents(self._ctx, _ptr(observers), Q, _ptr(goals), float(arrival_threshold),
+                                           int(no_action_max_step), _ptr(a["last_pose"]), _ptr(a["noact_count"]),
+                                           _ptr(a["retired_type"])))
+
+    @property
+    def retired_type(self) -> Optional[torch.Tensor]:
+        """uint8 [N, M] device tensor: the type of every slot an agent row retired, 255 elsewhere (None without agents)."""
+        a = getattr(self, "_agents", None)
+        return None if a is None else a["retired_type"]
+
+    def agents_epilogue(self, reset_trackers_on_done: bool = True) -> AgentEnvResult:
+        """Status, reward, terminated, truncated and IoU of every agent row of the last tick, retirement of the slots whose
+        rows settled, and the scenarios' done mask (no row NORMAL), in ONE launch (``t2d_agents_epilogue``).  With one row
+        per scenario on slot 0 and the ``set_goal`` target as its goal this is ``env_epilogue`` bit for bit."""
+        a = getattr(self, "_agents", None)
+        if a is None:
+            raise RuntimeError("call set_agents before agents_epilogue")
+        _lib.check(self.lib.t2d_agents_epilogue(
+            self._ctx, _ptr(self._out.flags), _ptr(a["reward"]), _ptr(a["terminated"]), _ptr(a["truncated"]), _ptr(a["status"]),
+            _ptr(a["iou"]), _ptr(a["done"]), _ptr(a["max_iou"]), _ptr(a["min_dist"]), _ptr(a["traffic"]),
+            1 if reset_trackers_on_done else 0, self._stream()))
+        return AgentEnvResult(a["reward"], a["terminated"], a["truncated"], a["status"], a["iou"], a["done"], a["traffic"])
+
+    def reset_agent_trackers(self):
+        """Forget every agent row's best IoU / distance of the previous episodes (``reset_env_trackers`` per row)."""
+        a = getattr(self, "_agents", None)
+        if a is not None:
+            a["max_iou"].fill_(-float("inf"))
+            a["min_dist"].fill_(float("inf"))
+
     def check_events(self) -> StepResult:
         """The detectors on the current poses, no physics (``EventBase.update``)."""
         o = self._out
@@ -678,19 +748,9 @@ class BatchedWorld:
                                         _ptr(obs.segment_index), self._stream()))
         return obs
 
-    def observe_agents(self, k_agents: int = 16, k_segments: int = 32, agent_range: float = 50.0,
-                       segment_range: float = 30.0, observers: Optional[torch.Tensor] = None,
-                       goals: Optional[torch.Tensor] = None) -> AgentObservation:
-        """``observe`` from the point of view of a list of observer slots per scenario, in one launch
-        (``t2d_observe_agents``; DESIGN.md section 1 "Per-agent vector observation").  ``observers``: int16 ``[N, Q]``
-        device tensor of slots, Q in 1..128 (a value outside ``[0, M)`` or an empty slot gives an absent row; duplicates
-        are allowed), or None for every slot (Q = M).  The agents of a row are the nearest other slots, slot 0 included.
-        ``goals``: fp32 ``[N, Q, 5]`` (cx, cy, heading, half_len, half_wid) per row, a NaN cx for none; without it the rows
-        observed by slot 0 take the ``set_goal`` target and the others none.  A row observed by slot 0 without ``goals``
-        equals ``observe``'s row.  The tensors are views of one buffer per ``(k_agents, k_segments, Q)`` that the next call
-        with those counts reuses."""
-        K, S = int(k_agents), int(k_segments)
-        # observers / goals reach the kernel as raw pointers: a host tensor, a wrong dtype or shape would be read out of bounds
+    def _agent_rows(self, observers, goals) -> int:
+        """Q of an observer list (M without one), after checking ``observers`` / ``goals``: they reach the kernels as raw
+        pointers, and a host tensor, a wrong dtype or shape would be read out of bounds."""
         if observers is None:
             Q = self.M
         else:
@@ -704,6 +764,21 @@ class BatchedWorld:
             if (not torch.is_tensor(goals) or goals.device != self.device or goals.dtype != torch.float32
                     or tuple(goals.shape) != (self.N, Q, 5) or not goals.is_contiguous()):
                 raise ValueError(f"goals must be a contiguous fp32 [{self.N}, {Q}, 5] tensor on {self.device}")
+        return Q
+
+    def observe_agents(self, k_agents: int = 16, k_segments: int = 32, agent_range: float = 50.0,
+                       segment_range: float = 30.0, observers: Optional[torch.Tensor] = None,
+                       goals: Optional[torch.Tensor] = None) -> AgentObservation:
+        """``observe`` from the point of view of a list of observer slots per scenario, in one launch
+        (``t2d_observe_agents``; DESIGN.md section 1 "Per-agent vector observation").  ``observers``: int16 ``[N, Q]``
+        device tensor of slots, Q in 1..128 (a value outside ``[0, M)`` or an empty slot gives an absent row; duplicates
+        are allowed), or None for every slot (Q = M).  The agents of a row are the nearest other slots, slot 0 included.
+        ``goals``: fp32 ``[N, Q, 5]`` (cx, cy, heading, half_len, half_wid) per row, a NaN cx for none; without it the rows
+        observed by slot 0 take the ``set_goal`` target and the others none.  A row observed by slot 0 without ``goals``
+        equals ``observe``'s row.  The tensors are views of one buffer per ``(k_agents, k_segments, Q)`` that the next call
+        with those counts reuses."""
+        K, S = int(k_agents), int(k_segments)
+        Q = self._agent_rows(observers, goals)
         cache = self.__dict__.setdefault("_agent_obs_out", {})
         obs = cache.get((K, S, Q))
         if obs is None:
