@@ -50,6 +50,11 @@
  *                        participants and nearest map segments of every scenario's ego
  *   t2d_observe_agents   (no reference counterpart) the same observation seen from a list of observer slots per scenario,
  *                        for multi-agent control
+ *   t2d_set_agents / t2d_agents_epilogue
+ *                        (no reference counterpart) status, reward and retirement of every agent row of an observer list
+ *   t2d_scatter_agent_action
+ *                        (no reference counterpart) one action per agent row, written into its slot of the action array
+ *   t2d_step_host_agents (no reference counterpart) the multi-agent step for a caller whose buffers live in host memory
  *
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types cross the ABI;
@@ -460,6 +465,37 @@ int t2d_set_agents(t2d_ctx* ctx, const int16_t* observers, int32_t n_observers, 
 int t2d_agents_epilogue(t2d_ctx* ctx, const uint8_t* flags, float* reward, uint8_t* terminated, uint8_t* truncated,
                         uint8_t* agent_status, float* iou, uint8_t* done, float* max_iou, float* min_dist,
                         uint8_t* traffic_status, int reset_trackers_on_done, void* stream);
+
+/* ---- per-agent action (no reference counterpart) ---------------------------------------------------------------------
+ * DESIGN.md section 1 "Per-agent action".  agent_action DEVICE fp32 [N][Q][2], one action per row of an observer list
+ * (observers DEVICE int16 [N][Q], Q = n_observers in 1..T2D_OBS_MAX_OBSERVERS, or NULL for slot q in row q, Q <= M), in
+ * the world's action order.  K11: for slot m of scenario n, let q* be the LOWEST q with observers[n][q] == m; when q*
+ * exists and type_id[n][m] < n_types, action[n][m] = agent_action[n][q*] (the fp32 bits as they are).  Nothing else is
+ * written: slots no row names, rows out of range, rows whose slot is empty or retired, and duplicate rows after the first
+ * leave action as it was.  Call it before t2d_control: a slot with a controller then takes its controller's action, and
+ * the controllers see the agents' own accelerations in last_accel.  While t2d_set_ego_action is bound, slot 0 still
+ * takes the ego action in t2d_control and t2d_step.  Needs no t2d_set_agents.  Rejected without a launch: n_observers
+ * outside 1..128, observers == NULL with n_observers > M, a NULL or not 8-byte aligned agent_action / action
+ * (T2D_E_INVALID), state not bound (T2D_E_STATE).  One launch, no allocation, no synchronisation: capturable in a CUDA
+ * graph. */
+int t2d_scatter_agent_action(t2d_ctx* ctx, const int16_t* observers /* DEVICE [N][Q] or NULL */, int32_t n_observers,
+                             const float* agent_action /* DEVICE [N][Q][2] */, float* action /* DEVICE [N][M][2] */,
+                             void* stream);
+/* One multi-agent step for a caller whose policy lives on the host: the counterpart of t2d_step_host_ego for the agents
+ * bound with t2d_set_agents (their observer list and Q).  Copies agent_action_host HOST [N][Q][2] (pinned memory
+ * recommended) into a device staging buffer with one host->device copy on `stream` (reallocated when Q changes, freed by
+ * t2d_destroy), scatters it into the caller's DEVICE action [N][M][2] with K11, runs t2d_control when controllers are
+ * set, the tick (log replay and drift as usual) and K10,
+ * copies reward (fp32), terminated, truncated, agent status (uint8; [N][Q] each) and done ([N]) back in ONE device->host
+ * copy and synchronises `stream`: the host arrays are valid on return.  flags [N][M], hit_index, hit_segment: DEVICE,
+ * any may be NULL (K10 then reads the library's own flags).  max_iou / min_dist: DEVICE [N][Q], the per-episode extrema
+ * of t2d_agents_epilogue.  Host outputs may be NULL, except done_host.  No reset inside the call.  Rejected without a
+ * launch: a NULL context, agent_action_host, action, max_iou, min_dist or done_host, an action that is not 8-byte
+ * aligned (T2D_E_INVALID), state not bound or no agents bound (T2D_E_STATE). */
+int t2d_step_host_agents(t2d_ctx* ctx, const float* agent_action_host /* HOST [N][Q][2] */, float* action /* DEVICE [N][M][2] */,
+                         uint8_t* flags, int16_t* hit_index, int16_t* hit_segment, float* max_iou, float* min_dist,
+                         int reset_trackers_on_done, float* reward_host, uint8_t* terminated_host, uint8_t* truncated_host,
+                         uint8_t* agent_status_host, uint8_t* done_host, void* stream);
 
 /* ---- done-mask exchange across the GPUs of one node, over peer memory (NVLink / NVSwitch) -------------------------
  * Scenarios are sharded across ranks (one process per GPU); the one exchange of the path is "every rank learns every

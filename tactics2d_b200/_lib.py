@@ -83,6 +83,8 @@ SYMBOLS = {
     "t2d_set_goal": (C.c_int, [_P, _P, C.c_float, C.c_int, _P, _P, _P]),
     "t2d_set_agents": (C.c_int, [_P, _P, C.c_int32, _P, C.c_float, C.c_int, _P, _P, _P]),
     "t2d_agents_epilogue": (C.c_int, [_P] + [_P] * 10 + [C.c_int, _P]),
+    "t2d_scatter_agent_action": (C.c_int, [_P, _P, C.c_int32, _P, _P, _P]),
+    "t2d_step_host_agents": (C.c_int, [_P] + [_P] * 7 + [C.c_int] + [_P] * 6),
     "t2d_reset": (C.c_int, [_P, _P, _P, C.c_int] + [_P] * 7),
     "t2d_lidar_scan": (C.c_int, [_P, C.c_int, C.c_float, _P, _P, _P]),
     "t2d_set_bev_styles": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int]),

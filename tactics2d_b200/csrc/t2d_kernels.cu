@@ -12,6 +12,7 @@
 // K8  t2d_obs_kernel       the ego-frame vector observation (t2d_obs.cuh).
 // K9  t2d_obs_agents_kernel the same observation from a list of observer slots per scenario (t2d_obs.cuh).
 // K10 t2d_agents_epilogue_kernel status, reward and retirement of every agent row of an observer list.
+// K11 t2d_agent_action_kernel    the action of every agent row of an observer list, scattered to its slot.
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory.
 //
 // Work decomposition of K1: a scenario (M <= 128 participants) is owned by a group of G lanes of
@@ -1417,6 +1418,62 @@ __global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(con
   }
 }
 
+// ---------------------------------------------------------------------------- K11 per-agent action
+// DESIGN.md section 1 "Per-agent action": slot m of scenario n takes row q* of agent_action, the lowest q with
+// observers[n][q] == m, when its type is active; nothing else is written.  One warp per scenario; lane l takes rows l,
+// l + 32, l + 64, l + 96 and claims their slots with atomicMin on a per-slot owner in shared memory, so the first row
+// wins whatever the order of the atomics.  Then one float2 copy per owned active slot (the fp32 bits as they are).
+struct ActionArgs {
+  const int16_t* observers;     // [N][Q] or nullptr: row q is slot q
+  const float* agent_action;    // [N][Q][2]
+  float* action;                // [N][M][2]
+  const uint8_t* type_id;       // [N][M]
+  int N, M, Q, n_types;
+};
+
+constexpr int K11_WARPS = 8;
+
+__global__ void __launch_bounds__(K11_WARPS * 32) t2d_agent_action_kernel(const __grid_constant__ ActionArgs A) {
+  __shared__ int s_owner[K11_WARPS][T2D_MAX_PARTICIPANTS];
+  const int lane = threadIdx.x & 31;
+  const long long n = (long long)blockIdx.x * K11_WARPS + (threadIdx.x >> 5);
+  if (n >= A.N) return;   // whole warps
+  const long long s0 = n * A.M, r0 = n * A.Q;
+  constexpr int K = T2D_MAX_PARTICIPANTS / 32;   // = T2D_OBS_MAX_OBSERVERS / 32: rows and slots per lane
+  // every independent load first: the observer and type loads of a lane are in flight together
+  int slot[K];
+  unsigned type[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const int q = lane + 32 * k, m = q;
+    slot[k] = q < A.Q ? (A.observers ? (int)A.observers[r0 + q] : q) : -1;
+    type[k] = m < A.M ? A.type_id[s0 + m] : 0xffu;
+  }
+  int* owner = s_owner[threadIdx.x >> 5];
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+    if (lane + 32 * k < A.M) owner[lane + 32 * k] = A.Q;   // Q: no row names the slot
+  __syncwarp();
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+    if (slot[k] >= 0 && slot[k] < A.M) atomicMin(&owner[slot[k]], lane + 32 * k);
+  __syncwarp();
+  const float2* src = reinterpret_cast<const float2*>(A.agent_action) + r0;
+  float2* dst = reinterpret_cast<float2*>(A.action) + s0;
+  float2 val[K];
+  bool put[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) {   // all loads, then all stores (the two arrays may alias as far as the compiler knows)
+    const int m = lane + 32 * k;
+    const int q = m < A.M ? owner[m] : A.Q;
+    put[k] = q < A.Q && type[k] < (unsigned)A.n_types;
+    if (put[k]) val[k] = src[q];
+  }
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+    if (put[k]) dst[lane + 32 * k] = val[k];
+}
+
 // ---------------------------------------------------------------------------- K3
 // ---------------------------------------------------------------------------- drift pre-pass
 // SingleTrackDrift participants of a tick, one per thread, before K1 (which then only builds their pose).
@@ -2108,6 +2165,14 @@ struct t2d_ctx {
   cudaStream_t hs_copy = nullptr;
   cudaEvent_t hs_begin = nullptr, hs_chunk[MAX_HOST_CHUNKS] = {};
   int host_chunks = 0;                 // 0 = pick from the batch size
+  // t2d_step_host_agents: device staging of the agents' actions, the packed outputs reward | terminated | truncated |
+  // status | done on the device and their pinned mirror, K10's iou, and the flags K10 needs when the caller keeps none;
+  // sized for ha_q rows per scenario
+  int ha_q = 0;
+  float* ha_action = nullptr;          // [N][Q][2]
+  uint8_t* ha_out = nullptr;           // [N][Q] fp32 reward, [3][N][Q] uint8, [N] uint8 done, then [N][Q] fp32 iou
+  uint8_t* ha_out_pinned = nullptr;    // pinned mirror of the part up to done
+  uint8_t* ha_flags = nullptr;         // [N][M]
   // BEV observation (t2d_set_bev_styles / t2d_bev_render)
   std::vector<int> tile_nseg;          // segments of every tile of the current map, in tile order
   int n_bev_styles = 0;                // 0: styles not set
@@ -2212,6 +2277,10 @@ int t2d_destroy(t2d_ctx* c) {
   if (c->hs_ego_pinned) cudaFreeHost(c->hs_ego_pinned);
   if (c->hs_out) cudaFree(c->hs_out);
   if (c->hs_out_pinned) cudaFreeHost(c->hs_out_pinned);
+  if (c->ha_action) cudaFree(c->ha_action);
+  if (c->ha_out) cudaFree(c->ha_out);
+  if (c->ha_out_pinned) cudaFreeHost(c->ha_out_pinned);
+  if (c->ha_flags) cudaFree(c->ha_flags);
   if (c->hs_begin) cudaEventDestroy(c->hs_begin);
   for (cudaEvent_t e : c->hs_chunk)
     if (e) cudaEventDestroy(e);
@@ -2736,16 +2805,25 @@ static int pick_wpc(long long tiles, int sm_count) {
 
 // Launches K1 over the scenarios [first, first + count) of the bound state; the per-participant / per-scenario
 // pointers passed in (action, flags, ..., done) address scenario `first` already.
+// The call-order checks of a tick with physics (a caller that launches other kernels first runs them up front).
+static int check_tick_state(const t2d_ctx* c) {
+  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (c->has_drift && !(c->wheel_f && c->wheel_r))
+    return fail(T2D_E_STATE, "the type table holds a SingleTrackDrift row: call t2d_bind_wheel_state first");
+  if (c->has_log && c->log_type_id != c->type_id)
+    return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+  return T2D_OK;
+}
+
 static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment,
                        uint8_t* scn_status, uint8_t* done, void* stream, int do_physics, int first = 0, int count = -1) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
   if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
   if (do_physics && !action) return fail(T2D_E_INVALID, "action is NULL");
-  if (do_physics && c->has_drift && !(c->wheel_f && c->wheel_r))
-    return fail(T2D_E_STATE, "the type table holds a SingleTrackDrift row: call t2d_bind_wheel_state first");
-  if (do_physics && c->has_log && c->log_type_id != c->type_id)
-    return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+  if (do_physics)
+    if (int r = check_tick_state(c)) return r;
   CUDA_TRY(cudaSetDevice(c->device));
   if (count < 0) count = c->N - first;
   if (first < 0 || count <= 0 || first + count > c->N) return fail(T2D_E_INVALID, "scenario range out of bounds");
@@ -3048,6 +3126,92 @@ int t2d_agents_epilogue(t2d_ctx* c, const uint8_t* flags, float* reward, uint8_t
   t2d_agents_epilogue_kernel<<<(c->N + K10_WARPS - 1) / K10_WARPS, K10_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
   g_launches.fetch_add(1);
   CUDA_TRY(cudaGetLastError());
+  return T2D_OK;
+}
+
+static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+
+// K11 over the bound state's type ids; the caller has checked the arguments
+static int launch_agent_action(t2d_ctx* c, const int16_t* observers, int Q, const float* agent_action, float* action,
+                               void* stream) {
+  CUDA_TRY(cudaSetDevice(c->device));
+  ActionArgs A{};
+  A.observers = observers; A.agent_action = agent_action; A.action = action; A.type_id = c->type_id;
+  A.N = c->N; A.M = c->M; A.Q = Q; A.n_types = c->n_types;
+  t2d_agent_action_kernel<<<(c->N + K11_WARPS - 1) / K11_WARPS, K11_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  g_launches.fetch_add(1);
+  CUDA_TRY(cudaGetLastError());
+  return T2D_OK;
+}
+
+int t2d_scatter_agent_action(t2d_ctx* c, const int16_t* observers, int32_t n_observers, const float* agent_action,
+                             float* action, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (n_observers < 1 || n_observers > T2D_OBS_MAX_OBSERVERS)
+    return fail(T2D_E_INVALID, "t2d_scatter_agent_action: n_observers must be in 1..128");
+  if (!observers && n_observers > c->M)
+    return fail(T2D_E_INVALID, "t2d_scatter_agent_action: without an observer list n_observers must not exceed the slots per scenario");
+  if (!agent_action || !action) return fail(T2D_E_INVALID, "t2d_scatter_agent_action: agent_action / action is NULL");
+  if (!aligned8(agent_action) || !aligned8(action))
+    return fail(T2D_E_INVALID, "t2d_scatter_agent_action: agent_action and action must be 8-byte aligned");
+  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  return launch_agent_action(c, observers, n_observers, agent_action, action, stream);
+}
+
+int t2d_step_host_agents(t2d_ctx* c, const float* agent_action_host, float* action, uint8_t* flags, int16_t* hit_index,
+                         int16_t* hit_segment, float* max_iou, float* min_dist, int reset_trackers_on_done, float* reward_host,
+                         uint8_t* terminated_host, uint8_t* truncated_host, uint8_t* agent_status_host, uint8_t* done_host,
+                         void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!agent_action_host || !action || !max_iou || !min_dist || !done_host)
+    return fail(T2D_E_INVALID, "t2d_step_host_agents: agent_action / action / max_iou / min_dist / done is NULL");
+  if (!aligned8(action)) return fail(T2D_E_INVALID, "t2d_step_host_agents: action must be 8-byte aligned");
+  if (int r = check_tick_state(c)) return r;
+  if (c->agent_q == 0) return fail(T2D_E_STATE, "t2d_step_host_agents: no agents bound: call t2d_set_agents first");
+  CUDA_TRY(cudaSetDevice(c->device));
+  const int N = c->N, M = c->M, Q = c->agent_q;
+  const size_t nq = (size_t)N * Q;
+  const size_t out_bytes = 7 * nq + N;                   // reward, terminated, truncated, status, done
+  const size_t iou_off = (out_bytes + 15) & ~(size_t)15;
+  if (c->ha_q != Q) {   // (re)size the staging for the bound Q
+    if (c->ha_action) { cudaFree(c->ha_action); c->ha_action = nullptr; }
+    if (c->ha_out) { cudaFree(c->ha_out); c->ha_out = nullptr; }
+    if (c->ha_out_pinned) { cudaFreeHost(c->ha_out_pinned); c->ha_out_pinned = nullptr; }
+    c->ha_q = 0;
+    CUDA_TRY(cudaMalloc(&c->ha_action, nq * 2 * sizeof(float)));
+    CUDA_TRY(cudaMalloc(&c->ha_out, iou_off + nq * sizeof(float)));
+    CUDA_TRY(cudaMallocHost(&c->ha_out_pinned, out_bytes));
+    c->ha_q = Q;
+  }
+  if (!flags && !c->ha_flags) CUDA_TRY(cudaMalloc(&c->ha_flags, (size_t)N * M));
+  uint8_t* fl = flags ? flags : c->ha_flags;
+  float* d_reward = reinterpret_cast<float*>(c->ha_out);
+  uint8_t* d_term = c->ha_out + 4 * nq;
+  uint8_t* d_trunc = d_term + nq;
+  uint8_t* d_status = d_trunc + nq;
+  uint8_t* d_done = d_status + nq;
+  float* d_iou = reinterpret_cast<float*>(c->ha_out + iou_off);
+  // One copy-engine transfer of the actions, as t2d_step_host (from pinned caller memory it is a DMA; pageable memory
+  // goes through the driver's staging).  Staging them in mapped host memory for K11 to read over PCIe, as
+  // t2d_step_host_ego does with its 8 N bytes, made the whole call about 1.5x slower at 2 MiB (DESIGN.md section 7).
+  cudaStream_t s = (cudaStream_t)stream;
+  CUDA_TRY(cudaMemcpyAsync(c->ha_action, agent_action_host, nq * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
+  if (int r = launch_agent_action(c, c->agent_observers, Q, c->ha_action, action, stream)) return r;
+  if (c->d_ctab)
+    if (int r = t2d_control(c, action, stream)) return r;
+  if (int r = launch_step(c, action, fl, hit_index, hit_segment, nullptr, nullptr, stream, 1)) return r;
+  if (int r = t2d_agents_epilogue(c, fl, d_reward, d_term, d_trunc, d_status, d_iou, d_done, max_iou, min_dist, nullptr,
+                                  reset_trackers_on_done, stream))
+    return r;
+  CUDA_TRY(cudaMemcpyAsync(c->ha_out_pinned, c->ha_out, out_bytes, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  const uint8_t* h = c->ha_out_pinned;
+  if (reward_host) memcpy(reward_host, h, 4 * nq);
+  if (terminated_host) memcpy(terminated_host, h + 4 * nq, nq);
+  if (truncated_host) memcpy(truncated_host, h + 5 * nq, nq);
+  if (agent_status_host) memcpy(agent_status_host, h + 6 * nq, nq);
+  memcpy(done_host, h + 7 * nq, (size_t)N);
   return T2D_OK;
 }
 

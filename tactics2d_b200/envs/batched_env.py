@@ -49,7 +49,7 @@ class BatchedTrafficEnv:
                  any_participant: bool = False, auto_reset: bool = True, target=None, arrival_threshold: float = 0.95,
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
-                 agent_rewards: bool = False):
+                 agent_rewards: bool = False, agent_actions: bool = False):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -70,16 +70,22 @@ class BatchedTrafficEnv:
         with the same ``observers`` / ``goals``, ``arrival_threshold`` and ``no_action_max_step``): ``step`` returns
         ``[N, Q]`` reward / terminated / truncated, ``info`` adds ``agent_status`` and ``agent_iou``, a settled agent's slot
         leaves the world until its scenario resets, and a scenario auto-resets when none of its agents is NORMAL.  The
-        per-row goals replace ``target``, which is then rejected."""
+        per-row goals replace ``target``, which is then rejected;
+        ``agent_actions``: with ``observation="agents"``, ``step`` takes one (steering, accel) per observer row, ``[N, Q,
+        2]``, and scatters it on the device into the slots the rows observe (``BatchedWorld.scatter_agent_action``; the
+        lowest row naming a slot wins, empty and retired slots take nothing)."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
             raise ValueError(f"observation must be 'state', 'bev', 'vector' or 'agents', got {observation!r}")
         if agent_rewards and observation != "agents":
             raise ValueError("agent_rewards needs observation='agents' (its observer list names the agents)")
+        if agent_actions and observation != "agents":
+            raise ValueError("agent_actions needs observation='agents' (its observer list names the agents)")
         if agent_rewards and target is not None:
             raise ValueError("agent_rewards takes per-row goals in vector_obs['goals'], not target")
         self.agent_rewards = bool(agent_rewards)
+        self.agent_actions = bool(agent_actions)
         self.observation = observation
         self.vector_obs = dict(vector_obs or {})
         keys = {"k_agents", "k_segments", "agent_range", "segment_range"}
@@ -127,6 +133,9 @@ class BatchedTrafficEnv:
         else:
             self.observation_space = {"shape": (n, m, 6), "dtype": "float32"}
         self.action_space = {"shape": (n, 2), "low": (-np.inf, -np.inf), "high": (np.inf, np.inf)}
+        if self.agent_actions:
+            obs = self.vector_obs.get("observers")
+            self.action_space["shape"] = (n, m if obs is None else int(obs.shape[1]), 2)
 
     # ------------------------------------------------------------------ helpers
     def _obs(self):
@@ -177,9 +186,22 @@ class BatchedTrafficEnv:
 
         Launches per call: the controllers (if set), the fused tick, the env epilogue (reward / terminated / truncated /
         TrafficStatus / done in one kernel) and the masked reset - no elementwise PyTorch.  The tensors in the returned
-        tuple and in ``info`` are views of buffers owned by the env: they hold this step's values until the next ``step``."""
+        tuple and in ``info`` are views of buffers owned by the env: they hold this step's values until the next ``step``.
+
+        With ``agent_actions``: ``action`` is exactly ``[N, Q, 2]``, one (steering, accel) per observer row, scattered into
+        the internal action array by one more launch in front of the controllers; ``npc_action`` [N, M, 2] optionally
+        fills that array first (the slots no agent row drives keep its rows)."""
         w = self.world
-        if action.dim() == 3:
+        if self.agent_actions:
+            if tuple(action.shape) != self.action_space["shape"]:
+                raise InvalidAction(f"Action of shape {tuple(action.shape)} is not in the action space.")
+            full = self._action
+            if npc_action is not None:
+                full.copy_(npc_action)
+            w.set_ego_action(None)
+            w.scatter_agent_action(action.to(device=w.device, dtype=full.dtype).contiguous(), full,
+                                   self.vector_obs.get("observers"))
+        elif action.dim() == 3:
             if tuple(action.shape) != (self.num_envs, self.num_participants, 2):
                 raise InvalidAction(f"Action of shape {tuple(action.shape)} is not in the action space.")
             full = action.contiguous()

@@ -607,6 +607,64 @@ class BatchedWorld:
             a["max_iou"].fill_(-float("inf"))
             a["min_dist"].fill_(float("inf"))
 
+    # ------------------------------------------------------------------ per-agent action
+    def _device_action(self, name: str, t, rows: int) -> torch.Tensor:
+        # the tensor reaches the kernel as a raw pointer: a host tensor, a wrong dtype or shape would be read out of bounds
+        if (not torch.is_tensor(t) or t.device != self.device or t.dtype != torch.float32
+                or tuple(t.shape) != (self.N, rows, 2) or not t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous fp32 [{self.N}, {rows}, 2] tensor on {self.device}")
+        return t
+
+    def scatter_agent_action(self, agent_action: torch.Tensor, action: torch.Tensor,
+                             observers: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Write one action per agent row into its slot of ``action`` [N, M, 2] (IN PLACE; ``t2d_scatter_agent_action``,
+        DESIGN.md section 1 "Per-agent action").  ``agent_action``: fp32 ``[N, Q, 2]`` device tensor in the world's action
+        order; ``observers``: int16 ``[N, Q]`` as in ``observe_agents`` (None: row q is slot q, Q <= M).  Slot m takes the
+        row of the lowest q naming it, when its type is active; every other row of ``action`` keeps its value.  Call it
+        before ``control`` and ``step``: a controlled slot then takes its controller's action, and a bound ego action
+        still drives slot 0."""
+        Q = self._agent_rows(observers, None)
+        self._device_action("agent_action", agent_action, Q)
+        self._device_action("action", action, self.M)
+        _lib.check(self.lib.t2d_scatter_agent_action(self._ctx, _ptr(observers), Q, _ptr(agent_action), _ptr(action),
+                                                     self._stream()))
+        return action
+
+    def step_host_agents(self, agent_action, action: Optional[torch.Tensor] = None, reset_trackers_on_done: bool = True):
+        """One multi-agent step for a host-side policy (``t2d_step_host_agents``): ``agent_action`` is a float32
+        ``[N, Q, 2]`` NumPy array or CPU tensor, one action per row of the agents bound with ``set_agents``.  It is
+        scattered into the DEVICE array ``action`` [N, M, 2] (default: an internal zero array, as ``step_host_ego``), then
+        the controllers (if set), the tick and ``agents_epilogue`` run, and the outputs come back in one copy.  Returns
+        ``(reward, terminated, truncated, status, done)`` as NumPy arrays ([N, Q] fp32 / bool / bool / uint8 and [N] uint8):
+        views of buffers owned by the world that hold their values until the next call.  The flags and hit indices stay on
+        the device in ``self.result``; the per-row extrema are those of ``agents_epilogue``, so the two may be mixed.  No
+        reset happens inside the call."""
+        a_ = getattr(self, "_agents", None)
+        if a_ is None:
+            raise RuntimeError("call set_agents before step_host_agents")
+        Q = a_["Q"]
+        a = agent_action if isinstance(agent_action, torch.Tensor) else torch.from_numpy(
+            np.ascontiguousarray(agent_action, dtype=np.float32))
+        if a.device.type != "cpu" or a.dtype != torch.float32 or tuple(a.shape) != (self.N, Q, 2) or not a.is_contiguous():
+            raise ValueError(f"agent_action must be a contiguous float32 host array [{self.N}, {Q}, 2]")
+        if action is None:
+            action = getattr(self, "_npc_action", None)
+            if action is None:
+                action = self._npc_action = torch.zeros((self.N, self.M, 2), dtype=torch.float32, device=self.device)
+        self._device_action("action", action, self.M)
+        hb = getattr(self, "_host_agents", None)
+        if hb is None or hb[0].shape[1] != Q:
+            hb = self._host_agents = (np.empty((self.N, Q), np.float32), np.empty((self.N, Q), np.bool_),
+                                      np.empty((self.N, Q), np.bool_), np.empty((self.N, Q), np.uint8),
+                                      np.empty(self.N, np.uint8))
+        o = self._out
+        _lib.check(self.lib.t2d_step_host_agents(
+            self._ctx, a.data_ptr(), _ptr(action), _ptr(o.flags), _ptr(o.hit_index), _ptr(o.hit_segment),
+            _ptr(a_["max_iou"]), _ptr(a_["min_dist"]), 1 if reset_trackers_on_done else 0,
+            *(h.ctypes.data for h in hb), self._stream()))
+        self.frame += self.interval
+        return hb
+
     def check_events(self) -> StepResult:
         """The detectors on the current poses, no physics (``EventBase.update``)."""
         o = self._out
