@@ -90,8 +90,9 @@ struct StepArgs {
   int map_bytes, map_in_smem;
   int n_types;
   int N, M, G;                     // G = lanes per scenario
-  int g_shift, mp_shift, ext, n_tiles, wpc, table_bytes;   // launch-shape constants (see the kernel prologue)
-  int off_poseA, off_poseB, off_hit, off_queue, off_posx, off_posy, off_qcount, off_bar;   // shared-memory carve
+  int g_shift, mp_shift, unused1, n_tiles, wpc, table_bytes;   // launch-shape constants (see the kernel prologue)
+  int off_poseA, off_poseB, off_hit, off_queue, off_sorted, unused0, off_qcount, off_bar;   // shared-memory carve
+  // (unused0, unused1: free slots that keep the parameter layout the drift pre-pass shares with K1)
   int n_steps;
   float dt, dt_rem;
   double dt_d, dt_rem_d, interval_d;   // the same steps in double (dynamics / point mass run in fp64)
@@ -270,11 +271,12 @@ __device__ __forceinline__ Pose load_pose(const float4* poseA, const float4* pos
 }
 
 constexpr int QCAP = 192;   // per-warp queue: candidate pairs, then static participants (0..127) + undecided segments (128..191)
-constexpr int POS_EXT_PER_WARP = 768;   // circularly extended x / y arrays: (32 / G) x EXT floats per warp, EXT = 1.5 MP + 16 rounded up to 4
 
 // Exact test of one candidate pair (tile indices ti, tj of the same scenario); a hit is recorded for both
-// ends as the minimum partner index (scenario-local), which is what "first hit in list order" means.
-__device__ __noinline__ void pair_resolve(int ti, int tj, int mp_shift, const float4* poseA, const float4* poseB, int* hitmin) {
+// ends as the minimum partner index (scenario-local), which is what "first hit in list order" means.  Inlined into the
+// drain: an out-of-line call taking the poses by value made every draining lane spill around an ABI call; only the rare
+// fp64 fallback (pair_exact) stays out of line, keeping its register footprint out of the kernel.
+__device__ __forceinline__ void pair_resolve(int ti, int tj, int mp_shift, const float4* poseA, const float4* poseB, int* hitmin) {
   const Pose a = load_pose(poseA, poseB, ti), b = load_pose(poseA, poseB, tj);
   if (pair_hit(a, b)) {
     const int mask = (1 << mp_shift) - 1;
@@ -283,113 +285,49 @@ __device__ __noinline__ void pair_resolve(int ti, int tj, int mp_shift, const fl
   }
 }
 
-// One word of the partner loop = IPW iterations x PPL own participants x 2 partners.  X / Y: the word's 2 * IPW partner
-// positions; nx / ny: the lane's own positions, negated; nthr: minus the squared broadphase reach.  The margin of a
-// pair, d^2 - thr, is <= 0 for a candidate; a NaN position (empty slot) gives a NaN margin, which neither the minimum nor
-// the comparison picks up.  FIRST: word 0, where the combinations with partner offset <= 0 (the lane's own participants
-// and pairs owned by the other end) are left out at compile time.
-constexpr int IPW = 16 / PPL;   // iterations per 32-bit word (2 * PPL bits each)
-
-// The margins of one own participant against the partners of iteration uu (2 uu and 2 uu + 1): two adds and two fused
-// multiply-adds each.  The two chains are interleaved step by step; written one margin after the other, the same
-// operations get a different schedule from ptxas.
-__device__ __forceinline__ void pair_margins(const float (&X)[2 * IPW], const float (&Y)[2 * IPW], int uu, float nx, float ny,
-                                             float nthr, float& d0, float& d1) {
-  const float dx0 = X[2 * uu] + nx, dx1 = X[2 * uu + 1] + nx;
-  const float dy0 = Y[2 * uu] + ny, dy1 = Y[2 * uu + 1] + ny;
-  const float e0 = fmaf(dy0, dy0, nthr), e1 = fmaf(dy1, dy1, nthr);
-  d0 = fmaf(dx0, dx0, e0);
-  d1 = fmaf(dx1, dx1, e1);
-}
-
-template <bool FIRST>
-__device__ __forceinline__ float pair_word_min(const float (&X)[2 * IPW], const float (&Y)[2 * IPW], const float (&nx)[PPL],
-                                               const float (&ny)[PPL], const float (&nthr)[PPL]) {
-  float m = INFINITY;
-#pragma unroll
-  for (int uu = 0; uu < IPW; ++uu) {
-#pragma unroll
-    for (int i = 0; i < PPL; ++i) {
-      const bool v0 = !FIRST || (2 * uu - i >= 1), v1 = !FIRST || (2 * uu + 1 - i >= 1);
-      if (!v0 && !v1) continue;
-      float d0, d1;
-      pair_margins(X, Y, uu, nx[i], ny[i], nthr[i], d0, d1);
-      if (v0 && v1) m = fminf(m, fminf(d0, d1));
-      else if (v0) m = fminf(m, d0);
-      else m = fminf(m, d1);
-    }
-  }
-  return m;
-}
-
-// The verdict bits of a word whose minimum margin was <= 0: bit ((uu * PPL + i) * 2 + e), the same margins recomputed.
-template <bool FIRST>
-__device__ __forceinline__ unsigned pair_word_bits(const float (&X)[2 * IPW], const float (&Y)[2 * IPW], const float (&nx)[PPL],
-                                                   const float (&ny)[PPL], const float (&nthr)[PPL]) {
-  unsigned bits = 0;
-#pragma unroll
-  for (int uu = 0; uu < IPW; ++uu) {
-#pragma unroll
-    for (int i = 0; i < PPL; ++i) {
-      const bool v0 = !FIRST || (2 * uu - i >= 1), v1 = !FIRST || (2 * uu + 1 - i >= 1);
-      if (!v0 && !v1) continue;
-      float d0, d1;
-      pair_margins(X, Y, uu, nx[i], ny[i], nthr[i], d0, d1);
-      if (v0 && d0 <= 0.0f) bits |= 1u << ((uu * PPL + i) * 2);
-      if (v1 && d1 <= 0.0f) bits |= 2u << ((uu * PPL + i) * 2);
-    }
-  }
-  return bits;
-}
-
-// Minus the squared broadphase reach of an own participant of bounding radius rb: conservative, since any partner's
-// bounding radius is <= rb_max.  The per-lane sweep and the compacted sweep form it from the same floats.
+// Minus the squared broadphase reach of an owner of bounding radius rb: conservative, since any partner's bounding
+// radius is <= rb_max.
 __device__ __forceinline__ float neg_reach2(float rb, float rb_max) {
   const float rr = rb + rb_max;
   return -fmaf(rr * rr, 1.00001f, 1e-12f);
 }
 
-// Box (xmin, xmax, ymin, ymax) of the 8 extended slots x[0..7], y[0..7] (16-byte aligned) a partner word reads.  A slot
-// whose x is NaN (non-solid, empty) is left out, its y too; an all-NaN window gives the empty box (+inf, -inf, +inf, -inf).
-__device__ __forceinline__ float4 window_box(const float* x, const float* y) {
-  float4 b = make_float4(INFINITY, -INFINITY, INFINITY, -INFINITY);
-#pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    const float4 xv = reinterpret_cast<const float4*>(x)[q], yv = reinterpret_cast<const float4*>(y)[q];
-    const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, ys[4] = {yv.x, yv.y, yv.z, yv.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float yk = xs[k] == xs[k] ? ys[k] : __int_as_float(0x7fc00000);
-      b.x = fminf(b.x, xs[k]); b.y = fmaxf(b.y, xs[k]);   // (fminf / fmaxf return the other operand for a NaN)
-      b.z = fminf(b.z, yk); b.w = fmaxf(b.w, yk);
-    }
+// Order-preserving map of a float (not NaN) to uint32 and back: a < b  <=>  f2ord(a) < f2ord(b) (-0 sorts before +0).
+__device__ __forceinline__ unsigned f2ord(float f) {
+  const unsigned u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float ord2f(unsigned o) { return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o); }
+
+// One entry of a scenario's x-sorted list (the tick's broadphase): position, minus the squared reach (neg_reach2) and
+// the sort key as bits; the key's low 7 bits are the participant's slot in its scenario.
+// The exact broadphase test of one pair {a, b} of a scenario: the circular enumeration's owner is the end from which the
+// other lies at circular offset 1 .. Mh (Mh = M / 2; at even M the pair at offset M / 2 is owned by BOTH ends, each
+// testing it with its own reach).  The margin d^2 - thr of owner o against partner r is fma(dx, dx, fma(dy, dy, -thr_o))
+// with dx = fl(x_r - x_o), dy = fl(y_r - y_o): for the other orientation fl(x_o - x_r) = -dx exactly, so both squares are
+// shared.  A pair whose owner's margin is <= 0 goes on the warp's queue as (owner, partner) tile indices; when the queue
+// is full the count keeps growing, and the caller then falls back to the exhaustive pass.  No function call may appear in
+// here: it is inlined into the scan loop, and a CALL makes the compiler keep only callee-saved registers live across it.
+__device__ __forceinline__ void sweep_pair(const float4& a, const float4& b, int tb, int M, int Mh, unsigned* queue, int* qcount) {
+  const int sa = (int)(__float_as_uint(a.w) & 127u), sb = (int)(__float_as_uint(b.w) & 127u);
+  int d = sb - sa;   // circular offset of b from a (the slots differ: 1 .. M - 1)
+  if (d < 0) d += M;
+  const float dx = b.x - a.x, dy = b.y - a.y;
+  if (d <= Mh && fmaf(dx, dx, fmaf(dy, dy, a.z)) <= 0.0f) {
+    const int slot = atomicAdd(qcount, 1);
+    if (slot < QCAP) queue[slot] = ((unsigned)(tb + sa) << 16) | (unsigned)(tb + sb);
   }
-  return b;
+  if (d >= M - Mh && fmaf(dx, dx, fmaf(dy, dy, b.z)) <= 0.0f) {
+    const int slot = atomicAdd(qcount, 1);
+    if (slot < QCAP) queue[slot] = ((unsigned)(tb + sb) << 16) | (unsigned)(tb + sa);
+  }
 }
 
-// Broadphase slow path.  `bits` holds the distance-test verdicts of four partner-loop iterations of this lane:
-// bit ((uu * PPL + i) * 2 + e) = own participant m0 + i against extended slot m0 + 2 (u_base + uu) + e.  Keep the
-// combinations whose partner offset q is 1..Mh (every unordered pair once; q <= 0 are the lane's own participants
-// or pairs owned by the other end) and push them on the warp's queue.
-__device__ __forceinline__ void pair_enqueue_bits(unsigned bits, int u_base, int t0, int tb, int m0, int M, int Mh,
-                                                  unsigned* queue, int* qcount) {
-  while (bits) {
-    const int b = __ffs(bits) - 1;
-    bits &= bits - 1;
-    const int e = b & 1, i = (b >> 1) & (PPL - 1), uu = (b >> 1) / PPL;   // PPL is a power of two
-    const int u = u_base + uu;
-    const int q = 2 * u + e - i;
-    if (q < 1 || q > Mh) continue;
-    int pj = m0 + 2 * u + e;          // < 2.5 M: at most two wraps
-    if (pj >= M) pj -= M;
-    if (pj >= M) pj -= M;
-    const int tj = tb + pj;
-    // No function call may appear in this loop: a CALL makes the compiler keep only callee-saved registers
-    // live across it and rematerialise everything else in every iteration of the partner loop.  When the
-    // queue is full the count keeps growing; the caller then falls back to the exhaustive pass.
-    const int slot = atomicAdd(qcount, 1);
-    if (slot < QCAP) queue[slot] = ((unsigned)(t0 + i) << 16) | (unsigned)tj;
-  }
+// The smallest margin a pair can have under any owner's reach (nglob = neg_reach2(rb_max, rb_max) <= every -thr, and the
+// margin is monotone in -thr): > 0 rules out a candidate in both orientations.  NaN positions give NaN, which fminf drops.
+__device__ __forceinline__ float pair_min_margin(const float4& a, const float4& b, float nglob) {
+  const float dx = b.x - a.x, dy = b.y - a.y;
+  return fmaf(dx, dx, fmaf(dy, dy, nglob));
 }
 
 // Dense-scene fallback (the candidate queue overflowed): every lane resolves all pairs of its own participants
@@ -411,7 +349,7 @@ __device__ __noinline__ void pair_exhaustive(int t0, int tb, int m0, int M, int 
 
 // Static level 2 for ONE participant (tile index ti), run by one lane: walk the grid cells under the bounding
 // circle, fp32-filtered segment test per listed segment, keep the lowest hit.  No function call in here (see
-// pair_enqueue_bits): a segment the filter cannot decide is pushed on the exact queue (entries QX0 .. QCAP-1
+// sweep_pair): a segment the filter cannot decide is pushed on the exact queue (entries QX0 .. QCAP-1
 // of the warp's queue, counter qcount) and decided after the loop; if that queue is full the participant is
 // marked (returns -2) for the out-of-line exact walk.
 constexpr int QX0 = 128;   // first exact-queue entry (entries below hold the compacted participant list)
@@ -651,8 +589,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
   float4* s_poseB = reinterpret_cast<float4*>(smem + A.off_poseB);
   int* s_hit = reinterpret_cast<int*>(smem + A.off_hit);
   unsigned* s_queue = reinterpret_cast<unsigned*>(smem + A.off_queue);
-  float* s_posx = reinterpret_cast<float*>(smem + A.off_posx);
-  float* s_posy = reinterpret_cast<float*>(smem + A.off_posy);
+  float4* s_sorted = reinterpret_cast<float4*>(smem + A.off_sorted);
   int* s_qcount = reinterpret_cast<int*>(smem + A.off_qcount);
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem + A.off_bar);
 
@@ -702,11 +639,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
   int* qcount = s_qcount + warp;
   const int tb = sub * MP, t0 = tb + m0;
   const int mp_shift = A.mp_shift;   // MP = 1 << mp_shift
-  // circularly extended positions of this scenario: slot k holds participant k mod M, so the partner loop reads
-  // consecutive slots (two per 64-bit load) without wrap-around logic
-  const int EXT = A.ext;   // (3 MP) / 2 + 16 >= (MP - PPL) + 2 * (partner pairs rounded up to whole words)
-  float* posx = s_posx + warp * POS_EXT_PER_WARP + sub * EXT;
-  float* posy = s_posy + warp * POS_EXT_PER_WARP + sub * EXT;
+  float4* sorted = s_sorted + warp * POSE_PER_WARP + tb;   // this scenario's x-sorted list (sweep_pair)
   const int Mh = M >> 1;                // partner offsets 1..Mh cover every unordered pair
 
   const int n_tiles = A.n_tiles;
@@ -880,22 +813,6 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       poseA[i * 32 + lane] = make_float4(px[i], py[i], rb[i], shd[i]);
       poseB[i * 32 + lane] = make_float4(ch[i], sh[i], g2.x, g2.y);
     }
-    // circularly extended positions: slot k holds participant k mod M, i.e. this lane's PPL participants go to
-    // m0 .. m0 + PPL - 1 and to the copies M and 2 M further on that still fit
-    if (m0 < M) {
-      if (nvalid == PPL && (M & (PPL - 1)) == 0) {   // whole, aligned groups: one vector store per copy
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const int k = m0 + c * M;
-          if (k < EXT) { st_vec<float, PPL>(posx + k, px); st_vec<float, PPL>(posy + k, py); }
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < PPL; ++i)
-          if (m0 + i < M)
-            for (int k = m0 + i; k < EXT; k += M) { posx[k] = px[i]; posy[k] = py[i]; }
-      }
-    }
     if (lane == 0) *qcount = 0;
     __syncwarp();
     // the step counter of the status section: fetched here - behind the state stores, so it cannot be hoisted to the top
@@ -925,133 +842,114 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
     }
 
     // ------------------------------------------------------------------ dynamic collision
-    // Every unordered pair once: participant i tests partners (i+1 .. i+M/2) mod M.  A lane walks the
-    // partners of its PPL participants together (one 128-bit pose load per partner, PPL distance tests);
-    // candidates (rare) go to the out-of-line narrowphase.  A confirmed hit is recorded for both ends:
-    // locally for i, by atomicMin in shared memory for the partner.
+    // Broadphase: every unordered pair of a scenario is tested in the orientation(s) of the circular enumeration - owner i,
+    // partner (i + 1 .. i + M/2) mod M (sweep_pair) - but only the pairs that can be candidates are enumerated: the group
+    // sorts its scenario's slots by x and each sorted entry is paired with the entries after it up to the reach.
+    // Candidates (rare) go on the warp's queue; after the sweep all 32 lanes drain it (narrowphase), recording a hit for
+    // both ends by atomicMin in shared memory on the scenario-local partner index.
     int hit[PPL];
     {
-      // hot loop: every lane runs it (idle slots hold NaN and never pass); branch-free; two partners per
-      // iteration.  Per pair the margin d^2 - thr is formed by two fused multiply-adds
-      // and folded into a running minimum over the 32 tests of a word; only a
-      // word whose minimum is <= 0 (rare) recomputes its verdict bits and goes to the out-of-line enqueue.
-      float nx[PPL], ny[PPL], nthr[PPL];
+      // (1) Sort.  Key of slot m0 + i: f2ord(x) with its low 7 bits replaced by the slot (MP <= 128), so the keys are
+      // distinct and one unsigned min / max moves key and payload together; a non-solid or padding slot (x NaN) takes
+      // 0xffffff80 | slot, above every solid key.  Bitonic network over element e = 4 gl + k of the group: strides 1
+      // and 2 are compare-exchanges inside the lane, larger strides __shfl_xor_sync inside the group (the group's lanes
+      // are aligned to G, so lane ^ j stays in it).  A tie in x is ordered by slot, which the scan below does not need.
+      unsigned key[PPL];
 #pragma unroll
-      for (int i = 0; i < PPL; ++i) {
-        nx[i] = -px[i];
-        ny[i] = -py[i];
-        nthr[i] = neg_reach2(rb[i], A.rb_max);
-      }
-      // partner pairs u = 0 .. U-1 cover offsets -(PPL-1) .. >= Mh; U is rounded up to whole words (the extended
-      // arrays are long enough), so the word body has no bounds test and its loads can be issued back to back
-      const int n_words = Mh > 0 ? (((Mh + PPL + 1) >> 1) + IPW - 1) / IPW : 0;
-      // one word = 2 * IPW consecutive partners: 128-bit loads (every scenario's window and m0 are 16-byte aligned)
-      auto load_word = [&](const float* wx, const float* wy, float (&X)[2 * IPW], float (&Y)[2 * IPW]) {
-#pragma unroll
-        for (int q = 0; q < IPW / 2; ++q) {
-          const float4 xv = reinterpret_cast<const float4*>(wx)[q], yv = reinterpret_cast<const float4*>(wy)[q];
-          X[4 * q] = xv.x; X[4 * q + 1] = xv.y; X[4 * q + 2] = xv.z; X[4 * q + 3] = xv.w;
-          Y[4 * q] = yv.x; Y[4 * q + 1] = yv.y; Y[4 * q + 2] = yv.z; Y[4 * q + 3] = yv.w;
-        }
+      for (int i = 0; i < PPL; ++i)
+        key[i] = (px[i] == px[i] ? (f2ord(px[i]) & ~127u) : 0xffffff80u) | (unsigned)(m0 + i);
+      auto cx = [&](int a, int b, bool desc) {
+        const unsigned lo = min(key[a], key[b]), hi = max(key[a], key[b]);
+        key[a] = desc ? hi : lo;
+        key[b] = desc ? lo : hi;
       };
-      // Box cull of words 1 .. n_words-1.  In an ordered scene most of them hold no partner within reach of any of the
-      // lane's participants, but nearly every warp has SOME lane that needs each word, so skipping words per warp never
-      // fires.  Instead every lane tests its own box against the box of each word's 8 partner slots, and the (lane, word)
-      // items that survive are compacted into a per-warp list that all 32 lanes sweep together.
-      //
-      // Why a culled word holds no candidate.  Let own participant i and partner j have the margin
-      // d = fma(dx, dx, fma(dy, dy, -thr)) <= 0, dx = fl(Xj - px_i), dy = fl(Yj - py_i), as the sweep computes it.  A NaN
-      // operand makes d NaN and an infinite dx or dy makes it +inf or NaN, so everything below is finite.  (a) Rounding is
-      // monotone and every v >= 2^-149 rounds to >= 2^-149 > 0, so d <= 0 means dx^2 + e < 2^-149 for e = fl(dy^2 - thr)
-      // >= -thr (thr is a float); likewise e < 2^-149 means dy^2 - thr < 2^-149.  Hence |dx|, |dy| < sqrt(thr) + 2^-74.
-      // (b) dx rounds the exact Xj - px_i with relative error 2^-24 (absolute 2^-150 among subnormals), so
-      // |Xj - px_i| < (sqrt(thr) + 2^-74)(1 + 2^-23) + 2^-149, and the same for y.  (c) thr = fl(fl(rr^2) * 1.00001f +
-      // 1e-12f), rr = fl(rb_i + rb_max), so sqrt(thr) <= rr * 1.0000051 * (1 + 2^-24) + 1.0000001e-6 and the bound of (b)
-      // is below D = rr * 1.0000054 + 1.1e-6.  (d) The lane box [lx0, lx1] x [ly0, ly1] is the exact min / max of the
-      // lane's positions whose x is not NaN, and the window box that of the word's 8 slots (window_box), so
-      // px_i - Xj >= lx0 - wx1 exactly.  The test rounds that difference once: g = fl(lx0 - wx1) > T with T a float
-      // implies lx0 - wx1 > T exactly (monotone rounding again), so no coordinate-dependent slack enters - at |x| = 1e4
-      // as at the origin - and T = fl(fma(max_i rr_i, 1.0001f, 1e-5f)) >= rr * 1.0000999 + 0.99e-5 > D.  So a word culled
-      // by any of the four sides has |Xj - px_i| > D or |Yj - py_i| > D for each of its 32 pairs: no candidate.  A NaN
-      // or infinite operand of the test (empty boxes against each other, inf - inf) makes a comparison false, i.e. keeps
-      // the word, which is always allowed; an empty lane or window box (+inf - finite) culls it, correctly.
-      //
-      // The window boxes live in the warp's queue area and the item list in its hit-minimum area: nothing is queued
-      // before the sweep (the table is dead once the list is built, and a __syncwarp separates the two), and the hit
-      // minima are first written after the sweep.
-      int n_items = 0;
-      uint8_t* items = reinterpret_cast<uint8_t*>(hitmin);   // (uw - 1) << 5 | lane: at most 32 x 8 bytes (M <= 128)
-      if (n_words > 1) {   // (M is uniform: so is n_words)
-        // window j of a scenario = extended slots 4 j .. 4 j + 7: lane gl, word uw reads window gl + 2 uw.  With M <= 4 G,
-        // n_words - 1 <= G / 4, so the 32 / G scenarios of a warp hold at most 32 / G x 1.5 G = 48 boxes = QCAP words.
-        const int wstride = G + 2 * (n_words - 1);
-        float4* wbox = reinterpret_cast<float4*>(queue) + sub * wstride;
-        for (int j = gl; j < wstride; j += G) wbox[j] = window_box(posx + 4 * j, posy + 4 * j);
-        float lx0 = INFINITY, lx1 = -INFINITY, ly0 = INFINITY, ly1 = -INFINITY, rr_max = 0.0f;
-#pragma unroll
-        for (int i = 0; i < PPL; ++i) {
-          const float yk = px[i] == px[i] ? py[i] : __int_as_float(0x7fc00000);
-          lx0 = fminf(lx0, px[i]); lx1 = fmaxf(lx1, px[i]); ly0 = fminf(ly0, yk); ly1 = fmaxf(ly1, yk);
-          rr_max = fmaxf(rr_max, rb[i] + A.rb_max);
-        }
-        const float reach = fmaf(rr_max, 1.0001f, 1e-5f);
-        __syncwarp();
-        for (int uw = 1; uw < n_words; ++uw) {
-          const float4 b = wbox[gl + 2 * uw];
-          const bool need = !(lx0 - b.y > reach || b.x - lx1 > reach || ly0 - b.w > reach || b.z - ly1 > reach);
-          const unsigned m = __ballot_sync(0xffffffffu, need);
-          if (need) items[n_items + __popc(m & ((1u << lane) - 1u))] = (uint8_t)(((uw - 1) << 5) | lane);
-          n_items += __popc(m);
-        }
-        __syncwarp();
-      }
-      if (n_words > 0) {   // word 0 also meets the lane's own participants (offset <= 0): those tests are compiled out
-        float X[2 * IPW], Y[2 * IPW];
-        load_word(posx + m0, posy + m0, X, Y);
-        if (pair_word_min<true>(X, Y, nx, ny, nthr) <= 0.0f) {
-          const unsigned bits = pair_word_bits<true>(X, Y, nx, ny, nthr);
-          if (bits) pair_enqueue_bits(bits, 0, t0, tb, m0, M, Mh, queue, qcount);
-        }
-      }
-      if ((n_items + 31) >> 5 < n_words - 1) {
-        // the list takes fewer warp passes than every lane sweeping all its words: an item reloads its owner's positions
-        // and reach from the pose tile; margins, verdict bits and queue entries are the per-lane sweep's, in another order
-        // (the narrowphase's atomicMin does not depend on it, and overflow is decided on the same count)
-        for (int k = lane; k < n_items; k += 32) {
-          const unsigned it = items[k];
-          const int ol = (int)(it & 31u), uw = (int)(it >> 5) + 1;
-          const int osub = ol >> A.g_shift, om0 = (ol & (G - 1)) * PPL, otb = osub * MP;
-          float onx[PPL], ony[PPL], onthr[PPL];
+      cx(0, 1, false); cx(2, 3, true);   // sorted runs of 2, alternating in direction (element bit 1)
+      for (int S = PPL; S <= MP; S <<= 1) {           // merge into sorted runs of S (the last one, S = MP, ascending)
+        const bool desc = (gl & (S >> 2)) != 0;       // element bit log2(S) = lane bit log2(S / 4)
+        for (int j = S >> 3; j > 0; j >>= 1) {        // element stride 4 j = lane stride j
+          const bool keep_max = ((gl & j) != 0) != desc;
 #pragma unroll
           for (int i = 0; i < PPL; ++i) {
-            const float4 a = poseA[i * 32 + ol];
-            onx[i] = -a.x;
-            ony[i] = -a.y;
-            onthr[i] = neg_reach2(a.z, A.rb_max);
-          }
-          const int off = osub * EXT + om0 + uw * 2 * IPW;
-          float X[2 * IPW], Y[2 * IPW];
-          load_word(s_posx + warp * POS_EXT_PER_WARP + off, s_posy + warp * POS_EXT_PER_WARP + off, X, Y);
-          if (pair_word_min<false>(X, Y, onx, ony, onthr) <= 0.0f) {
-            const unsigned bits = pair_word_bits<false>(X, Y, onx, ony, onthr);
-            if (bits) pair_enqueue_bits(bits, uw * IPW, otb + om0, otb, om0, M, Mh, queue, qcount);
+            const unsigned o = __shfl_xor_sync(0xffffffffu, key[i], j);
+            key[i] = keep_max ? max(key[i], o) : min(key[i], o);
           }
         }
-      } else {
-        // unordered scenes: nearly every word is needed, and the lanes sweep their own words from registers
-        for (int uw = 1; uw < n_words; ++uw) {
-          float X[2 * IPW], Y[2 * IPW];
-          load_word(posx + m0 + uw * 2 * IPW, posy + m0 + uw * 2 * IPW, X, Y);
-          if (pair_word_min<false>(X, Y, nx, ny, nthr) <= 0.0f) {
-            const unsigned bits = pair_word_bits<false>(X, Y, nx, ny, nthr);
-            if (bits) pair_enqueue_bits(bits, uw * IPW, t0, tb, m0, M, Mh, queue, qcount);
-          }
+        cx(0, 2, desc); cx(1, 3, desc); cx(0, 1, desc); cx(2, 3, desc);
+      }
+      // (2) Stage the sorted list: entry 4 gl + k = (x, y, -thr, key) of the slot the key names, from the pose tile.
+      float4 own[PPL];
+#pragma unroll
+      for (int i = 0; i < PPL; ++i) {
+        const float4 a = poseA[pslot(tb + (int)(key[i] & 127u))];
+        own[i] = make_float4(a.x, a.y, neg_reach2(a.z, A.rb_max), __uint_as_float(key[i]));
+        sorted[m0 + i] = own[i];
+      }
+      __syncwarp();
+      // (3) Scan.  Entry p is paired with every entry q > p of its scenario up to the first q whose bucket floor
+      // lo_q = ord2f(key_q & ~127) satisfies fl(lo_q - xmax) > T, where xmax >= x_p (the max over the lane's own entries)
+      // and T = fl(fma(2 rb_max, 1.0001f, 1e-5f)).
+      //
+      // Why no pair beyond the stop is a candidate, in either orientation.  Let owner o, partner r have the margin
+      // fma(dx, dx, fma(dy, dy, -thr_o)) <= 0 with dx = fl(x_r - x_o), as sweep_pair computes it.  A NaN or infinite
+      // operand makes the margin NaN or +inf, so both positions are finite.  (a) Rounding is monotone and every
+      // v >= 2^-149 rounds to >= 2^-149 > 0, so the margin <= 0 means dx^2 + e < 2^-149 for e = fl(dy^2 - thr_o) >= -thr_o
+      // (thr_o is a float): |dx| < sqrt(thr_o) + 2^-74.  (b) dx rounds the exact x_r - x_o with relative error 2^-24
+      // (absolute 2^-150 among subnormals), so |x_r - x_o| < (sqrt(thr_o) + 2^-74)(1 + 2^-23) + 2^-149.  (c) thr_o =
+      // fl(fl(rr^2) * 1.00001f + 1e-12f) with rr = fl(rb_o + rb_max) <= 2 rb_max (exact doubling, monotone rounding), so
+      // sqrt(thr_o) <= rr * 1.0000051 * (1 + 2^-24) + 1.0000001e-6 and |x_r - x_o| < D = 2 rb_max * 1.0000054 + 1.1e-6,
+      // whichever end owns the pair.  (d) T >= (2 rb_max * 1.0001f + 1e-5f)(1 - 2^-24) > D.  (e) The keys are sorted, so
+      // for q' >= q the bucket floors are ordered, lo_q' >= lo_q, and x_q' >= lo_q' (f2ord is monotone and clearing low
+      // bits only lowers it); every own p has x_p <= xmax.  A stop with fl(lo_q - xmax) > T means lo_q - xmax > T exactly
+      // (T is a float and rounding is monotone), so x_q' - x_p > T > D: no candidate, at any coordinate magnitude.  A NaN
+      // test stops the scan too; that happens only when lo_q is NaN (q non-solid, so are all later entries; or x_q = -inf,
+      // whose bucket holds no finite x, so every own x is -inf as well) or when lo_q = xmax = +inf: in each case every
+      // remaining pair has a non-finite position.  An own entry that is not solid has x NaN, which fmaxf leaves out; a
+      // lane with no solid entry has xmax NaN and stops at once (its own pairs have NaN margins).
+      //
+      // The pairs enumerated are each unordered pair of sorted ranks {p < q} at most once (by the lane holding p), and
+      // sweep_pair decides owner and margin exactly as the circular sweep does, so the queue receives the same set of
+      // (owner, partner) entries - only in another order, which the atomicMin drain does not see - and an overflow
+      // triggers on the same count.  At C2 (64 participants over 200 m of x, T = 5.65 m) an entry has about 1.8
+      // x-neighbours within T, so a lane scans its 6 own pairs and one group of 4 entries beyond them.
+      const float T = fmaf(2.0f * A.rb_max, 1.0001f, 1e-5f);
+      const float nglob = neg_reach2(A.rb_max, A.rb_max);
+      const float xmax = fmaxf(fmaxf(own[0].x, own[1].x), fmaxf(own[2].x, own[3].x));
+      {
+        float m = INFINITY;
+#pragma unroll
+        for (int a = 0; a < PPL; ++a)
+#pragma unroll
+          for (int b = a + 1; b < PPL; ++b) m = fminf(m, pair_min_margin(own[a], own[b], nglob));
+        if (m <= 0.0f) {
+#pragma unroll
+          for (int a = 0; a < PPL; ++a)
+#pragma unroll
+            for (int b = a + 1; b < PPL; ++b) sweep_pair(own[a], own[b], tb, M, Mh, queue, qcount);
         }
       }
-      __syncwarp();   // the item list is dead: the hit minima take its place
+      if (xmax == xmax) {
+        for (int q0 = m0 + PPL; q0 < MP; q0 += PPL) {   // four entries per round, loaded together (MP is a multiple of 4)
+          float4 e[PPL];
+#pragma unroll
+          for (int k = 0; k < PPL; ++k) e[k] = sorted[q0 + k];
+          bool stop = false;
+#pragma unroll
+          for (int k = 0; k < PPL; ++k) {
+            if (!(ord2f(__float_as_uint(e[k].w) & ~127u) - xmax <= T)) { stop = true; break; }
+            float m = INFINITY;
+#pragma unroll
+            for (int a = 0; a < PPL; ++a) m = fminf(m, pair_min_margin(own[a], e[k], nglob));
+            if (m <= 0.0f) {
+#pragma unroll
+              for (int a = 0; a < PPL; ++a) sweep_pair(own[a], e[k], tb, M, Mh, queue, qcount);
+            }
+          }
+          if (stop) break;
+        }
+      }
 #pragma unroll
       for (int i = 0; i < PPL; ++i) hitmin[i * 32 + lane] = 0x7fffffff;
-      __syncwarp();
+      __syncwarp();   // the queue holds every candidate
       // narrowphase: the queued candidate pairs, one per lane (or the exhaustive pass if the queue overflowed)
       const int n_q = *qcount;
       if (n_q <= QCAP) {
@@ -2875,8 +2773,7 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
     A.off_poseB = off; off += wpc * POSE_PER_WARP * (int)sizeof(float4);
     A.off_hit = off; off += wpc * POSE_PER_WARP * (int)sizeof(int);
     A.off_queue = off; off += wpc * QCAP * 4;
-    A.off_posx = off; off += wpc * POS_EXT_PER_WARP * 4;
-    A.off_posy = off; off += wpc * POS_EXT_PER_WARP * 4;
+    A.off_sorted = off; off += wpc * POSE_PER_WARP * (int)sizeof(float4);
     A.off_qcount = off; off += ((wpc + 3) & ~3) * 4;
     A.off_bar = off; off += 16;
     A.wpc = wpc;
@@ -2887,7 +2784,6 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
     const int MP = c->G * PPL;
     A.mp_shift = 0;
     while ((1 << A.mp_shift) < MP) ++A.mp_shift;
-    A.ext = ((3 * MP) / 2 + 16 + 3) & ~3;   // a multiple of 4 floats: every scenario's window starts 16-byte aligned
   }
   const int smem = A.off_bar + 16;
   if (smem > c->max_smem_optin) return fail(T2D_E_UNSUPPORTED, "shared memory budget exceeded");
