@@ -179,7 +179,9 @@ int t2d_set_map_polygons(t2d_ctx* ctx, const float* segments, int n_seg, const i
 /* One tile = the static objects + boundary of one map (host arrays, copied).  tile_id: DEVICE uint16 [N], owned by the
  * caller and read by every tick: the tile of each scenario (may be rewritten between ticks, e.g. by a reset that draws a
  * new parking lot); NULL is allowed when n_tiles == 1.  Every scenario then collides with its own tile's objects, is
- * bounded by its own tile's box, and t2d_lidar_scan sees its own tile's segments. */
+ * bounded by its own tile's box, and t2d_lidar_scan sees its own tile's segments.
+ * t2d_set_map / t2d_set_map_polygons / t2d_set_map_table: n_tiles == 0 (no segments and no bounds) unbinds.  Rejected
+ * (the previous map, its tile_id and its per-segment BEV styles stay bound): any malformed tile. */
 #define T2D_MAX_TILES 4096
 typedef struct {
   const float* segments;     /* [n_seg][4] */
@@ -406,7 +408,8 @@ int t2d_set_controllers(t2d_ctx* ctx, const t2d_controller_params* table, int n_
                         const int16_t* lead_index, const int16_t* path_id, float* last_accel);
 
 /* Pure-pursuit paths: HOST arrays, copied.  xy [V][2] vertices of all paths back to back, offsets [n_paths + 1] (path p
- * owns vertices offsets[p] .. offsets[p + 1] - 1, at least 2). */
+ * owns vertices offsets[p] .. offsets[p + 1] - 1, at least 2).  n_paths == 0 or xy == NULL unbinds.  Rejected (the
+ * previous paths stay bound): malformed offsets. */
 int t2d_set_paths(t2d_ctx* ctx, const float* xy, const int32_t* offsets, int n_paths);
 
 /* Overwrites action[n][m] = (accel, steer) ((steer, accel) with T2D_CFG_STEER_FIRST) of every controlled participant from

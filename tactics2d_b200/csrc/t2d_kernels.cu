@@ -31,6 +31,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cmath>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -1982,6 +1983,40 @@ static int fail(int code, const std::string& msg) {
     if (_e != cudaSuccess) return fail(T2D_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
   } while (0)
 
+// Owners of the context's device and pinned host buffers.  Dropping one frees its buffer, so whatever replaces or drops
+// one runs with the context's device current.
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+struct CudaFreeHost {
+  void operator()(void* p) const { cudaFreeHost(p); }
+};
+template <class T> using dev_ptr = std::unique_ptr<T, CudaFree>;
+template <class T> using host_ptr = std::unique_ptr<T, CudaFreeHost>;
+
+template <class T> static int dev_alloc(dev_ptr<T>& out, size_t n) {
+  T* p = nullptr;
+  CUDA_TRY(cudaMalloc(&p, n * sizeof(T)));
+  out.reset(p);
+  return T2D_OK;
+}
+
+template <class T> static int host_alloc(host_ptr<T>& out, size_t n, unsigned flags = cudaHostAllocDefault) {
+  T* p = nullptr;
+  CUDA_TRY(cudaHostAlloc(&p, n * sizeof(T), flags));
+  out.reset(p);
+  return T2D_OK;
+}
+
+// n host elements copied to a fresh device buffer; `out` changes only on success
+template <class T> static int upload(dev_ptr<T>& out, const T* src, size_t n) {
+  dev_ptr<T> d;
+  if (int r = dev_alloc(d, n)) return r;
+  CUDA_TRY(cudaMemcpy(d.get(), src, n * sizeof(T), cudaMemcpyHostToDevice));
+  out = std::move(d);
+  return T2D_OK;
+}
+
 struct t2d_exchange {
   int device = 0, world = 0, rank = 0, n_local = 0, slots = 0;
   size_t bytes = 0;
@@ -1995,6 +2030,70 @@ struct t2d_exchange {
   unsigned* word(int i) const { return reinterpret_cast<unsigned*>(base + flag_off()) + T2D_MAX_RANKS + i; }   // 0 steps done, 3 error
 };
 
+// The bound map (t2d_set_map_table), replaced as a whole: a new map also drops the per-segment BEV styles of the old one
+struct DeviceMap {
+  dev_ptr<unsigned char> blob;         // the tiles back to back, each 128-byte aligned
+  dev_ptr<uint32_t> tile_off;          // [n_tiles] byte offsets of the tiles inside blob
+  const uint16_t* tile_id = nullptr;   // caller-owned DEVICE [N] (more than one tile)
+  int n_tiles = 0;
+  bool has_segments = false;
+  bool has_bounds = false;             // any tile has a boundary box
+  MapHeader mh{};                      // tile 0's header
+  int smem_bytes = 0;                  // what a single tile stages into shared memory
+  std::vector<int> tile_nseg;          // segments of every tile, in tile order
+  dev_ptr<uint8_t> seg_style;          // BEV style per segment, tiles back to back; nullptr: the default ring / open styles
+  dev_ptr<uint32_t> seg_base;          // [n_tiles] first entry of every tile in seg_style
+};
+
+// The bound log (t2d_set_log / K7), replaced as a whole
+struct DeviceLog {
+  dev_ptr<ReplayTrack> tracks;
+  dev_ptr<uint8_t> track_type;
+  dev_ptr<float> rec;
+  dev_ptr<int32_t> t0;
+  dev_ptr<int32_t> slot_off;           // [n_rows * M + 1] schedule offsets
+  dev_ptr<ReplayEntry> entries;
+  dev_ptr<int32_t> slot_track1;        // [n_rows * M] instead of the two above when no schedule has two entries
+  int n_tracks = 0, n_rows = 0;
+  int32_t* row = nullptr;              // caller-owned DEVICE [N]
+  int32_t* track_out = nullptr;        // caller-owned DEVICE [N][M] or nullptr
+  uint8_t* type_id = nullptr;          // writable alias of type_id, checked against the bound one before every launch
+  std::vector<uint8_t> track_type_host;   // host copy: t2d_set_type_table keeps these rows static
+};
+
+// Staging of the host steps (t2d_step_host, t2d_step_host_ego, t2d_step_host_agents); every piece is created whole the
+// first time a step needs it.
+static constexpr int MAX_HOST_CHUNKS = 8;
+
+struct ChunkedUpload {   // t2d_step_host: device copy of the actions, the copy stream and its events
+  dev_ptr<float> action;               // [N][M][2]
+  cudaStream_t copy = nullptr;
+  cudaEvent_t begin = nullptr, chunk[MAX_HOST_CHUNKS] = {};
+  ~ChunkedUpload() {
+    if (begin) cudaEventDestroy(begin);
+    for (cudaEvent_t e : chunk)
+      if (e) cudaEventDestroy(e);
+    if (copy) cudaStreamDestroy(copy);
+  }
+};
+
+struct Mirror {   // a packed block of device outputs and its pinned host mirror
+  dev_ptr<uint8_t> dev;
+  host_ptr<uint8_t> host;
+};
+
+struct MappedEgo {   // t2d_step_host_ego: [N][2] pinned + mapped host staging of the ego actions ...
+  host_ptr<float> host;
+  const float* dev = nullptr;          // ... and its device-side address: the kernels read it over PCIe, no copy engine involved
+};
+
+struct AgentStaging {   // t2d_step_host_agents, sized for q rows per scenario
+  int q = 0;
+  dev_ptr<float> action;               // [N][Q][2]
+  Mirror out;                          // device: [N][Q] fp32 reward, [3][N][Q] uint8, [N] uint8 done, then [N][Q] fp32 iou;
+                                       // host: the part up to done
+};
+
 struct t2d_ctx {
   int device = 0, N = 0, M = 0, G = 0;
   t2d_config cfg{};
@@ -2004,16 +2103,8 @@ struct t2d_ctx {
   bool kin_only = false;
   float *wheel_f = nullptr, *wheel_r = nullptr;
   const float *reset_pool_wf = nullptr, *reset_pool_wr = nullptr;   // t2d_bind_reset_wheel_pool
-  Params* d_table = nullptr;
-  unsigned char* d_map = nullptr;
-  uint32_t* d_tile_off = nullptr;   // [n_tiles] byte offsets of the tiles inside d_map
-  const uint16_t* tile_id = nullptr;   // caller-owned DEVICE [N] (more than one tile)
-  int n_tiles = 0;
-  bool has_segments = false;
-  MapHeader mh{};
-  int map_bytes = 0;
-  bool has_bounds = false;
-  float bounds[4] = {0, 0, 0, 0};
+  dev_ptr<Params> d_table;
+  DeviceMap map;
   float *x = nullptr, *y = nullptr, *h = nullptr, *v = nullptr, *vx = nullptr, *vy = nullptr;
   const uint8_t* type_id = nullptr;
   int32_t* step_count = nullptr;
@@ -2044,57 +2135,69 @@ struct t2d_ctx {
   int occ_val[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   int occ_variant[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   // NPC controllers (t2d_set_controllers / t2d_set_paths / t2d_control)
-  t2d_controller_params* d_ctab = nullptr;
+  dev_ptr<t2d_controller_params> d_ctab;
   int n_ctrl = 0;
   const uint8_t* ctrl_id = nullptr;
   const int16_t* ctrl_lead = nullptr;
   const int16_t* ctrl_path = nullptr;
   float* ctrl_last_accel = nullptr;
-  PathVertex* d_path_v = nullptr;
-  int* d_path_off = nullptr;
+  dev_ptr<PathVertex> d_path_v;
+  dev_ptr<int> d_path_off;
   int n_paths = 0;
-  // t2d_step_host: device staging for the host-resident action / status / done, the copy stream and its events
-  static constexpr int MAX_HOST_CHUNKS = 8;
-  float* hs_action = nullptr;          // [N][M][2]
-  float* hs_ego_pinned = nullptr;      // [N][2] pinned + mapped host staging of the ego actions (t2d_step_host_ego) ...
-  const float* hs_ego_dev = nullptr;   // ... and its device-side address: the kernels read it over PCIe, no copy engine involved
-  uint8_t* hs_out = nullptr;           // [2][N] status, done
-  uint8_t* hs_out_pinned = nullptr;    // pinned host mirror of hs_out
-  cudaStream_t hs_copy = nullptr;
-  cudaEvent_t hs_begin = nullptr, hs_chunk[MAX_HOST_CHUNKS] = {};
+  // host steps
+  std::unique_ptr<ChunkedUpload> hs_upload;
+  Mirror hs_out;                       // [2][N] status, done (t2d_step_host and t2d_step_host_ego)
+  MappedEgo hs_ego;
+  AgentStaging ha;
+  dev_ptr<uint8_t> ha_flags;           // [N][M]: the flags K10 needs when the caller keeps none
   int host_chunks = 0;                 // 0 = pick from the batch size
-  // t2d_step_host_agents: device staging of the agents' actions, the packed outputs reward | terminated | truncated |
-  // status | done on the device and their pinned mirror, K10's iou, and the flags K10 needs when the caller keeps none;
-  // sized for ha_q rows per scenario
-  int ha_q = 0;
-  float* ha_action = nullptr;          // [N][Q][2]
-  uint8_t* ha_out = nullptr;           // [N][Q] fp32 reward, [3][N][Q] uint8, [N] uint8 done, then [N][Q] fp32 iou
-  uint8_t* ha_out_pinned = nullptr;    // pinned mirror of the part up to done
-  uint8_t* ha_flags = nullptr;         // [N][M]
   // BEV observation (t2d_set_bev_styles / t2d_bev_render)
-  std::vector<int> tile_nseg;          // segments of every tile of the current map, in tile order
   int n_bev_styles = 0;                // 0: styles not set
   t2d_bev_style bev_style[bev::MAX_STYLES] = {};
   uint8_t bev_type_style[T2D_MAX_TYPES] = {};
   int bev_target_style = bev::NO_STYLE;
-  uint8_t* d_seg_style = nullptr;      // per segment, tiles back to back; nullptr: the default ring / open styles
-  uint32_t* d_seg_base = nullptr;      // [n_tiles] first entry of every tile in d_seg_style
-  // log replay (t2d_set_log / K7)
-  bool has_log = false;
-  int log_tracks = 0, log_rows = 0;
-  ReplayTrack* d_log_tracks = nullptr;
-  uint8_t* d_log_track_type = nullptr;
-  float* d_log_rec = nullptr;
-  int32_t* d_log_t0 = nullptr;
-  int32_t* d_log_slot_off = nullptr;   // [n_rows * M + 1] schedule offsets
-  ReplayEntry* d_log_entries = nullptr;
-  int32_t* d_log_slot_track1 = nullptr; // [n_rows * M] instead of the two above when no schedule has two entries
-  int32_t* log_row = nullptr;          // caller-owned DEVICE [N]
-  int32_t* log_track_out = nullptr;    // caller-owned DEVICE [N][M] or nullptr
-  uint8_t* log_type_id = nullptr;      // writable alias of type_id, checked against the bound one before every launch
-  std::vector<uint8_t> log_track_type; // host copy: t2d_set_type_table keeps these rows static
+  std::unique_ptr<DeviceLog> log;      // nullptr: no log bound
   std::vector<int> type_model;         // host copy of the current type table's model ids
 };
+
+enum : unsigned { NEED_STATE = 1, NEED_TABLE = 2, NEED_TICK = 4 };
+
+// The call-order preconditions, checked in this order: the bound state, the type table, and what a tick with physics
+// needs besides (a caller that launches other kernels first checks them up front).
+static int require(const t2d_ctx* c, unsigned need) {
+  if ((need & NEED_STATE) && !c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if ((need & NEED_TABLE) && (!c->d_table || c->n_types == 0))
+    return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (need & NEED_TICK) {
+    if (c->has_drift && !(c->wheel_f && c->wheel_r))
+      return fail(T2D_E_STATE, "the type table holds a SingleTrackDrift row: call t2d_bind_wheel_state first");
+    if (c->log && c->log->type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+  }
+  return T2D_OK;
+}
+
+// after every launch: count it and report a launch error
+static int launched() {
+  g_launches.fetch_add(1);
+  CUDA_TRY(cudaGetLastError());
+  return T2D_OK;
+}
+
+// grid of a grid-stride kernel: one CTA per `per_cta` items, at most `per_sm` CTAs per SM
+static int capped_grid(long long items, int per_cta, int sm_count, int per_sm) {
+  return (int)std::max(1LL, std::min((items + per_cta - 1) / per_cta, (long long)sm_count * per_sm));
+}
+
+// the integration steps of one interval, for the tick and t2d_physics_step
+template <class Args> static void set_time_step(Args& A, int interval_ms, int delta_t_ms) {
+  const int delta_t = std::min(delta_t_ms, interval_ms);
+  A.n_steps = interval_ms / delta_t;                            // single_track_kinematics.py:129
+  A.dt = (float)((double)delta_t / 1000.0);                     // :128
+  A.dt_rem = (float)((double)(interval_ms % delta_t) / 1000.0);   // :130,152
+  A.dt_d = (double)delta_t / 1000.0;
+  A.dt_rem_d = (double)(interval_ms % delta_t) / 1000.0;
+  A.interval_d = (double)interval_ms / 1000.0;                  // point_mass.py:86
+}
 
 extern "C" {
 
@@ -2131,7 +2234,7 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
     const int v = atoi(e);
     if (v >= 1 && v <= MAX_WARPS_PER_CTA) c->wpc_override = v;
   }
-  if (const char* e = getenv("T2D_HOST_CHUNKS")) c->host_chunks = std::max(0, std::min(atoi(e), (int)t2d_ctx::MAX_HOST_CHUNKS));
+  if (const char* e = getenv("T2D_HOST_CHUNKS")) c->host_chunks = std::max(0, std::min(atoi(e), MAX_HOST_CHUNKS));
   int g = 1;
   while (g * PPL < m_participants) g <<= 1;
   c->G = g;
@@ -2144,45 +2247,9 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
   return T2D_OK;
 }
 
-static void free_log(t2d_ctx* c) {
-  if (c->d_log_tracks) cudaFree(c->d_log_tracks);
-  if (c->d_log_track_type) cudaFree(c->d_log_track_type);
-  if (c->d_log_rec) cudaFree(c->d_log_rec);
-  if (c->d_log_t0) cudaFree(c->d_log_t0);
-  if (c->d_log_slot_off) cudaFree(c->d_log_slot_off);
-  if (c->d_log_entries) cudaFree(c->d_log_entries);
-  if (c->d_log_slot_track1) cudaFree(c->d_log_slot_track1);
-  c->d_log_tracks = nullptr; c->d_log_track_type = nullptr; c->d_log_rec = nullptr; c->d_log_t0 = nullptr;
-  c->d_log_slot_off = nullptr; c->d_log_entries = nullptr; c->d_log_slot_track1 = nullptr;
-  c->has_log = false; c->log_tracks = c->log_rows = 0; c->log_row = nullptr; c->log_type_id = nullptr;
-  c->log_track_out = nullptr;
-  c->log_track_type.clear();
-}
-
 int t2d_destroy(t2d_ctx* c) {
   if (!c) return T2D_OK;
-  cudaSetDevice(c->device);
-  if (c->d_table) cudaFree(c->d_table);
-  if (c->d_map) cudaFree(c->d_map);
-  if (c->d_tile_off) cudaFree(c->d_tile_off);
-  if (c->d_ctab) cudaFree(c->d_ctab);
-  if (c->d_path_v) cudaFree(c->d_path_v);
-  if (c->d_path_off) cudaFree(c->d_path_off);
-  if (c->d_seg_style) cudaFree(c->d_seg_style);
-  if (c->d_seg_base) cudaFree(c->d_seg_base);
-  free_log(c);
-  if (c->hs_action) cudaFree(c->hs_action);
-  if (c->hs_ego_pinned) cudaFreeHost(c->hs_ego_pinned);
-  if (c->hs_out) cudaFree(c->hs_out);
-  if (c->hs_out_pinned) cudaFreeHost(c->hs_out_pinned);
-  if (c->ha_action) cudaFree(c->ha_action);
-  if (c->ha_out) cudaFree(c->ha_out);
-  if (c->ha_out_pinned) cudaFreeHost(c->ha_out_pinned);
-  if (c->ha_flags) cudaFree(c->ha_flags);
-  if (c->hs_begin) cudaEventDestroy(c->hs_begin);
-  for (cudaEvent_t e : c->hs_chunk)
-    if (e) cudaEventDestroy(e);
-  if (c->hs_copy) cudaStreamDestroy(c->hs_copy);
+  cudaSetDevice(c->device);   // the owners free on the current device
   delete c;
   return T2D_OK;
 }
@@ -2198,11 +2265,11 @@ int t2d_set_type_table(t2d_ctx* c, const t2d_type_params* table, int n_types) {
   if (!c || !table) return fail(T2D_E_INVALID, "ctx/table is NULL");
   if (n_types <= 0 || n_types > T2D_MAX_TYPES) return fail(T2D_E_INVALID, "n_types must be in 1..64");
   static_assert(sizeof(t2d_type_params) == sizeof(AbiParams), "type table layout");
-  for (uint8_t row : c->log_track_type)   // a bound log's tracks must stay static rows (K1 would integrate on the log)
-    if (row >= n_types || table[row].model != T2D_MODEL_STATIC)
-      return fail(T2D_E_INVALID, "type table: row " + std::to_string(row) + " of a replayed track must exist and be T2D_MODEL_STATIC");
-  c->has_pointmass = false;
-  bool has_drift = false;
+  if (c->log)
+    for (uint8_t row : c->log->track_type_host)   // a bound log's tracks must stay static rows (K1 would integrate on the log)
+      if (row >= n_types || table[row].model != T2D_MODEL_STATIC)
+        return fail(T2D_E_INVALID, "type table: row " + std::to_string(row) + " of a replayed track must exist and be T2D_MODEL_STATIC");
+  bool has_pointmass = false, has_drift = false, kin_only = true;
   float rb_max = 0.0f;
   for (int i = 0; i < n_types; ++i) {
     const t2d_type_params& p = table[i];
@@ -2220,41 +2287,37 @@ int t2d_set_type_table(t2d_ctx* c, const t2d_type_params* table, int n_types) {
     if (p.shape == T2D_SHAPE_OBB && !(p.half_len >= 0.0f && p.half_wid >= 0.0f))
       return fail(T2D_E_INVALID, "type table: negative OBB half extent");
     if (p.shape == T2D_SHAPE_CIRCLE && !(p.radius >= 0.0f)) return fail(T2D_E_INVALID, "type table: negative radius");
-    if (p.model == T2D_MODEL_POINTMASS_NEWTON || p.model == T2D_MODEL_POINTMASS_EULER) c->has_pointmass = true;
+    if (p.model == T2D_MODEL_POINTMASS_NEWTON || p.model == T2D_MODEL_POINTMASS_EULER) has_pointmass = true;
+    if (p.model != T2D_MODEL_KINEMATICS && p.model != T2D_MODEL_STATIC) kin_only = false;
+  }
+  std::vector<Params> rows(n_types + 1);
+  for (int i = 0; i < n_types; ++i) {
+    AbiParams a;
+    memcpy(&a, &table[i], sizeof(AbiParams));
+    rows[i] = derive_params(a);
+  }
+  {
+    // row n_types: the neutral kinematic row that K1's 4-chain loop gives to slots holding another model or nothing
+    // (zero speed and action in, unbounded ranges: every product stays finite and the result is discarded)
+    AbiParams a{};
+    a.lf = 1.0f; a.lr = 1.0f;
+    a.steer_lo = a.speed_lo = a.accel_lo = -INFINITY;
+    a.steer_hi = a.speed_hi = a.accel_hi = INFINITY;
+    a.model = MODEL_KINEMATICS; a.shape = SHAPE_NONE;
+    rows[n_types] = derive_params(a);
   }
   CUDA_TRY(cudaSetDevice(c->device));
-  if (!c->d_table) CUDA_TRY(cudaMalloc(&c->d_table, (T2D_MAX_TYPES + 1) * sizeof(Params)));
-  {
-    std::vector<Params> rows(n_types + 1);
-    for (int i = 0; i < n_types; ++i) {
-      AbiParams a;
-      memcpy(&a, &table[i], sizeof(AbiParams));
-      rows[i] = derive_params(a);
-    }
-    {
-      // row n_types: the neutral kinematic row that K1's 4-chain loop gives to slots holding another model or nothing
-      // (zero speed and action in, unbounded ranges: every product stays finite and the result is discarded)
-      AbiParams a{};
-      a.lf = 1.0f; a.lr = 1.0f;
-      a.steer_lo = a.speed_lo = a.accel_lo = -INFINITY;
-      a.steer_hi = a.speed_hi = a.accel_hi = INFINITY;
-      a.model = MODEL_KINEMATICS; a.shape = SHAPE_NONE;
-      rows[n_types] = derive_params(a);
-    }
-    CUDA_TRY(cudaMemcpy(c->d_table, rows.data(), (n_types + 1) * sizeof(Params), cudaMemcpyHostToDevice));
-  }
+  if (int r = upload(c->d_table, rows.data(), rows.size())) return r;
   c->n_types = n_types;
   c->type_model.resize(n_types);
   for (int i = 0; i < n_types; ++i) c->type_model[i] = table[i].model;
+  c->has_pointmass = has_pointmass;
   c->has_drift = has_drift;
   c->rb_max = rb_max;
-  c->kin_only = true;
-  for (int i = 0; i < n_types; ++i)
-    if (table[i].model != T2D_MODEL_KINEMATICS && table[i].model != T2D_MODEL_STATIC) c->kin_only = false;
+  c->kin_only = kin_only;
   for (int w = 0; w < 9; ++w) c->occ_smem[w] = -1;
   return T2D_OK;
 }
-
 // Host-side build of one static-geometry tile: the segments in list order (+ which of them close up to polygons), a
 // uniform grid over their bounding box grown by one cell, per cell the ascending list of the segments that touch it and
 // the "dilated" list of those within one cell of it, the clearance fields, the tile's boundary box.
@@ -2454,18 +2517,9 @@ int t2d_set_map_table(t2d_ctx* c, const t2d_map_tile* tiles, int n_tiles, const 
   if (n_tiles < 0 || n_tiles > T2D_MAX_TILES) return fail(T2D_E_INVALID, "n_tiles must be in 0..T2D_MAX_TILES");
   if (n_tiles > 0 && !tiles) return fail(T2D_E_INVALID, "tiles is NULL");
   if (n_tiles > 1 && !tile_id) return fail(T2D_E_INVALID, "tile_id is NULL (needed with more than one tile)");
-  CUDA_TRY(cudaSetDevice(c->device));
-  if (c->d_map) { cudaFree(c->d_map); c->d_map = nullptr; }
-  if (c->d_tile_off) { cudaFree(c->d_tile_off); c->d_tile_off = nullptr; }
-  if (c->d_seg_style) { cudaFree(c->d_seg_style); c->d_seg_style = nullptr; }   // a new map: default segment styles
-  if (c->d_seg_base) { cudaFree(c->d_seg_base); c->d_seg_base = nullptr; }
-  c->tile_nseg.clear();
-  c->map_bytes = 0; c->n_tiles = 0; c->tile_id = nullptr; c->has_bounds = false; c->has_segments = false;
-  c->mh = MapHeader{};
-  if (n_tiles == 0) return T2D_OK;
+  DeviceMap m;
   std::vector<unsigned char> all;
   std::vector<uint32_t> offs((size_t)n_tiles);
-  bool any_bounds = false, any_seg = false;
   for (int i = 0; i < n_tiles; ++i) {
     TileIn t{tiles[i].segments, tiles[i].n_seg, tiles[i].poly_start, tiles[i].n_poly, tiles[i].bounds};
     std::vector<unsigned char> blob;
@@ -2473,20 +2527,20 @@ int t2d_set_map_table(t2d_ctx* c, const t2d_map_tile* tiles, int n_tiles, const 
     offs[i] = (uint32_t)all.size();
     all.insert(all.end(), blob.begin(), blob.end());
     all.resize((all.size() + 127) / 128 * 128, 0);   // every tile starts 128-byte aligned
-    any_bounds = any_bounds || tiles[i].bounds != nullptr;
-    any_seg = any_seg || tiles[i].n_seg > 0;
-    if (i == 0) memcpy(&c->mh, blob.data(), sizeof(MapHeader));
+    m.has_bounds = m.has_bounds || tiles[i].bounds != nullptr;
+    m.has_segments = m.has_segments || tiles[i].n_seg > 0;
+    m.tile_nseg.push_back(tiles[i].n_seg);
+    if (i == 0) memcpy(&m.mh, blob.data(), sizeof(MapHeader));
   }
-  CUDA_TRY(cudaMalloc(&c->d_map, all.size()));
-  CUDA_TRY(cudaMemcpy(c->d_map, all.data(), all.size(), cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMalloc(&c->d_tile_off, sizeof(uint32_t) * (size_t)n_tiles));
-  CUDA_TRY(cudaMemcpy(c->d_tile_off, offs.data(), sizeof(uint32_t) * (size_t)n_tiles, cudaMemcpyHostToDevice));
-  c->n_tiles = n_tiles;
-  for (int i = 0; i < n_tiles; ++i) c->tile_nseg.push_back(tiles[i].n_seg);
-  c->tile_id = n_tiles > 1 ? tile_id : nullptr;
-  c->map_bytes = (int)c->mh.smem_bytes;     // what a single tile stages into shared memory
-  c->has_bounds = any_bounds; c->has_segments = any_seg;
-  if (c->mh.has_bounds) { c->bounds[0] = c->mh.bxmin; c->bounds[1] = c->mh.bxmax; c->bounds[2] = c->mh.bymin; c->bounds[3] = c->mh.bymax; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  if (n_tiles > 0) {
+    if (int r = upload(m.blob, all.data(), all.size())) return r;
+    if (int r = upload(m.tile_off, offs.data(), offs.size())) return r;
+  }
+  m.n_tiles = n_tiles;
+  m.tile_id = n_tiles > 1 ? tile_id : nullptr;
+  m.smem_bytes = (int)m.mh.smem_bytes;   // what a single tile stages into shared memory
+  c->map = std::move(m);
   return T2D_OK;
 }
 
@@ -2531,8 +2585,7 @@ int t2d_bind_reset_wheel_pool(t2d_ctx* c, const float* pool_omega_front, const f
 static int set_log(t2d_ctx* c, const t2d_log* L, const char* who, const int32_t* slot_off, const int32_t* slot_track,
                    int n_entries, int32_t* track_out) {
   const std::string fn = who;
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   if (L->n_tracks <= 0 || L->n_rows <= 0) return fail(T2D_E_INVALID, fn + ": n_tracks and n_rows must be >= 1");
   if (!L->first_ms || !L->n_frames || !L->period_ms || !L->type_row || !L->records || !L->t0_ms || !L->log_row || !L->type_id)
     return fail(T2D_E_INVALID, fn + ": NULL array");
@@ -2602,37 +2655,27 @@ static int set_log(t2d_ctx* c, const t2d_log* L, const char* who, const int32_t*
     std::copy(slot_off, slot_off + PM + 1, off.begin());
   }
   // at most one entry per slot (every row_track binding): the slots' tracks as one array, no search
-  std::vector<int32_t> one;
   bool single = true;
   for (long long s = 0; s < PM && single; ++s) single = off[s + 1] - off[s] <= 1;
+  CUDA_TRY(cudaSetDevice(c->device));
+  auto g = std::make_unique<DeviceLog>();
   if (single) {
-    one.assign((size_t)PM, -1);
+    std::vector<int32_t> one((size_t)PM, -1);
     for (long long s = 0; s < PM; ++s)
       if (off[s + 1] > off[s]) one[s] = entries[off[s]].track;
-  }
-  CUDA_TRY(cudaSetDevice(c->device));
-  free_log(c);
-  CUDA_TRY(cudaMalloc(&c->d_log_tracks, sizeof(ReplayTrack) * (size_t)K));
-  CUDA_TRY(cudaMalloc(&c->d_log_track_type, (size_t)K));
-  CUDA_TRY(cudaMalloc(&c->d_log_rec, sizeof(float) * 5 * (size_t)n_rec));
-  CUDA_TRY(cudaMalloc(&c->d_log_t0, sizeof(int32_t) * (size_t)L->n_rows));
-  if (single) {
-    CUDA_TRY(cudaMalloc(&c->d_log_slot_track1, sizeof(int32_t) * one.size()));
-    CUDA_TRY(cudaMemcpy(c->d_log_slot_track1, one.data(), sizeof(int32_t) * one.size(), cudaMemcpyHostToDevice));
+    if (int r = upload(g->slot_track1, one.data(), one.size())) return r;
   } else {
-    CUDA_TRY(cudaMalloc(&c->d_log_slot_off, sizeof(int32_t) * off.size()));
-    CUDA_TRY(cudaMalloc(&c->d_log_entries, sizeof(ReplayEntry) * entries.size()));
-    CUDA_TRY(cudaMemcpy(c->d_log_slot_off, off.data(), sizeof(int32_t) * off.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(c->d_log_entries, entries.data(), sizeof(ReplayEntry) * entries.size(), cudaMemcpyHostToDevice));
+    if (int r = upload(g->slot_off, off.data(), off.size())) return r;
+    if (int r = upload(g->entries, entries.data(), entries.size())) return r;
   }
-  CUDA_TRY(cudaMemcpy(c->d_log_tracks, tracks.data(), sizeof(ReplayTrack) * (size_t)K, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(c->d_log_track_type, L->type_row, (size_t)K, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(c->d_log_rec, L->records, sizeof(float) * 5 * (size_t)n_rec, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(c->d_log_t0, L->t0_ms, sizeof(int32_t) * (size_t)L->n_rows, cudaMemcpyHostToDevice));
-  c->log_track_type.assign(L->type_row, L->type_row + K);
-  c->log_tracks = K; c->log_rows = L->n_rows;
-  c->log_row = L->log_row; c->log_type_id = L->type_id; c->log_track_out = track_out;
-  c->has_log = true;
+  if (int r = upload(g->tracks, tracks.data(), tracks.size())) return r;
+  if (int r = upload(g->track_type, L->type_row, (size_t)K)) return r;
+  if (int r = upload(g->rec, L->records, 5 * (size_t)n_rec)) return r;
+  if (int r = upload(g->t0, L->t0_ms, (size_t)L->n_rows)) return r;
+  g->track_type_host.assign(L->type_row, L->type_row + K);
+  g->n_tracks = K; g->n_rows = L->n_rows;
+  g->row = L->log_row; g->type_id = L->type_id; g->track_out = track_out;
+  c->log = std::move(g);
   return T2D_OK;
 }
 
@@ -2640,7 +2683,7 @@ int t2d_set_log(t2d_ctx* c, const t2d_log* L) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (!L) {
     CUDA_TRY(cudaSetDevice(c->device));
-    free_log(c);
+    c->log.reset();
     return T2D_OK;
   }
   return set_log(c, L, "t2d_set_log", nullptr, nullptr, 0, nullptr);
@@ -2656,26 +2699,23 @@ int t2d_set_log_schedule(t2d_ctx* c, const t2d_log* L, const int32_t* slot_off, 
 // K7 over the scenarios [first, first + count): tick mode (mask == nullptr, offset 1) or reset mode (the masked scenarios
 // take row pool_index[n] / n, offset 0).
 static int launch_replay(t2d_ctx* c, void* stream, int first, int count, int offset, const uint8_t* mask, const int32_t* pool_index) {
-  if (c->log_type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+  const DeviceLog& g = *c->log;
+  if (g.type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
   const size_t p0 = (size_t)first * c->M;
   ReplayArgs R{};
   R.x = c->x + p0; R.y = c->y + p0; R.h = c->h + p0; R.v = c->v + p0; R.vx = c->vx + p0; R.vy = c->vy + p0;
-  R.type_id = c->log_type_id + p0;
+  R.type_id = g.type_id + p0;
   R.step_count = c->step_count + first;
-  R.log_row = c->log_row + first;
+  R.log_row = g.row + first;
   R.mask = mask ? mask + first : nullptr;
   R.pool_index = pool_index ? pool_index + first : nullptr;
-  R.log_row_out = mask ? c->log_row + first : nullptr;
-  R.tracks = c->d_log_tracks; R.track_type = c->d_log_track_type; R.rec = c->d_log_rec;
-  R.t0 = c->d_log_t0; R.slot_off = c->d_log_slot_off; R.entries = c->d_log_entries; R.slot_track1 = c->d_log_slot_track1;
-  R.track_out = c->log_track_out ? c->log_track_out + p0 : nullptr;
-  R.N = count; R.M = c->M; R.n_rows = c->log_rows; R.offset = offset; R.interval_ms = c->cfg.interval_ms;
-  const long long total = (long long)count * c->M;
-  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)c->sm_count * 8);
-  t2d_replay_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(R);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  R.log_row_out = mask ? g.row + first : nullptr;
+  R.tracks = g.tracks.get(); R.track_type = g.track_type.get(); R.rec = g.rec.get();
+  R.t0 = g.t0.get(); R.slot_off = g.slot_off.get(); R.entries = g.entries.get(); R.slot_track1 = g.slot_track1.get();
+  R.track_out = g.track_out ? g.track_out + p0 : nullptr;
+  R.N = count; R.M = c->M; R.n_rows = g.n_rows; R.offset = offset; R.interval_ms = c->cfg.interval_ms;
+  t2d_replay_kernel<<<capped_grid((long long)count * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(R);
+  return launched();
 }
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -2701,56 +2741,41 @@ static int pick_wpc(long long tiles, int sm_count) {
   return best;
 }
 
-// Launches K1 over the scenarios [first, first + count) of the bound state; the per-participant / per-scenario
-// pointers passed in (action, flags, ..., done) address scenario `first` already.
-// The call-order checks of a tick with physics (a caller that launches other kernels first runs them up front).
-static int check_tick_state(const t2d_ctx* c) {
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
-  if (c->has_drift && !(c->wheel_f && c->wheel_r))
-    return fail(T2D_E_STATE, "the type table holds a SingleTrackDrift row: call t2d_bind_wheel_state first");
-  if (c->has_log && c->log_type_id != c->type_id)
-    return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
-  return T2D_OK;
-}
-
-static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment,
+// Launches K1 over the scenarios [first, first + count) of the bound state with the ego action `ego` (nullptr: row 0 of
+// `action`); the per-participant / per-scenario pointers passed in (action, flags, ..., done) address scenario `first`
+// already, `ego` scenario 0.
+static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment,
                        uint8_t* scn_status, uint8_t* done, void* stream, int do_physics, int first = 0, int count = -1) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   if (do_physics && !action) return fail(T2D_E_INVALID, "action is NULL");
   if (do_physics)
-    if (int r = check_tick_state(c)) return r;
+    if (int r = require(c, NEED_TICK)) return r;
   CUDA_TRY(cudaSetDevice(c->device));
   if (count < 0) count = c->N - first;
   if (first < 0 || count <= 0 || first + count > c->N) return fail(T2D_E_INVALID, "scenario range out of bounds");
+  const DeviceMap& map = c->map;
   const size_t p0 = (size_t)first * c->M;
   StepArgs A{};
   A.x = c->x + p0; A.y = c->y + p0; A.h = c->h + p0; A.v = c->v + p0; A.vx = c->vx + p0; A.vy = c->vy + p0;
   A.type_id = c->type_id + p0; A.step_count = c->step_count + first;
   A.wheel_f = c->wheel_f ? c->wheel_f + p0 : nullptr; A.wheel_r = c->wheel_r ? c->wheel_r + p0 : nullptr;
-  A.action = action; A.ego_action = c->ego_action ? c->ego_action + 2 * (size_t)first : nullptr; A.flags = flags; A.hit_index = hit_index; A.hit_segment = hit_segment;
+  A.action = action; A.ego_action = ego ? ego + 2 * (size_t)first : nullptr; A.flags = flags; A.hit_index = hit_index; A.hit_segment = hit_segment;
   A.scn_status = scn_status; A.done = done;
-  const bool map_table = c->n_tiles > 1;
-  A.map_blob = c->d_map; A.map_bytes = c->map_bytes; A.mh = c->mh;
-  A.tile_off = c->d_tile_off; A.tile_id = map_table ? c->tile_id + first : nullptr;
-  A.map_in_smem = (!map_table && c->d_map && c->mh.n_seg > 0 && c->map_bytes <= MAP_SMEM_LIMIT) ? 1 : 0;
-  A.table = c->d_table; A.n_types = c->n_types;
+  const bool map_table = map.n_tiles > 1;
+  A.map_blob = map.blob.get(); A.map_bytes = map.smem_bytes; A.mh = map.mh;
+  A.tile_off = map.tile_off.get(); A.tile_id = map_table ? map.tile_id + first : nullptr;
+  A.map_in_smem = (!map_table && map.blob && map.mh.n_seg > 0 && map.smem_bytes <= MAP_SMEM_LIMIT) ? 1 : 0;
+  A.table = c->d_table.get(); A.n_types = c->n_types;
   A.N = count; A.M = c->M; A.G = c->G;
-  const int delta_t = std::min(c->cfg.delta_t_ms, c->cfg.interval_ms);
-  A.n_steps = c->cfg.interval_ms / delta_t;                       // single_track_kinematics.py:129
-  A.dt = (float)((double)delta_t / 1000.0);                      // :128
-  A.dt_rem = (float)((double)(c->cfg.interval_ms % delta_t) / 1000.0);   // :130,152
-  A.dt_d = (double)delta_t / 1000.0;
-  A.dt_rem_d = (double)(c->cfg.interval_ms % delta_t) / 1000.0;
-  A.interval_d = (double)c->cfg.interval_ms / 1000.0;                  // point_mass.py:86
+  set_time_step(A, c->cfg.interval_ms, c->cfg.delta_t_ms);
   A.max_step = c->cfg.max_step; A.cfg_flags = c->cfg.flags;
-  A.do_physics = do_physics; A.has_bounds = c->has_bounds ? 1 : 0;
-  A.bxmin = c->bounds[0]; A.bxmax = c->bounds[1]; A.bymin = c->bounds[2]; A.bymax = c->bounds[3];
+  // the boundary box: tile 0's (with a map table every lane reads its own tile's)
+  A.do_physics = do_physics; A.has_bounds = map.has_bounds ? 1 : 0;
+  A.bxmin = map.mh.bxmin; A.bxmax = map.mh.bxmax; A.bymin = map.mh.bymin; A.bymax = map.mh.bymax;
   A.prefetch = c->prefetch_override >= 0 ? c->prefetch_override : (g_exchanges_alive.load() == 0 ? 1 : 0);
   // (drift / replay: K1 passes the pre-pass's vx, vy through)
-  A.needs_vel_in = (c->has_pointmass || c->has_drift || (do_physics && c->has_log)) ? 1 : 0;
+  A.needs_vel_in = (c->has_pointmass || c->has_drift || (do_physics && c->log)) ? 1 : 0;
   bool vec = (c->M % PPL == 0) && aligned16(A.x) && aligned16(A.y) && aligned16(A.h) && aligned16(A.v) && aligned16(A.vx) &&
              aligned16(A.vy) && (reinterpret_cast<uintptr_t>(A.type_id) % 4 == 0) && (!action || aligned16(action)) &&
              (!flags || reinterpret_cast<uintptr_t>(flags) % 4 == 0) && (!hit_index || reinterpret_cast<uintptr_t>(hit_index) % 8 == 0) &&
@@ -2802,14 +2827,11 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
       configured = smem;
     }
   }
-  if (do_physics && c->has_log)
+  if (do_physics && c->log)
     if (int r = launch_replay(c, stream, first, count, 1, nullptr, nullptr)) return r;
   if (do_physics && c->has_drift) {
-    const long long total = (long long)count * c->M;
-    const int dgrid = (int)std::min<long long>((total + 127) / 128, (long long)c->sm_count * 16);
-    t2d_drift_kernel<<<dgrid, 128, 0, (cudaStream_t)stream>>>(A);
-    g_launches.fetch_add(1);
-    CUDA_TRY(cudaGetLastError());
+    t2d_drift_kernel<<<capped_grid((long long)count * c->M, 128, c->sm_count, 16), 128, 0, (cudaStream_t)stream>>>(A);
+    if (int r = launched()) return r;
   }
   const long long ctas_needed = (tiles + wpc - 1) / wpc;
   if (c->occ_smem[wpc] != smem || c->occ_variant[wpc] != (map_table ? 1 : 0)) {
@@ -2823,22 +2845,63 @@ static int launch_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t*
   if (c->grid_limit > 0) per_sm_ctas = std::min(per_sm_ctas, c->grid_limit);   // T2D_GRID_LIMIT: leave CTA slots to other streams
   const long long resident = (long long)c->sm_count * per_sm_ctas;
   const int grid = (int)std::max(1LL, std::min(ctas_needed, resident));
-  {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3((unsigned)(wpc * 32));
-    cfg.dynamicSmemBytes = (size_t)smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = c->use_pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, A));
-  }
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3((unsigned)(wpc * 32));
+  cfg.dynamicSmemBytes = (size_t)smem;
+  cfg.stream = (cudaStream_t)stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = c->use_pdl ? 1 : 0;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, A));
+  return launched();
+}
+
+// K5 with the ego action `ego` (nullptr: row 0 of `action`)
+static int launch_control(t2d_ctx* c, float* action, const float* ego, void* stream) {
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (!c->d_ctab) return fail(T2D_E_STATE, "controllers not set: call t2d_set_controllers first");
+  if (!action) return fail(T2D_E_INVALID, "action is NULL");
+  if (reinterpret_cast<uintptr_t>(action) % 8 != 0) return fail(T2D_E_INVALID, "action must be 8-byte aligned");
+  CUDA_TRY(cudaSetDevice(c->device));
+  CtrlArgs A{};
+  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
+  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.lead = c->ctrl_lead; A.path_id = c->ctrl_path;
+  A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.last_accel = c->ctrl_last_accel; A.action = action; A.ego_action = ego;
+  A.N = c->N; A.M = c->M; A.steer_first = (c->cfg.flags & T2D_CFG_STEER_FIRST) ? 1 : 0;
+  const int warps_per_cta = 4;
+  t2d_control_kernel<<<capped_grid(c->N, warps_per_cta, c->sm_count, 16), warps_per_cta * 32, 0, (cudaStream_t)stream>>>(A);
+  return launched();
+}
+
+struct HostPart {   // a part of a packed read-back that goes to a caller's array (dst == nullptr: not wanted)
+  void* dst;
+  size_t off, bytes;
+};
+
+// Copies the first `bytes` of a packed device block to its pinned mirror, waits for the stream, and copies the parts out
+static int read_back(const Mirror& m, size_t bytes, cudaStream_t s, std::initializer_list<HostPart> parts) {
+  CUDA_TRY(cudaMemcpyAsync(m.host.get(), m.dev.get(), bytes, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (const HostPart& p : parts)
+    if (p.dst) memcpy(p.dst, m.host.get() + p.off, p.bytes);
   return T2D_OK;
+}
+
+static int make_mirror(Mirror& out, size_t dev_bytes, size_t host_bytes) {
+  Mirror m;
+  if (int r = dev_alloc(m.dev, dev_bytes)) return r;
+  if (int r = host_alloc(m.host, host_bytes)) return r;
+  out = std::move(m);
+  return T2D_OK;
+}
+
+// the [2][N] status / done block of t2d_step_host and t2d_step_host_ego
+static int status_done_staging(t2d_ctx* c) {
+  return c->hs_out.dev ? T2D_OK : make_mirror(c->hs_out, 2 * (size_t)c->N, 2 * (size_t)c->N);
 }
 
 int t2d_set_goal(t2d_ctx* c, const float* target, float arrival_threshold, int no_action_max_step, float* iou_out, float* last_pose,
@@ -2853,7 +2916,7 @@ int t2d_set_goal(t2d_ctx* c, const float* target, float arrival_threshold, int n
 
 int t2d_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment, uint8_t* scn_status,
              uint8_t* done, void* stream) {
-  return launch_step(c, action, flags, hit_index, hit_segment, scn_status, done, stream, 1);
+  return launch_step(c, action, c ? c->ego_action : nullptr, flags, hit_index, hit_segment, scn_status, done, stream, 1);
 }
 
 int t2d_step_host(t2d_ctx* c, const float* action_host, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment,
@@ -2862,48 +2925,47 @@ int t2d_step_host(t2d_ctx* c, const float* action_host, uint8_t* flags, int16_t*
   if (!action_host) return fail(T2D_E_INVALID, "action is NULL");
   CUDA_TRY(cudaSetDevice(c->device));
   const int N = c->N, M = c->M;
-  if (!c->hs_action) {
-    CUDA_TRY(cudaMalloc(&c->hs_action, (size_t)N * M * 2 * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->hs_out, 2 * (size_t)N));
-    CUDA_TRY(cudaMallocHost(&c->hs_out_pinned, 2 * (size_t)N));
-    CUDA_TRY(cudaStreamCreateWithFlags(&c->hs_copy, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreateWithFlags(&c->hs_begin, cudaEventDisableTiming));
-    for (cudaEvent_t& e : c->hs_chunk) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  if (!c->hs_upload) {
+    auto u = std::make_unique<ChunkedUpload>();
+    if (int r = dev_alloc(u->action, (size_t)N * M * 2)) return r;
+    CUDA_TRY(cudaStreamCreateWithFlags(&u->copy, cudaStreamNonBlocking));
+    CUDA_TRY(cudaEventCreateWithFlags(&u->begin, cudaEventDisableTiming));
+    for (cudaEvent_t& e : u->chunk) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    c->hs_upload = std::move(u);
   }
+  if (int r = status_done_staging(c)) return r;
+  ChunkedUpload& u = *c->hs_upload;
+  uint8_t* out = c->hs_out.dev.get();
   // Chunks of whole scenarios: the copy of chunk k + 1 (copy engine, own stream) runs under the kernel of chunk k.
   // A kernel that does not fill the GPU lasts one tile's lifetime whatever the batch, so splitting a small upload only
   // adds a fixed cost per chunk; it pays once a chunk alone fills the GPU, i.e. from ~1 M participants (8 MiB of
   // actions) per chunk upwards.
   int chunks = c->host_chunks;
-  if (chunks <= 0) chunks = (int)std::min<long long>(t2d_ctx::MAX_HOST_CHUNKS, std::max<long long>(1, (long long)N * M / (1 << 20)));
+  if (chunks <= 0) chunks = (int)std::min<long long>(MAX_HOST_CHUNKS, std::max<long long>(1, (long long)N * M / (1 << 20)));
   int per = (N + chunks - 1) / chunks;
   per = (per + 31) & ~31;   // whole warp tiles (<= 32 scenarios per warp): a chunked tick groups lanes exactly as t2d_step does
   cudaStream_t s = (cudaStream_t)stream;
   const bool split = per < N;   // a single chunk needs no second stream
   if (split) {
-    CUDA_TRY(cudaEventRecord(c->hs_begin, s));            // the copies follow whatever the caller queued on `stream`
-    CUDA_TRY(cudaStreamWaitEvent(c->hs_copy, c->hs_begin, 0));
+    CUDA_TRY(cudaEventRecord(u.begin, s));            // the copies follow whatever the caller queued on `stream`
+    CUDA_TRY(cudaStreamWaitEvent(u.copy, u.begin, 0));
   }
   int k = 0;
   for (int first = 0; first < N; first += per, ++k) {
     const int count = std::min(per, N - first);
     const size_t a0 = (size_t)first * M * 2;
-    CUDA_TRY(cudaMemcpyAsync(c->hs_action + a0, action_host + a0, (size_t)count * M * 2 * sizeof(float), cudaMemcpyHostToDevice,
-                             split ? c->hs_copy : s));
+    CUDA_TRY(cudaMemcpyAsync(u.action.get() + a0, action_host + a0, (size_t)count * M * 2 * sizeof(float), cudaMemcpyHostToDevice,
+                             split ? u.copy : s));
     if (split) {
-      CUDA_TRY(cudaEventRecord(c->hs_chunk[k], c->hs_copy));
-      CUDA_TRY(cudaStreamWaitEvent(s, c->hs_chunk[k], 0));
+      CUDA_TRY(cudaEventRecord(u.chunk[k], u.copy));
+      CUDA_TRY(cudaStreamWaitEvent(s, u.chunk[k], 0));
     }
     const size_t p0 = (size_t)first * M;
-    if (int r = launch_step(c, c->hs_action + a0, flags ? flags + p0 : nullptr, hit_index ? hit_index + p0 : nullptr,
-                            hit_segment ? hit_segment + p0 : nullptr, c->hs_out + first, c->hs_out + N + first, stream, 1, first, count))
+    if (int r = launch_step(c, u.action.get() + a0, c->ego_action, flags ? flags + p0 : nullptr, hit_index ? hit_index + p0 : nullptr,
+                            hit_segment ? hit_segment + p0 : nullptr, out + first, out + N + first, stream, 1, first, count))
       return r;
   }
-  CUDA_TRY(cudaMemcpyAsync(c->hs_out_pinned, c->hs_out, 2 * (size_t)N, cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  if (scn_status_host) memcpy(scn_status_host, c->hs_out_pinned, (size_t)N);
-  if (done_host) memcpy(done_host, c->hs_out_pinned + N, (size_t)N);
-  return T2D_OK;
+  return read_back(c->hs_out, 2 * (size_t)N, s, {{scn_status_host, 0, (size_t)N}, {done_host, (size_t)N, (size_t)N}});
 }
 
 int t2d_set_prefetch(t2d_ctx* c, int mode) {
@@ -2926,46 +2988,36 @@ int t2d_step_host_ego(t2d_ctx* c, const float* ego_action_host, float* action, u
   if (!ego_action_host || !action) return fail(T2D_E_INVALID, "ego_action / action is NULL");
   CUDA_TRY(cudaSetDevice(c->device));
   const int N = c->N;
-  if (!c->hs_ego_pinned) {
+  if (!c->hs_ego.host) {
     // pinned AND mapped: the first kernel of the step reads the 8 N bytes straight from host memory (one PCIe round trip
     // inside the kernel) instead of waiting for a copy-engine transfer and the stream dependency behind it
-    CUDA_TRY(cudaHostAlloc(&c->hs_ego_pinned, (size_t)N * 2 * sizeof(float), cudaHostAllocMapped));
+    MappedEgo e;
+    if (int r = host_alloc(e.host, (size_t)N * 2, cudaHostAllocMapped)) return r;
     float* dev = nullptr;
-    CUDA_TRY(cudaHostGetDevicePointer(&dev, c->hs_ego_pinned, 0));
-    c->hs_ego_dev = dev;
+    CUDA_TRY(cudaHostGetDevicePointer(&dev, e.host.get(), 0));
+    e.dev = dev;
+    c->hs_ego = std::move(e);
   }
-  if (!c->hs_out) {
-    CUDA_TRY(cudaMalloc(&c->hs_out, 2 * (size_t)N));
-    CUDA_TRY(cudaMallocHost(&c->hs_out_pinned, 2 * (size_t)N));
-  }
-  cudaStream_t s = (cudaStream_t)stream;
-  memcpy(c->hs_ego_pinned, ego_action_host, (size_t)N * 2 * sizeof(float));
-  const float* saved = c->ego_action;
-  int r = T2D_OK;
+  if (int r = status_done_staging(c)) return r;
+  memcpy(c->hs_ego.host.get(), ego_action_host, (size_t)N * 2 * sizeof(float));
+  const float* ego = c->hs_ego.dev;
   if (c->d_ctab) {
     // the controllers' launch fetches the ego actions and writes them into row 0 of `action`; the other participants'
     // actions never leave the device; the tick then reads everything from `action`
-    c->ego_action = c->hs_ego_dev;
-    r = t2d_control(c, action, stream);
-    c->ego_action = nullptr;
-  } else {
-    c->ego_action = c->hs_ego_dev;
+    if (int r = launch_control(c, action, ego, stream)) return r;
+    ego = nullptr;
   }
-  if (r == T2D_OK) r = launch_step(c, action, flags, hit_index, hit_segment, c->hs_out, c->hs_out + N, stream, 1);
-  c->ego_action = saved;
-  if (r != T2D_OK) return r;
-  CUDA_TRY(cudaMemcpyAsync(c->hs_out_pinned, c->hs_out, 2 * (size_t)N, cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  if (scn_status_host) memcpy(scn_status_host, c->hs_out_pinned, (size_t)N);
-  if (done_host) memcpy(done_host, c->hs_out_pinned + N, (size_t)N);
-  return T2D_OK;
+  uint8_t* out = c->hs_out.dev.get();
+  if (int r = launch_step(c, action, ego, flags, hit_index, hit_segment, out, out + N, stream, 1)) return r;
+  return read_back(c->hs_out, 2 * (size_t)N, (cudaStream_t)stream,
+                   {{scn_status_host, 0, (size_t)N}, {done_host, (size_t)N, (size_t)N}});
 }
 
 int t2d_env_epilogue(t2d_ctx* c, const uint8_t* flags, const uint8_t* scn_status, float* reward, uint8_t* terminated,
                      uint8_t* truncated, uint8_t* traffic_status, uint8_t* done, float* max_iou, float* min_dist,
                      int reset_trackers_on_done, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (int r = require(c, NEED_STATE)) return r;
   if (!flags || !scn_status || !reward) return fail(T2D_E_INVALID, "t2d_env_epilogue: flags / scn_status / reward is NULL");
   CUDA_TRY(cudaSetDevice(c->device));
   EnvArgs A{};
@@ -2974,12 +3026,8 @@ int t2d_env_epilogue(t2d_ctx* c, const uint8_t* flags, const uint8_t* scn_status
   A.max_iou = max_iou; A.min_dist = min_dist;
   A.reward = reward; A.terminated = terminated; A.truncated = truncated; A.done = done; A.traffic_status = traffic_status;
   A.N = c->N; A.M = c->M; A.max_step = c->cfg.max_step; A.reset_trackers = reset_trackers_on_done ? 1 : 0;
-  const long long total = (long long)c->N * c->M;
-  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)c->sm_count * 8);
-  t2d_env_epilogue_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  t2d_env_epilogue_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(A);
+  return launched();
 }
 
 int t2d_set_agents(t2d_ctx* c, const int16_t* observers, int32_t n_observers, const float* goals, float arrival_threshold,
@@ -3004,8 +3052,7 @@ int t2d_agents_epilogue(t2d_ctx* c, const uint8_t* flags, float* reward, uint8_t
                         uint8_t* agent_status, float* iou, uint8_t* done, float* max_iou, float* min_dist, uint8_t* traffic_status,
                         int reset_trackers_on_done, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   if (c->agent_q == 0) return fail(T2D_E_STATE, "t2d_agents_epilogue: no agents bound: call t2d_set_agents first");
   if (!flags || !reward || !terminated || !truncated || !agent_status || !iou || !done || !max_iou || !min_dist)
     return fail(T2D_E_INVALID, "t2d_agents_epilogue: NULL array");
@@ -3014,15 +3061,13 @@ int t2d_agents_epilogue(t2d_ctx* c, const uint8_t* flags, float* reward, uint8_t
   A.g.goal_target = c->agent_goals; A.g.goal_iou = iou; A.g.goal_last_pose = c->agent_last_pose;
   A.g.goal_noact_count = c->agent_noact_count; A.g.goal_threshold = c->agent_threshold; A.g.goal_noact_max = c->agent_noact_max;
   A.flags = flags; A.observers = c->agent_observers; A.x = c->x; A.y = c->y; A.h = c->h;
-  A.type_id = const_cast<uint8_t*>(c->type_id); A.retired = c->agent_retired; A.step_count = c->step_count; A.table = c->d_table;
+  A.type_id = const_cast<uint8_t*>(c->type_id); A.retired = c->agent_retired; A.step_count = c->step_count; A.table = c->d_table.get();
   A.max_iou = max_iou; A.min_dist = min_dist; A.reward = reward; A.terminated = terminated; A.truncated = truncated;
   A.status = agent_status; A.done = done; A.traffic_status = traffic_status;
   A.N = c->N; A.M = c->M; A.Q = c->agent_q; A.n_types = c->n_types; A.max_step = c->cfg.max_step;
   A.reset_trackers = reset_trackers_on_done ? 1 : 0;
   t2d_agents_epilogue_kernel<<<(c->N + K10_WARPS - 1) / K10_WARPS, K10_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  return launched();
 }
 
 static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
@@ -3035,9 +3080,7 @@ static int launch_agent_action(t2d_ctx* c, const int16_t* observers, int Q, cons
   A.observers = observers; A.agent_action = agent_action; A.action = action; A.type_id = c->type_id;
   A.N = c->N; A.M = c->M; A.Q = Q; A.n_types = c->n_types;
   t2d_agent_action_kernel<<<(c->N + K11_WARPS - 1) / K11_WARPS, K11_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  return launched();
 }
 
 int t2d_scatter_agent_action(t2d_ctx* c, const int16_t* observers, int32_t n_observers, const float* agent_action,
@@ -3050,8 +3093,7 @@ int t2d_scatter_agent_action(t2d_ctx* c, const int16_t* observers, int32_t n_obs
   if (!agent_action || !action) return fail(T2D_E_INVALID, "t2d_scatter_agent_action: agent_action / action is NULL");
   if (!aligned8(agent_action) || !aligned8(action))
     return fail(T2D_E_INVALID, "t2d_scatter_agent_action: agent_action and action must be 8-byte aligned");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   return launch_agent_action(c, observers, n_observers, agent_action, action, stream);
 }
 
@@ -3063,66 +3105,59 @@ int t2d_step_host_agents(t2d_ctx* c, const float* agent_action_host, float* acti
   if (!agent_action_host || !action || !max_iou || !min_dist || !done_host)
     return fail(T2D_E_INVALID, "t2d_step_host_agents: agent_action / action / max_iou / min_dist / done is NULL");
   if (!aligned8(action)) return fail(T2D_E_INVALID, "t2d_step_host_agents: action must be 8-byte aligned");
-  if (int r = check_tick_state(c)) return r;
+  if (int r = require(c, NEED_STATE | NEED_TABLE | NEED_TICK)) return r;
   if (c->agent_q == 0) return fail(T2D_E_STATE, "t2d_step_host_agents: no agents bound: call t2d_set_agents first");
   CUDA_TRY(cudaSetDevice(c->device));
   const int N = c->N, M = c->M, Q = c->agent_q;
   const size_t nq = (size_t)N * Q;
   const size_t out_bytes = 7 * nq + N;                   // reward, terminated, truncated, status, done
   const size_t iou_off = (out_bytes + 15) & ~(size_t)15;
-  if (c->ha_q != Q) {   // (re)size the staging for the bound Q
-    if (c->ha_action) { cudaFree(c->ha_action); c->ha_action = nullptr; }
-    if (c->ha_out) { cudaFree(c->ha_out); c->ha_out = nullptr; }
-    if (c->ha_out_pinned) { cudaFreeHost(c->ha_out_pinned); c->ha_out_pinned = nullptr; }
-    c->ha_q = 0;
-    CUDA_TRY(cudaMalloc(&c->ha_action, nq * 2 * sizeof(float)));
-    CUDA_TRY(cudaMalloc(&c->ha_out, iou_off + nq * sizeof(float)));
-    CUDA_TRY(cudaMallocHost(&c->ha_out_pinned, out_bytes));
-    c->ha_q = Q;
+  if (c->ha.q != Q) {   // staging for the bound Q
+    AgentStaging a;
+    if (int r = dev_alloc(a.action, nq * 2)) return r;
+    if (int r = make_mirror(a.out, iou_off + nq * sizeof(float), out_bytes)) return r;
+    a.q = Q;
+    c->ha = std::move(a);
   }
-  if (!flags && !c->ha_flags) CUDA_TRY(cudaMalloc(&c->ha_flags, (size_t)N * M));
-  uint8_t* fl = flags ? flags : c->ha_flags;
-  float* d_reward = reinterpret_cast<float*>(c->ha_out);
-  uint8_t* d_term = c->ha_out + 4 * nq;
+  if (!flags && !c->ha_flags)
+    if (int r = dev_alloc(c->ha_flags, (size_t)N * M)) return r;
+  uint8_t* fl = flags ? flags : c->ha_flags.get();
+  uint8_t* o = c->ha.out.dev.get();
+  float* d_reward = reinterpret_cast<float*>(o);
+  uint8_t* d_term = o + 4 * nq;
   uint8_t* d_trunc = d_term + nq;
   uint8_t* d_status = d_trunc + nq;
   uint8_t* d_done = d_status + nq;
-  float* d_iou = reinterpret_cast<float*>(c->ha_out + iou_off);
+  float* d_iou = reinterpret_cast<float*>(o + iou_off);
   // One copy-engine transfer of the actions, as t2d_step_host (from pinned caller memory it is a DMA; pageable memory
   // goes through the driver's staging).  Staging them in mapped host memory for K11 to read over PCIe, as
   // t2d_step_host_ego does with its 8 N bytes, made the whole call about 1.5x slower at 2 MiB (DESIGN.md section 7).
   cudaStream_t s = (cudaStream_t)stream;
-  CUDA_TRY(cudaMemcpyAsync(c->ha_action, agent_action_host, nq * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
-  if (int r = launch_agent_action(c, c->agent_observers, Q, c->ha_action, action, stream)) return r;
+  CUDA_TRY(cudaMemcpyAsync(c->ha.action.get(), agent_action_host, nq * 2 * sizeof(float), cudaMemcpyHostToDevice, s));
+  if (int r = launch_agent_action(c, c->agent_observers, Q, c->ha.action.get(), action, stream)) return r;
   if (c->d_ctab)
-    if (int r = t2d_control(c, action, stream)) return r;
-  if (int r = launch_step(c, action, fl, hit_index, hit_segment, nullptr, nullptr, stream, 1)) return r;
+    if (int r = launch_control(c, action, c->ego_action, stream)) return r;
+  if (int r = launch_step(c, action, c->ego_action, fl, hit_index, hit_segment, nullptr, nullptr, stream, 1)) return r;
   if (int r = t2d_agents_epilogue(c, fl, d_reward, d_term, d_trunc, d_status, d_iou, d_done, max_iou, min_dist, nullptr,
                                   reset_trackers_on_done, stream))
     return r;
-  CUDA_TRY(cudaMemcpyAsync(c->ha_out_pinned, c->ha_out, out_bytes, cudaMemcpyDeviceToHost, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  const uint8_t* h = c->ha_out_pinned;
-  if (reward_host) memcpy(reward_host, h, 4 * nq);
-  if (terminated_host) memcpy(terminated_host, h + 4 * nq, nq);
-  if (truncated_host) memcpy(truncated_host, h + 5 * nq, nq);
-  if (agent_status_host) memcpy(agent_status_host, h + 6 * nq, nq);
-  memcpy(done_host, h + 7 * nq, (size_t)N);
-  return T2D_OK;
+  return read_back(c->ha.out, out_bytes, s,
+                   {{reward_host, 0, 4 * nq}, {terminated_host, 4 * nq, nq}, {truncated_host, 5 * nq, nq},
+                    {agent_status_host, 6 * nq, nq}, {done_host, 7 * nq, (size_t)N}});
 }
 
 int t2d_check_events(t2d_ctx* c, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment, void* stream) {
-  return launch_step(c, nullptr, flags, hit_index, hit_segment, nullptr, nullptr, stream, 0);
+  return launch_step(c, nullptr, c ? c->ego_action : nullptr, flags, hit_index, hit_segment, nullptr, nullptr, stream, 0);
 }
 
 int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x, const float* pool_y,
               const float* pool_heading, const float* pool_speed, const float* pool_vx, const float* pool_vy, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (int r = require(c, NEED_STATE)) return r;
   if (!mask || !pool_x || !pool_y || !pool_heading || !pool_speed) return fail(T2D_E_INVALID, "t2d_reset: NULL array");
   if (n_pool <= 0) return fail(T2D_E_INVALID, "n_pool must be > 0");
-  if (c->has_log && n_pool != c->log_rows) return fail(T2D_E_INVALID, "t2d_reset: with a log bound, pool row p is episode row p (n_pool == n_rows)");
-  if (c->has_log && c->log_type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+  if (c->log && n_pool != c->log->n_rows) return fail(T2D_E_INVALID, "t2d_reset: with a log bound, pool row p is episode row p (n_pool == n_rows)");
+  if (c->log && c->log->type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
   CUDA_TRY(cudaSetDevice(c->device));
   ResetArgs A{};
   A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy; A.step_count = c->step_count;
@@ -3130,43 +3165,37 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   A.px = pool_x; A.py = pool_y; A.ph = pool_heading; A.pv = pool_speed; A.pvx = pool_vx; A.pvy = pool_vy;
   A.goal_last_pose = c->goal_last_pose; A.goal_noact_count = c->goal_noact_count;
   A.wheel_f = c->wheel_f; A.wheel_r = c->wheel_r; A.pool_wf = c->reset_pool_wf; A.pool_wr = c->reset_pool_wr;
-  A.last_accel = c->ctrl_last_accel; A.type_id = c->type_id; A.table = c->d_table; A.n_types = c->n_types;
+  A.last_accel = c->ctrl_last_accel; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
   A.N = c->N; A.M = c->M; A.n_pool = n_pool;
   if (c->agent_q > 0) {   // the bound type_id is the caller's writable device array (K10 retires slots in it)
     A.agent_type_id = const_cast<uint8_t*>(c->type_id); A.agent_retired = c->agent_retired;
     A.agent_last_pose = c->agent_last_pose; A.agent_noact_count = c->agent_noact_count; A.agent_q = c->agent_q;
   }
-  const long long total = (long long)c->N * c->M;
-  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)c->sm_count * 8);
-  t2d_reset_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  if (c->has_log) return launch_replay(c, stream, 0, c->N, 0, mask, pool_index);   // the new episode's traffic at t0
+  t2d_reset_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(A);
+  if (int r = launched()) return r;
+  if (c->log) return launch_replay(c, stream, 0, c->N, 0, mask, pool_index);   // the new episode's traffic at t0
   return T2D_OK;
 }
 
 int t2d_lidar_scan(t2d_ctx* c, int n_beams, float max_range, const double* beam_cos_sin, float* scan, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   if (n_beams <= 0 || !(max_range > 0.0f) || !beam_cos_sin || !scan) return fail(T2D_E_INVALID, "t2d_lidar_scan: bad argument");
   CUDA_TRY(cudaSetDevice(c->device));
   LidarArgs A{};
-  A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table; A.n_types = c->n_types;
-  A.map_blob = c->d_map; A.tile_off = c->d_tile_off; A.tile_id = c->n_tiles > 1 ? c->tile_id : nullptr;
+  A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
+  A.map_blob = c->map.blob.get(); A.tile_off = c->map.tile_off.get(); A.tile_id = c->map.n_tiles > 1 ? c->map.tile_id : nullptr;
   A.beam_cs = beam_cos_sin; A.scan = scan;
   A.N = c->N; A.M = c->M; A.n_beams = n_beams; A.range = (double)max_range;
   const int grid = (c->N + LIDAR_WARPS - 1) / LIDAR_WARPS;
   t2d_lidar_kernel<<<grid, LIDAR_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  return launched();
 }
 
 int t2d_set_bev_styles(t2d_ctx* c, const t2d_bev_style* table, int n_styles, const uint8_t* type_style, const uint8_t* seg_style,
                        int n_seg_total, int target_style) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+  if (int r = require(c, NEED_TABLE)) return r;
   if (!table || n_styles < 4 || n_styles > T2D_MAX_BEV_STYLES) return fail(T2D_E_INVALID, "n_styles must be in 4..64");
   if (!type_style) return fail(T2D_E_INVALID, "type_style is NULL");
   for (int i = 0; i < n_styles; ++i)
@@ -3176,38 +3205,39 @@ int t2d_set_bev_styles(t2d_ctx* c, const t2d_bev_style* table, int n_styles, con
   for (int t = 0; t < c->n_types; ++t)
     if (!ok(type_style[t])) return fail(T2D_E_INVALID, "type_style: no such style");
   if (!ok(target_style)) return fail(T2D_E_INVALID, "target_style: no such style");
+  const std::vector<int>& nseg = c->map.tile_nseg;
   long long total = 0;
-  for (int k : c->tile_nseg) total += k;
+  for (int k : nseg) total += k;
   if (seg_style) {
     if (n_seg_total != total) return fail(T2D_E_INVALID, "n_seg_total differs from the segments of the map's tiles");
     for (long long s = 0; s < total; ++s)
       if (!ok(seg_style[s])) return fail(T2D_E_INVALID, "seg_style: no such style");
   }
   CUDA_TRY(cudaSetDevice(c->device));
-  if (c->d_seg_style) { cudaFree(c->d_seg_style); c->d_seg_style = nullptr; }
-  if (c->d_seg_base) { cudaFree(c->d_seg_base); c->d_seg_base = nullptr; }
+  dev_ptr<uint8_t> d_style;
+  dev_ptr<uint32_t> d_base;
   if (seg_style && total > 0) {
-    std::vector<uint32_t> base(c->tile_nseg.size());
+    std::vector<uint32_t> base(nseg.size());
     uint32_t acc = 0;
-    for (size_t i = 0; i < base.size(); ++i) { base[i] = acc; acc += (uint32_t)c->tile_nseg[i]; }
-    CUDA_TRY(cudaMalloc(&c->d_seg_style, (size_t)total));
-    CUDA_TRY(cudaMemcpy(c->d_seg_style, seg_style, (size_t)total, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMalloc(&c->d_seg_base, sizeof(uint32_t) * base.size()));
-    CUDA_TRY(cudaMemcpy(c->d_seg_base, base.data(), sizeof(uint32_t) * base.size(), cudaMemcpyHostToDevice));
+    for (size_t i = 0; i < base.size(); ++i) { base[i] = acc; acc += (uint32_t)nseg[i]; }
+    if (int r = upload(d_style, seg_style, (size_t)total)) return r;
+    if (int r = upload(d_base, base.data(), base.size())) return r;
   }
+  // opt in to the kernel's shared memory here: t2d_bev_render must stay free of anything a graph capture rejects
+  CUDA_TRY(cudaFuncSetAttribute(bev::t2d_bev_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(bev::Smem)));
+  c->map.seg_style = std::move(d_style);
+  c->map.seg_base = std::move(d_base);
   memcpy(c->bev_style, table, sizeof(t2d_bev_style) * (size_t)n_styles);
   memset(c->bev_type_style, bev::NO_STYLE, sizeof(c->bev_type_style));
   memcpy(c->bev_type_style, type_style, (size_t)c->n_types);
   c->bev_target_style = target_style;
   c->n_bev_styles = n_styles;
-  // opt in to the kernel's shared memory here: t2d_bev_render must stay free of anything a graph capture rejects
-  CUDA_TRY(cudaFuncSetAttribute(bev::t2d_bev_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(bev::Smem)));
   return T2D_OK;
 }
 
 int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rgb, uint8_t* out, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+  if (int r = require(c, NEED_STATE)) return r;
   if (c->n_bev_styles == 0) return fail(T2D_E_STATE, "BEV styles not set: call t2d_set_bev_styles first");
   if (!range || !out) return fail(T2D_E_INVALID, "t2d_bev_render: range / out is NULL");
   if (width < 1 || height < 1 || width > bev::MAX_SIDE || height > bev::MAX_SIDE)
@@ -3235,88 +3265,69 @@ int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rg
     A.style_z[s] = st.z;
   }
   memcpy(A.type_style, c->bev_type_style, sizeof(A.type_style));
-  A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table; A.n_types = c->n_types;
+  A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
   A.N = c->N; A.M = c->M;
-  A.map_blob = c->d_map; A.tile_off = c->d_tile_off; A.tile_id = c->n_tiles > 1 ? c->tile_id : nullptr;
-  A.seg_style = c->d_seg_style; A.seg_base = c->d_seg_base;
+  A.map_blob = c->map.blob.get(); A.tile_off = c->map.tile_off.get(); A.tile_id = c->map.n_tiles > 1 ? c->map.tile_id : nullptr;
+  A.seg_style = c->map.seg_style.get(); A.seg_base = c->map.seg_base.get();
   A.target = c->goal_target; A.target_style = c->bev_target_style;
   A.ring_style = T2D_BEV_STYLE_RING; A.open_style = T2D_BEV_STYLE_OPEN;
   A.W = width; A.H = height; A.rgb = rgb ? 1 : 0; A.out = out;
   CUDA_TRY(cudaSetDevice(c->device));
   bev::t2d_bev_kernel<<<c->N, bev::CTA, sizeof(bev::Smem), (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
+  return launched();
+}
+
+// What t2d_observe and t2d_observe_agents share: the checks of cfg and out (messages prefixed with fn) and K8's arguments
+static int obs_args(const t2d_ctx* c, const std::string& fn, const t2d_obs_config* cfg, float* out, int16_t* agent_index,
+                    int16_t* segment_index, obs::Args& A) {
+  if (!cfg) return fail(T2D_E_INVALID, fn + ": cfg is NULL");
+  if (cfg->k_agents < 0 || cfg->k_agents > T2D_OBS_MAX_AGENTS) return fail(T2D_E_INVALID, fn + ": k_agents must be in 0..127");
+  if (cfg->k_segments < 0 || cfg->k_segments > T2D_OBS_MAX_SEGMENTS)
+    return fail(T2D_E_INVALID, fn + ": k_segments must be in 0..256");
+  if (!(cfg->agent_range > 0.0f && cfg->agent_range <= 1.0e5f) || !(cfg->segment_range > 0.0f && cfg->segment_range <= 1.0e5f))
+    return fail(T2D_E_INVALID, fn + ": agent_range and segment_range must be in (0, 1e5] m");
+  if (!out) return fail(T2D_E_INVALID, fn + ": out is NULL");
+  static_assert(T2D_OBS_MAX_AGENTS == obs::MAX_K && T2D_OBS_MAX_SEGMENTS == obs::MAX_S, "K8's shared lists hold the ABI's limits");
+  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy;
+  A.type_id = c->type_id; A.step_count = c->step_count; A.table = c->d_table.get(); A.n_types = c->n_types;
+  A.N = c->N; A.M = c->M; A.max_step = c->cfg.max_step;
+  A.map_blob = c->map.blob.get(); A.tile_off = c->map.tile_off.get(); A.tile_id = c->map.n_tiles > 1 ? c->map.tile_id : nullptr;
+  A.target = c->goal_target;
+  A.K = cfg->k_agents; A.S = cfg->k_segments;
+  A.F = obs::EGO_F + obs::GOAL_F + obs::AGENT_F * A.K + obs::SEG_F * A.S;
+  const double ra = cfg->agent_range, rs = cfg->segment_range;
+  A.ra2 = ra * ra; A.rs2 = rs * rs;
+  A.out = out; A.agent_index = agent_index; A.segment_index = segment_index;
   return T2D_OK;
 }
 
 int t2d_observe(t2d_ctx* c, const t2d_obs_config* cfg, float* out, int16_t* agent_index, int16_t* segment_index, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!cfg) return fail(T2D_E_INVALID, "t2d_observe: cfg is NULL");
-  if (cfg->k_agents < 0 || cfg->k_agents > T2D_OBS_MAX_AGENTS) return fail(T2D_E_INVALID, "t2d_observe: k_agents must be in 0..127");
-  if (cfg->k_segments < 0 || cfg->k_segments > T2D_OBS_MAX_SEGMENTS)
-    return fail(T2D_E_INVALID, "t2d_observe: k_segments must be in 0..256");
-  if (!(cfg->agent_range > 0.0f && cfg->agent_range <= 1.0e5f) || !(cfg->segment_range > 0.0f && cfg->segment_range <= 1.0e5f))
-    return fail(T2D_E_INVALID, "t2d_observe: agent_range and segment_range must be in (0, 1e5] m");
-  if (!out) return fail(T2D_E_INVALID, "t2d_observe: out is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
-  static_assert(T2D_OBS_MAX_AGENTS == obs::MAX_K && T2D_OBS_MAX_SEGMENTS == obs::MAX_S, "K8's shared lists hold the ABI's limits");
   obs::Args A{};
-  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy;
-  A.type_id = c->type_id; A.step_count = c->step_count; A.table = c->d_table; A.n_types = c->n_types;
-  A.N = c->N; A.M = c->M; A.max_step = c->cfg.max_step;
-  A.map_blob = c->d_map; A.tile_off = c->d_tile_off; A.tile_id = c->n_tiles > 1 ? c->tile_id : nullptr;
-  A.target = c->goal_target;
-  A.K = cfg->k_agents; A.S = cfg->k_segments;
-  A.F = obs::EGO_F + obs::GOAL_F + obs::AGENT_F * A.K + obs::SEG_F * A.S;
-  const double ra = cfg->agent_range, rs = cfg->segment_range;
-  A.ra2 = ra * ra; A.rs2 = rs * rs;
-  A.out = out; A.agent_index = agent_index; A.segment_index = segment_index;
+  if (int r = obs_args(c, "t2d_observe", cfg, out, agent_index, segment_index, A)) return r;
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   CUDA_TRY(cudaSetDevice(c->device));
   const int grid = (c->N + obs::WARPS - 1) / obs::WARPS;
   obs::t2d_obs_kernel<<<grid, obs::WARPS * 32, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  return launched();
 }
 
 int t2d_observe_agents(t2d_ctx* c, const t2d_obs_config* cfg, const int16_t* observers, int32_t n_observers,
                        const float* goals, float* out, int16_t* agent_index, int16_t* segment_index, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!cfg) return fail(T2D_E_INVALID, "t2d_observe_agents: cfg is NULL");
-  if (cfg->k_agents < 0 || cfg->k_agents > T2D_OBS_MAX_AGENTS)
-    return fail(T2D_E_INVALID, "t2d_observe_agents: k_agents must be in 0..127");
-  if (cfg->k_segments < 0 || cfg->k_segments > T2D_OBS_MAX_SEGMENTS)
-    return fail(T2D_E_INVALID, "t2d_observe_agents: k_segments must be in 0..256");
-  if (!(cfg->agent_range > 0.0f && cfg->agent_range <= 1.0e5f) || !(cfg->segment_range > 0.0f && cfg->segment_range <= 1.0e5f))
-    return fail(T2D_E_INVALID, "t2d_observe_agents: agent_range and segment_range must be in (0, 1e5] m");
-  if (!out) return fail(T2D_E_INVALID, "t2d_observe_agents: out is NULL");
+  obs::AgentArgs G{};
+  if (int r = obs_args(c, "t2d_observe_agents", cfg, out, agent_index, segment_index, G.a)) return r;
   if (n_observers < 1 || n_observers > T2D_OBS_MAX_OBSERVERS)
     return fail(T2D_E_INVALID, "t2d_observe_agents: n_observers must be in 1..128");
   if (!observers && n_observers > c->M)
     return fail(T2D_E_INVALID, "t2d_observe_agents: without an observer list n_observers must not exceed the slots per scenario");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
-  obs::AgentArgs G{};
-  obs::Args& A = G.a;
-  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy;
-  A.type_id = c->type_id; A.step_count = c->step_count; A.table = c->d_table; A.n_types = c->n_types;
-  A.N = c->N; A.M = c->M; A.max_step = c->cfg.max_step;
-  A.map_blob = c->d_map; A.tile_off = c->d_tile_off; A.tile_id = c->n_tiles > 1 ? c->tile_id : nullptr;
-  A.target = c->goal_target;
-  A.K = cfg->k_agents; A.S = cfg->k_segments;
-  A.F = obs::EGO_F + obs::GOAL_F + obs::AGENT_F * A.K + obs::SEG_F * A.S;
-  const double ra = cfg->agent_range, rs = cfg->segment_range;
-  A.ra2 = ra * ra; A.rs2 = rs * rs;
-  A.out = out; A.agent_index = agent_index; A.segment_index = segment_index;
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   G.observers = observers; G.goals = goals; G.Q = n_observers;
   CUDA_TRY(cudaSetDevice(c->device));
   const long long rows = (long long)c->N * n_observers;
   const int grid = (int)std::min<long long>((rows + obs::WARPS - 1) / obs::WARPS, 1ll << 30);   // the kernel strides past 2^32 rows
   obs::t2d_obs_agents_kernel<<<grid, obs::WARPS * 32, 0, (cudaStream_t)stream>>>(G);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  return launched();
 }
 
 int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_rows, const uint8_t* ctrl_id,
@@ -3324,8 +3335,8 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   CUDA_TRY(cudaSetDevice(c->device));
   if (!table) {
-    if (c->d_ctab) cudaFree(c->d_ctab);
-    c->d_ctab = nullptr; c->n_ctrl = 0; c->ctrl_id = nullptr; c->ctrl_lead = nullptr; c->ctrl_path = nullptr;
+    c->d_ctab.reset();
+    c->n_ctrl = 0; c->ctrl_id = nullptr; c->ctrl_lead = nullptr; c->ctrl_path = nullptr;
     c->ctrl_last_accel = nullptr;
     return T2D_OK;
   }
@@ -3339,9 +3350,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
     if (p.kind >= T2D_CTRL_CRUISE && p.target_speed < 0.0f)
       return fail(T2D_E_INVALID, "target_speed must be non-negative");          // acceleration_controller.py:48-49
   }
-  if (c->d_ctab) { cudaFree(c->d_ctab); c->d_ctab = nullptr; }
-  CUDA_TRY(cudaMalloc(&c->d_ctab, sizeof(t2d_controller_params) * n_rows));
-  CUDA_TRY(cudaMemcpy(c->d_ctab, table, sizeof(t2d_controller_params) * n_rows, cudaMemcpyHostToDevice));
+  if (int r = upload(c->d_ctab, table, (size_t)n_rows)) return r;
   c->n_ctrl = n_rows; c->ctrl_id = ctrl_id; c->ctrl_lead = lead_index; c->ctrl_path = path_id; c->ctrl_last_accel = last_accel;
   return T2D_OK;
 }
@@ -3349,10 +3358,10 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
 int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_paths) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   CUDA_TRY(cudaSetDevice(c->device));
-  if (c->d_path_v) { cudaFree(c->d_path_v); c->d_path_v = nullptr; }
-  if (c->d_path_off) { cudaFree(c->d_path_off); c->d_path_off = nullptr; }
-  c->n_paths = 0;
-  if (n_paths == 0 || !xy) return T2D_OK;
+  if (n_paths == 0 || !xy) {   // unbind
+    c->d_path_v.reset(); c->d_path_off.reset(); c->n_paths = 0;
+    return T2D_OK;
+  }
   if (n_paths < 0 || !offsets) return fail(T2D_E_INVALID, "t2d_set_paths: bad argument");
   if (offsets[0] != 0) return fail(T2D_E_INVALID, "offsets[0] must be 0");
   for (int p = 0; p < n_paths; ++p)
@@ -3371,36 +3380,18 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
       }
     }
   }
-  CUDA_TRY(cudaMalloc(&c->d_path_v, sizeof(PathVertex) * (size_t)V));
-  CUDA_TRY(cudaMemcpy(c->d_path_v, pv.data(), sizeof(PathVertex) * (size_t)V, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMalloc(&c->d_path_off, sizeof(int) * (size_t)(n_paths + 1)));
-  CUDA_TRY(cudaMemcpy(c->d_path_off, offsets, sizeof(int) * (size_t)(n_paths + 1), cudaMemcpyHostToDevice));
-  c->n_paths = n_paths;
+  dev_ptr<PathVertex> d_v;
+  dev_ptr<int> d_off;
+  if (int r = upload(d_v, pv.data(), pv.size())) return r;
+  if (int r = upload(d_off, offsets, (size_t)n_paths + 1)) return r;
+  c->d_path_v = std::move(d_v); c->d_path_off = std::move(d_off); c->n_paths = n_paths;
   return T2D_OK;
 }
 
 int t2d_control(t2d_ctx* c, float* action, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (!c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
-  if (!c->d_table || c->n_types == 0) return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
-  if (!c->d_ctab) return fail(T2D_E_STATE, "controllers not set: call t2d_set_controllers first");
-  if (!action) return fail(T2D_E_INVALID, "action is NULL");
-  if (reinterpret_cast<uintptr_t>(action) % 8 != 0) return fail(T2D_E_INVALID, "action must be 8-byte aligned");
-  CUDA_TRY(cudaSetDevice(c->device));
-  CtrlArgs A{};
-  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.type_id = c->type_id; A.table = c->d_table; A.n_types = c->n_types;
-  A.ctab = c->d_ctab; A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.lead = c->ctrl_lead; A.path_id = c->ctrl_path;
-  A.path_v = c->d_path_v; A.path_off = c->d_path_off; A.n_paths = c->n_paths;
-  A.last_accel = c->ctrl_last_accel; A.action = action; A.ego_action = c->ego_action;
-  A.N = c->N; A.M = c->M; A.steer_first = (c->cfg.flags & T2D_CFG_STEER_FIRST) ? 1 : 0;
-  const int warps_per_cta = 4;
-  const int grid = std::max(1, std::min((c->N + warps_per_cta - 1) / warps_per_cta, c->sm_count * 16));
-  t2d_control_kernel<<<grid, warps_per_cta * 32, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  return launch_control(c, action, c->ego_action, stream);
 }
-
 int t2d_exchange_create(t2d_exchange** out, int device, int world, int rank, int n_local, int slots, void* ipc_handle_out) {
   if (!out || !ipc_handle_out) return fail(T2D_E_INVALID, "out / ipc_handle_out is NULL");
   *out = nullptr;
@@ -3518,20 +3509,11 @@ int t2d_physics_step(int device, const t2d_type_params* params, int interval_ms,
   }
   A.x = x; A.y = y; A.h = heading; A.v = speed; A.vx = vx; A.vy = vy; A.action = action; A.applied = applied;
   A.n = n;
-  const int delta_t = std::min(delta_t_ms, interval_ms);
-  A.n_steps = interval_ms / delta_t;
-  A.dt = (float)((double)delta_t / 1000.0);
-  A.dt_rem = (float)((double)(interval_ms % delta_t) / 1000.0);
-  A.dt_d = (double)delta_t / 1000.0;
-  A.dt_rem_d = (double)(interval_ms % delta_t) / 1000.0;
-  A.interval_d = (double)interval_ms / 1000.0;
+  set_time_step(A, interval_ms, delta_t_ms);
   int sms = 0;
   CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-  const int grid = std::min((n + 255) / 256, sms * 8);
-  t2d_physics_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(A);
-  g_launches.fetch_add(1);
-  CUDA_TRY(cudaGetLastError());
-  return T2D_OK;
+  t2d_physics_kernel<<<capped_grid(n, 256, sms, 8), 256, 0, (cudaStream_t)stream>>>(A);
+  return launched();
 }
 
 }  // extern "C"

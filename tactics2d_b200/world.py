@@ -253,8 +253,10 @@ class BatchedWorld:
         tid = torch.as_tensor(np.asarray(tile_id) if not torch.is_tensor(tile_id) else tile_id).to(torch.int64)
         if tid.numel() != self.N or int(tid.min()) < 0 or int(tid.max()) >= len(tiles):
             raise ValueError(f"tile_id must hold {self.N} indices into the {len(tiles)} tiles")
-        self.tile_id = tid.to(torch.int16).to(self.device).contiguous()   # (bit pattern of uint16 for ids < 32768)
-        _lib.check(self.lib.t2d_set_map_table(self._ctx, rows, len(tiles), _ptr(self.tile_id), float(cell_size)))
+        tid = tid.to(torch.int16).to(self.device).contiguous()   # (bit pattern of uint16 for ids < 32768)
+        # a rejected table leaves the previous map bound, and with it the previous tile_id tensor
+        _lib.check(self.lib.t2d_set_map_table(self._ctx, rows, len(tiles), _ptr(tid), float(cell_size)))
+        self.tile_id = tid
         self.tiles = [dict(segments=k[0], bounds=None if k[1] is None else tuple(float(v) for v in k[1]), poly_start=k[2]) for k in keep]
         self.segments, self.poly_start, self.bounds = None, None, None
         self._seg_style_keys = [self._check_style_keys(t.get("style"), 0 if k[0] is None else k[0].shape[0])
@@ -266,34 +268,35 @@ class BatchedWorld:
         or None to disable.  Enables ``Arrival`` (IoU >= threshold -> COMPLETED, arrival.py:32-47) and ``NoAction``
         (IoU with the previous pose > 0.999 for more than ``no_action_max_step`` ticks, no_action.py:32-53) inside
         ``step``; ``StepResult.iou`` then holds the ego/target IoU."""
+        # the library keeps the pointers of the previous goal until a call succeeds: replace the tensors only then
         if target is None:
+            _lib.check(self.lib.t2d_set_goal(self._ctx, _ptr(None), 0.95, 0, _ptr(None), _ptr(None), _ptr(None)))
             self._goal = None
             self._out.iou = None
-            _lib.check(self.lib.t2d_set_goal(self._ctx, _ptr(None), 0.95, 0, _ptr(None), _ptr(None), _ptr(None)))
             return
         t = torch.as_tensor(np.asarray(target, dtype=np.float32) if not torch.is_tensor(target) else target)
         t = t.to(device=self.device, dtype=torch.float32).reshape(self.N, 5).contiguous()
-        self._goal = dict(target=t, iou=torch.zeros(self.N, dtype=torch.float32, device=self.device),
-                          last_pose=torch.zeros((self.N, 4), dtype=torch.float32, device=self.device),
-                          count=torch.zeros(self.N, dtype=torch.int32, device=self.device))
-        self._out.iou = self._goal["iou"]
-        g = self._goal
+        g = dict(target=t, iou=torch.zeros(self.N, dtype=torch.float32, device=self.device),
+                 last_pose=torch.zeros((self.N, 4), dtype=torch.float32, device=self.device),
+                 count=torch.zeros(self.N, dtype=torch.int32, device=self.device))
         _lib.check(self.lib.t2d_set_goal(self._ctx, _ptr(g["target"]), float(arrival_threshold), int(no_action_max_step),
                                          _ptr(g["iou"]), _ptr(g["last_pose"]), _ptr(g["count"])))
+        self._goal = g
+        self._out.iou = g["iou"]
 
     # ------------------------------------------------------------------ NPC controllers
     def set_paths(self, paths):
         """Pure-pursuit waypoint polylines: a list of ``[V_p, 2]`` arrays (the ``waypoints`` of
         ``PurePursuitController.step``, pure_pursuit_controller.py:76); ``path_id`` of ``set_controllers`` indexes it."""
         paths = [np.ascontiguousarray(np.asarray(p, dtype=np.float32).reshape(-1, 2)) for p in paths]
-        self.paths = paths
         if not paths:
             _lib.check(self.lib.t2d_set_paths(self._ctx, _ptr(None), _ptr(None), 0))
-            return
-        xy = np.ascontiguousarray(np.concatenate(paths, 0))
-        off = np.zeros(len(paths) + 1, np.int32)
-        off[1:] = np.cumsum([len(p) for p in paths])
-        _lib.check(self.lib.t2d_set_paths(self._ctx, C.c_void_p(xy.ctypes.data), C.c_void_p(off.ctypes.data), len(paths)))
+        else:
+            xy = np.ascontiguousarray(np.concatenate(paths, 0))
+            off = np.zeros(len(paths) + 1, np.int32)
+            off[1:] = np.cumsum([len(p) for p in paths])
+            _lib.check(self.lib.t2d_set_paths(self._ctx, C.c_void_p(xy.ctypes.data), C.c_void_p(off.ctypes.data), len(paths)))
+        self.paths = paths
 
     def set_controllers(self, controllers, ctrl_id, lead_index=None, path_id=None, last_accel=None):
         """Hand the non-ego agents to on-device controllers.  ``controllers``: list of ``tactics2d_b200.controller``
@@ -302,8 +305,8 @@ class BatchedWorld:
         none; ``path_id`` [N, M] int16: its pure-pursuit path (``set_paths``), -1 for none; ``last_accel`` [N, M]:
         ``State.accel`` of the previous tick (default zeros).  ``None`` for ``controllers`` removes them."""
         if controllers is None:
-            self._ctrl = None
             _lib.check(self.lib.t2d_set_controllers(self._ctx, _ptr(None), 0, _ptr(None), _ptr(None), _ptr(None), _ptr(None)))
+            self._ctrl = None
             return
         rows = [c if isinstance(c, _lib.ControllerParamsC) else c.params() for c in controllers]
         arr = (_lib.ControllerParamsC * len(rows))(*rows)
@@ -320,8 +323,8 @@ class BatchedWorld:
         la = dev(last_accel, torch.float32, 0.0)
         if la is None:
             la = torch.zeros((self.N, self.M), dtype=torch.float32, device=self.device)
-        self._ctrl = dict(rows=arr, ctrl_id=cid, lead_index=lead, path_id=pid, last_accel=la)
         _lib.check(self.lib.t2d_set_controllers(self._ctx, arr, len(rows), _ptr(cid), _ptr(lead), _ptr(pid), _ptr(la)))
+        self._ctrl = dict(rows=arr, ctrl_id=cid, lead_index=lead, path_id=pid, last_accel=la)
 
     @property
     def last_accel(self) -> Optional[torch.Tensor]:
@@ -491,8 +494,8 @@ class BatchedWorld:
             if (ego_action.device != self.device or ego_action.dtype != torch.float32 or tuple(ego_action.shape) != (self.N, 2)
                     or not ego_action.is_contiguous()):
                 raise ValueError(f"ego_action must be a contiguous fp32 [{self.N}, 2] tensor on {self.device}")
-        self._ego_action = ego_action   # keeps the tensor alive while the library holds its pointer
         _lib.check(self.lib.t2d_set_ego_action(self._ctx, _ptr(ego_action)))
+        self._ego_action = ego_action   # keeps the tensor alive while the library holds its pointer
 
     def step_host_ego(self, ego_action, action: Optional[torch.Tensor] = None):
         """One tick for a host-side policy that drives only the ego: ``ego_action`` is a float32 ``[N, 2]`` NumPy array
@@ -562,7 +565,7 @@ class BatchedWorld:
         outputs of ``agents_epilogue``; a settled row retires its slot (type 255) until ``reset`` restores it."""
         Q = self._agent_rows(observers, goals)
         f32, dev = torch.float32, self.device
-        self._agents = dict(
+        a = dict(
             observers=observers, goals=goals, Q=Q,
             last_pose=torch.zeros((self.N, Q, 4), dtype=f32, device=dev),
             noact_count=torch.zeros((self.N, Q), dtype=torch.int32, device=dev),
@@ -576,10 +579,10 @@ class BatchedWorld:
             traffic=torch.ones((self.N, self.M), dtype=torch.uint8, device=dev),
             max_iou=torch.full((self.N, Q), -float("inf"), dtype=f32, device=dev),
             min_dist=torch.full((self.N, Q), float("inf"), dtype=f32, device=dev))
-        a = self._agents
         _lib.check(self.lib.t2d_set_agents(self._ctx, _ptr(observers), Q, _ptr(goals), float(arrival_threshold),
                                            int(no_action_max_step), _ptr(a["last_pose"]), _ptr(a["noact_count"]),
                                            _ptr(a["retired_type"])))
+        self._agents = a
 
     @property
     def retired_type(self) -> Optional[torch.Tensor]:
