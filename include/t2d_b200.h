@@ -28,6 +28,8 @@
  *                        TimeExceed.update                tactics2d/traffic/event_detection/time_exceed.py:26-33
  *   t2d_set_goal         Arrival.update / NoAction.update  tactics2d/traffic/event_detection/arrival.py:32-47, no_action.py:32-53
  *   t2d_lidar_scan       SingleLineLidar._scan_obstacles   tactics2d/sensor/lidar.py:128-221
+ *   t2d_lidar_scan_agents
+ *                        (no reference counterpart: the reference's SingleLineLidar bound to each row's slot)
  *   t2d_set_bev_styles   the colour / z-order tables of MatplotlibRenderer   tactics2d/renderer/matplotlib_config.py,
  *                                                         sensor/camera.py:56-87 (style key of an element)
  *   t2d_bev_render       BEVCamera.update + MatplotlibRenderer.update / save_single_frame(return_array=True)
@@ -297,6 +299,22 @@ int t2d_set_log_schedule(t2d_ctx* ctx, const t2d_log* log, const int32_t* slot_o
  * (lidar.py:160); scan: DEVICE float [N][n_beams], +inf where nothing is hit within the range.  Obstacles are the map
  * segments given to t2d_set_map and the pose rings of the other box-shaped participants. */
 int t2d_lidar_scan(t2d_ctx* ctx, int n_beams, float max_range, const double* beam_cos_sin, float* scan, void* stream);
+
+/* Per-agent lidar: t2d_lidar_scan with the sensor on any list of observer slots per scenario (the reference's
+ * SingleLineLidar bound with bind_with(j) to each row's slot; DESIGN.md section 1 "Per-agent lidar").  Row (n, q), q < Q =
+ * n_observers (1..T2D_OBS_MAX_OBSERVERS), is the scan from slot j = observers[n][q] at its fp32 (x, y, heading), whatever
+ * j's shape: the beams are in j's frame, the obstacles are the scenario's map segments and the pose rings of every other
+ * active box-shaped slot, slot 0 included.  observers: DEVICE int16 [N][Q], or NULL for slot q in row q of every scenario
+ * (needs Q <= M).  A value outside [0, M) or an empty slot (type_id >= n_types, a retired one included) gives an absent
+ * row (every beam +inf); duplicates give identical rows.  beam_cos_sin as t2d_lidar_scan; scan: DEVICE float
+ * [N][Q][n_beams] (64-bit offsets: N·Q·n_beams may exceed 2^31).  With observers NULL and Q = 1 the call is
+ * t2d_lidar_scan.  Rejected without a launch: n_observers outside 1..128, observers == NULL with n_observers > M,
+ * n_beams <= 0, max_range not > 0 (NaN included), beam_cos_sin or scan NULL (T2D_E_INVALID), state or type table not bound
+ * (T2D_E_STATE), more than 2^33 rows (T2D_E_UNSUPPORTED).  One launch, no allocation, no synchronisation: capturable in
+ * a CUDA graph. */
+int t2d_lidar_scan_agents(t2d_ctx* ctx, const int16_t* observers /* DEVICE [N][Q] or NULL */, int32_t n_observers /* Q */,
+                          int n_beams, float max_range, const double* beam_cos_sin, float* scan /* DEVICE [N][Q][n_beams] */,
+                          void* stream);
 
 /* ---- bird's-eye-view observation of the ego of every scenario ------------------------------------------------------
  * t2d_set_bev_styles + t2d_bev_render replace BEVCamera.update (tactics2d/sensor/camera.py:333-386) followed by

@@ -1561,6 +1561,10 @@ __global__ void __launch_bounds__(256) t2d_physics_kernel(const __grid_constant_
 // together with their beam window (beam_window below), and the warp walks the edges with its lanes sharing the beams of
 // each window.  fp64 throughout (from the fp32 state): every tested pair gives exactly the float64 oracle's value, the
 // untested pairs are ones the reference's own filters reject.
+// The sensor may sit on any slot (t2d_lidar_scan_agents; the reference's SingleLineLidar bound with bind_with(j), whose
+// scan skips participant j and sees every other one, :146-148): one warp per (scenario, observer) row n·Q + q, the rows
+// of a scenario in adjacent warps so that they share its slots through L1.  t2d_lidar_scan is the row list {0} (Q = 1,
+// no list): the walk over the other slots below visits exactly the slots 1 .. M-1 then, in the same rounds.
 constexpr int LIDAR_EDGES = 144;   // edges per shared-memory chunk per warp (4 doubles + a beam window each)
 constexpr int LIDAR_WARPS = 4;
 constexpr int LIDAR_BEAMS = 512;   // beams per pass (running minima in shared memory)
@@ -1573,9 +1577,10 @@ struct LidarArgs {
   const unsigned char* map_blob;
   const uint32_t* tile_off;   // map table: byte offsets of the tiles; the scenario's tile id, or nullptr = tile 0 for all
   const uint16_t* tile_id;
-  const double* beam_cs;   // [n_beams][2] cos, sin of the beam angles (host float64)
-  float* scan;             // [N][n_beams]
-  int N, M, n_beams;
+  const double* beam_cs;      // [n_beams][2] cos, sin of the beam angles (host float64)
+  const int16_t* observers;   // [N][Q]: the slot carrying the sensor of row n·Q + q, or nullptr: row q is slot q
+  float* scan;                // [N][Q][n_beams]
+  int N, M, Q, n_beams;
   double range;
 };
 
@@ -1594,20 +1599,23 @@ __global__ void __launch_bounds__(LIDAR_WARPS * 32, 7) t2d_lidar_kernel(const __
   __shared__ float s_best[LIDAR_WARPS][LIDAR_BEAMS];
   __shared__ int s_cnt[LIDAR_WARPS];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long n = (long long)blockIdx.x * LIDAR_WARPS + warp;
-  if (n >= A.N) return;
+  const long long row = (long long)blockIdx.x * LIDAR_WARPS + warp;
+  if (row >= (long long)A.N * A.Q) return;
+  // (the ego scan divides by nothing, and a 32-bit division serves every row index below 2^32)
+  const long long n = A.Q == 1 ? row : row <= 0xffffffffll ? (long long)((unsigned)row / (unsigned)A.Q) : row / A.Q;
+  const int q = (int)(row - n * A.Q);
+  const int jo = A.observers ? (int)A.observers[row] : q;   // the slot carrying the sensor
   double(*edge)[4] = s_edge[warp];
   BeamWindow* win = s_win[warp];
   float* best = s_best[warp];
   int* cnt = &s_cnt[warp];
   const long long base = n * A.M;
-  const int t_ego = A.type_id[base];
-  float* out = A.scan + n * A.n_beams;
-  if (t_ego >= A.n_types) {   // no ego: nothing is seen
+  float* out = A.scan + row * A.n_beams;
+  if (jo < 0 || jo >= A.M || A.type_id[base + jo] >= A.n_types) {   // not a slot, or an empty one: nothing is seen
     for (int b = lane; b < A.n_beams; b += 32) out[b] = INFINITY;
     return;
   }
-  const double x0 = A.x[base], y0 = A.y[base], th = A.h[base];
+  const double x0 = A.x[base + jo], y0 = A.y[base + jo], th = A.h[base + jo];
   double sa, ca;
   sincos(th, &sa, &ca);
   const double xoff = -x0 * ca - y0 * sa, yoff = x0 * sa - y0 * ca;   // lidar.py:116-121
@@ -1628,7 +1636,8 @@ __global__ void __launch_bounds__(LIDAR_WARPS * 32, 7) t2d_lidar_kernel(const __
     // with their beam window; the chunk is scanned whenever the next round might not fit.
     for (int r = 0; r < part_rounds + seg_rounds; ++r) {
       if (r < part_rounds) {
-        const int j = 1 + r * 32 + lane;
+        const int i = r * 32 + lane;
+        const int j = i < jo ? i : i + 1;   // the i-th slot other than the observer's
         const int tj = j < A.M ? (int)A.type_id[base + j] : 255;
         if (tj < A.n_types && A.table[tj].shape() == SHAPE_OBB) {
           const Params& pj = A.table[tj];
@@ -3177,19 +3186,39 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   return T2D_OK;
 }
 
-int t2d_lidar_scan(t2d_ctx* c, int n_beams, float max_range, const double* beam_cos_sin, float* scan, void* stream) {
-  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
-  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
-  if (n_beams <= 0 || !(max_range > 0.0f) || !beam_cos_sin || !scan) return fail(T2D_E_INVALID, "t2d_lidar_scan: bad argument");
+// K4 over the rows of an observer list (observers == nullptr: row q is slot q); the callers have checked their arguments
+static int launch_lidar(t2d_ctx* c, const int16_t* observers, int Q, int n_beams, float max_range, const double* beam_cos_sin,
+                        float* scan, void* stream) {
   CUDA_TRY(cudaSetDevice(c->device));
   LidarArgs A{};
   A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
   A.map_blob = c->map.blob.get(); A.tile_off = c->map.tile_off.get(); A.tile_id = c->map.n_tiles > 1 ? c->map.tile_id : nullptr;
-  A.beam_cs = beam_cos_sin; A.scan = scan;
-  A.N = c->N; A.M = c->M; A.n_beams = n_beams; A.range = (double)max_range;
-  const int grid = (c->N + LIDAR_WARPS - 1) / LIDAR_WARPS;
-  t2d_lidar_kernel<<<grid, LIDAR_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  A.beam_cs = beam_cos_sin; A.observers = observers; A.scan = scan;
+  A.N = c->N; A.M = c->M; A.Q = Q; A.n_beams = n_beams; A.range = (double)max_range;
+  const long long grid = ((long long)c->N * Q + LIDAR_WARPS - 1) / LIDAR_WARPS;
+  if (grid > INT32_MAX) return fail(T2D_E_UNSUPPORTED, "lidar: more than 2^33 rows (one warp per row)");
+  t2d_lidar_kernel<<<(unsigned)grid, LIDAR_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
+}
+
+int t2d_lidar_scan(t2d_ctx* c, int n_beams, float max_range, const double* beam_cos_sin, float* scan, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (n_beams <= 0 || !(max_range > 0.0f) || !beam_cos_sin || !scan) return fail(T2D_E_INVALID, "t2d_lidar_scan: bad argument");
+  return launch_lidar(c, nullptr, 1, n_beams, max_range, beam_cos_sin, scan, stream);
+}
+
+int t2d_lidar_scan_agents(t2d_ctx* c, const int16_t* observers, int32_t n_observers, int n_beams, float max_range,
+                          const double* beam_cos_sin, float* scan, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (n_observers < 1 || n_observers > T2D_OBS_MAX_OBSERVERS)
+    return fail(T2D_E_INVALID, "t2d_lidar_scan_agents: n_observers must be in 1..128");
+  if (n_beams <= 0 || !(max_range > 0.0f) || !beam_cos_sin || !scan)
+    return fail(T2D_E_INVALID, "t2d_lidar_scan_agents: n_beams must be > 0, max_range > 0, beam_cos_sin and scan not NULL");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (!observers && n_observers > c->M)
+    return fail(T2D_E_INVALID, "t2d_lidar_scan_agents: without an observer list n_observers must not exceed the slots per scenario");
+  return launch_lidar(c, observers, n_observers, n_beams, max_range, beam_cos_sin, scan, stream);
 }
 
 int t2d_set_bev_styles(t2d_ctx* c, const t2d_bev_style* table, int n_styles, const uint8_t* type_style, const uint8_t* seg_style,

@@ -49,7 +49,7 @@ class BatchedTrafficEnv:
                  any_participant: bool = False, auto_reset: bool = True, target=None, arrival_threshold: float = 0.95,
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
-                 agent_rewards: bool = False, agent_actions: bool = False):
+                 agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -73,7 +73,12 @@ class BatchedTrafficEnv:
         per-row goals replace ``target``, which is then rejected;
         ``agent_actions``: with ``observation="agents"``, ``step`` takes one (steering, accel) per observer row, ``[N, Q,
         2]``, and scatters it on the device into the slots the rows observe (``BatchedWorld.scatter_agent_action``; the
-        lowest row naming a slot wins, empty and retired slots take nothing)."""
+        lowest row naming a slot wins, empty and retired slots take nothing);
+        ``lidar``: e.g. ``dict(n_beams=360, max_range=20.0)`` (``ParkingEnv``'s lidar, parking.py:303-304) adds
+        ``info["lidar"]`` to ``reset`` and ``step``, the reference env's ``infos["lidar"]`` (parking.py:206-217), scanned
+        after the auto-reset like the observation: fp32 ``[N, n_beams]`` from every ego (``BatchedWorld.lidar_scan``), or
+        with ``observation="agents"`` ``[N, Q, n_beams]`` from every observer row (``BatchedWorld.lidar_scan_agents`` on
+        ``vector_obs["observers"]``)."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -94,6 +99,11 @@ class BatchedTrafficEnv:
         unknown = set(self.vector_obs) - keys
         if unknown:
             raise ValueError(f"vector_obs: unknown keys {sorted(unknown)}")
+        self.lidar = None if lidar is None else dict(lidar)
+        if self.lidar is not None:
+            unknown = set(self.lidar) - {"n_beams", "max_range"}
+            if unknown:
+                raise ValueError(f"lidar: unknown keys {sorted(unknown)}")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -154,6 +164,15 @@ class BatchedTrafficEnv:
             info["track"] = self.world.replay_track
         return info
 
+    def _add_lidar(self, info):
+        """``info["lidar"]`` when the env has a lidar; called after the auto-reset, so that the scan sees the new episodes."""
+        if self.lidar is not None:
+            if self.observation == "agents":
+                info["lidar"] = self.world.lidar_scan_agents(**self.lidar, observers=self.vector_obs.get("observers"))
+            else:
+                info["lidar"] = self.world.lidar_scan(**self.lidar)
+        return info
+
     # ------------------------------------------------------------------ gym surface
     def reset(self, seed: int = None, options: dict = None):
         import torch
@@ -176,8 +195,10 @@ class BatchedTrafficEnv:
         traffic = torch.full((self.num_envs, self.num_participants), int(TrafficStatus.NORMAL), dtype=torch.uint8,
                              device=self.world.device)
         o = self.world._out
-        return self._obs(), self._info(status, traffic, torch.zeros_like(o.flags), torch.full_like(o.hit_index, -1),
-                                       torch.full_like(o.hit_segment, -1))
+        obs = self._obs()
+        info = self._info(status, traffic, torch.zeros_like(o.flags), torch.full_like(o.hit_index, -1),
+                          torch.full_like(o.hit_segment, -1))
+        return obs, self._add_lidar(info)
 
     def step(self, action, npc_action=None):
         """``action``: fp32 device tensor [N, 2] = (steering, accel) of the ego (participant 0), or [N, M, 2] for
@@ -223,7 +244,8 @@ class BatchedTrafficEnv:
             info["agent_status"], info["agent_iou"] = a.status, a.iou
             if self.auto_reset:
                 self.scenario_manager.reset(mask=a.done, pool_index=w.log_row)
-            return self._obs(), a.reward, a.terminated, a.truncated, info
+            obs = self._obs()
+            return obs, a.reward, a.terminated, a.truncated, self._add_lidar(info)
         status, traffic = self.scenario_manager.check_status()
         e = self.scenario_manager.env_result
         r = w.result
@@ -232,7 +254,8 @@ class BatchedTrafficEnv:
             info["iou"] = r.iou
         if self.auto_reset:
             self.scenario_manager.reset(mask=e.done, pool_index=w.log_row)   # (a log: restart the scenario's row)
-        return self._obs(), e.reward, e.terminated, e.truncated, info
+        obs = self._obs()
+        return obs, e.reward, e.terminated, e.truncated, self._add_lidar(info)
 
     def render(self):
         raise NotImplementedError("rendering is outside this hot path")

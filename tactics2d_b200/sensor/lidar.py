@@ -2,7 +2,8 @@
 ``point_density = max(int(freq_detect / freq_scan), 1)`` beams over a full turn, ``angle_resolution = 2 pi /
 point_density``, range ``perception_range``.  ``scan(world)`` runs ``_scan_obstacles`` (:128-221) for the ego of
 every scenario of a :class:`tactics2d_b200.BatchedWorld` in one kernel launch and returns the [N, point_density]
-distance tensor (``inf`` = nothing within range), i.e. the batched ``scan_result``."""
+distance tensor (``inf`` = nothing within range), i.e. the batched ``scan_result``; ``scan_agents(world, observers)``
+scans from every row of an observer list instead, [N, Q, point_density]."""
 
 from __future__ import annotations
 
@@ -30,6 +31,12 @@ class SingleLineLidar:
     def scan(self, world):
         self.scan_result = world.lidar_scan(self.point_density, self.max_perception_distance)
         return self.scan_result
+
+    def scan_agents(self, world, observers=None):
+        """The same sensor bound to a list of observer slots per scenario (``bind_with(j)`` for each row's slot j;
+        ``BatchedWorld.lidar_scan_agents``): fp32 [N, Q, point_density].  ``observers``: int16 [N, Q] device tensor, or
+        None for every slot.  Does not touch ``scan_result``, which stays the ego's scan."""
+        return world.lidar_scan_agents(self.point_density, self.max_perception_distance, observers)
 
     def get_points(self, world):
         """Point cloud in the global frame (``_get_points``, lidar.py:223-243): [N, point_density, 2], NaN where no hit."""

@@ -688,6 +688,27 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_lidar_scan(self._ctx, int(n_beams), float(max_range), _ptr(cache[1]), _ptr(cache[2]), self._stream()))
         return cache[2]
 
+    def lidar_scan_agents(self, n_beams: int = 500, max_range: float = 12.0,
+                          observers: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``lidar_scan`` with the sensor on a list of observer slots per scenario, in one launch
+        (``t2d_lidar_scan_agents``; DESIGN.md section 1 "Per-agent lidar"): the reference's ``SingleLineLidar`` bound to
+        each row's slot, which sees the map and every other box-shaped participant, slot 0 included.  ``observers``: int16
+        ``[N, Q]`` device tensor as in ``observe_agents`` (None: every slot, Q = M); a value outside ``[0, M)`` or an empty
+        slot gives a row of ``inf``.  Returns fp32 ``[N, Q, n_beams]``, a buffer per ``(n_beams, max_range, Q)`` that the
+        next call with those values reuses.  A row observed by slot 0 equals ``lidar_scan``'s row."""
+        Q = self._agent_rows(observers, None)
+        key = (int(n_beams), float(max_range), Q)
+        cache = self.__dict__.setdefault("_agent_lidar", {})
+        entry = cache.get(key)
+        if entry is None:
+            theta = np.linspace(0, 2 * np.pi, int(n_beams), endpoint=False)          # lidar.py:160
+            cs = torch.from_numpy(np.stack([np.cos(theta), np.sin(theta)], 1)).to(self.device)   # float64, host trig
+            scan = torch.empty((self.N, Q, int(n_beams)), dtype=torch.float32, device=self.device)
+            entry = cache[key] = (cs.contiguous(), scan)
+        _lib.check(self.lib.t2d_lidar_scan_agents(self._ctx, _ptr(observers), Q, int(n_beams), float(max_range),
+                                                  _ptr(entry[0]), _ptr(entry[1]), self._stream()))
+        return entry[1]
+
     # ------------------------------------------------------------------ BEV observation
     @staticmethod
     def _check_style_keys(keys, n_seg):
