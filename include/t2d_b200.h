@@ -563,6 +563,11 @@ int t2d_set_prefetch(t2d_ctx* ctx, int mode);
 /* Number of kernels this library has launched since load (bench.py's gpu_launches). */
 int64_t t2d_launch_count(void);
 
+/* Number of ticks launched through the tick kernel's instance compiled for M = 64: kinematic types only, aligned
+   state, no ego action and no goal (the others run the generic instance, which computes the same bits).
+   The environment variable T2D_TICK_GENERIC=1, read at t2d_create, keeps a world on the generic instance. */
+int64_t t2d_tick_fixed_count(void);
+
 #ifdef __cplusplus
 }
 #endif

@@ -108,6 +108,7 @@ SYMBOLS = {
     "t2d_set_log_schedule": (C.c_int, [_P, C.POINTER(LogC), _P, _P, C.c_int32, _P]),
     "t2d_set_prefetch": (C.c_int, [_P, C.c_int]),
     "t2d_launch_count": (C.c_int64, []),
+    "t2d_tick_fixed_count": (C.c_int64, []),
 }
 
 _lib = None

@@ -555,19 +555,47 @@ __device__ __noinline__ unsigned ego_goal_events(const StepArgs& A, long long n,
   return r;
 }
 
+// The launch shape K1's FIXED instance is compiled for (C2: M = 64 participants, so G = 16 lanes and MP = 64 padded
+// slots per scenario; kinematic physics on, vector access, no velocity inputs, no ego action, no goal).  The host
+// launches it exactly when a tick has this shape and the generic instance otherwise.
+constexpr int FIX_M = 64, FIX_G = 16, FIX_G_SHIFT = 4, FIX_MP_SHIFT = 6;
+
 // L2 prefetch of the lines a lane's PPL participants will load (state, action, type ids).
+template <bool FIXED>
 __device__ __forceinline__ void prefetch_tile_l2(const StepArgs& A, long long i) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.x + i));
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.y + i));
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.h + i));
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.v + i));
-  if (A.action) asm volatile("prefetch.global.L2 [%0];" ::"l"(A.action + 2 * i));
+  if (FIXED || A.action) asm volatile("prefetch.global.L2 [%0];" ::"l"(A.action + 2 * i));
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.type_id + i));
-  if (A.needs_vel_in) {
+  if (!FIXED && A.needs_vel_in) {
     asm volatile("prefetch.global.L2 [%0];" ::"l"(A.vx + i));
     asm volatile("prefetch.global.L2 [%0];" ::"l"(A.vy + i));
   }
 }
+
+// ---------------------------------------------------------------------------- K1 phase timeline (measurement build)
+// Built with -DT2D_TICK_TIMELINE (bench_tick_phases.py compiles such a library on the side), lane 0 of every warp
+// records %globaltimer and %clock64 at TL_POINTS points of its first tile: entry, after griddepcontrol.wait, loads
+// consumed, physics done, sort done, sweep done, drain done, static done, exit.  A point waits for the value `dep` it is
+// given, so that it marks when that value was available rather than when its instruction was issued.  In the shipped
+// build T2D_TL expands to nothing and the kernel is unchanged.
+#ifdef T2D_TICK_TIMELINE
+constexpr int TL_POINTS = 9, TL_MAX_WARPS = 4096;
+__device__ unsigned long long t2d_timeline[TL_MAX_WARPS][TL_POINTS][2];
+#define T2D_TL(k, on, slot, dep)                                                                                    \
+  do {                                                                                                              \
+    if ((on) && (slot) < TL_MAX_WARPS) {                                                                            \
+      unsigned long long g_, c_;                                                                                    \
+      asm volatile("mov.u64 %0, %%globaltimer;\n\tmov.u64 %1, %%clock64;" : "=l"(g_), "=l"(c_) : "f"(dep) : "memory"); \
+      t2d_timeline[slot][k][0] = g_;                                                                                \
+      t2d_timeline[slot][k][1] = c_;                                                                                \
+    }                                                                                                               \
+  } while (0)
+#else
+#define T2D_TL(k, on, slot, dep)
+#endif
 
 // ---------------------------------------------------------------------------- K1
 // KIN_ONLY: every type in the table is SingleTrackKinematics or static - the fp64 models are compiled out
@@ -575,9 +603,15 @@ __device__ __forceinline__ void prefetch_tile_l2(const StepArgs& A, long long i)
 // MAP_TABLE: every scenario names its own static-geometry tile (t2d_set_map_table); the tiles are then read from global
 // memory, header included.  Otherwise one tile serves all scenarios: header in the constant bank, sections staged into
 // shared memory once per CTA.
-template <bool KIN_ONLY, bool MAP_TABLE>
+// FIXED: the tick has the C2 launch shape (FIX_M ...): every shape value is a compile-time constant, so the sort network
+// and the status reduction unroll, addresses fold, and the tests for features that shape excludes go away.  The
+// physics and every other operation on the data are the generic instance's: only control flow and addresses differ.
+// (The sub-step loop keeps its runtime trip count: unrolled, the compiler fuses multiplies and adds that the loop keeps
+// in separate blocks into FMAs, which changes result bits.)
+template <bool KIN_ONLY, bool MAP_TABLE, bool FIXED>
 __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_constant__ StepArgs A) {
   extern __shared__ __align__(128) unsigned char smem[];
+  T2D_TL(0, (threadIdx.x & 31) == 0, (int)(blockIdx.x * A.wpc + (threadIdx.x >> 5)), 0.0f);
   // carve: [map blob | 16B aligned] [type table] [pose tiles, hit mins, queues, positions] [mbarrier]; every
   // offset, shift and count that depends only on the launch shape comes precomputed from the host
   // (kernel-parameter constant bank) instead of integer divisions / loops per thread
@@ -618,17 +652,20 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
   // peer-memory done exchange running under the tick the burst of prefetches competes with the exchange kernel's peer
   // stores and system-scope fence, and the exchange chain then sets the pace, so the host leaves it off while an
   // exchange object is alive in the process (T2D_PREFETCH=0 / 1 overrides).
+  // a launch-shape parameter, or the constant it is in the FIXED instance (read where it is used, as before)
+#define K1_SHAPE(field, fixed_value) (FIXED ? (fixed_value) : A.field)
   {
-    const long long n_ = ((long long)blockIdx.x * wpc + warp) * (32 >> A.g_shift) + (lane >> A.g_shift);
-    const int m_ = (lane & (A.G - 1)) * PPL;
-    if (A.prefetch && n_ < A.N && m_ < A.M) prefetch_tile_l2(A, n_ * A.M + m_);   // (inside the arrays: a hint, but no stray addresses)
+    const long long n_ = ((long long)blockIdx.x * wpc + warp) * (32 >> K1_SHAPE(g_shift, FIX_G_SHIFT)) + (lane >> K1_SHAPE(g_shift, FIX_G_SHIFT));
+    const int m_ = (lane & (K1_SHAPE(G, FIX_G) - 1)) * PPL;
+    if (A.prefetch && n_ < A.N && m_ < K1_SHAPE(M, FIX_M)) prefetch_tile_l2<FIXED>(A, n_ * K1_SHAPE(M, FIX_M) + m_);   // (inside the arrays: a hint, but no stray addresses)
   }
   // ... and wait here, before the first access to the state the previous tick wrote, until that grid has
   // completed and flushed (no-op when the kernel was not launched as a programmatic dependent).
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  const int G = A.G, M = A.M;
-  const int spw = 32 >> A.g_shift;      // scenarios per warp
-  const int sub = lane >> A.g_shift;    // scenario slot inside the warp
+  T2D_TL(1, lane == 0, (int)blockIdx.x * wpc + warp, 0.0f);
+  const int G = K1_SHAPE(G, FIX_G), M = K1_SHAPE(M, FIX_M);
+  const int spw = 32 >> K1_SHAPE(g_shift, FIX_G_SHIFT);   // scenarios per warp
+  const int sub = lane >> K1_SHAPE(g_shift, FIX_G_SHIFT);   // scenario slot inside the warp
   const int gl = lane & (G - 1);        // lane inside the group
   const int m0 = gl * PPL;              // first participant of this lane
   const int MP = G * PPL;               // padded participants per scenario
@@ -639,7 +676,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
   unsigned* queue = s_queue + warp * QCAP;
   int* qcount = s_qcount + warp;
   const int tb = sub * MP, t0 = tb + m0;
-  const int mp_shift = A.mp_shift;   // MP = 1 << mp_shift
+  const int mp_shift = K1_SHAPE(mp_shift, FIX_MP_SHIFT);   // MP = 1 << mp_shift
   float4* sorted = s_sorted + warp * POSE_PER_WARP + tb;   // this scenario's x-sorted list (sweep_pair)
   const int Mh = M >> 1;                // partner offsets 1..Mh cover every unordered pair
 
@@ -647,9 +684,13 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
   for (int tile = (int)blockIdx.x * wpc + warp; tile < n_tiles; tile += (int)gridDim.x * wpc) {
     const long long n = (long long)tile * spw + sub;
     const bool scn_ok = n < A.N;
-    int nvalid = scn_ok ? min(PPL, M - m0) : 0;
+    int nvalid = scn_ok ? (FIXED ? PPL : min(PPL, M - m0)) : 0;
     if (nvalid < 0) nvalid = 0;
     const long long idx0 = n * M + m0;
+#ifdef T2D_TICK_TIMELINE
+    const bool tl_on = lane == 0 && tile == (int)blockIdx.x * wpc + warp;
+    const int tl_slot = tile;
+#endif
 
     // ------------------------------------------------------------------ load
     float sx[PPL], sy[PPL], shd[PPL], sv[PPL], svx[PPL], svy[PPL], a0[PPL], a1[PPL];
@@ -659,7 +700,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       sx[i] = sy[i] = shd[i] = sv[i] = svx[i] = svy[i] = a0[i] = a1[i] = 0.0f;
       tidv[i] = T2D_TYPE_INACTIVE;
     }
-    if (nvalid == PPL && A.vec_ok) {
+    if (nvalid == PPL && K1_SHAPE(vec_ok, 1)) {
       ld_vec<float, PPL>(A.x + idx0, sx);
       ld_vec<float, PPL>(A.y + idx0, sy);
       ld_vec<float, PPL>(A.h + idx0, shd);
@@ -668,7 +709,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       ld_vec<uint8_t, PPL>(A.type_id + idx0, tb8);
 #pragma unroll
       for (int i = 0; i < PPL; ++i) tidv[i] = tb8[i];
-      if (A.do_physics) {
+      if (K1_SHAPE(do_physics, 1)) {
         float2 act[PPL];
         float lo[4], hi[4];
         ld_vec<float, 4>(A.action + 2 * idx0, lo);
@@ -677,7 +718,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         act[2] = make_float2(hi[0], hi[1]); act[3] = make_float2(hi[2], hi[3]);
 #pragma unroll
         for (int i = 0; i < PPL; ++i) { a0[i] = act[i].x; a1[i] = act[i].y; }
-        if (A.needs_vel_in) {
+        if (K1_SHAPE(needs_vel_in, 0)) {
           ld_vec<float, PPL>(A.vx + idx0, svx);
           ld_vec<float, PPL>(A.vy + idx0, svy);
         }
@@ -690,19 +731,19 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         if (i < nvalid) {
           sx[i] = A.x[idx0 + i]; sy[i] = A.y[idx0 + i]; shd[i] = A.h[idx0 + i]; sv[i] = A.v[idx0 + i];
           tidv[i] = A.type_id[idx0 + i];
-          if (A.do_physics) {
+          if (K1_SHAPE(do_physics, 1)) {
             a0[i] = A.action[2 * (idx0 + i)]; a1[i] = A.action[2 * (idx0 + i) + 1];
-            if (A.needs_vel_in) { svx[i] = A.vx[idx0 + i]; svy[i] = A.vy[idx0 + i]; }
+            if (K1_SHAPE(needs_vel_in, 0)) { svx[i] = A.vx[idx0 + i]; svy[i] = A.vy[idx0 + i]; }
           }
         }
       }
     }
     {   // several tiles per warp (persistent CTAs): the next tile's lines start their way to L2 now
       const long long n_next = n + (long long)gridDim.x * wpc * spw;
-      if (A.prefetch && n_next < A.N && m0 < M) prefetch_tile_l2(A, n_next * M + m0);
+      if (A.prefetch && n_next < A.N && m0 < M) prefetch_tile_l2<FIXED>(A, n_next * M + m0);
     }
-    if (A.ego_action != nullptr && A.do_physics && gl == 0 && scn_ok) {   // the ego's action comes from its own [N, 2] array
-      const float2 ea = reinterpret_cast<const float2*>(A.ego_action)[n];
+    if (K1_SHAPE(ego_action, nullptr) != nullptr && K1_SHAPE(do_physics, 1) && gl == 0 && scn_ok) {   // the ego's action comes from its own [N, 2] array
+      const float2 ea = reinterpret_cast<const float2*>(K1_SHAPE(ego_action, nullptr))[n];
       a0[0] = ea.x; a1[0] = ea.y;
     }
     if (!staged) {   // table + map tile landed? (first tile only)
@@ -725,6 +766,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       lane_any_kin = lane_any_kin || kin[i];
       ch[i] = 1.0f; sh[i] = 0.0f;
     }
+    T2D_TL(2, tl_on, tl_slot, sx[PPL - 1] + sy[PPL - 1] + shd[PPL - 1] + sv[PPL - 1] + a0[PPL - 1] + a1[PPL - 1] + (float)model[PPL - 1]);
     if (A.cfg_flags & T2D_CFG_STEER_FIRST) {
 #pragma unroll
       for (int i = 0; i < PPL; ++i)
@@ -732,7 +774,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
     }
 
     // ------------------------------------------------------------------ physics
-    if (A.do_physics) {
+    if (K1_SHAPE(do_physics, 1)) {
       // Kinematic participants of the whole warp advance together in the 4-chain loop; slots holding another
       // model (or nothing) ride along on a neutral row (zero speed / action, unbounded ranges) and are discarded.
       if (__any_sync(0xffffffffu, lane_any_kin)) {
@@ -777,7 +819,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       bool all_active = true;
 #pragma unroll
       for (int i = 0; i < PPL; ++i) all_active = all_active && active[i];
-      if (nvalid == PPL && A.vec_ok && all_active) {   // (an inactive slot keeps its state: vx, vy may not even be loaded)
+      if (nvalid == PPL && K1_SHAPE(vec_ok, 1) && all_active) {   // (an inactive slot keeps its state: vx, vy may not even be loaded)
         st_vec<float, PPL>(A.x + idx0, sx);
         st_vec<float, PPL>(A.y + idx0, sy);
         st_vec<float, PPL>(A.h + idx0, shd);
@@ -797,6 +839,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
 #pragma unroll
       for (int i = 0; i < PPL; ++i) sincos_fast(shd[i], &sh[i], &ch[i]);
     }
+    T2D_TL(3, tl_on, tl_slot, sx[0] + sy[PPL - 1] + ch[0] + sh[PPL - 1]);
 
     // ------------------------------------------------------------------ poses -> shared
     // Only (x, y, bounding radius) stay in registers; the full pose lives in the warp's smem tile.
@@ -819,7 +862,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
     // the step counter of the status section: fetched here - behind the state stores, so it cannot be hoisted to the top
     // of the tile (where ptxas spilled it, stalling the warp on HBM before its state loads were even issued), and with
     // the whole collision phase in front of its first use
-    const int cnt_in = (A.do_physics && gl == 0 && scn_ok) ? A.step_count[n] : 0;
+    const int cnt_in = (K1_SHAPE(do_physics, 1) && gl == 0 && scn_ok) ? A.step_count[n] : 0;
 
     // static broadphase level 1 (clearance field: one byte per participant through L1/L2), issued here so that
     // its global-load latency hides behind the partner loop
@@ -877,6 +920,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         }
         cx(0, 2, desc); cx(1, 3, desc); cx(0, 1, desc); cx(2, 3, desc);
       }
+      T2D_TL(4, tl_on, tl_slot, __uint_as_float(key[0] ^ key[PPL - 1]));
       // (2) Stage the sorted list: entry 4 gl + k = (x, y, -thr, key) of the slot the key names, from the pose tile.
       float4 own[PPL];
 #pragma unroll
@@ -948,6 +992,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
           if (stop) break;
         }
       }
+      T2D_TL(5, tl_on, tl_slot, xmax);
 #pragma unroll
       for (int i = 0; i < PPL; ++i) hitmin[i * 32 + lane] = 0x7fffffff;
       __syncwarp();   // the queue holds every candidate
@@ -971,6 +1016,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       if (lane == 0) *qcount = 0;
       __syncwarp();
     }
+    T2D_TL(6, tl_on, tl_slot, (float)(hit[0] + hit[PPL - 1]));
 
     // ------------------------------------------------------------------ static collision
     int hseg[PPL];
@@ -990,6 +1036,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         }
       }
     }
+    T2D_TL(7, tl_on, tl_slot, (float)(hseg[0] + hseg[PPL - 1]));
 
     // ------------------------------------------------------------------ out of bound + flags
     // the boundary box of this lane's scenario (Map.boundary of its tile)
@@ -1017,7 +1064,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       for (int i = 0; i < PPL; ++i)
         if (((oob_check >> i) & 1u) && oob_slow(poseA, poseB, t0 + i, bxmin, bxmax, bymin, bymax)) fl[i] |= T2D_F_OUTBOUND;
     }
-    if (nvalid == PPL && A.vec_ok) {
+    if (nvalid == PPL && K1_SHAPE(vec_ok, 1)) {
       int16_t h16[PPL], s16[PPL];
 #pragma unroll
       for (int i = 0; i < PPL; ++i) { h16[i] = (int16_t)hit[i]; s16[i] = (int16_t)hseg[i]; }
@@ -1036,7 +1083,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
     }
 
     // ------------------------------------------------------------------ scenario status
-    if (A.do_physics) {
+    if (K1_SHAPE(do_physics, 1)) {
       unsigned agg;
       if (A.cfg_flags & T2D_CFG_ANY_PARTICIPANT) {
         agg = 0;
@@ -1051,7 +1098,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         A.step_count[n] = cnt;
         uint8_t st = T2D_STATUS_NORMAL;
         unsigned goal = 0;
-        if (A.goal_target != nullptr) {   // the ego is participant 0 = this lane's first slot
+        if (K1_SHAPE(goal_target, nullptr) != nullptr) {   // the ego is participant 0 = this lane's first slot
           const float4 ea = poseA[pslot(t0)], eb = poseB[pslot(t0)];
           if (ea.x == ea.x && eb.w >= 0.0f) goal = ego_goal_events(A, n, ea.x, ea.y, ea.w, eb.z, eb.w);
         }
@@ -1065,9 +1112,11 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         if (A.done) A.done[n] = st != T2D_STATUS_NORMAL;             // parking.py:243-248
       }
     }
+    T2D_TL(8, tl_on, tl_slot, 0.0f);
     __syncwarp();   // pose tile is reused by the next tile
   }
   if (!staged) mbar_wait(s_bar, 0);   // never leave a bulk copy in flight at exit
+#undef K1_SHAPE
 }
 
 // ---------------------------------------------------------------------------- K2
@@ -1978,9 +2027,10 @@ using namespace t2d;
 
 static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
+static std::atomic<long long> g_fixed_ticks{0};   // ticks launched through K1's FIXED instance
 static std::atomic<int> g_exchanges_alive{0};   // peer-memory done exchanges in this process (see StepArgs::prefetch)
 static std::mutex g_smem_mutex;
-static int g_smem_configured[64][4];   // [device][kernel variant]: dynamic shared memory opted in so far (process-wide)
+static int g_smem_configured[64][6];   // [device][kernel variant]: dynamic shared memory opted in so far (process-wide)
 
 static int fail(int code, const std::string& msg) {
   g_err = msg;
@@ -2140,6 +2190,7 @@ struct t2d_ctx {
   int prefetch_override = -1;      // T2D_PREFETCH=0 / 1 (experiments; -1 = on unless a done exchange is alive)
   int wpc_override = 0;            // T2D_WPC=w: warps per CTA of the tick (experiments; 0 = pick from the batch size)
   int grid_limit = 0;              // T2D_GRID_LIMIT=k: at most k CTAs of the persistent tick grid per SM (experiments; 0 = occupancy)
+  bool tick_generic = false;       // T2D_TICK_GENERIC=1: never launch K1's FIXED instance (tests compare the two)
   int occ_smem[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};   // per warps-per-CTA: smem the cached occupancy was computed for
   int occ_val[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   int occ_variant[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -2213,6 +2264,22 @@ extern "C" {
 int t2d_version(void) { return T2D_VERSION; }
 const char* t2d_last_error(void) { return g_err.c_str(); }
 int64_t t2d_launch_count(void) { return (int64_t)g_launches.load(); }
+int64_t t2d_tick_fixed_count(void) { return (int64_t)g_fixed_ticks.load(); }
+
+#ifdef T2D_TICK_TIMELINE
+// The phase timeline of the last tick (measurement build only): [TL_MAX_WARPS][TL_POINTS][globaltimer, clock64],
+// zeroed after the copy when `clear` is set.
+int t2d_tick_timeline(void* dst, int64_t bytes, int clear) {
+  if (!dst || bytes != (int64_t)sizeof(t2d_timeline)) return fail(T2D_E_INVALID, "timeline buffer size");
+  CUDA_TRY(cudaMemcpyFromSymbol(dst, t2d_timeline, sizeof(t2d_timeline)));
+  if (clear) {
+    void* p = nullptr;
+    CUDA_TRY(cudaGetSymbolAddress(&p, t2d_timeline));
+    CUDA_TRY(cudaMemset(p, 0, sizeof(t2d_timeline)));
+  }
+  return T2D_OK;
+}
+#endif
 
 static int check_cfg(const t2d_config* cfg) {
   if (!cfg) return fail(T2D_E_INVALID, "cfg is NULL");
@@ -2238,6 +2305,7 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
   c->M = m_participants;
   if (const char* e = getenv("T2D_PDL")) c->use_pdl = atoi(e) != 0;
   if (const char* e = getenv("T2D_GRID_LIMIT")) c->grid_limit = std::max(0, atoi(e));
+  if (const char* e = getenv("T2D_TICK_GENERIC")) c->tick_generic = atoi(e) != 0;
   if (const char* e = getenv("T2D_PREFETCH")) c->prefetch_override = atoi(e) != 0 ? 1 : 0;
   if (const char* e = getenv("T2D_WPC")) {
     const int v = atoi(e);
@@ -2823,12 +2891,16 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
   if (smem > c->max_smem_optin) return fail(T2D_E_UNSUPPORTED, "shared memory budget exceeded");
   using kernel_t = void (*)(StepArgs);
   kernel_t kern;
-  if (c->kin_only) kern = map_table ? (kernel_t)t2d_step_kernel<true, true> : (kernel_t)t2d_step_kernel<true, false>;
-  else kern = map_table ? (kernel_t)t2d_step_kernel<false, true> : (kernel_t)t2d_step_kernel<false, false>;
+  // the C2-shaped instance exactly when this tick has the shape it is compiled for (FIX_M ...)
+  const bool fixed = c->kin_only && !c->tick_generic && c->M == FIX_M && c->G == FIX_G && do_physics && A.vec_ok &&
+                     !A.needs_vel_in && A.ego_action == nullptr && A.goal_target == nullptr;
+  if (fixed) kern = map_table ? (kernel_t)t2d_step_kernel<true, true, true> : (kernel_t)t2d_step_kernel<true, false, true>;
+  else if (c->kin_only) kern = map_table ? (kernel_t)t2d_step_kernel<true, true, false> : (kernel_t)t2d_step_kernel<true, false, false>;
+  else kern = map_table ? (kernel_t)t2d_step_kernel<false, true, false> : (kernel_t)t2d_step_kernel<false, false, false>;
+  const int variant = (fixed ? 4 : c->kin_only ? 2 : 0) + (map_table ? 1 : 0);
   {
     // cudaFuncSetAttribute applies to the kernel function for the whole process and SETS the value: worlds of
     // different sizes share it, so the opt-in is tracked per (device, kernel variant) and only ever raised.
-    const int variant = (c->kin_only ? 2 : 0) + (map_table ? 1 : 0);
     std::lock_guard<std::mutex> lock(g_smem_mutex);
     int& configured = g_smem_configured[c->device % 64][variant];
     if (smem > configured) {
@@ -2843,12 +2915,12 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
     if (int r = launched()) return r;
   }
   const long long ctas_needed = (tiles + wpc - 1) / wpc;
-  if (c->occ_smem[wpc] != smem || c->occ_variant[wpc] != (map_table ? 1 : 0)) {
+  if (c->occ_smem[wpc] != smem || c->occ_variant[wpc] != variant) {
     int per_sm = 1;
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, wpc * 32, smem));
     c->occ_val[wpc] = per_sm < 1 ? 1 : per_sm;
     c->occ_smem[wpc] = smem;
-    c->occ_variant[wpc] = map_table ? 1 : 0;
+    c->occ_variant[wpc] = variant;
   }
   int per_sm_ctas = c->occ_val[wpc];
   if (c->grid_limit > 0) per_sm_ctas = std::min(per_sm_ctas, c->grid_limit);   // T2D_GRID_LIMIT: leave CTA slots to other streams
@@ -2865,6 +2937,7 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, A));
+  if (fixed) g_fixed_ticks.fetch_add(1);
   return launched();
 }
 
