@@ -568,6 +568,14 @@ int64_t t2d_launch_count(void);
    The environment variable T2D_TICK_GENERIC=1, read at t2d_create, keeps a world on the generic instance. */
 int64_t t2d_tick_fixed_count(void);
 
+/* Number of launches of the tick kernel (t2d_step and every call that ticks or checks events) since load that the CUDA
+   runtime accepted (a fault while the kernel runs is not seen here), per instance:
+   k = 0 / 1: fp64 models compiled in (the table holds a type that is neither kinematic nor static), one map tile / a map
+   table; k = 2 / 3: kinematic and static types only, one tile / table; k = 4 / 5: the M = 64 instance of
+   t2d_tick_fixed_count, one tile / table.  k = 6: launches with one map tile too large for shared memory, which read it
+   from global memory.  Returns -1 for any other k. */
+int64_t t2d_tick_instance_count(int k);
+
 #ifdef __cplusplus
 }
 #endif

@@ -109,6 +109,7 @@ SYMBOLS = {
     "t2d_set_prefetch": (C.c_int, [_P, C.c_int]),
     "t2d_launch_count": (C.c_int64, []),
     "t2d_tick_fixed_count": (C.c_int64, []),
+    "t2d_tick_instance_count": (C.c_int64, [C.c_int]),
 }
 
 _lib = None

@@ -2027,7 +2027,8 @@ using namespace t2d;
 
 static thread_local std::string g_err;
 static std::atomic<long long> g_launches{0};
-static std::atomic<long long> g_fixed_ticks{0};   // ticks launched through K1's FIXED instance
+// K1 launches per instance (launch_step's `variant`), then the one-tile launches that read the map from global memory
+static std::atomic<long long> g_tick_instances[7] = {};
 static std::atomic<int> g_exchanges_alive{0};   // peer-memory done exchanges in this process (see StepArgs::prefetch)
 static std::mutex g_smem_mutex;
 static int g_smem_configured[64][6];   // [device][kernel variant]: dynamic shared memory opted in so far (process-wide)
@@ -2264,7 +2265,8 @@ extern "C" {
 int t2d_version(void) { return T2D_VERSION; }
 const char* t2d_last_error(void) { return g_err.c_str(); }
 int64_t t2d_launch_count(void) { return (int64_t)g_launches.load(); }
-int64_t t2d_tick_fixed_count(void) { return (int64_t)g_fixed_ticks.load(); }
+int64_t t2d_tick_fixed_count(void) { return (int64_t)(g_tick_instances[4].load() + g_tick_instances[5].load()); }
+int64_t t2d_tick_instance_count(int k) { return k >= 0 && k < 7 ? (int64_t)g_tick_instances[k].load() : -1; }
 
 #ifdef T2D_TICK_TIMELINE
 // The phase timeline of the last tick (measurement build only): [TL_MAX_WARPS][TL_POINTS][globaltimer, clock64],
@@ -2937,8 +2939,10 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, A));
-  if (fixed) g_fixed_ticks.fetch_add(1);
-  return launched();
+  if (int r = launched()) return r;
+  g_tick_instances[variant].fetch_add(1);
+  if (!map_table && map.blob && map.mh.n_seg > 0 && !A.map_in_smem) g_tick_instances[6].fetch_add(1);
+  return T2D_OK;
 }
 
 // K5 with the ego action `ego` (nullptr: row 0 of `action`)
