@@ -121,14 +121,8 @@ T2D_HD void pixel_world(const View& v, const Window& w, int r, int c, double& X,
 #if defined(__CUDACC__)
 namespace bev {
 
-struct Args {
-  const float *x, *y, *h;
-  const uint8_t* type_id;
-  const Params* table;
-  int n_types, N, M;
-  const unsigned char* map_blob;   // tiles as in K1 / the lidar; nullptr when no tile has geometry
-  const uint32_t* tile_off;
-  const uint16_t* tile_id;         // nullptr: tile 0 for every scenario
+struct Args : WorldArgs {
+  MapArgs map;
   const uint8_t* seg_style;        // per segment, tiles back to back (seg_base[tile] + segment), or nullptr: defaults
   const uint32_t* seg_base;        // [n_tiles]
   const float* target;             // [N][5] goal rectangles, or nullptr
@@ -314,7 +308,7 @@ __global__ void __launch_bounds__(CTA) t2d_bev_kernel(const __grid_constant__ Ar
   const long long n = blockIdx.x;
   const int tid = threadIdx.x;
   if (tid == 0) {
-    const unsigned char* blob = A.map_blob ? A.map_blob + (A.tile_id ? A.tile_off[A.tile_id[n]] : 0u) : nullptr;
+    const unsigned char* blob = tile_blob(A.map, n);
     const MapHeader* mh = reinterpret_cast<const MapHeader*>(blob);
     S.blob = blob;
     S.n_seg = blob ? mh->n_seg : 0;
@@ -324,7 +318,7 @@ __global__ void __launch_bounds__(CTA) t2d_bev_kernel(const __grid_constant__ Ar
     S.pbox = blob ? reinterpret_cast<const float4*>(blob + mh->off_pbox) : nullptr;
     S.ring_lo = S.n_poly > 0 ? S.pstart[0] : 0;
     S.ring_hi = S.n_poly > 0 ? S.pstart[S.n_poly] : 0;
-    S.sstyle = A.seg_style ? A.seg_style + A.seg_base[A.tile_id ? A.tile_id[n] : 0] : nullptr;
+    S.sstyle = A.seg_style ? A.seg_style + A.seg_base[A.map.tile_id ? A.map.tile_id[n] : 0] : nullptr;
     S.n_cand = 1 + S.n_poly + S.n_seg + 2 * A.M;
     View v;
     const int t0 = A.type_id[n * A.M];

@@ -72,6 +72,39 @@ struct MapHeader {   // 128 bytes, start of a tile's blob
 constexpr float CLEAR_QUANT = 0.125f;   // metres per unit of the byte-quantised fine clearance field
 static_assert(sizeof(MapHeader) == 128, "MapHeader must be 128 bytes");
 
+// The bound world as t2d_ctx holds it (world_args): the state and the type table every kernel besides K1, its drift
+// pre-pass and K7 reads.  Their argument structs derive from it.
+struct WorldArgs {
+  float *x, *y, *h, *v, *vx, *vy;  // [N][M]
+  const uint8_t* type_id;          // [N][M]
+  int32_t* step_count;             // [N]
+  const Params* table;             // device
+  int n_types, N, M;
+};
+
+// The bound map as K4, K6 and K8 / K9 read it (map_args); tile_blob finds a scenario's tile in it.
+struct MapArgs {
+  const unsigned char* map_blob;   // device: the tiles' blobs, one after the other; nullptr when no tile has segments
+  const uint32_t* tile_off;        // [n_tiles] byte offset of every tile's blob
+  const uint16_t* tile_id;         // [N] the tile of every scenario, or nullptr: every scenario uses tile 0
+};
+
+// The blob of scenario n's tile, or nullptr when no tile has geometry (tile 0 starts the blob: no table, no lookup)
+__device__ __forceinline__ const unsigned char* tile_blob(const MapArgs& m, long long n) {
+  return m.map_blob ? m.map_blob + (m.tile_id ? m.tile_off[m.tile_id[n]] : 0u) : nullptr;
+}
+
+// The Arrival / NoAction detector state of a set of rows (ego_goal_events): the ego of every scenario (t2d_set_goal,
+// [N] rows) or every agent row (t2d_set_agents, [N][Q] rows).
+struct GoalArgs {
+  const float* target;             // [rows][5] cx, cy, heading, half_len, half_wid of the target area, or nullptr
+  float* iou;                      // [rows]
+  float* last_pose;                // [rows][4] x, y, heading, valid
+  int32_t* noact_count;            // [rows]
+  float threshold;
+  int noact_max;
+};
+
 struct StepArgs {
   float *x, *y, *h, *v, *vx, *vy;
   const uint8_t* type_id;
@@ -102,12 +135,7 @@ struct StepArgs {
   int prefetch;                    // L2 prefetch of tile inputs ahead of their loads (see the kernel prologue)
   float bxmin, bxmax, bymin, bymax;
   float rb_max;                    // largest bounding radius in the type table (broadphase threshold)
-  const float* goal_target;        // [N][5] cx, cy, heading, half_len, half_wid of the target area, or nullptr
-  float* goal_iou;                 // [N]
-  float* goal_last_pose;           // [N][4] x, y, heading, valid
-  int32_t* goal_noact_count;       // [N]
-  float goal_threshold;
-  int goal_noact_max;
+  GoalArgs goal;                   // the ego's; goal.target == nullptr: no goal
   float *wheel_f, *wheel_r;        // [N][M] wheel angular speeds of the SingleTrackDrift participants, or nullptr
 };
 
@@ -533,25 +561,30 @@ __device__ __noinline__ bool oob_slow(const float4* poseA, const float4* poseB, 
   return r != 0;
 }
 
-// Arrival (arrival.py:32-47) and NoAction (no_action.py:32-53) for the ego of scenario n; returns bit0 = arrived,
-// bit1 = no action for more than max_step consecutive ticks.  One lane per scenario, fp64, out of line.
-__device__ __noinline__ unsigned ego_goal_events(const StepArgs& A, long long n, float ex, float ey, float eh, float el, float ew) {
+// Arrival (arrival.py:32-47) and NoAction (no_action.py:32-53) for row n of the detector record A.goal; returns bit0 =
+// arrived, bit1 = no action for more than max_step consecutive ticks.  One lane per row, fp64, out of line: K1 (the ego)
+// and K10 (the agent rows) run the same code, so that their detectors agree bit for bit.  It takes the kernel's whole
+// argument block rather than &A.goal: the address of a member of a kernel parameter is loop-invariant, and K1 would hold
+// it in two registers across its tile loop.
+template <class Args>
+__device__ __noinline__ unsigned ego_goal_events(const Args& A, long long n, float ex, float ey, float eh, float el, float ew) {
+  const GoalArgs& G = A.goal;
   unsigned r = 0;
-  float* last = A.goal_last_pose + 4 * n;
-  if (A.goal_noact_max > 0) {
-    int cnt = A.goal_noact_count[n];
+  float* last = G.last_pose + 4 * n;
+  if (G.noact_max > 0) {
+    int cnt = G.noact_count[n];
     if (last[3] != 0.0f) {                                          // no_action.py:40-50
       const double iou = rect_iou_f64(ex, ey, eh, el, ew, last[0], last[1], last[2], el, ew);
       cnt = iou > 0.999 ? cnt + 1 : 0;
     }
-    A.goal_noact_count[n] = cnt;
-    if (cnt > A.goal_noact_max) r |= 2u;                            // no_action.py:53
+    G.noact_count[n] = cnt;
+    if (cnt > G.noact_max) r |= 2u;                                 // no_action.py:53
   }
   last[0] = ex; last[1] = ey; last[2] = eh; last[3] = 1.0f;         // no_action.py:39,51
-  const float* tg = A.goal_target + 5 * n;
+  const float* tg = G.target + 5 * n;
   const double iou = rect_iou_f64(ex, ey, eh, el, ew, tg[0], tg[1], tg[2], tg[3], tg[4]);   // arrival.py:42-44
-  A.goal_iou[n] = (float)iou;
-  if (iou >= (double)A.goal_threshold) r |= 1u;                     // arrival.py:45
+  G.iou[n] = (float)iou;
+  if (iou >= (double)G.threshold) r |= 1u;                          // arrival.py:45
   return r;
 }
 
@@ -1098,7 +1131,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         A.step_count[n] = cnt;
         uint8_t st = T2D_STATUS_NORMAL;
         unsigned goal = 0;
-        if (K1_SHAPE(goal_target, nullptr) != nullptr) {   // the ego is participant 0 = this lane's first slot
+        if (K1_SHAPE(goal.target, nullptr) != nullptr) {   // the ego is participant 0 = this lane's first slot
           const float4 ea = poseA[pslot(t0)], eb = poseB[pslot(t0)];
           if (ea.x == ea.x && eb.w >= 0.0f) goal = ego_goal_events(A, n, ea.x, ea.y, ea.w, eb.z, eb.w);
         }
@@ -1120,28 +1153,21 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
 }
 
 // ---------------------------------------------------------------------------- K2
-struct ResetArgs {
-  float *x, *y, *h, *v, *vx, *vy;
-  int32_t* step_count;
+struct ResetArgs : WorldArgs {
   const uint8_t* mask;
   const int32_t* pool_index;
   const float *px, *py, *ph, *pv, *pvx, *pvy;
-  float* goal_last_pose;
-  int32_t* goal_noact_count;
+  GoalArgs goal;                       // the ego's NoAction state starts fresh
   // per-participant state owned by the world besides x .. vy: the SingleTrackDrift wheel speeds and the controllers'
   // State.accel of the previous tick - a new episode must not inherit them from the old one
   float *wheel_f, *wheel_r;            // [N][M] or nullptr
   const float *pool_wf, *pool_wr;      // [n_pool][M] initial wheel speeds, or nullptr: free rolling, speed / wheel radius
   float* last_accel;                   // [N][M] or nullptr
-  const uint8_t* type_id;
-  const Params* table;
-  int n_types;
-  int N, M, n_pool;
+  int n_pool;
   // t2d_set_agents: the slots K10 retired take their types back, and the per-row NoAction state starts fresh
   uint8_t* agent_type_id;              // writable alias of type_id, or nullptr: no agents bound
   uint8_t* agent_retired;              // [N][M], 255 = not retired
-  float* agent_last_pose;              // [N][Q][4]
-  int32_t* agent_noact_count;          // [N][Q]
+  GoalArgs agent;
   int agent_q;
 };
 
@@ -1160,8 +1186,8 @@ __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
       const uint8_t rt = A.agent_retired[i];
       if (rt != 0xff) { A.agent_type_id[i] = rt; A.agent_retired[i] = 0xff; }
       for (int q = m; q < A.agent_q; q += A.M) {   // NoAction.reset of every row
-        A.agent_last_pose[4 * ((long long)n * A.agent_q + q) + 3] = 0.0f;
-        A.agent_noact_count[(long long)n * A.agent_q + q] = 0;
+        A.agent.last_pose[4 * ((long long)n * A.agent_q + q) + 3] = 0.0f;
+        A.agent.noact_count[(long long)n * A.agent_q + q] = 0;
       }
     }
     if (A.wheel_f != nullptr) {
@@ -1177,8 +1203,8 @@ __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
     if (A.last_accel != nullptr) A.last_accel[i] = 0.0f;   // a fresh State has no acceleration (state.py:171-185)
     if (m == 0) {
       A.step_count[n] = 0;
-      if (A.goal_last_pose) A.goal_last_pose[4 * (long long)n + 3] = 0.0f;   // NoAction.reset / last_pose = None
-      if (A.goal_noact_count) A.goal_noact_count[n] = 0;
+      if (A.goal.last_pose) A.goal.last_pose[4 * (long long)n + 3] = 0.0f;   // NoAction.reset / last_pose = None
+      if (A.goal.noact_count) A.goal.noact_count[n] = 0;
     }
   }
 }
@@ -1190,11 +1216,9 @@ __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
 // (_max_iou, _min_dist_to_target) and the done mask that drives the masked reset.  One thread per participant slot;
 // the thread of slot 0 also does the per-scenario part.  Reads the ego's flags through the same array, so the launch
 // has no other input than the tick's outputs.
-struct EnvArgs {
+struct EnvArgs : WorldArgs {   // (the state after the tick: the ego's position for the distance shaping)
   const uint8_t* flags;        // [N][M] event byte of the tick
   const uint8_t* status;       // [N] ScenarioStatus of the tick
-  const int32_t* step_count;   // [N]
-  const float *x, *y;          // [N][M] state after the tick (the ego's position for the distance shaping)
   const float* iou;            // [N] IoU(ego pose, target) of the tick, or nullptr (no goal)
   const float* target;         // [N][5] or nullptr
   float* max_iou;              // [N] in/out, or nullptr
@@ -1202,7 +1226,7 @@ struct EnvArgs {
   float* reward;               // [N]
   uint8_t *terminated, *truncated, *done;   // [N]
   uint8_t* traffic_status;     // [N][M]
-  int N, M, max_step, reset_trackers;
+  int max_step, reset_trackers;
 };
 
 // The reward chain of _get_reward (parking.py:148-190) for one scored participant: st its ScenarioStatus, ts its
@@ -1269,25 +1293,18 @@ __global__ void __launch_bounds__(256) t2d_env_epilogue_kernel(const __grid_cons
 // DESIGN.md section 1 "Per-agent status and reward": the status chain, terminated / truncated and the reward chain of the
 // env epilogue for every row (n, q) of an observer list, retirement of the slots whose rows settle, and the done mask
 // "no row of the scenario is NORMAL".  One warp per scenario; lane l takes rows l, l + 32, l + 64, l + 96.
-struct AgentArgs {
-  // Arrival / NoAction go through K1's ego_goal_events, which reads its arrays from a StepArgs and indexes them by its
-  // second argument: here only the goal_* fields are set, to the per-row arrays, and the index is the row n·Q + q.  K1
-  // and K10 so run one compiled copy of the detectors (bit-exact agreement) and K1's code is untouched.
-  StepArgs g;                   // goal_target = goals [N][Q][5] or nullptr, goal_iou = iou [N][Q], goal_last_pose [N][Q][4],
-                                // goal_noact_count [N][Q], goal_threshold, goal_noact_max
+// The state is the tick's result; a settled row's slot becomes 255 in type_id, the caller's writable array ...
+struct AgentArgs : WorldArgs {
+  GoalArgs goal;                // the rows' detectors, indexed by the row n·Q + q (target [N][Q][5] or nullptr)
   const uint8_t* flags;         // [N][M] event byte of the tick
   const int16_t* observers;     // [N][Q] or nullptr: row q is slot q
-  const float *x, *y, *h;       // [N][M] state after the tick
-  uint8_t* type_id;             // [N][M]: a settled row's slot becomes 255 ...
   uint8_t* retired;             // [N][M]: ... and keeps its type here (255: not retired)
-  const int32_t* step_count;    // [N]
-  const Params* table;
   float *max_iou, *min_dist;    // [N][Q] per-episode extrema
   float* reward;                // [N][Q]
   uint8_t *terminated, *truncated, *status;   // [N][Q]
   uint8_t* done;                // [N]
   uint8_t* traffic_status;      // [N][M] or nullptr
-  int N, M, Q, n_types, max_step, reset_trackers;
+  int Q, max_step, reset_trackers;
 };
 
 constexpr int K10_WARPS = 8;
@@ -1316,22 +1333,22 @@ __global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(con
     const int j = A.observers ? A.observers[r] : q;
     const int t = (j >= 0 && j < A.M) ? A.type_id[s0 + j] : 0xff;
     if (t >= A.n_types) {   // absent row
-      A.status[r] = 0; A.reward[r] = 0.0f; A.terminated[r] = 0; A.truncated[r] = 0; A.g.goal_iou[r] = 0.0f;
+      A.status[r] = 0; A.reward[r] = 0.0f; A.terminated[r] = 0; A.truncated[r] = 0; A.goal.iou[r] = 0.0f;
       continue;
     }
     const long long i = s0 + j;
     const float x = A.x[i], y = A.y[i];
-    const float* goal = A.g.goal_target ? A.g.goal_target + 5 * r : nullptr;
+    const float* goal = A.goal.target ? A.goal.target + 5 * r : nullptr;
     const bool has_goal = goal != nullptr && goal[0] == goal[0];
     unsigned ev = 0;
     float iou = 0.0f;
     const Vec4 g2 = params_group(A.table + t, 2);   // (pose_l, pose_w, rbound, model | shape << 8)
     // K1's condition for the ego: a solid box (pose tile: x not NaN, pose_w >= 0)
     if (has_goal && x == x && (__float_as_int(g2.w) >> 8) != SHAPE_NONE && g2.y >= 0.0f) {
-      ev = ego_goal_events(A.g, r, x, y, A.h[i], g2.x, g2.y);   // writes goal_iou[r]
-      iou = A.g.goal_iou[r];
+      ev = ego_goal_events(A, r, x, y, A.h[i], g2.x, g2.y);   // writes goal.iou[r]
+      iou = A.goal.iou[r];
     } else {
-      A.g.goal_iou[r] = 0.0f;
+      A.goal.iou[r] = 0.0f;
     }
     const unsigned f = A.flags[i];
     int st = T2D_STATUS_NORMAL;                                                 // parking.py:366-390, lowest priority first
@@ -1362,7 +1379,7 @@ __global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(con
     const int q = lane + 32 * k;
     if (q >= A.Q) break;
     if (A.reset_trackers && done) { A.max_iou[r0 + q] = -INFINITY; A.min_dist[r0 + q] = INFINITY; }
-    if ((settle >> k) & 1u) A.type_id[s0 + (A.observers ? A.observers[r0 + q] : q)] = 0xff;
+    if ((settle >> k) & 1u) const_cast<uint8_t*>(A.type_id)[s0 + (A.observers ? A.observers[r0 + q] : q)] = 0xff;
   }
 }
 
@@ -1371,12 +1388,11 @@ __global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(con
 // observers[n][q] == m, when its type is active; nothing else is written.  One warp per scenario; lane l takes rows l,
 // l + 32, l + 64, l + 96 and claims their slots with atomicMin on a per-slot owner in shared memory, so the first row
 // wins whatever the order of the atomics.  Then one float2 copy per owned active slot (the fp32 bits as they are).
-struct ActionArgs {
+struct ActionArgs : WorldArgs {
   const int16_t* observers;     // [N][Q] or nullptr: row q is slot q
   const float* agent_action;    // [N][Q][2]
   float* action;                // [N][M][2]
-  const uint8_t* type_id;       // [N][M]
-  int N, M, Q, n_types;
+  int Q;
 };
 
 constexpr int K11_WARPS = 8;
@@ -1618,18 +1634,12 @@ constexpr int LIDAR_EDGES = 144;   // edges per shared-memory chunk per warp (4 
 constexpr int LIDAR_WARPS = 4;
 constexpr int LIDAR_BEAMS = 512;   // beams per pass (running minima in shared memory)
 
-struct LidarArgs {
-  const float *x, *y, *h;
-  const uint8_t* type_id;
-  const Params* table;
-  int n_types;
-  const unsigned char* map_blob;
-  const uint32_t* tile_off;   // map table: byte offsets of the tiles; the scenario's tile id, or nullptr = tile 0 for all
-  const uint16_t* tile_id;
+struct LidarArgs : WorldArgs {
+  MapArgs map;
   const double* beam_cs;      // [n_beams][2] cos, sin of the beam angles (host float64)
   const int16_t* observers;   // [N][Q]: the slot carrying the sensor of row n·Q + q, or nullptr: row q is slot q
   float* scan;                // [N][Q][n_beams]
-  int N, M, Q, n_beams;
+  int Q, n_beams;
   double range;
 };
 
@@ -1670,7 +1680,7 @@ __global__ void __launch_bounds__(LIDAR_WARPS * 32, 7) t2d_lidar_kernel(const __
   const double xoff = -x0 * ca - y0 * sa, yoff = x0 * sa - y0 * ca;   // lidar.py:116-121
   const double R = A.range, R2 = R * R;
   // the scenario's static-geometry tile (its header is read from global memory: one warp, a handful of words)
-  const unsigned char* blob = A.map_blob ? A.map_blob + (A.tile_id ? A.tile_off[A.tile_id[n]] : 0u) : nullptr;
+  const unsigned char* blob = tile_blob(A.map, n);
   const MapHeader* tmh = reinterpret_cast<const MapHeader*>(blob);
   const int n_seg = blob ? tmh->n_seg : 0;
   const float4* seg = n_seg > 0 ? reinterpret_cast<const float4*>(blob + tmh->off_seg) : nullptr;
@@ -1861,11 +1871,7 @@ __global__ void __launch_bounds__(512) t2d_exchange_allgather_kernel(const __gri
 // leader's, previous tick) happen before the warp barrier, all writes (this tick) after it.
 struct PathVertex { double x, y, cum, len; };   // vertex, arc length up to it, length of the segment that starts here
 
-struct CtrlArgs {
-  const float *x, *y, *h, *v;
-  const uint8_t* type_id;
-  const Params* table;
-  int n_types;
+struct CtrlArgs : WorldArgs {
   const t2d_controller_params* ctab;
   int n_ctrl;
   const uint8_t* ctrl_id;
@@ -1877,7 +1883,7 @@ struct CtrlArgs {
   float* last_accel;
   float* action;
   const float* ego_action;   // [N][2] or nullptr: participant 0's action (written into its row of `action` as well)
-  int N, M, steer_first;
+  int steer_first;
 };
 
 __device__ __forceinline__ double clip_np(double v, double lo, double hi) {   // np.clip: NaN propagates
@@ -2094,7 +2100,7 @@ struct t2d_exchange {
 struct DeviceMap {
   dev_ptr<unsigned char> blob;         // the tiles back to back, each 128-byte aligned
   dev_ptr<uint32_t> tile_off;          // [n_tiles] byte offsets of the tiles inside blob
-  const uint16_t* tile_id = nullptr;   // caller-owned DEVICE [N] (more than one tile)
+  const uint16_t* tile_id = nullptr;   // caller-owned DEVICE [N]; nullptr unless there is more than one tile
   int n_tiles = 0;
   bool has_segments = false;
   bool has_bounds = false;             // any tile has a boundary box
@@ -2172,20 +2178,11 @@ struct t2d_ctx {
   int max_smem_optin = 0;
   float rb_max = 0.0f;
   const float* ego_action = nullptr;   // t2d_set_ego_action
-  const float* goal_target = nullptr;
-  float* goal_iou = nullptr;
-  float* goal_last_pose = nullptr;
-  int32_t* goal_noact_count = nullptr;
-  float goal_threshold = 0.95f;
-  int goal_noact_max = 0;
+  GoalArgs goal{};                     // t2d_set_goal
   // per-agent status and reward (t2d_set_agents / K10); agent_q == 0: not bound
   int agent_q = 0;
   const int16_t* agent_observers = nullptr;
-  const float* agent_goals = nullptr;
-  float agent_threshold = 0.95f;
-  int agent_noact_max = 0;
-  float* agent_last_pose = nullptr;
-  int32_t* agent_noact_count = nullptr;
+  GoalArgs agent{};                    // iou: the t2d_agents_epilogue argument
   uint8_t* agent_retired = nullptr;
   bool use_pdl = true;            // T2D_PDL=0 disables programmatic dependent launch
   int prefetch_override = -1;      // T2D_PREFETCH=0 / 1 (experiments; -1 = on unless a done exchange is alive)
@@ -2235,6 +2232,15 @@ static int require(const t2d_ctx* c, unsigned need) {
     if (c->log && c->log->type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
   }
   return T2D_OK;
+}
+
+static WorldArgs world_args(const t2d_ctx* c) {
+  return {c->x, c->y, c->h, c->v, c->vx, c->vy, c->type_id, c->step_count, c->d_table.get(), c->n_types, c->N, c->M};
+}
+
+// from scenario `first` on (t2d_set_map_table keeps tile_id only with more than one tile)
+static MapArgs map_args(const DeviceMap& map, int first = 0) {
+  return {map.blob.get(), map.tile_off.get(), map.tile_id ? map.tile_id + first : nullptr};
 }
 
 // after every launch: count it and report a launch error
@@ -2842,8 +2848,8 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
   A.action = action; A.ego_action = ego ? ego + 2 * (size_t)first : nullptr; A.flags = flags; A.hit_index = hit_index; A.hit_segment = hit_segment;
   A.scn_status = scn_status; A.done = done;
   const bool map_table = map.n_tiles > 1;
-  A.map_blob = map.blob.get(); A.map_bytes = map.smem_bytes; A.mh = map.mh;
-  A.tile_off = map.tile_off.get(); A.tile_id = map_table ? map.tile_id + first : nullptr;
+  const MapArgs mp = map_args(map, first);
+  A.map_blob = mp.map_blob; A.tile_off = mp.tile_off; A.tile_id = mp.tile_id; A.map_bytes = map.smem_bytes; A.mh = map.mh;
   A.map_in_smem = (!map_table && map.blob && map.mh.n_seg > 0 && map.smem_bytes <= MAP_SMEM_LIMIT) ? 1 : 0;
   A.table = c->d_table.get(); A.n_types = c->n_types;
   A.N = count; A.M = c->M; A.G = c->G;
@@ -2862,10 +2868,10 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
   A.vec_ok = vec ? 1 : 0;
 
   A.rb_max = c->rb_max;
-  A.goal_target = c->goal_target ? c->goal_target + 5 * (size_t)first : nullptr;
-  A.goal_iou = c->goal_iou ? c->goal_iou + first : nullptr;
-  A.goal_last_pose = c->goal_last_pose ? c->goal_last_pose + 4 * (size_t)first : nullptr;
-  A.goal_noact_count = c->goal_noact_count ? c->goal_noact_count + first : nullptr; A.goal_threshold = c->goal_threshold; A.goal_noact_max = c->goal_noact_max;
+  A.goal = c->goal;
+  if (A.goal.target) {   // the rows from `first` on (t2d_set_goal binds the three outputs with every target)
+    A.goal.target += 5 * (size_t)first; A.goal.iou += first; A.goal.last_pose += 4 * (size_t)first; A.goal.noact_count += first;
+  }
   const int table_bytes = (((c->n_types + 1) * (int)sizeof(Params) + 15) / 16) * 16;   // + the neutral row
   const int spw = 32 / c->G;
   const long long tiles = ((long long)count + spw - 1) / spw;
@@ -2895,7 +2901,7 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
   kernel_t kern;
   // the C2-shaped instance exactly when this tick has the shape it is compiled for (FIX_M ...)
   const bool fixed = c->kin_only && !c->tick_generic && c->M == FIX_M && c->G == FIX_G && do_physics && A.vec_ok &&
-                     !A.needs_vel_in && A.ego_action == nullptr && A.goal_target == nullptr;
+                     !A.needs_vel_in && A.ego_action == nullptr && A.goal.target == nullptr;
   if (fixed) kern = map_table ? (kernel_t)t2d_step_kernel<true, true, true> : (kernel_t)t2d_step_kernel<true, false, true>;
   else if (c->kin_only) kern = map_table ? (kernel_t)t2d_step_kernel<true, true, false> : (kernel_t)t2d_step_kernel<true, false, false>;
   else kern = map_table ? (kernel_t)t2d_step_kernel<false, true, false> : (kernel_t)t2d_step_kernel<false, false, false>;
@@ -2952,12 +2958,11 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
   if (!action) return fail(T2D_E_INVALID, "action is NULL");
   if (reinterpret_cast<uintptr_t>(action) % 8 != 0) return fail(T2D_E_INVALID, "action must be 8-byte aligned");
   CUDA_TRY(cudaSetDevice(c->device));
-  CtrlArgs A{};
-  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
+  CtrlArgs A{world_args(c)};
   A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.lead = c->ctrl_lead; A.path_id = c->ctrl_path;
   A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
   A.last_accel = c->ctrl_last_accel; A.action = action; A.ego_action = ego;
-  A.N = c->N; A.M = c->M; A.steer_first = (c->cfg.flags & T2D_CFG_STEER_FIRST) ? 1 : 0;
+  A.steer_first = (c->cfg.flags & T2D_CFG_STEER_FIRST) ? 1 : 0;
   const int warps_per_cta = 4;
   t2d_control_kernel<<<capped_grid(c->N, warps_per_cta, c->sm_count, 16), warps_per_cta * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
@@ -2995,8 +3000,7 @@ int t2d_set_goal(t2d_ctx* c, const float* target, float arrival_threshold, int n
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (target && (!iou_out || !last_pose || !no_action_count)) return fail(T2D_E_INVALID, "t2d_set_goal: NULL output array");
   if (target && !(arrival_threshold > 0.0f && arrival_threshold <= 1.0f)) return fail(T2D_E_INVALID, "arrival_threshold must be in (0, 1]");
-  c->goal_target = target; c->goal_iou = iou_out; c->goal_last_pose = last_pose; c->goal_noact_count = no_action_count;
-  c->goal_threshold = arrival_threshold; c->goal_noact_max = no_action_max_step;
+  c->goal = {target, iou_out, last_pose, no_action_count, arrival_threshold, no_action_max_step};
   return T2D_OK;
 }
 
@@ -3106,12 +3110,12 @@ int t2d_env_epilogue(t2d_ctx* c, const uint8_t* flags, const uint8_t* scn_status
   if (int r = require(c, NEED_STATE)) return r;
   if (!flags || !scn_status || !reward) return fail(T2D_E_INVALID, "t2d_env_epilogue: flags / scn_status / reward is NULL");
   CUDA_TRY(cudaSetDevice(c->device));
-  EnvArgs A{};
-  A.flags = flags; A.status = scn_status; A.step_count = c->step_count; A.x = c->x; A.y = c->y;
-  A.iou = c->goal_target ? c->goal_iou : nullptr; A.target = c->goal_target;
+  EnvArgs A{world_args(c)};
+  A.flags = flags; A.status = scn_status;
+  A.iou = c->goal.target ? c->goal.iou : nullptr; A.target = c->goal.target;
   A.max_iou = max_iou; A.min_dist = min_dist;
   A.reward = reward; A.terminated = terminated; A.truncated = truncated; A.done = done; A.traffic_status = traffic_status;
-  A.N = c->N; A.M = c->M; A.max_step = c->cfg.max_step; A.reset_trackers = reset_trackers_on_done ? 1 : 0;
+  A.max_step = c->cfg.max_step; A.reset_trackers = reset_trackers_on_done ? 1 : 0;
   t2d_env_epilogue_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(A);
   return launched();
 }
@@ -3120,17 +3124,15 @@ int t2d_set_agents(t2d_ctx* c, const int16_t* observers, int32_t n_observers, co
                    int no_action_max_step, float* last_pose, int32_t* noact_count, uint8_t* retired_type) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (!observers && n_observers == 0) {   // unbind
-    c->agent_q = 0; c->agent_observers = nullptr; c->agent_goals = nullptr;
-    c->agent_last_pose = nullptr; c->agent_noact_count = nullptr; c->agent_retired = nullptr;
+    c->agent_q = 0; c->agent_observers = nullptr; c->agent = {}; c->agent_retired = nullptr;
     return T2D_OK;
   }
   if (n_observers < 1 || n_observers > T2D_OBS_MAX_OBSERVERS) return fail(T2D_E_INVALID, "t2d_set_agents: n_observers must be in 1..128");
   if (!observers && n_observers > c->M) return fail(T2D_E_INVALID, "t2d_set_agents: without observers row q is slot q (n_observers <= M)");
   if (!last_pose || !noact_count || !retired_type) return fail(T2D_E_INVALID, "t2d_set_agents: NULL state array");
   if (goals && !(arrival_threshold > 0.0f && arrival_threshold <= 1.0f)) return fail(T2D_E_INVALID, "arrival_threshold must be in (0, 1]");
-  c->agent_q = n_observers; c->agent_observers = observers; c->agent_goals = goals;
-  c->agent_threshold = arrival_threshold; c->agent_noact_max = no_action_max_step;
-  c->agent_last_pose = last_pose; c->agent_noact_count = noact_count; c->agent_retired = retired_type;
+  c->agent_q = n_observers; c->agent_observers = observers; c->agent_retired = retired_type;
+  c->agent = {goals, nullptr, last_pose, noact_count, arrival_threshold, no_action_max_step};
   return T2D_OK;
 }
 
@@ -3143,14 +3145,12 @@ int t2d_agents_epilogue(t2d_ctx* c, const uint8_t* flags, float* reward, uint8_t
   if (!flags || !reward || !terminated || !truncated || !agent_status || !iou || !done || !max_iou || !min_dist)
     return fail(T2D_E_INVALID, "t2d_agents_epilogue: NULL array");
   CUDA_TRY(cudaSetDevice(c->device));
-  AgentArgs A{};
-  A.g.goal_target = c->agent_goals; A.g.goal_iou = iou; A.g.goal_last_pose = c->agent_last_pose;
-  A.g.goal_noact_count = c->agent_noact_count; A.g.goal_threshold = c->agent_threshold; A.g.goal_noact_max = c->agent_noact_max;
-  A.flags = flags; A.observers = c->agent_observers; A.x = c->x; A.y = c->y; A.h = c->h;
-  A.type_id = const_cast<uint8_t*>(c->type_id); A.retired = c->agent_retired; A.step_count = c->step_count; A.table = c->d_table.get();
+  AgentArgs A{world_args(c)};
+  A.goal = c->agent; A.goal.iou = iou;
+  A.flags = flags; A.observers = c->agent_observers; A.retired = c->agent_retired;
   A.max_iou = max_iou; A.min_dist = min_dist; A.reward = reward; A.terminated = terminated; A.truncated = truncated;
   A.status = agent_status; A.done = done; A.traffic_status = traffic_status;
-  A.N = c->N; A.M = c->M; A.Q = c->agent_q; A.n_types = c->n_types; A.max_step = c->cfg.max_step;
+  A.Q = c->agent_q; A.max_step = c->cfg.max_step;
   A.reset_trackers = reset_trackers_on_done ? 1 : 0;
   t2d_agents_epilogue_kernel<<<(c->N + K10_WARPS - 1) / K10_WARPS, K10_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
@@ -3162,9 +3162,8 @@ static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7
 static int launch_agent_action(t2d_ctx* c, const int16_t* observers, int Q, const float* agent_action, float* action,
                                void* stream) {
   CUDA_TRY(cudaSetDevice(c->device));
-  ActionArgs A{};
-  A.observers = observers; A.agent_action = agent_action; A.action = action; A.type_id = c->type_id;
-  A.N = c->N; A.M = c->M; A.Q = Q; A.n_types = c->n_types;
+  ActionArgs A{world_args(c)};
+  A.observers = observers; A.agent_action = agent_action; A.action = action; A.Q = Q;
   t2d_agent_action_kernel<<<(c->N + K11_WARPS - 1) / K11_WARPS, K11_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
 }
@@ -3245,17 +3244,15 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   if (c->log && n_pool != c->log->n_rows) return fail(T2D_E_INVALID, "t2d_reset: with a log bound, pool row p is episode row p (n_pool == n_rows)");
   if (c->log && c->log->type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
   CUDA_TRY(cudaSetDevice(c->device));
-  ResetArgs A{};
-  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy; A.step_count = c->step_count;
+  ResetArgs A{world_args(c)};
   A.mask = mask; A.pool_index = pool_index;
   A.px = pool_x; A.py = pool_y; A.ph = pool_heading; A.pv = pool_speed; A.pvx = pool_vx; A.pvy = pool_vy;
-  A.goal_last_pose = c->goal_last_pose; A.goal_noact_count = c->goal_noact_count;
+  A.goal = c->goal;
   A.wheel_f = c->wheel_f; A.wheel_r = c->wheel_r; A.pool_wf = c->reset_pool_wf; A.pool_wr = c->reset_pool_wr;
-  A.last_accel = c->ctrl_last_accel; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
-  A.N = c->N; A.M = c->M; A.n_pool = n_pool;
+  A.last_accel = c->ctrl_last_accel; A.n_pool = n_pool;
   if (c->agent_q > 0) {   // the bound type_id is the caller's writable device array (K10 retires slots in it)
     A.agent_type_id = const_cast<uint8_t*>(c->type_id); A.agent_retired = c->agent_retired;
-    A.agent_last_pose = c->agent_last_pose; A.agent_noact_count = c->agent_noact_count; A.agent_q = c->agent_q;
+    A.agent = c->agent; A.agent_q = c->agent_q;
   }
   t2d_reset_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(A);
   if (int r = launched()) return r;
@@ -3267,11 +3264,10 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
 static int launch_lidar(t2d_ctx* c, const int16_t* observers, int Q, int n_beams, float max_range, const double* beam_cos_sin,
                         float* scan, void* stream) {
   CUDA_TRY(cudaSetDevice(c->device));
-  LidarArgs A{};
-  A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
-  A.map_blob = c->map.blob.get(); A.tile_off = c->map.tile_off.get(); A.tile_id = c->map.n_tiles > 1 ? c->map.tile_id : nullptr;
+  LidarArgs A{world_args(c)};
+  A.map = map_args(c->map);
   A.beam_cs = beam_cos_sin; A.observers = observers; A.scan = scan;
-  A.N = c->N; A.M = c->M; A.Q = Q; A.n_beams = n_beams; A.range = (double)max_range;
+  A.Q = Q; A.n_beams = n_beams; A.range = (double)max_range;
   const long long grid = ((long long)c->N * Q + LIDAR_WARPS - 1) / LIDAR_WARPS;
   if (grid > INT32_MAX) return fail(T2D_E_UNSUPPORTED, "lidar: more than 2^33 rows (one warp per row)");
   t2d_lidar_kernel<<<(unsigned)grid, LIDAR_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
@@ -3360,7 +3356,7 @@ int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rg
   if (wh / ww > aspect) { nw = wh / aspect; nh = wh; }
   else { nw = ww; nh = ww * aspect; }
   const double nx0 = cx - nw / 2, nx1 = cx + nw / 2, ny0 = cy - nh / 2, ny1 = cy + nh / 2;
-  bev::Args A{};
+  bev::Args A{world_args(c)};
   A.win.xmin = nx0; A.win.ymax = ny1;
   A.win.px = (nx1 - nx0) / width; A.win.py = (ny1 - ny0) / height;
   for (int s = 0; s < c->n_bev_styles; ++s) {
@@ -3371,11 +3367,8 @@ int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rg
     A.style_z[s] = st.z;
   }
   memcpy(A.type_style, c->bev_type_style, sizeof(A.type_style));
-  A.x = c->x; A.y = c->y; A.h = c->h; A.type_id = c->type_id; A.table = c->d_table.get(); A.n_types = c->n_types;
-  A.N = c->N; A.M = c->M;
-  A.map_blob = c->map.blob.get(); A.tile_off = c->map.tile_off.get(); A.tile_id = c->map.n_tiles > 1 ? c->map.tile_id : nullptr;
-  A.seg_style = c->map.seg_style.get(); A.seg_base = c->map.seg_base.get();
-  A.target = c->goal_target; A.target_style = c->bev_target_style;
+  A.map = map_args(c->map); A.seg_style = c->map.seg_style.get(); A.seg_base = c->map.seg_base.get();
+  A.target = c->goal.target; A.target_style = c->bev_target_style;
   A.ring_style = T2D_BEV_STYLE_RING; A.open_style = T2D_BEV_STYLE_OPEN;
   A.W = width; A.H = height; A.rgb = rgb ? 1 : 0; A.out = out;
   CUDA_TRY(cudaSetDevice(c->device));
@@ -3394,11 +3387,8 @@ static int obs_args(const t2d_ctx* c, const std::string& fn, const t2d_obs_confi
     return fail(T2D_E_INVALID, fn + ": agent_range and segment_range must be in (0, 1e5] m");
   if (!out) return fail(T2D_E_INVALID, fn + ": out is NULL");
   static_assert(T2D_OBS_MAX_AGENTS == obs::MAX_K && T2D_OBS_MAX_SEGMENTS == obs::MAX_S, "K8's shared lists hold the ABI's limits");
-  A.x = c->x; A.y = c->y; A.h = c->h; A.v = c->v; A.vx = c->vx; A.vy = c->vy;
-  A.type_id = c->type_id; A.step_count = c->step_count; A.table = c->d_table.get(); A.n_types = c->n_types;
-  A.N = c->N; A.M = c->M; A.max_step = c->cfg.max_step;
-  A.map_blob = c->map.blob.get(); A.tile_off = c->map.tile_off.get(); A.tile_id = c->map.n_tiles > 1 ? c->map.tile_id : nullptr;
-  A.target = c->goal_target;
+  static_cast<WorldArgs&>(A) = world_args(c);
+  A.max_step = c->cfg.max_step; A.map = map_args(c->map); A.target = c->goal.target;
   A.K = cfg->k_agents; A.S = cfg->k_segments;
   A.F = obs::EGO_F + obs::GOAL_F + obs::AGENT_F * A.K + obs::SEG_F * A.S;
   const double ra = cfg->agent_range, rs = cfg->segment_range;

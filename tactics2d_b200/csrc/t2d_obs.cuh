@@ -28,15 +28,9 @@ constexpr int MAX_S = 256;            // segments per row
 constexpr int EGO_F = 8, GOAL_F = 8, AGENT_F = 11, SEG_F = 9;
 constexpr unsigned long long NO_KEY = ~0ull;
 
-struct Args {
-  const float *x, *y, *h, *v, *vx, *vy;
-  const uint8_t* type_id;
-  const int32_t* step_count;
-  const Params* table;
-  int n_types, N, M, max_step;
-  const unsigned char* map_blob;   // tiles as K4 reads them; nullptr when the map is empty
-  const uint32_t* tile_off;
-  const uint16_t* tile_id;         // nullptr: tile 0 for every scenario
+struct Args : WorldArgs {
+  int max_step;
+  MapArgs map;
   const float* target;             // [N][5] goal rectangles, or nullptr
   int K, S, F;
   double ra2, rs2;                 // squared ranges
@@ -148,7 +142,7 @@ __device__ __forceinline__ void observe_row(const Args& A, Smem& sm, int lane, l
   sincos_angle(h0, &f.s, &f.c);
 
   // ---- the tile (as K4 finds it)
-  const unsigned char* blob = A.map_blob ? A.map_blob + (A.tile_id ? A.tile_off[A.tile_id[n]] : 0u) : nullptr;
+  const unsigned char* blob = tile_blob(A.map, n);
   const MapHeader* mh = reinterpret_cast<const MapHeader*>(blob);
   const int n_seg = blob ? mh->n_seg : 0;
   const float4* seg = n_seg > 0 ? reinterpret_cast<const float4*>(blob + mh->off_seg) : nullptr;
