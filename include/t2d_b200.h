@@ -35,13 +35,15 @@
  *   t2d_bev_render       BEVCamera.update + MatplotlibRenderer.update / save_single_frame(return_array=True)
  *                                                         tactics2d/sensor/camera.py:333-386,
  *                                                         renderer/matplotlib_renderer.py:542-768
- *   t2d_set_controllers  IDMController / AccelerationController / PurePursuitController objects
+ *   t2d_set_controllers  IDMController / AccelerationController / PurePursuitController / PIDController objects
  *                                                         tactics2d/controller/idm_controller.py:33-58,
- *                                                         acceleration_controller.py:33-80, pure_pursuit_controller.py:26-49
+ *                                                         acceleration_controller.py:33-80, pure_pursuit_controller.py:26-49,
+ *                                                         pid_controller.py:41-157
  *   t2d_set_paths        the `waypoints` LineString of PurePursuitController.step   pure_pursuit_controller.py:76,92
+ *   t2d_set_pid          the PIDController keyword targets and its per-object state, per slot   pid_controller.py:126-132
  *   t2d_control          ControllerBase.step for every controlled participant
  *                                                         idm_controller.py:59-141, acceleration_controller.py:82-145,
- *                                                         pure_pursuit_controller.py:51-98
+ *                                                         pure_pursuit_controller.py:51-98, pid_controller.py:159-406
  *   t2d_check_events     the same detectors on caller-supplied poses (no physics)
  *   t2d_reset            ScenarioManager.reset / ParticipantBase.reset
  *                                                         tactics2d/envs/parking.py:397-441, participant_base.py:236-246
@@ -239,7 +241,7 @@ int t2d_set_goal(t2d_ctx* ctx, const float* target, float arrival_threshold, int
  * with mask[n] != 0 copy row pool_index[n] (row n when pool_index is NULL) of the [n_pool, M] pool arrays into the bound
  * state and zero step_count[n]; pool_vx / pool_vy may be NULL (then speed x (cos, sin)(heading)).  Everything else the
  * world owns per participant starts fresh too: the NoAction detector state of t2d_set_goal, the controllers' last_accel
- * (0), and the SingleTrackDrift wheel speeds bound with t2d_bind_wheel_state - from the pool columns of
+ * (0), the PID state of t2d_set_pid (0), and the SingleTrackDrift wheel speeds bound with t2d_bind_wheel_state - from the pool columns of
  * t2d_bind_reset_wheel_pool when bound, else free rolling (speed / wheel_radius).  With agents bound (t2d_set_agents)
  * the retired slots take their types back and the per-row NoAction state is cleared. */
 int t2d_reset(t2d_ctx* ctx, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x,
@@ -398,12 +400,28 @@ int t2d_observe_agents(t2d_ctx* ctx, const t2d_obs_config* cfg, const int16_t* o
  * are the reference's attribute names.  kind selects the law:
  *   T2D_CTRL_IDM           IDMController.step               (steering 0; free flow, or car following when a leader is set)
  *   T2D_CTRL_CRUISE        AccelerationController.step      (steering 0; cruise, or adaptive cruise with a leader)
- *   T2D_CTRL_PURE_PURSUIT  PurePursuitController.step       (pure-pursuit steering on a path + the cruise laws) */
+ *   T2D_CTRL_PURE_PURSUIT  PurePursuitController.step       (pure-pursuit steering on a path + the cruise laws)
+ *   T2D_CTRL_PID           PIDController.step               (PID steering and acceleration with per-slot state, t2d_set_pid) */
 #define T2D_CTRL_EXTERNAL 0 /* the caller's action is kept */
 #define T2D_CTRL_IDM 1
 #define T2D_CTRL_CRUISE 2
 #define T2D_CTRL_PURE_PURSUIT 3
+#define T2D_CTRL_PID 4
 #define T2D_MAX_CONTROLLERS 64
+
+/* Where a PID row takes its lateral error from (pid_controller.py:249-283).  HEADING / CROSS_TRACK read column 1 of the
+ * t2d_set_pid target (target_heading in rad / cross_track_error in m); the PATH_* sources derive it from the slot's
+ * path_id polyline (t2d_set_paths): PATH_CROSS_TRACK is the signed offset of the closest path point, positive when the
+ * path lies to the vehicle's left, PATH_HEADING the direction of the closest segment as target_heading.  NONE: steering 0
+ * and the lateral half of the state untouched (control_mode "longitudinal"). */
+#define T2D_PID_LAT_NONE 0
+#define T2D_PID_LAT_HEADING 1
+#define T2D_PID_LAT_CROSS_TRACK 2
+#define T2D_PID_LAT_PATH_HEADING 3
+#define T2D_PID_LAT_PATH_CROSS_TRACK 4
+/* Longitudinal error: TARGET = target_speed (column 0 of the target) - speed; NONE: acceleration 0 ("lateral") */
+#define T2D_PID_LON_NONE 0
+#define T2D_PID_LON_TARGET 1
 
 typedef struct t2d_controller_params {
   int32_t kind; /* T2D_CTRL_* */
@@ -413,7 +431,12 @@ typedef struct t2d_controller_params {
   float target_speed, kp, accel_change_rate, delta_t, max_accel, min_accel, interval;
   /* PurePursuitController: min_pre_aiming_distance, interval (pure_pursuit_controller.py:26-36), wheel_base (:76) */
   float min_pre_aiming_distance, pp_interval, wheel_base;
-} t2d_controller_params;
+  /* PIDController attributes, pid_controller.py:41-134 (after update_driving_style, :136-157).  The channel's limits are
+   * max_accel / min_accel above; a CROSS_TRACK / PATH_CROSS_TRACK row scales the lateral output by 2.0 / wheel_base. */
+  int32_t pid_lateral;      /* T2D_PID_LAT_* */
+  int32_t pid_longitudinal; /* T2D_PID_LON_* */
+  double dt, kp_lat, ki_lat, kd_lat, max_steering, kp_lon, ki_lon, kd_lon, derivative_filter_alpha;
+} t2d_controller_params; /* 152 bytes: 4 bytes of padding before dt */
 
 /* table: HOST array of n_rows (<= T2D_MAX_CONTROLLERS) rows, copied.  The rest are DEVICE arrays owned by the caller:
  * ctrl_id [N, M] uint8 = row of the participant's controller (255, or a row of kind EXTERNAL: not controlled);
@@ -421,7 +444,9 @@ typedef struct t2d_controller_params {
  * -1 for none (NULL: nobody has one); path_id [N, M] int16 = the pure-pursuit path, -1 for none (NULL allowed);
  * last_accel [N, M] float = |acceleration| each participant applied on the previous tick (State.accel,
  * participant/trajectory/state.py:171-185), read and rewritten by t2d_control; zero it before the first tick.
- * table == NULL removes the controllers. */
+ * table == NULL removes the controllers.  Rejected (the previous binding stays whole): an unknown kind, and a PID row with
+ * dt <= 0, max_steering <= 0, max_accel <= 0, min_accel >= 0, max_accel <= min_accel, derivative_filter_alpha outside
+ * (0, 1], an unknown source, or wheel_base <= 0 with a cross-track source. */
 int t2d_set_controllers(t2d_ctx* ctx, const t2d_controller_params* table, int n_rows, const uint8_t* ctrl_id,
                         const int16_t* lead_index, const int16_t* path_id, float* last_accel);
 
@@ -435,6 +460,15 @@ int t2d_set_paths(t2d_ctx* ctx, const float* xy, const int32_t* offsets, int n_p
  * to the type's range; point masses: |(ax, ay)|).  Call it after the external actions are in the buffer and before
  * t2d_step.  action: DEVICE [N, M, 2] fp32. */
 int t2d_control(t2d_ctx* ctx, float* action, void* stream);
+
+/* Inputs and memory of the PID rows: DEVICE arrays owned by the caller.  target [N][M][2] fp32 = (target_speed, lateral
+ * target: target_heading in rad for HEADING rows, cross_track_error in m for CROSS_TRACK rows; PATH rows ignore it);
+ * state [N][M][6] fp64 = (lat_integral, lat_prev_error, lat_prev_derivative, lon_integral, lon_prev_error,
+ * lon_prev_derivative) of every slot, all zero for a freshly reset controller.  t2d_control reads and rewrites the state
+ * row of each slot a PID row drives (only the half of an enabled channel); t2d_reset zeroes the rows of the reset
+ * scenarios.  state == NULL unbinds both; a target without a state is rejected.  While a PID row is bound, t2d_control
+ * refuses (T2D_E_INVALID, nothing launched) without a state, or without a target when a row reads it. */
+int t2d_set_pid(t2d_ctx* ctx, const float* target, double* state);
 
 /* ---- the env layer: ego action, host-resident ego caller, reward / terminated / truncated ------------------------------
  * ParkingEnv.step takes ONE action, the ego's (steering, accel) (envs/parking.py:219-239); the other participants of a

@@ -41,7 +41,9 @@ class ControllerParamsC(C.Structure):
     _fields_ = [("kind", C.c_int32)] + [(n, C.c_float) for n in (
         "desired_speed", "time_headway", "min_spacing", "max_acceleration", "comfortable_deceleration", "delta",
         "target_speed", "kp", "accel_change_rate", "delta_t", "max_accel", "min_accel", "interval",
-        "min_pre_aiming_distance", "pp_interval", "wheel_base")]
+        "min_pre_aiming_distance", "pp_interval", "wheel_base")] + [
+        ("pid_lateral", C.c_int32), ("pid_longitudinal", C.c_int32)] + [(n, C.c_double) for n in (
+        "dt", "kp_lat", "ki_lat", "kd_lat", "max_steering", "kp_lon", "ki_lon", "kd_lon", "derivative_filter_alpha")]
 
 
 class BevStyleC(C.Structure):
@@ -95,6 +97,7 @@ SYMBOLS = {
     "t2d_set_controllers": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P]),
     "t2d_set_paths": (C.c_int, [_P, _P, _P, C.c_int]),
     "t2d_control": (C.c_int, [_P, _P, _P]),
+    "t2d_set_pid": (C.c_int, [_P, _P, _P]),
     "t2d_exchange_create": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "t2d_exchange_connect": (C.c_int, [_P, _P]),
     "t2d_exchange_allgather": (C.c_int, [_P, _P, _P, _P]),

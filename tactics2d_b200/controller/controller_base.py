@@ -10,7 +10,10 @@ import numpy as np
 
 from .. import _lib
 
-CTRL_EXTERNAL, CTRL_IDM, CTRL_CRUISE, CTRL_PURE_PURSUIT = range(4)
+CTRL_EXTERNAL, CTRL_IDM, CTRL_CRUISE, CTRL_PURE_PURSUIT, CTRL_PID = range(5)
+# t2d_controller_params.pid_lateral / pid_longitudinal (T2D_PID_LAT_* / T2D_PID_LON_*)
+PID_LAT_NONE, PID_LAT_HEADING, PID_LAT_CROSS_TRACK, PID_LAT_PATH_HEADING, PID_LAT_PATH_CROSS_TRACK = range(5)
+PID_LON_NONE, PID_LON_TARGET = range(2)
 NO_CONTROLLER = 255
 
 

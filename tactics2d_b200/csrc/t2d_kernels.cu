@@ -7,7 +7,7 @@
 // K2  t2d_reset_kernel     masked re-initialisation from a pool of initial states.
 // K3  t2d_physics_kernel   flat batch through one physics model (PhysicsModelBase.step).
 // K4  t2d_lidar_kernel     single-line lidar of every scenario's ego (per-edge beam windows).
-// K5  t2d_control_kernel   NPC controllers: IDM, cruise / adaptive cruise, pure pursuit.
+// K5  t2d_control_kernel   NPC controllers: IDM, cruise / adaptive cruise, pure pursuit, PID.
 // K7  t2d_replay_kernel    log replay: recorded tracks pose the replayed slots before K1 / after K2.
 // K8  t2d_obs_kernel       the ego-frame vector observation (t2d_obs.cuh).
 // K9  t2d_obs_agents_kernel the same observation from a list of observer slots per scenario (t2d_obs.cuh).
@@ -24,6 +24,7 @@
 // grid) into shared memory ONCE with a TMA bulk copy (cp.async.bulk + mbarrier) that overlaps
 // the first tile's physics.
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -1163,6 +1164,7 @@ struct ResetArgs : WorldArgs {
   float *wheel_f, *wheel_r;            // [N][M] or nullptr
   const float *pool_wf, *pool_wr;      // [n_pool][M] initial wheel speeds, or nullptr: free rolling, speed / wheel radius
   float* last_accel;                   // [N][M] or nullptr
+  double* pid_state;                   // [N][M][6] or nullptr: the PID controllers' integral / previous error / derivative
   int n_pool;
   // t2d_set_agents: the slots K10 retired take their types back, and the per-row NoAction state starts fresh
   uint8_t* agent_type_id;              // writable alias of type_id, or nullptr: no agents bound
@@ -1201,6 +1203,8 @@ __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
       A.wheel_f[i] = wf; A.wheel_r[i] = wr;
     }
     if (A.last_accel != nullptr) A.last_accel[i] = 0.0f;   // a fresh State has no acceleration (state.py:171-185)
+    if (A.pid_state != nullptr)                            // PIDController.reset, pid_controller.py:408-418
+      for (int k = 0; k < 6; ++k) A.pid_state[6 * i + k] = 0.0;
     if (m == 0) {
       A.step_count[n] = 0;
       if (A.goal.last_pose) A.goal.last_pose[4 * (long long)n + 3] = 0.0f;   // NoAction.reset / last_pose = None
@@ -1871,6 +1875,18 @@ __global__ void __launch_bounds__(512) t2d_exchange_allgather_kernel(const __gri
 // leader's, previous tick) happen before the warp barrier, all writes (this tick) after it.
 struct PathVertex { double x, y, cum, len; };   // vertex, arc length up to it, length of the segment that starts here
 
+// The leading fields of t2d_controller_params, the only ones the IDM / cruise / pure-pursuit laws read.  The row also
+// holds doubles (the PID part), so it is 8-byte aligned; read through this 4-byte-aligned view, those laws load their
+// fields one by one as they did before the row grew.
+struct CtrlLawRow {
+  int32_t kind;
+  float desired_speed, time_headway, min_spacing, max_acceleration, comfortable_deceleration, delta;
+  float target_speed, kp, accel_change_rate, delta_t, max_accel, min_accel, interval;
+  float min_pre_aiming_distance, pp_interval, wheel_base;
+};
+static_assert(alignof(CtrlLawRow) == 4 && offsetof(CtrlLawRow, wheel_base) == offsetof(t2d_controller_params, wheel_base),
+              "CtrlLawRow is the float prefix of t2d_controller_params");
+
 struct CtrlArgs : WorldArgs {
   const t2d_controller_params* ctab;
   int n_ctrl;
@@ -1884,6 +1900,8 @@ struct CtrlArgs : WorldArgs {
   float* action;
   const float* ego_action;   // [N][2] or nullptr: participant 0's action (written into its row of `action` as well)
   int steer_first;
+  const float* pid_target;   // [N][M][2] (target_speed, lateral target) or nullptr; read by the HAS_PID instance only
+  double* pid_state;         // [N][M][6] or nullptr; read and written by the HAS_PID instance only
 };
 
 __device__ __forceinline__ double clip_np(double v, double lo, double hi) {   // np.clip: NaN propagates
@@ -1891,7 +1909,7 @@ __device__ __forceinline__ double clip_np(double v, double lo, double hi) {   //
 }
 
 // acceleration_controller.py:82-130: cruise, or adaptive cruise when a leader is given
-__device__ double longitudinal_law(const t2d_controller_params& p, double v, double x, double y, double a_last, bool has_lead,
+__device__ double longitudinal_law(const CtrlLawRow& p, double v, double x, double y, double a_last, bool has_lead,
                                    double vl, double xl, double yl, double al) {
   const double kp = (double)p.kp;
   double a;
@@ -1918,7 +1936,7 @@ __device__ __forceinline__ double idm_pow(double r, double delta) {
 }
 
 // idm_controller.py:59-141
-__device__ double idm_law(const t2d_controller_params& p, double v, double x, double y, bool has_lead, double vl, double xl,
+__device__ double idm_law(const CtrlLawRow& p, double v, double x, double y, bool has_lead, double vl, double xl,
                           double yl) {
   const double vd = (double)p.desired_speed, am = (double)p.max_acceleration, b = (double)p.comfortable_deceleration;
   double a;
@@ -1941,7 +1959,7 @@ __device__ double idm_law(const t2d_controller_params& p, double v, double x, do
 }
 
 // pure_pursuit_controller.py:51-74,90-92; LineString.interpolate = arc-length walk from the first vertex
-__device__ double pure_pursuit_law(const t2d_controller_params& p, const PathVertex* pv, int n_vert, double v, double x, double y,
+__device__ double pure_pursuit_law(const CtrlLawRow& p, const PathVertex* pv, int n_vert, double v, double x, double y,
                                    double heading) {
   const double d = fmax(v * (double)p.pp_interval, (double)p.min_pre_aiming_distance);     // :90-91
   double px = pv[n_vert - 1].x, py = pv[n_vert - 1].y;
@@ -1959,6 +1977,109 @@ __device__ double pure_pursuit_law(const t2d_controller_params& p, const PathVer
   return atan(2.0 * (double)p.wheel_base * sin(ang - heading) / dist);                      // :68-70
 }
 
+// pid_controller.py:159-234, one channel.  s = (integral, prev_error, prev_derivative) is rewritten in place.  Every
+// operation rounds once (no FMA contraction) in the reference's order; `limited` selects the output_limits branch.
+__device__ double pid_channel(const t2d_controller_params& p, double e, double s[3], double kp, double ki, double kd,
+                              bool limited, double lo, double hi) {
+  const double alpha = p.derivative_filter_alpha;
+  const double p_term = __dmul_rn(kp, e);                                                     // :191
+  const double raw = __ddiv_rn(__dsub_rn(e, s[1]), p.dt);                                     // :194
+  const double d = __dadd_rn(__dmul_rn(alpha, raw), __dmul_rn(__dsub_rn(1.0, alpha), s[2]));   // :195-198
+  double out = __dadd_rn(p_term, __dmul_rn(kd, d));                                          // :199-202
+  bool saturated = false;
+  if (limited) {                                                                             // :205-214
+    if (out > hi) { saturated = true; out = hi; }
+    else if (out < lo) { saturated = true; out = lo; }
+  }
+  s[0] = saturated ? __dmul_rn(s[0], 0.99) : __dadd_rn(s[0], __dmul_rn(e, p.dt));            // :217-222
+  out = __dadd_rn(out, __dmul_rn(ki, s[0]));                                                 // :224-227
+  if (limited) out = clip_np(out, lo, hi);                                                   // :230-232
+  s[1] = e;
+  s[2] = d;
+  return out;
+}
+
+// The lateral error of a PATH_* source (no reference counterpart): the closest point c of the polyline to (x, y) - the
+// first strict minimum of |p - c|^2 over the segments of non-zero length, c the clamped projection - and that segment's
+// unit tangent u.  PATH_CROSS_TRACK: e = u.x (c.y - y) - u.y (c.x - x), positive when the path lies to the left;
+// PATH_HEADING: target_heading = atan2(u.y, u.x).  fp64, one rounding per operation, in this order.  false: no segment.
+__device__ bool path_lateral_error(const PathVertex* pv, int n_vert, double x, double y, double heading, bool cross,
+                                   double& e) {
+  double best = 0.0, cx = 0.0, cy = 0.0, ux = 0.0, uy = 0.0;
+  bool found = false;
+  for (int i = 0; i + 1 < n_vert; ++i) {
+    const double ax = pv[i].x, ay = pv[i].y;
+    const double dx = __dsub_rn(pv[i + 1].x, ax), dy = __dsub_rn(pv[i + 1].y, ay);
+    const double l2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
+    if (!(l2 > 0.0)) continue;
+    double t = __ddiv_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, ax), dx), __dmul_rn(__dsub_rn(y, ay), dy)), l2);
+    t = fmin(fmax(t, 0.0), 1.0);
+    const double qx = __dadd_rn(ax, __dmul_rn(t, dx)), qy = __dadd_rn(ay, __dmul_rn(t, dy));
+    const double ex = __dsub_rn(x, qx), ey = __dsub_rn(y, qy);
+    const double d2 = __dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey));
+    if (!found || d2 < best) {
+      const double len = __dsqrt_rn(l2);
+      best = d2; cx = qx; cy = qy; ux = __ddiv_rn(dx, len); uy = __ddiv_rn(dy, len);
+      found = true;
+    }
+  }
+  if (!found) return false;
+  if (cross) {
+    e = __dsub_rn(__dmul_rn(ux, __dsub_rn(cy, y)), __dmul_rn(uy, __dsub_rn(cx, x)));
+  } else {
+    const double err = __dsub_rn(atan2(uy, ux), heading);
+    e = atan2(sin(err), cos(err));
+  }
+  return true;
+}
+
+// pid_controller.py:309-406 for slot i: (steering, acceleration) into steer / acc; the slot's state row is rewritten
+// for each channel that runs.  A channel whose source is NONE, or whose error is missing (a PATH source without a usable
+// path: the combined mode's missing keyword), gives 0 and leaves its half of the row alone.
+__device__ void pid_law(const t2d_controller_params& p, const CtrlArgs& A, size_t i, double x, double y, double v,
+                        double heading, double& steer, double& acc) {
+  double* st = A.pid_state + 6 * i;
+  steer = 0.0;
+  acc = 0.0;
+  const int lat = p.pid_lateral;
+  if (lat != T2D_PID_LAT_NONE) {
+    double e = 0.0;
+    bool have = true;
+    if (lat == T2D_PID_LAT_HEADING) {                                                       // :267-274
+      const double err = __dsub_rn((double)A.pid_target[2 * i + 1], heading);
+      e = atan2(sin(err), cos(err));
+    } else if (lat == T2D_PID_LAT_CROSS_TRACK) {                                             // :275-279
+      e = (double)A.pid_target[2 * i + 1];
+    } else {
+      const int pid = A.path_id ? (int)A.path_id[i] : -1;
+      have = pid >= 0 && pid < A.n_paths &&
+             path_lateral_error(A.path_v + A.path_off[pid], A.path_off[pid + 1] - A.path_off[pid], x, y, heading,
+                                lat == T2D_PID_LAT_PATH_CROSS_TRACK, e);
+    }
+    if (have) {
+      double s[3] = {st[0], st[1], st[2]};
+      const double out = pid_channel(p, e, s, p.kp_lat, p.ki_lat, p.kd_lat, false, 0.0, 0.0);   // :338-348
+      const bool cross = lat == T2D_PID_LAT_CROSS_TRACK || lat == T2D_PID_LAT_PATH_CROSS_TRACK;
+      steer = cross ? __dmul_rn(out, __ddiv_rn(2.0, (double)p.wheel_base)) : out;            // :355-365
+      steer = clip_np(steer, -p.max_steering, p.max_steering);                               // :368
+      st[0] = s[0]; st[1] = s[1]; st[2] = s[2];
+    }
+  }
+  if (p.pid_longitudinal == T2D_PID_LON_TARGET) {
+    const double e = __dsub_rn((double)A.pid_target[2 * i], v);                              // :306-307
+    double s[3] = {st[3], st[4], st[5]};
+    const double lo = (double)p.min_accel, hi = (double)p.max_accel;
+    acc = clip_np(pid_channel(p, e, s, p.kp_lon, p.ki_lon, p.kd_lon, true, lo, hi), lo, hi);   // :383-397
+    st[3] = s[0]; st[4] = s[1]; st[5] = s[2];
+  }
+}
+
+__device__ __forceinline__ const CtrlLawRow& law_row(const t2d_controller_params* ctab, int cid) {
+  return *reinterpret_cast<const CtrlLawRow*>(reinterpret_cast<const char*>(ctab) + (size_t)cid * sizeof(t2d_controller_params));
+}
+
+// HAS_PID: the instance with the PID law, launched when the bound table holds a PID row; the other one is today's K5.
+template <bool HAS_PID>
 __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant__ CtrlArgs A) {
   const int lane = threadIdx.x & 31;
   const int warps = (gridDim.x * blockDim.x) >> 5;
@@ -1980,8 +2101,8 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
       out[j] = reinterpret_cast<const float2*>(A.action)[base + m];
       if (m == 0 && A.ego_action != nullptr) { out[j] = reinterpret_cast<const float2*>(A.ego_action)[n]; ctl[j] = true; }   // row 0 <- the ego's action
       const int cid = A.ctrl_id[base + m];
-      if (cid < A.n_ctrl && A.ctab[cid].kind != T2D_CTRL_EXTERNAL) {
-        const t2d_controller_params& p = A.ctab[cid];
+      if (cid < A.n_ctrl && law_row(A.ctab, cid).kind != T2D_CTRL_EXTERNAL) {
+        const CtrlLawRow& p = law_row(A.ctab, cid);
         const double x = A.x[base + m], y = A.y[base + m], v = A.v[base + m];
         const int li = A.lead ? (int)A.lead[base + m] : -1;
         const bool has = li >= 0 && li < A.M && li != m && A.type_id[base + li] < A.n_types;
@@ -1990,7 +2111,9 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
           xl = A.x[base + li]; yl = A.y[base + li]; vl = A.v[base + li]; al = A.last_accel[base + li];
         }
         double acc, steer = 0.0;
-        if (p.kind == T2D_CTRL_IDM) {
+        if (HAS_PID && p.kind == T2D_CTRL_PID) {
+          pid_law(A.ctab[cid], A, base + m, x, y, v, (double)A.h[base + m], steer, acc);
+        } else if (p.kind == T2D_CTRL_IDM) {
           acc = idm_law(p, v, x, y, has, vl, xl, yl);
         } else {
           acc = longitudinal_law(p, v, x, y, (double)A.last_accel[base + m], has, vl, xl, yl, al);
@@ -2199,6 +2322,10 @@ struct t2d_ctx {
   const int16_t* ctrl_lead = nullptr;
   const int16_t* ctrl_path = nullptr;
   float* ctrl_last_accel = nullptr;
+  bool ctrl_has_pid = false;          // the table holds a T2D_CTRL_PID row: K5 runs its PID instance
+  bool ctrl_pid_reads_target = false; // ... and one of them reads the target array
+  const float* pid_target = nullptr;  // t2d_set_pid: [N][M][2]
+  double* pid_state = nullptr;        // t2d_set_pid: [N][M][6]
   dev_ptr<PathVertex> d_path_v;
   dev_ptr<int> d_path_off;
   int n_paths = 0;
@@ -2952,9 +3079,19 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
 }
 
 // K5 with the ego action `ego` (nullptr: row 0 of `action`)
+// A call K5 could not complete is refused before anything is launched: PID rows without their state or target.
+static int check_pid_binding(const t2d_ctx* c) {
+  if (!c->ctrl_has_pid) return T2D_OK;
+  if (!c->pid_state) return fail(T2D_E_INVALID, "a PID controller row is bound without its state: call t2d_set_pid first");
+  if (c->ctrl_pid_reads_target && !c->pid_target)
+    return fail(T2D_E_INVALID, "a PID controller row reads the target, and none is bound: call t2d_set_pid with one");
+  return T2D_OK;
+}
+
 static int launch_control(t2d_ctx* c, float* action, const float* ego, void* stream) {
   if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   if (!c->d_ctab) return fail(T2D_E_STATE, "controllers not set: call t2d_set_controllers first");
+  if (int r = check_pid_binding(c)) return r;
   if (!action) return fail(T2D_E_INVALID, "action is NULL");
   if (reinterpret_cast<uintptr_t>(action) % 8 != 0) return fail(T2D_E_INVALID, "action must be 8-byte aligned");
   CUDA_TRY(cudaSetDevice(c->device));
@@ -2963,8 +3100,10 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
   A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
   A.last_accel = c->ctrl_last_accel; A.action = action; A.ego_action = ego;
   A.steer_first = (c->cfg.flags & T2D_CFG_STEER_FIRST) ? 1 : 0;
+  A.pid_target = c->pid_target; A.pid_state = c->pid_state;
   const int warps_per_cta = 4;
-  t2d_control_kernel<<<capped_grid(c->N, warps_per_cta, c->sm_count, 16), warps_per_cta * 32, 0, (cudaStream_t)stream>>>(A);
+  auto kern = c->ctrl_has_pid ? t2d_control_kernel<true> : t2d_control_kernel<false>;
+  kern<<<capped_grid(c->N, warps_per_cta, c->sm_count, 16), warps_per_cta * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
 }
 
@@ -3089,6 +3228,8 @@ int t2d_step_host_ego(t2d_ctx* c, const float* ego_action_host, float* action, u
     c->hs_ego = std::move(e);
   }
   if (int r = status_done_staging(c)) return r;
+  if (c->d_ctab)
+    if (int r = check_pid_binding(c)) return r;
   memcpy(c->hs_ego.host.get(), ego_action_host, (size_t)N * 2 * sizeof(float));
   const float* ego = c->hs_ego.dev;
   if (c->d_ctab) {
@@ -3192,6 +3333,8 @@ int t2d_step_host_agents(t2d_ctx* c, const float* agent_action_host, float* acti
   if (!aligned8(action)) return fail(T2D_E_INVALID, "t2d_step_host_agents: action must be 8-byte aligned");
   if (int r = require(c, NEED_STATE | NEED_TABLE | NEED_TICK)) return r;
   if (c->agent_q == 0) return fail(T2D_E_STATE, "t2d_step_host_agents: no agents bound: call t2d_set_agents first");
+  if (c->d_ctab)
+    if (int r = check_pid_binding(c)) return r;
   CUDA_TRY(cudaSetDevice(c->device));
   const int N = c->N, M = c->M, Q = c->agent_q;
   const size_t nq = (size_t)N * Q;
@@ -3249,7 +3392,7 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   A.px = pool_x; A.py = pool_y; A.ph = pool_heading; A.pv = pool_speed; A.pvx = pool_vx; A.pvy = pool_vy;
   A.goal = c->goal;
   A.wheel_f = c->wheel_f; A.wheel_r = c->wheel_r; A.pool_wf = c->reset_pool_wf; A.pool_wr = c->reset_pool_wr;
-  A.last_accel = c->ctrl_last_accel; A.n_pool = n_pool;
+  A.last_accel = c->ctrl_last_accel; A.pid_state = c->pid_state; A.n_pool = n_pool;
   if (c->agent_q > 0) {   // the bound type_id is the caller's writable device array (K10 retires slots in it)
     A.agent_type_id = const_cast<uint8_t*>(c->type_id); A.agent_retired = c->agent_retired;
     A.agent = c->agent; A.agent_q = c->agent_q;
@@ -3434,13 +3577,33 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
     c->d_ctab.reset();
     c->n_ctrl = 0; c->ctrl_id = nullptr; c->ctrl_lead = nullptr; c->ctrl_path = nullptr;
     c->ctrl_last_accel = nullptr;
+    c->ctrl_has_pid = c->ctrl_pid_reads_target = false;
     return T2D_OK;
   }
   if (n_rows <= 0 || n_rows > T2D_MAX_CONTROLLERS) return fail(T2D_E_INVALID, "n_rows must be in 1..T2D_MAX_CONTROLLERS");
   if (!ctrl_id || !last_accel) return fail(T2D_E_INVALID, "t2d_set_controllers: ctrl_id / last_accel is NULL");
+  bool has_pid = false, reads_target = false;
   for (int i = 0; i < n_rows; ++i) {
     const t2d_controller_params& p = table[i];
-    if (p.kind < T2D_CTRL_EXTERNAL || p.kind > T2D_CTRL_PURE_PURSUIT) return fail(T2D_E_INVALID, "unknown controller kind");
+    if (p.kind < T2D_CTRL_EXTERNAL || p.kind > T2D_CTRL_PID) return fail(T2D_E_INVALID, "unknown controller kind");
+    if (p.kind == T2D_CTRL_PID) {   // PIDController.__init__'s checks, pid_controller.py:81-102
+      if (!(p.dt > 0.0)) return fail(T2D_E_INVALID, "PID row: dt must be positive");
+      if (!(p.max_steering > 0.0)) return fail(T2D_E_INVALID, "PID row: max_steering must be positive");
+      if (!(p.max_accel > 0.0f)) return fail(T2D_E_INVALID, "PID row: max_accel must be positive");
+      if (!(p.min_accel < 0.0f)) return fail(T2D_E_INVALID, "PID row: min_accel must be negative (deceleration)");
+      if (!(p.max_accel > p.min_accel)) return fail(T2D_E_INVALID, "PID row: max_accel must be greater than min_accel");
+      if (!(p.derivative_filter_alpha > 0.0 && p.derivative_filter_alpha <= 1.0))
+        return fail(T2D_E_INVALID, "PID row: derivative_filter_alpha must be in range (0, 1]");
+      if (p.pid_lateral < T2D_PID_LAT_NONE || p.pid_lateral > T2D_PID_LAT_PATH_CROSS_TRACK)
+        return fail(T2D_E_INVALID, "PID row: unknown lateral source");
+      if (p.pid_longitudinal != T2D_PID_LON_NONE && p.pid_longitudinal != T2D_PID_LON_TARGET)
+        return fail(T2D_E_INVALID, "PID row: unknown longitudinal source");
+      if ((p.pid_lateral == T2D_PID_LAT_CROSS_TRACK || p.pid_lateral == T2D_PID_LAT_PATH_CROSS_TRACK) && !(p.wheel_base > 0.0f))
+        return fail(T2D_E_INVALID, "PID row: wheel_base must be positive");   // pid_controller.py:357-358
+      has_pid = true;
+      reads_target = reads_target || p.pid_longitudinal == T2D_PID_LON_TARGET || p.pid_lateral == T2D_PID_LAT_HEADING ||
+                     p.pid_lateral == T2D_PID_LAT_CROSS_TRACK;
+    }
     if (p.kind == T2D_CTRL_PURE_PURSUIT && !(p.min_pre_aiming_distance > 0.0f))
       return fail(T2D_E_INVALID, "min_pre_aiming_distance must be positive");   // pure_pursuit_controller.py:30-31
     if (p.kind >= T2D_CTRL_CRUISE && p.target_speed < 0.0f)
@@ -3448,6 +3611,20 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
   }
   if (int r = upload(c->d_ctab, table, (size_t)n_rows)) return r;
   c->n_ctrl = n_rows; c->ctrl_id = ctrl_id; c->ctrl_lead = lead_index; c->ctrl_path = path_id; c->ctrl_last_accel = last_accel;
+  c->ctrl_has_pid = has_pid; c->ctrl_pid_reads_target = reads_target;
+  return T2D_OK;
+}
+
+int t2d_set_pid(t2d_ctx* c, const float* target, double* state) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!state) {
+    if (target) return fail(T2D_E_INVALID, "t2d_set_pid: a target needs a state");
+    c->pid_target = nullptr; c->pid_state = nullptr;
+    return T2D_OK;
+  }
+  if (reinterpret_cast<uintptr_t>(target) % 8 != 0 || reinterpret_cast<uintptr_t>(state) % 8 != 0)
+    return fail(T2D_E_INVALID, "t2d_set_pid: target / state must be 8-byte aligned");
+  c->pid_target = target; c->pid_state = state;
   return T2D_OK;
 }
 

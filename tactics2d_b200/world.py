@@ -298,14 +298,23 @@ class BatchedWorld:
             _lib.check(self.lib.t2d_set_paths(self._ctx, C.c_void_p(xy.ctypes.data), C.c_void_p(off.ctypes.data), len(paths)))
         self.paths = paths
 
-    def set_controllers(self, controllers, ctrl_id, lead_index=None, path_id=None, last_accel=None):
+    def set_controllers(self, controllers, ctrl_id, lead_index=None, path_id=None, last_accel=None, pid_target=None,
+                        pid_state=None):
         """Hand the non-ego agents to on-device controllers.  ``controllers``: list of ``tactics2d_b200.controller``
         objects (or ``ControllerParamsC`` rows); ``ctrl_id`` [N, M] uint8: the participant's row, 255 for "action comes
         from the caller"; ``lead_index`` [N, M] int16: its leading vehicle (``leading_state`` / ``front_state``), -1 for
-        none; ``path_id`` [N, M] int16: its pure-pursuit path (``set_paths``), -1 for none; ``last_accel`` [N, M]:
-        ``State.accel`` of the previous tick (default zeros).  ``None`` for ``controllers`` removes them."""
+        none; ``path_id`` [N, M] int16: its pure-pursuit path or the PID rows' path (``set_paths``), -1 for none;
+        ``last_accel`` [N, M]: ``State.accel`` of the previous tick (default zeros).  ``None`` for ``controllers``
+        removes them.
+
+        PID rows (``PIDController``): ``pid_target`` [N, M, 2] = (target_speed, target_heading or cross_track_error),
+        fp32, read every tick (write new targets into ``self.pid_target`` in place).  Their memory is ``self.pid_state``,
+        fp64 [N, M, 6] = (lat_integral, lat_prev_error, lat_prev_derivative, lon_integral, lon_prev_error,
+        lon_prev_derivative): a fresh zeroed tensor, or ``pid_state`` when given; ``reset`` zeroes the rows of the
+        reset scenarios."""
         if controllers is None:
             _lib.check(self.lib.t2d_set_controllers(self._ctx, _ptr(None), 0, _ptr(None), _ptr(None), _ptr(None), _ptr(None)))
+            _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(None), _ptr(None)))
             self._ctrl = None
             return
         rows = [c if isinstance(c, _lib.ControllerParamsC) else c.params() for c in controllers]
@@ -323,13 +332,39 @@ class BatchedWorld:
         la = dev(last_accel, torch.float32, 0.0)
         if la is None:
             la = torch.zeros((self.N, self.M), dtype=torch.float32, device=self.device)
+        from .controller.controller_base import CTRL_PID
+
+        tgt, st = None, None
+        if any(r.kind == CTRL_PID for r in rows):
+            if pid_target is not None:
+                t = pid_target if torch.is_tensor(pid_target) else torch.from_numpy(np.ascontiguousarray(np.asarray(pid_target)))
+                tgt = t.to(device=self.device, dtype=torch.float32).reshape(self.N, self.M, 2).contiguous()
+            if pid_state is None:
+                st = torch.zeros((self.N, self.M, 6), dtype=torch.float64, device=self.device)
+            else:
+                if (not torch.is_tensor(pid_state) or pid_state.dtype != torch.float64 or pid_state.device != self.device
+                        or tuple(pid_state.shape) != (self.N, self.M, 6) or not pid_state.is_contiguous()):
+                    raise ValueError(f"pid_state must be a contiguous fp64 [{self.N}, {self.M}, 6] tensor on the world's device")
+                st = pid_state
+        # the controllers first: a rejected table leaves the previous binding, PID arrays included, as it was
         _lib.check(self.lib.t2d_set_controllers(self._ctx, arr, len(rows), _ptr(cid), _ptr(lead), _ptr(pid), _ptr(la)))
-        self._ctrl = dict(rows=arr, ctrl_id=cid, lead_index=lead, path_id=pid, last_accel=la)
+        _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(tgt), _ptr(st)))
+        self._ctrl = dict(rows=arr, ctrl_id=cid, lead_index=lead, path_id=pid, last_accel=la, pid_target=tgt, pid_state=st)
 
     @property
     def last_accel(self) -> Optional[torch.Tensor]:
         c = getattr(self, "_ctrl", None)
         return None if c is None else c["last_accel"]
+
+    @property
+    def pid_target(self) -> Optional[torch.Tensor]:
+        c = getattr(self, "_ctrl", None)
+        return None if c is None else c["pid_target"]
+
+    @property
+    def pid_state(self) -> Optional[torch.Tensor]:
+        c = getattr(self, "_ctrl", None)
+        return None if c is None else c["pid_state"]
 
     def control(self, action: torch.Tensor) -> torch.Tensor:
         """Fill the rows of ``action`` [N, M, 2] that belong to controlled participants (IN PLACE; the other rows keep
