@@ -102,7 +102,7 @@ class AgentObservation:
     segments: torch.Tensor       # fp32 [N, Q, S, 9]   (SEGMENT_FIELDS), nearest first
     agent_index: torch.Tensor    # int16 [N, Q, K]: the participant slot of each agent row, -1 for padding
     segment_index: torch.Tensor  # int16 [N, Q, S]: the segment's index in its tile, -1 for padding
-    observers: Optional[torch.Tensor]   # int16 [N, Q] as passed, or None: row q is slot q
+    observers: Optional[torch.Tensor] = None   # int16 [N, Q] as passed, or None: row q is slot q
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -160,7 +160,11 @@ class BatchedWorld:
         self.poly_start = None
         self.tiles, self.tile_id = None, None
         self.bounds = None
-        self._goal = None
+        self.paths = None
+        # what the setters bind (None until they are called) and the output buffers made on first use
+        self._goal = self._ctrl = self._log = self._agents = self._ego_action = None
+        self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
+        self._agent_lidar, self._obs_out, self._agent_obs_out = {}, {}, {}
         self._seg_style_keys = []
         self._bev_cfg = None
 
@@ -171,6 +175,33 @@ class BatchedWorld:
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _device_tensor(self, name: str, t, dtype: torch.dtype, shape) -> torch.Tensor:
+        """``t`` itself, after checking that it is a contiguous ``dtype`` tensor of exactly ``shape`` on the world's device.
+        Such a tensor reaches the kernels as a raw pointer: a host tensor, another dtype or shape would be read out of
+        bounds."""
+        if not (torch.is_tensor(t) and t.device == self.device and t.dtype == dtype and t.shape == shape
+                and t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous {dtype} {list(shape)} tensor on {self.device}")
+        return t
+
+    @staticmethod
+    def _host_tensor(name: str, a, shape) -> torch.Tensor:
+        """``a`` as a contiguous fp32 CPU tensor of exactly ``shape``, for the host steps: any array-like is converted to
+        float32, a tensor must already be one."""
+        t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
+        if not (t.device.type == "cpu" and t.dtype == torch.float32 and t.shape == shape and t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous float32 host array {list(shape)}")
+        return t
+
+    def _to_device(self, a, dtype: torch.dtype, shape) -> torch.Tensor:
+        """``a`` (a tensor on any device, or anything array-like) as a contiguous ``dtype`` tensor of ``shape`` on the
+        world's device; a copy unless ``a`` is one already."""
+        t = (a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))).to(device=self.device, dtype=dtype)
+        return (t if t.shape == shape else t.reshape(shape)).contiguous()
+
+    def _put(self, dst: torch.Tensor, src):
+        dst.copy_(self._to_device(src, dst.dtype, dst.shape))
 
     def close(self):
         if getattr(self, "_ctx", None) is not None and self._ctx.value:
@@ -196,11 +227,22 @@ class BatchedWorld:
 
     def set_type_table(self, type_table: TypeTable):
         """Replace the type table.  The map stays as it was built: its dilated cell lists cover the reach of the table
-        that was current at ``set_map``, and a participant whose type reaches further takes the slower exhaustive walk."""
+        that was current at ``set_map``, and a participant whose type reaches further takes the slower exhaustive walk.
+
+        Once BEV styles are chosen (``set_bev_styles``, or the first ``bev``), they are pushed again for the new table
+        at once: a table with as many rows keeps the per-type styles, any other falls back on ``default_type_style`` of
+        its rows; the target keeps its style."""
+        from .sensor.camera import default_type_style
+
         if any(r.model == MODEL_DRIFT for r in type_table.rows) and self.omega_front is None:
             raise ValueError("a SingleTrackDrift row needs a world created with one (its wheel speeds are allocated there)")
         _lib.check(self.lib.t2d_set_type_table(self._ctx, type_table.to_c_array(), len(type_table)))
         self.type_table = type_table
+        if self._bev_cfg is not None:
+            type_styles, target = self._bev_cfg
+            if len(type_styles) != len(type_table):
+                self._bev_cfg = ([default_type_style(r) for r in type_table.rows], target)
+            self._push_bev_styles()
 
     def set_map(self, segments=None, bounds: Optional[Sequence[float]] = None, cell_size: float = 0.0, poly_start=None,
                 style=None):
@@ -253,7 +295,7 @@ class BatchedWorld:
         tid = torch.as_tensor(np.asarray(tile_id) if not torch.is_tensor(tile_id) else tile_id).to(torch.int64)
         if tid.numel() != self.N or int(tid.min()) < 0 or int(tid.max()) >= len(tiles):
             raise ValueError(f"tile_id must hold {self.N} indices into the {len(tiles)} tiles")
-        tid = tid.to(torch.int16).to(self.device).contiguous()   # (bit pattern of uint16 for ids < 32768)
+        tid = self._to_device(tid, torch.int16, tid.shape)   # (bit pattern of uint16 for ids < 32768)
         # a rejected table leaves the previous map bound, and with it the previous tile_id tensor
         _lib.check(self.lib.t2d_set_map_table(self._ctx, rows, len(tiles), _ptr(tid), float(cell_size)))
         self.tile_id = tid
@@ -274,9 +316,8 @@ class BatchedWorld:
             self._goal = None
             self._out.iou = None
             return
-        t = torch.as_tensor(np.asarray(target, dtype=np.float32) if not torch.is_tensor(target) else target)
-        t = t.to(device=self.device, dtype=torch.float32).reshape(self.N, 5).contiguous()
-        g = dict(target=t, iou=torch.zeros(self.N, dtype=torch.float32, device=self.device),
+        g = dict(target=self._to_device(target, torch.float32, (self.N, 5)),
+                 iou=torch.zeros(self.N, dtype=torch.float32, device=self.device),
                  last_pose=torch.zeros((self.N, 4), dtype=torch.float32, device=self.device),
                  count=torch.zeros(self.N, dtype=torch.int32, device=self.device))
         _lib.check(self.lib.t2d_set_goal(self._ctx, _ptr(g["target"]), float(arrival_threshold), int(no_action_max_step),
@@ -319,33 +360,22 @@ class BatchedWorld:
             return
         rows = [c if isinstance(c, _lib.ControllerParamsC) else c.params() for c in controllers]
         arr = (_lib.ControllerParamsC * len(rows))(*rows)
-
-        def dev(a, dtype, fill):
-            if a is None:
-                return None
-            t = a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(np.asarray(a)))
-            return t.to(device=self.device, dtype=dtype).reshape(self.N, self.M).contiguous()
-
-        cid = dev(ctrl_id, torch.uint8, 255)
-        lead = dev(lead_index, torch.int16, -1)
-        pid = dev(path_id, torch.int16, -1)
-        la = dev(last_accel, torch.float32, 0.0)
+        NM = (self.N, self.M)
+        dev = lambda a, dtype: None if a is None else self._to_device(a, dtype, NM)
+        cid, lead, pid = dev(ctrl_id, torch.uint8), dev(lead_index, torch.int16), dev(path_id, torch.int16)
+        la = dev(last_accel, torch.float32)
         if la is None:
-            la = torch.zeros((self.N, self.M), dtype=torch.float32, device=self.device)
+            la = torch.zeros(NM, dtype=torch.float32, device=self.device)
         from .controller.controller_base import CTRL_PID
 
         tgt, st = None, None
         if any(r.kind == CTRL_PID for r in rows):
             if pid_target is not None:
-                t = pid_target if torch.is_tensor(pid_target) else torch.from_numpy(np.ascontiguousarray(np.asarray(pid_target)))
-                tgt = t.to(device=self.device, dtype=torch.float32).reshape(self.N, self.M, 2).contiguous()
+                tgt = self._to_device(pid_target, torch.float32, NM + (2,))
             if pid_state is None:
-                st = torch.zeros((self.N, self.M, 6), dtype=torch.float64, device=self.device)
+                st = torch.zeros(NM + (6,), dtype=torch.float64, device=self.device)
             else:
-                if (not torch.is_tensor(pid_state) or pid_state.dtype != torch.float64 or pid_state.device != self.device
-                        or tuple(pid_state.shape) != (self.N, self.M, 6) or not pid_state.is_contiguous()):
-                    raise ValueError(f"pid_state must be a contiguous fp64 [{self.N}, {self.M}, 6] tensor on the world's device")
-                st = pid_state
+                st = self._device_tensor("pid_state", pid_state, torch.float64, NM + (6,))
         # the controllers first: a rejected table leaves the previous binding, PID arrays included, as it was
         _lib.check(self.lib.t2d_set_controllers(self._ctx, arr, len(rows), _ptr(cid), _ptr(lead), _ptr(pid), _ptr(la)))
         _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(tgt), _ptr(st)))
@@ -353,27 +383,21 @@ class BatchedWorld:
 
     @property
     def last_accel(self) -> Optional[torch.Tensor]:
-        c = getattr(self, "_ctrl", None)
-        return None if c is None else c["last_accel"]
+        return None if self._ctrl is None else self._ctrl["last_accel"]
 
     @property
     def pid_target(self) -> Optional[torch.Tensor]:
-        c = getattr(self, "_ctrl", None)
-        return None if c is None else c["pid_target"]
+        return None if self._ctrl is None else self._ctrl["pid_target"]
 
     @property
     def pid_state(self) -> Optional[torch.Tensor]:
-        c = getattr(self, "_ctrl", None)
-        return None if c is None else c["pid_state"]
+        return None if self._ctrl is None else self._ctrl["pid_state"]
 
     def control(self, action: torch.Tensor) -> torch.Tensor:
         """Fill the rows of ``action`` [N, M, 2] that belong to controlled participants (IN PLACE; the other rows keep
         the caller's values) and refresh ``last_accel`` - ``ControllerBase.step`` of every NPC in one launch.  Call it
         after writing the external (ego) actions and before ``step``."""
-        if action.device != self.device or action.dtype != torch.float32:
-            raise ValueError("action must be an fp32 tensor on the world's device")
-        if tuple(action.shape) != (self.N, self.M, 2) or not action.is_contiguous():
-            raise ValueError(f"action must be contiguous [{self.N}, {self.M}, 2]")
+        self._device_tensor("action", action, torch.float32, (self.N, self.M, 2))
         _lib.check(self.lib.t2d_control(self._ctx, _ptr(action), self._stream()))
         return action
 
@@ -436,30 +460,26 @@ class BatchedWorld:
     def replay_track(self) -> Optional[torch.Tensor]:
         """int32 [N, M] device tensor: the track each slot shows, -1 while it shows none or is not replayed (None unless a
         log is bound with a ``schedule``).  Every replay - each tick and each reset of a scenario - rewrites its slots."""
-        lg = getattr(self, "_log", None)
-        return None if lg is None else lg["track"]
+        return None if self._log is None else self._log["track"]
 
     @property
     def log_row(self) -> Optional[torch.Tensor]:
         """int32 [N] device tensor: the episode row every scenario runs (None without a log).  ``reset`` writes it; it may
         be rewritten between ticks."""
-        lg = getattr(self, "_log", None)
-        return None if lg is None else lg["log_row"]
+        return None if self._log is None else self._log["log_row"]
 
     # ------------------------------------------------------------------ state
     def set_wheel_state(self, omega_front, omega_rear):
         """Wheel angular speeds [N, M] of the SingleTrackDrift participants (``omega_wf`` / ``omega_wr``)."""
         if self.omega_front is None:
             raise ValueError("the type table holds no SingleTrackDrift row")
-        for dst, src in ((self.omega_front, omega_front), (self.omega_rear, omega_rear)):
-            dst.copy_(torch.as_tensor(np.asarray(src) if not torch.is_tensor(src) else src).to(dst.dtype).reshape(dst.shape))
+        self._put(self.omega_front, omega_front)
+        self._put(self.omega_rear, omega_rear)
 
     def set_state(self, x, y, heading, speed=None, vx=None, vy=None, type_id=None):
         """Copy host or device arrays [N, M] into the SoA state.  Missing ``vx, vy`` are derived as
         ``State.velocity`` does (state.py:160-165); missing ``speed`` as ``State.speed`` (:143-146)."""
-        def put(dst, src):
-            dst.copy_(torch.as_tensor(np.asarray(src) if not torch.is_tensor(src) else src).to(dst.dtype).reshape(dst.shape))
-
+        put = self._put
         put(self.x, x); put(self.y, y); put(self.heading, heading)
         if speed is None and (vx is None or vy is None):
             raise ValueError("give speed, or vx and vy")
@@ -486,10 +506,7 @@ class BatchedWorld:
     def step(self, action: torch.Tensor) -> StepResult:
         """One tick.  ``action``: fp32 device tensor [N, M, 2] = (accel, steer) per bicycle
         (``(steer, accel)`` when built with ``steer_first``), (ax, ay) per point mass."""
-        if action.device != self.device or action.dtype != torch.float32:
-            raise ValueError("action must be an fp32 tensor on the world's device")
-        if tuple(action.shape) != (self.N, self.M, 2) or not action.is_contiguous():
-            raise ValueError(f"action must be contiguous [{self.N}, {self.M}, 2]")
+        self._device_tensor("action", action, torch.float32, (self.N, self.M, 2))
         o = self._out
         _lib.check(self.lib.t2d_step(self._ctx, _ptr(action), _ptr(o.flags), _ptr(o.hit_index), _ptr(o.hit_segment),
                                      _ptr(o.status), _ptr(o.done), self._stream()))
@@ -508,17 +525,25 @@ class BatchedWorld:
         ``done`` tensors this call does not touch).  The copies are
         inside the call (``t2d_step_host``): chunked host->device copy overlapped with the kernel, one
         device->host read-back, one stream synchronisation."""
-        a = action if isinstance(action, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(action, dtype=np.float32))
-        if a.device.type != "cpu" or a.dtype != torch.float32 or tuple(a.shape) != (self.N, self.M, 2) or not a.is_contiguous():
-            raise ValueError(f"action must be a contiguous float32 host array [{self.N}, {self.M}, 2]")
-        hb = getattr(self, "_host_out", None)
-        if hb is None:
-            hb = self._host_out = (np.empty(self.N, np.uint8), np.empty(self.N, np.uint8))
+        a = self._host_tensor("action", action, (self.N, self.M, 2))
+        hb = self._host_status()
         o = self._out
         _lib.check(self.lib.t2d_step_host(self._ctx, a.data_ptr(), _ptr(o.flags), _ptr(o.hit_index), _ptr(o.hit_segment),
                                           hb[1].ctypes.data, hb[0].ctypes.data, self._stream()))
         self.frame += self.interval
         return hb[0], hb[1]
+
+    def _host_status(self):
+        """The (done, status) host buffers the ego host steps return."""
+        if self._host_out is None:
+            self._host_out = (np.empty(self.N, np.uint8), np.empty(self.N, np.uint8))
+        return self._host_out
+
+    def _npc_zero_action(self) -> torch.Tensor:
+        """The internal zero [N, M, 2] action of the host steps called without a device ``action``."""
+        if self._npc_action is None:
+            self._npc_action = torch.zeros((self.N, self.M, 2), dtype=torch.float32, device=self.device)
+        return self._npc_action
 
     # ------------------------------------------------------------------ env layer
     def set_ego_action(self, ego_action: Optional[torch.Tensor]):
@@ -526,9 +551,7 @@ class BatchedWorld:
         ``step`` take the action of participant 0 of every scenario from it - the reference env's single action
         (envs/parking.py:219-239) - instead of row 0 of the full action array."""
         if ego_action is not None:
-            if (ego_action.device != self.device or ego_action.dtype != torch.float32 or tuple(ego_action.shape) != (self.N, 2)
-                    or not ego_action.is_contiguous()):
-                raise ValueError(f"ego_action must be a contiguous fp32 [{self.N}, 2] tensor on {self.device}")
+            self._device_tensor("ego_action", ego_action, torch.float32, (self.N, 2))
         _lib.check(self.lib.t2d_set_ego_action(self._ctx, _ptr(ego_action)))
         self._ego_action = ego_action   # keeps the tensor alive while the library holds its pointer
 
@@ -537,19 +560,12 @@ class BatchedWorld:
         or CPU tensor; the other participants take the rows of the DEVICE array ``action`` [N, M, 2] (default: an
         internal zero array), which ``set_controllers`` fills on the device.  Per step 8 N bytes go up and 2 N come back
         (``t2d_step_host_ego``).  Returns ``(done, status)`` as uint8 NumPy arrays [N]."""
-        a = ego_action if isinstance(ego_action, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(ego_action, dtype=np.float32))
-        if a.device.type != "cpu" or a.dtype != torch.float32 or tuple(a.shape) != (self.N, 2) or not a.is_contiguous():
-            raise ValueError(f"ego_action must be a contiguous float32 host array [{self.N}, 2]")
+        a = self._host_tensor("ego_action", ego_action, (self.N, 2))
         if action is None:
-            action = getattr(self, "_npc_action", None)
-            if action is None:
-                action = self._npc_action = torch.zeros((self.N, self.M, 2), dtype=torch.float32, device=self.device)
-        elif action.device != self.device or action.dtype != torch.float32 or tuple(action.shape) != (self.N, self.M, 2) \
-                or not action.is_contiguous():
-            raise ValueError(f"action must be contiguous fp32 [{self.N}, {self.M}, 2] on {self.device}")
-        hb = getattr(self, "_host_out", None)
-        if hb is None:
-            hb = self._host_out = (np.empty(self.N, np.uint8), np.empty(self.N, np.uint8))
+            action = self._npc_zero_action()
+        else:
+            self._device_tensor("action", action, torch.float32, (self.N, self.M, 2))
+        hb = self._host_status()
         o = self._out
         _lib.check(self.lib.t2d_step_host_ego(self._ctx, a.data_ptr(), _ptr(action), _ptr(o.flags), _ptr(o.hit_index),
                                               _ptr(o.hit_segment), hb[1].ctypes.data, hb[0].ctypes.data, self._stream()))
@@ -564,7 +580,7 @@ class BatchedWorld:
     def env_epilogue(self, reset_trackers_on_done: bool = True) -> "EnvResult":
         """Reward, terminated, truncated, done and the per-participant TrafficStatus of the last tick in ONE launch
         (``t2d_env_epilogue``: ParkingEnv.step after check_status, envs/parking.py:240-256 and _get_reward :148-190)."""
-        e = getattr(self, "_env", None)
+        e = self._env
         if e is None:
             u8 = dict(dtype=torch.uint8, device=self.device)
             e = self._env = dict(
@@ -584,10 +600,9 @@ class BatchedWorld:
 
     def reset_env_trackers(self):
         """``ParkingEnv.reset``: forget the best IoU / distance of the previous episodes (parking.py:276-277)."""
-        e = getattr(self, "_env", None)
-        if e is not None:
-            e["max_iou"].fill_(-float("inf"))
-            e["min_dist"].fill_(float("inf"))
+        if self._env is not None:
+            self._env["max_iou"].fill_(-float("inf"))
+            self._env["min_dist"].fill_(float("inf"))
 
     # ------------------------------------------------------------------ per-agent status and reward
     def set_agents(self, observers: Optional[torch.Tensor] = None, goals: Optional[torch.Tensor] = None,
@@ -622,14 +637,13 @@ class BatchedWorld:
     @property
     def retired_type(self) -> Optional[torch.Tensor]:
         """uint8 [N, M] device tensor: the type of every slot an agent row retired, 255 elsewhere (None without agents)."""
-        a = getattr(self, "_agents", None)
-        return None if a is None else a["retired_type"]
+        return None if self._agents is None else self._agents["retired_type"]
 
     def agents_epilogue(self, reset_trackers_on_done: bool = True) -> AgentEnvResult:
         """Status, reward, terminated, truncated and IoU of every agent row of the last tick, retirement of the slots whose
         rows settled, and the scenarios' done mask (no row NORMAL), in ONE launch (``t2d_agents_epilogue``).  With one row
         per scenario on slot 0 and the ``set_goal`` target as its goal this is ``env_epilogue`` bit for bit."""
-        a = getattr(self, "_agents", None)
+        a = self._agents
         if a is None:
             raise RuntimeError("call set_agents before agents_epilogue")
         _lib.check(self.lib.t2d_agents_epilogue(
@@ -640,19 +654,11 @@ class BatchedWorld:
 
     def reset_agent_trackers(self):
         """Forget every agent row's best IoU / distance of the previous episodes (``reset_env_trackers`` per row)."""
-        a = getattr(self, "_agents", None)
-        if a is not None:
-            a["max_iou"].fill_(-float("inf"))
-            a["min_dist"].fill_(float("inf"))
+        if self._agents is not None:
+            self._agents["max_iou"].fill_(-float("inf"))
+            self._agents["min_dist"].fill_(float("inf"))
 
     # ------------------------------------------------------------------ per-agent action
-    def _device_action(self, name: str, t, rows: int) -> torch.Tensor:
-        # the tensor reaches the kernel as a raw pointer: a host tensor, a wrong dtype or shape would be read out of bounds
-        if (not torch.is_tensor(t) or t.device != self.device or t.dtype != torch.float32
-                or tuple(t.shape) != (self.N, rows, 2) or not t.is_contiguous()):
-            raise ValueError(f"{name} must be a contiguous fp32 [{self.N}, {rows}, 2] tensor on {self.device}")
-        return t
-
     def scatter_agent_action(self, agent_action: torch.Tensor, action: torch.Tensor,
                              observers: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Write one action per agent row into its slot of ``action`` [N, M, 2] (IN PLACE; ``t2d_scatter_agent_action``,
@@ -662,8 +668,8 @@ class BatchedWorld:
         before ``control`` and ``step``: a controlled slot then takes its controller's action, and a bound ego action
         still drives slot 0."""
         Q = self._agent_rows(observers, None)
-        self._device_action("agent_action", agent_action, Q)
-        self._device_action("action", action, self.M)
+        self._device_tensor("agent_action", agent_action, torch.float32, (self.N, Q, 2))
+        self._device_tensor("action", action, torch.float32, (self.N, self.M, 2))
         _lib.check(self.lib.t2d_scatter_agent_action(self._ctx, _ptr(observers), Q, _ptr(agent_action), _ptr(action),
                                                      self._stream()))
         return action
@@ -677,20 +683,16 @@ class BatchedWorld:
         views of buffers owned by the world that hold their values until the next call.  The flags and hit indices stay on
         the device in ``self.result``; the per-row extrema are those of ``agents_epilogue``, so the two may be mixed.  No
         reset happens inside the call."""
-        a_ = getattr(self, "_agents", None)
+        a_ = self._agents
         if a_ is None:
             raise RuntimeError("call set_agents before step_host_agents")
         Q = a_["Q"]
-        a = agent_action if isinstance(agent_action, torch.Tensor) else torch.from_numpy(
-            np.ascontiguousarray(agent_action, dtype=np.float32))
-        if a.device.type != "cpu" or a.dtype != torch.float32 or tuple(a.shape) != (self.N, Q, 2) or not a.is_contiguous():
-            raise ValueError(f"agent_action must be a contiguous float32 host array [{self.N}, {Q}, 2]")
+        a = self._host_tensor("agent_action", agent_action, (self.N, Q, 2))
         if action is None:
-            action = getattr(self, "_npc_action", None)
-            if action is None:
-                action = self._npc_action = torch.zeros((self.N, self.M, 2), dtype=torch.float32, device=self.device)
-        self._device_action("action", action, self.M)
-        hb = getattr(self, "_host_agents", None)
+            action = self._npc_zero_action()
+        else:
+            self._device_tensor("action", action, torch.float32, (self.N, self.M, 2))
+        hb = self._host_agents
         if hb is None or hb[0].shape[1] != Q:
             hb = self._host_agents = (np.empty((self.N, Q), np.float32), np.empty((self.N, Q), np.bool_),
                                       np.empty((self.N, Q), np.bool_), np.empty((self.N, Q), np.uint8),
@@ -714,12 +716,10 @@ class BatchedWorld:
         fp32 [N, n_beams] distances, ``inf`` where nothing is hit within ``max_range``.  Defaults are the
         reference's (range 12 m, freq_detect / freq_scan = 5000 / 10 = 500 beams, lidar.py:35-50)."""
         key = (int(n_beams), float(max_range))
-        cache = getattr(self, "_lidar", None)
+        cache = self._lidar
         if cache is None or cache[0] != key:
-            theta = np.linspace(0, 2 * np.pi, int(n_beams), endpoint=False)          # lidar.py:160
-            cs = torch.from_numpy(np.stack([np.cos(theta), np.sin(theta)], 1)).to(self.device)   # float64, host trig
             scan = torch.empty((self.N, int(n_beams)), dtype=torch.float32, device=self.device)
-            self._lidar = cache = (key, cs.contiguous(), scan)
+            self._lidar = cache = (key, self._beam_table(n_beams), scan)
         _lib.check(self.lib.t2d_lidar_scan(self._ctx, int(n_beams), float(max_range), _ptr(cache[1]), _ptr(cache[2]), self._stream()))
         return cache[2]
 
@@ -733,16 +733,18 @@ class BatchedWorld:
         next call with those values reuses.  A row observed by slot 0 equals ``lidar_scan``'s row."""
         Q = self._agent_rows(observers, None)
         key = (int(n_beams), float(max_range), Q)
-        cache = self.__dict__.setdefault("_agent_lidar", {})
-        entry = cache.get(key)
+        entry = self._agent_lidar.get(key)
         if entry is None:
-            theta = np.linspace(0, 2 * np.pi, int(n_beams), endpoint=False)          # lidar.py:160
-            cs = torch.from_numpy(np.stack([np.cos(theta), np.sin(theta)], 1)).to(self.device)   # float64, host trig
             scan = torch.empty((self.N, Q, int(n_beams)), dtype=torch.float32, device=self.device)
-            entry = cache[key] = (cs.contiguous(), scan)
+            entry = self._agent_lidar[key] = (self._beam_table(n_beams), scan)
         _lib.check(self.lib.t2d_lidar_scan_agents(self._ctx, _ptr(observers), Q, int(n_beams), float(max_range),
                                                   _ptr(entry[0]), _ptr(entry[1]), self._stream()))
         return entry[1]
+
+    def _beam_table(self, n_beams) -> torch.Tensor:
+        """fp64 [n_beams, 2] device tensor: (cos, sin) of every beam's angle, the trig done on the host."""
+        theta = np.linspace(0, 2 * np.pi, int(n_beams), endpoint=False)          # lidar.py:160
+        return torch.from_numpy(np.stack([np.cos(theta), np.sin(theta)], 1)).to(self.device).contiguous()
 
     # ------------------------------------------------------------------ BEV observation
     @staticmethod
@@ -764,7 +766,8 @@ class BatchedWorld:
         :data:`tactics2d_b200.sensor.camera.BEV_STYLES`.  ``type_styles``: one key (or None = not drawn) per type-table
         row, default from each row's template name (:func:`~tactics2d_b200.sensor.camera.default_type_style`);
         ``target``: the style of the ``set_goal`` rectangle, None = not drawn.  Map segments take the ``style`` given to
-        ``set_map`` / ``set_map_table``."""
+        ``set_map`` / ``set_map_table``.  The per-type styles belong to the current table: ``set_type_table`` keeps them
+        for a table with as many rows and puts any other table's rows back on their defaults."""
         from .sensor.camera import BEV_STYLES, default_type_style
 
         if type_styles is None:
@@ -827,7 +830,7 @@ class BatchedWorld:
         pr = perception_range
         rng = np.ascontiguousarray(np.asarray([pr] * 4 if np.ndim(pr) == 0 else pr, dtype=np.float32).reshape(4))
         key = (w, h, bool(rgb))
-        cache = getattr(self, "_bev_out", None)
+        cache = self._bev_out
         if cache is None or cache[0] != key:
             if not (1 <= w <= 1024 and 1 <= h <= 1024):
                 raise ValueError("resolution: width and height must be in 1..1024")
@@ -846,41 +849,40 @@ class BatchedWorld:
         first, ties to the lower index; absent rows are zeros with index -1 (DESIGN.md section 1 "Vector observation").
         The tensors are views of one buffer per ``(k_agents, k_segments)`` that the next call with those counts reuses."""
         K, S = int(k_agents), int(k_segments)
-        cache = self.__dict__.setdefault("_obs_out", {})
-        obs = cache.get((K, S))
+        obs = self._obs_out.get((K, S))
         if obs is None:
-            if not (0 <= K <= 127 and 0 <= S <= 256):
-                raise ValueError("k_agents must be in 0..127 and k_segments in 0..256")
-            flat = torch.empty((self.N, vector_obs_width(K, S)), dtype=torch.float32, device=self.device)
-            a0 = len(EGO_FIELDS) + len(GOAL_FIELDS)
-            s0 = a0 + len(AGENT_FIELDS) * K
-            obs = cache[(K, S)] = VectorObservation(
-                flat=flat, ego=flat[:, :len(EGO_FIELDS)], goal=flat[:, len(EGO_FIELDS):a0],
-                agents=flat[:, a0:s0].view(self.N, K, len(AGENT_FIELDS)),
-                segments=flat[:, s0:].view(self.N, S, len(SEGMENT_FIELDS)),
-                agent_index=torch.empty((self.N, K), dtype=torch.int16, device=self.device),
-                segment_index=torch.empty((self.N, S), dtype=torch.int16, device=self.device))
+            obs = self._obs_out[(K, S)] = self._obs_buffer(VectorObservation, (self.N,), K, S)
         cfg = _lib.ObsConfigC(K, S, float(agent_range), float(segment_range))
         _lib.check(self.lib.t2d_observe(self._ctx, C.byref(cfg), _ptr(obs.flat), _ptr(obs.agent_index),
                                         _ptr(obs.segment_index), self._stream()))
         return obs
 
+    def _obs_buffer(self, cls, lead, K: int, S: int):
+        """A ``VectorObservation`` / ``AgentObservation`` over one new buffer, leading shape ``lead`` = (N,) or (N, Q)."""
+        if not (0 <= K <= 127 and 0 <= S <= 256):
+            raise ValueError("k_agents must be in 0..127 and k_segments in 0..256")
+        flat = torch.empty(lead + (vector_obs_width(K, S),), dtype=torch.float32, device=self.device)
+        a0 = len(EGO_FIELDS) + len(GOAL_FIELDS)
+        s0 = a0 + len(AGENT_FIELDS) * K
+        i16 = dict(dtype=torch.int16, device=self.device)
+        return cls(flat=flat, ego=flat[..., :len(EGO_FIELDS)], goal=flat[..., len(EGO_FIELDS):a0],
+                   agents=flat[..., a0:s0].view(lead + (K, len(AGENT_FIELDS))),
+                   segments=flat[..., s0:].view(lead + (S, len(SEGMENT_FIELDS))),
+                   agent_index=torch.empty(lead + (K,), **i16), segment_index=torch.empty(lead + (S,), **i16))
+
     def _agent_rows(self, observers, goals) -> int:
-        """Q of an observer list (M without one), after checking ``observers`` / ``goals``: they reach the kernels as raw
-        pointers, and a host tensor, a wrong dtype or shape would be read out of bounds."""
+        """Q of an observer list (M without one), after checking ``observers`` / ``goals``."""
         if observers is None:
             Q = self.M
         else:
-            if (not torch.is_tensor(observers) or observers.device != self.device or observers.dtype != torch.int16
-                    or observers.dim() != 2 or observers.shape[0] != self.N or not observers.is_contiguous()):
+            if not (torch.is_tensor(observers) and observers.dim() == 2):
                 raise ValueError(f"observers must be a contiguous int16 [{self.N}, Q] tensor on {self.device}")
             Q = int(observers.shape[1])
+            self._device_tensor("observers", observers, torch.int16, (self.N, Q))
         if not 1 <= Q <= 128:
             raise ValueError("the number of observers per scenario must be in 1..128")
         if goals is not None:
-            if (not torch.is_tensor(goals) or goals.device != self.device or goals.dtype != torch.float32
-                    or tuple(goals.shape) != (self.N, Q, 5) or not goals.is_contiguous()):
-                raise ValueError(f"goals must be a contiguous fp32 [{self.N}, {Q}, 5] tensor on {self.device}")
+            self._device_tensor("goals", goals, torch.float32, (self.N, Q, 5))
         return Q
 
     def observe_agents(self, k_agents: int = 16, k_segments: int = 32, agent_range: float = 50.0,
@@ -896,20 +898,9 @@ class BatchedWorld:
         with those counts reuses."""
         K, S = int(k_agents), int(k_segments)
         Q = self._agent_rows(observers, goals)
-        cache = self.__dict__.setdefault("_agent_obs_out", {})
-        obs = cache.get((K, S, Q))
+        obs = self._agent_obs_out.get((K, S, Q))
         if obs is None:
-            if not (0 <= K <= 127 and 0 <= S <= 256):
-                raise ValueError("k_agents must be in 0..127 and k_segments in 0..256")
-            flat = torch.empty((self.N, Q, vector_obs_width(K, S)), dtype=torch.float32, device=self.device)
-            a0 = len(EGO_FIELDS) + len(GOAL_FIELDS)
-            s0 = a0 + len(AGENT_FIELDS) * K
-            obs = cache[(K, S, Q)] = AgentObservation(
-                flat=flat, ego=flat[..., :len(EGO_FIELDS)], goal=flat[..., len(EGO_FIELDS):a0],
-                agents=flat[..., a0:s0].view(self.N, Q, K, len(AGENT_FIELDS)),
-                segments=flat[..., s0:].view(self.N, Q, S, len(SEGMENT_FIELDS)),
-                agent_index=torch.empty((self.N, Q, K), dtype=torch.int16, device=self.device),
-                segment_index=torch.empty((self.N, Q, S), dtype=torch.int16, device=self.device), observers=None)
+            obs = self._agent_obs_out[(K, S, Q)] = self._obs_buffer(AgentObservation, (self.N, Q), K, S)
         obs.observers = observers
         cfg = _lib.ObsConfigC(K, S, float(agent_range), float(segment_range))
         _lib.check(self.lib.t2d_observe_agents(self._ctx, C.byref(cfg), _ptr(observers), Q, _ptr(goals), _ptr(obs.flat),
@@ -924,19 +915,17 @@ class BatchedWorld:
         n_pool = px.shape[0]
         cols = ["x", "y", "heading", "speed"] + [k for k in ("vx", "vy", "omega_wf", "omega_wr") if pool.get(k) is not None]
         for k in cols:
-            t = pool[k]
-            if t.device != self.device or t.dtype != torch.float32 or tuple(t.shape) != (n_pool, self.M) or not t.is_contiguous():
-                raise ValueError(f"pool[{k!r}] must be a contiguous fp32 [{n_pool}, {self.M}] tensor on {self.device}")
+            self._device_tensor(f"pool[{k!r}]", pool[k], torch.float32, (n_pool, self.M))
         if (pool.get("vx") is None) != (pool.get("vy") is None):
             raise ValueError("give both pool['vx'] and pool['vy'], or neither")
-        # mask / pool_index reach the kernel as raw pointers: a host tensor or a wrong length would be an illegal address
+        # mask / pool_index reach the kernel as raw pointers: a wrong length would be an illegal address
         if not torch.is_tensor(mask) or mask.numel() != self.N:
             raise ValueError(f"mask must be a tensor of {self.N} scenarios")
-        mask = mask.to(device=self.device, dtype=torch.uint8).contiguous()
+        mask = self._to_device(mask, torch.uint8, (self.N,))
         if pool_index is not None:
             if not torch.is_tensor(pool_index) or pool_index.numel() != self.N:
                 raise ValueError(f"pool_index must be a tensor of {self.N} scenarios")
-            pool_index = pool_index.to(device=self.device, dtype=torch.int32).contiguous()
+            pool_index = self._to_device(pool_index, torch.int32, (self.N,))
         if pool_index is None and n_pool < self.N:
             raise ValueError("without pool_index the pool needs one row per scenario")
         if self.omega_front is not None:
