@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench_tick_phases.py - where one tick's time goes, phase by phase, at C2 (4096 x 64, kinematics, grid map).
 
-    python bench_tick_phases.py [--ticks K] [--warmup W] [--lib PATH]
+    python bench_tick_phases.py [--ticks K] [--warmup W] [--lib PATH] [--cohorts C]
 
 Compiles `t2d_kernels.cu` with -DT2D_TICK_TIMELINE into a temporary directory (or takes a library built that way from
 --lib) and loads it in place of the in-tree build.  In that build lane 0 of every warp of the tick records %globaltimer
@@ -11,10 +11,12 @@ instance, the other is kept on the generic instance (T2D_TICK_GENERIC=1 at its c
 each tick on its own with the L2 flushed before it, and after each tick the timeline is read back.
 
 Printed, one JSON line per instance: per phase the median and p99 over all warps and ticks of its duration in SM
-cycles and in ns (cycles converted at the clock measured over the warps' lifetimes), the spread of the warps' entry
-and post-wait times relative to the first warp of the tick, the median warp lifetime and the median tick span (first
-entry to last exit).  The timeline build is a measurement build: the recording itself costs time, so its spans are
-longer than the shipped tick's.  Nothing is written to the tree.
+cycles and in ns (cycles converted at the clock measured over the warps' lifetimes), the spread of the warps' entry,
+post-wait and loads-consumed times relative to the first warp of the tick, the median warp lifetime and the median
+tick span (first entry to last exit).  Then the same once per cohort: the warps of every CTA split into C equal groups
+by their index in the CTA (default 2: the C2-shaped instance's cohorts A and B, which issue their first loads one after
+the other), with times still taken from the tick's first entry.  The timeline build is a measurement build: the
+recording itself costs time, so its spans are longer than the shipped tick's.  Nothing is written to the tree.
 """
 
 from __future__ import annotations
@@ -35,6 +37,7 @@ if ROOT not in sys.path:
 
 POINTS = ["entry", "wait", "loads", "physics", "sort", "sweep", "drain", "static", "exit"]
 TL_MAX_WARPS = 4096   # t2d_kernels.cu: TL_MAX_WARPS, TL_POINTS
+WPC = 8               # warps per CTA of the tick at C2 (2048 warp tiles: pick_wpc's largest CTA); a warp's slot is its tile
 
 
 def build_timeline_lib(out_dir):
@@ -47,19 +50,24 @@ def build_timeline_lib(out_dir):
     return out
 
 
-def summarise(records):
-    """records: list of [warps, points, 2] arrays (globaltimer ns, clock64) of one tick each."""
-    durs, starts, waits, life_ns, spans = [], [], [], [], []
+def summarise(records, sel=None):
+    """records: list of [warps, points, 2] arrays (globaltimer ns, clock64) of one tick each; sel: a boolean mask over
+    the warp slots to summarise (None: all).  Times relative to the tick's start are taken from all its warps."""
+    durs, starts, waits, loads, life_ns, spans = [], [], [], [], [], []
     cyc_total = ns_total = 0
     for r in records:
         ok = (r[:, :, 0] != 0).all(axis=1)
+        t0 = r[ok, 0, 0].astype(np.int64).min()
+        if sel is not None:
+            ok &= sel
         g = r[ok, :, 0].astype(np.int64)
         c = r[ok, :, 1].astype(np.int64)
         durs.append(np.diff(c, axis=1))
-        starts.append(g[:, 0] - g[:, 0].min())
-        waits.append(g[:, 1] - g[:, 0].min())
+        starts.append(g[:, 0] - t0)
+        waits.append(g[:, 1] - t0)
+        loads.append(g[:, 2] - t0)
         life_ns.append(g[:, -1] - g[:, 0])
-        spans.append(int(g[:, -1].max() - g[:, 0].min()))
+        spans.append(int(g[:, -1].max() - t0))
         cyc_total += int((c[:, -1] - c[:, 0]).sum())
         ns_total += int((g[:, -1] - g[:, 0]).sum())
     d = np.concatenate(durs)
@@ -70,11 +78,12 @@ def summarise(records):
         phases[f"{POINTS[k]}->{POINTS[k + 1]}"] = {
             "median_cycles": float(np.median(col)), "p99_cycles": float(np.percentile(col, 99)),
             "median_ns": float(np.median(col) / ghz), "p99_ns": float(np.percentile(col, 99) / ghz)}
-    s, w = np.concatenate(starts), np.concatenate(waits)
+    dist = lambda a: {"median": float(np.median(a)), "p99": float(np.percentile(a, 99)), "max": float(a.max())}
     return {"warps_per_tick": int(d.shape[0] // len(records)), "ticks": len(records), "sm_clock_ghz": round(ghz, 4),
             "phases": phases,
-            "entry_spread_ns": {"median": float(np.median(s)), "p99": float(np.percentile(s, 99)), "max": float(s.max())},
-            "wait_done_ns": {"median": float(np.median(w)), "p99": float(np.percentile(w, 99)), "max": float(w.max())},
+            "entry_spread_ns": dist(np.concatenate(starts)),
+            "wait_done_ns": dist(np.concatenate(waits)),
+            "loads_done_ns": dist(np.concatenate(loads)),
             "warp_life_ns_median": float(np.median(np.concatenate(life_ns))),
             "tick_span_ns_median": float(np.median(spans))}
 
@@ -84,6 +93,7 @@ def main():
     ap.add_argument("--ticks", type=int, default=50, help="timed ticks per instance")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--lib", default=None, help="a library built with -DT2D_TICK_TIMELINE (default: build one in a temp dir)")
+    ap.add_argument("--cohorts", type=int, default=2, help="also summarise the warps of each CTA in this many equal groups")
     args = ap.parse_args()
 
     tmp = tempfile.mkdtemp(prefix="t2d_timeline_")
@@ -142,8 +152,13 @@ def main():
     except Exception:
         smi = None
     print(json.dumps({"gpu": props.name, "nvidia_smi": smi, "scene": scene.name, "N": n, "M": m}), flush=True)
+    slot = np.arange(TL_MAX_WARPS) % WPC
     for name in worlds:
         print(json.dumps({"instance": name, **summarise(records[name])}), flush=True)
+        for k in range(args.cohorts):
+            sel = slot * args.cohorts // WPC == k
+            print(json.dumps({"instance": name, "cohort": k, "warps": f"{k * WPC // args.cohorts}-{(k + 1) * WPC // args.cohorts - 1}",
+                              **summarise(records[name], sel)}), flush=True)
     for w in worlds.values():
         w.close()
 

@@ -594,6 +594,20 @@ __device__ __noinline__ unsigned ego_goal_events(const Args& A, long long n, flo
 // launches it exactly when a tick has this shape and the generic instance otherwise.
 constexpr int FIX_M = 64, FIX_G = 16, FIX_G_SHIFT = 4, FIX_MP_SHIFT = 6;
 
+// Load cohorts of the FIXED instance.  Its tick is one wave, so every warp issues its loads within a fraction of a
+// microsecond of the others and then waits for the whole transfer, and the SMs have nothing to issue meanwhile.  The
+// first half of every CTA's warps (cohort A) issue their first tile's loads and then arrive on this named barrier; the
+// second half (cohort B) wait on it before issuing theirs, so their requests queue behind A's and A runs its physics
+// while B's bytes stream in.  Only A prefetches into L2 before griddepcontrol.wait, for the same reason.  The barrier
+// counts every thread of the CTA, so each thread must reach it exactly once (see the tile loop).
+constexpr int COHORT_BAR = 1;   // (0 is __syncthreads')
+__device__ __forceinline__ void cohort_arrive(int threads) {
+  asm volatile("barrier.arrive %0, %1;" ::"n"(COHORT_BAR), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void cohort_wait(int threads) {
+  asm volatile("barrier.sync %0, %1;" ::"n"(COHORT_BAR), "r"(threads) : "memory");
+}
+
 // L2 prefetch of the lines a lane's PPL participants will load (state, action, type ids).
 template <bool FIXED>
 __device__ __forceinline__ void prefetch_tile_l2(const StepArgs& A, long long i) {
@@ -688,10 +702,12 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
   // exchange object is alive in the process (T2D_PREFETCH=0 / 1 overrides).
   // a launch-shape parameter, or the constant it is in the FIXED instance (read where it is used, as before)
 #define K1_SHAPE(field, fixed_value) (FIXED ? (fixed_value) : A.field)
+  const bool cohorts = FIXED && wpc > 1;                 // warps [0, wpc / 2) are cohort A, the rest cohort B
+  const bool cohort_b = cohorts && warp >= (wpc >> 1);
   {
     const long long n_ = ((long long)blockIdx.x * wpc + warp) * (32 >> K1_SHAPE(g_shift, FIX_G_SHIFT)) + (lane >> K1_SHAPE(g_shift, FIX_G_SHIFT));
     const int m_ = (lane & (K1_SHAPE(G, FIX_G) - 1)) * PPL;
-    if (A.prefetch && n_ < A.N && m_ < K1_SHAPE(M, FIX_M)) prefetch_tile_l2<FIXED>(A, n_ * K1_SHAPE(M, FIX_M) + m_);   // (inside the arrays: a hint, but no stray addresses)
+    if (!cohort_b && A.prefetch && n_ < A.N && m_ < K1_SHAPE(M, FIX_M)) prefetch_tile_l2<FIXED>(A, n_ * K1_SHAPE(M, FIX_M) + m_);   // (inside the arrays: a hint, but no stray addresses)
   }
   // ... and wait here, before the first access to the state the previous tick wrote, until that grid has
   // completed and flushed (no-op when the kernel was not launched as a programmatic dependent).
@@ -715,7 +731,13 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
   const int Mh = M >> 1;                // partner offsets 1..Mh cover every unordered pair
 
   const int n_tiles = A.n_tiles;
-  for (int tile = (int)blockIdx.x * wpc + warp; tile < n_tiles; tile += (int)gridDim.x * wpc) {
+  const int tile0 = (int)blockIdx.x * wpc + warp;
+  // The cohort barrier, once per thread: B waits here, before its first tile; A arrives right after issuing its first
+  // tile's loads, or here when it has no tile (a partial last CTA, where B has none either).  Later tiles of a
+  // persistent launch do not touch it.
+  if (cohort_b) cohort_wait(wpc * 32);
+  else if (cohorts && tile0 >= n_tiles) cohort_arrive(wpc * 32);
+  for (int tile = tile0; tile < n_tiles; tile += (int)gridDim.x * wpc) {
     const long long n = (long long)tile * spw + sub;
     const bool scn_ok = n < A.N;
     int nvalid = scn_ok ? (FIXED ? PPL : min(PPL, M - m0)) : 0;
@@ -772,6 +794,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         }
       }
     }
+    if (cohorts && !cohort_b && tile == tile0) cohort_arrive(wpc * 32);   // issued, not landed: B's requests queue behind
     {   // several tiles per warp (persistent CTAs): the next tile's lines start their way to L2 now
       const long long n_next = n + (long long)gridDim.x * wpc * spw;
       if (A.prefetch && n_next < A.N && m0 < M) prefetch_tile_l2<FIXED>(A, n_next * M + m0);
