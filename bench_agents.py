@@ -33,35 +33,10 @@ from __future__ import annotations
 
 import argparse
 import json
-import time
 
 import numpy as np
 
-PEAK_BYTES_PER_S = 3.35e12
-
-
-def _gpu_info():
-    import subprocess
-
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = (v.strip() for v in out.split(","))
-        return name, power
-    except Exception:
-        import torch
-
-        return torch.cuda.get_device_name(0), "unknown"
-
-
-def _scene(name):
-    from tactics2d_b200 import synthetic
-    from tactics2d_b200.map import load_collidable_segments
-
-    if name == "c2":
-        return synthetic.config2(4096, 64, seed=1)
-    seg, b = load_collidable_segments("inD_1")
-    return synthetic.config4(16384, 32, seed=4, segments=seg, bounds=b)
+from benchlib import PEAK_BYTES_PER_S, alternate, gpu_info, require_cuda, scene, time_graph
 
 
 def _goals(s, device):
@@ -83,13 +58,13 @@ def k10_bytes(n, m, q, observers=False, goals=True):
     return n * q * (row_read + row_write) + n * m * (1 + 1) + n * (4 + 1)   # + flag / TrafficStatus per slot, steps / done
 
 
-def time_k10(name, seconds, reps=20):
+def time_k10(name, seconds):
     import ctypes as C
 
     import torch
     from tactics2d_b200 import BatchedWorld
 
-    s = _scene(name)
+    s = scene(name)
     n, m = s.shape
     w = BatchedWorld(n, m, s.table)
     w.set_map(s.segments, s.bounds)
@@ -103,66 +78,39 @@ def time_k10(name, seconds, reps=20):
     def launch():
         w.lib.t2d_agents_epilogue(w._ctx, p(zero_flags), *args, 1, w._stream())
 
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        for _ in range(3):
-            launch()
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(reps):
-            launch()
-    for _ in range(5):
-        g.replay()
-    torch.cuda.synchronize()
+    us, _ = time_graph(launch, seconds, per_graph=20)
     assert int((a["status"] == 1).sum()) == int((w.type_id < len(w.type_table)).sum()), "a row settled"
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    calls, ms = 0, 0.0
-    t_end = time.perf_counter() + seconds
-    while time.perf_counter() < t_end:
-        e0.record()
-        for _ in range(10):
-            g.replay()
-        e1.record()
-        e1.synchronize()
-        ms += e0.elapsed_time(e1)
-        calls += 10 * reps
-    us = ms * 1e3 / calls
     b = k10_bytes(n, m, m)
     w.close()
     return dict(us_per_call=round(us, 3), bytes=b, hbm_bound_us=round(b / PEAK_BYTES_PER_S * 1e6, 3),
                 share_of_hbm_peak=round(b / PEAK_BYTES_PER_S * 1e6 / us, 3), n=n, m=m, q=m)
 
 
-def time_env(name, rounds, steps):
-    import torch
+def _envs(s, **variants):
+    """{label: a reset ``BatchedTrafficEnv`` with every slot observing (K = 16, S = 32), the goals of ``_goals`` and the
+    keyword arguments of ``variants[label]``}."""
     from tactics2d_b200.envs import BatchedTrafficEnv
 
-    s = _scene(name)
-    n, m = s.shape
     envs = {}
-    for rewards in (False, True):
+    for label, kw in variants.items():
         cfg = dict(k_agents=16, k_segments=32, goals=_goals(s, "cuda:0"))
-        envs[rewards] = BatchedTrafficEnv(s, max_step=200, observation="agents", vector_obs=cfg, agent_rewards=rewards)
-        envs[rewards].reset(seed=0)
+        envs[label] = BatchedTrafficEnv(s, max_step=200, observation="agents", vector_obs=cfg, **kw)
+        envs[label].reset(seed=0)
+    return envs
+
+
+def time_env(name, rounds, steps):
+    import torch
+
+    s = scene(name)
+    n, m = s.shape
+    envs = _envs(s, ego_only=dict(agent_rewards=False), agent_rewards=dict(agent_rewards=True))
     act = torch.full((n, 2), 0.05, device="cuda:0")
-    for env in envs.values():   # warm-up
-        for _ in range(3):
-            env.step(act)
-    torch.cuda.synchronize()
-    times = {False: [], True: []}
-    for _ in range(rounds):
-        for rewards, env in envs.items():
-            t0 = time.perf_counter()
-            for _ in range(steps):
-                env.step(act)
-            torch.cuda.synchronize()
-            times[rewards].append((time.perf_counter() - t0) * 1e6 / steps)
+    times = alternate({k: (lambda env=env: env.step(act)) for k, env in envs.items()}, rounds, steps)
     for env in envs.values():
         env.close()
-    return dict(us_per_step_ego_only=[round(v, 1) for v in times[False]],
-                us_per_step_agent_rewards=[round(v, 1) for v in times[True]], n=n, m=m, q=m)
+    return dict(us_per_step_ego_only=[round(v, 1) for v in times["ego_only"]],
+                us_per_step_agent_rewards=[round(v, 1) for v in times["agent_rewards"]], n=n, m=m, q=m)
 
 
 def k11_bytes(n, m, q, observers):
@@ -179,43 +127,18 @@ def _duplicate_list(n, m, seed=0):
     return obs
 
 
-def time_k11(name, seconds, with_list, reps=20):
+def time_k11(name, seconds, with_list):
     import torch
     from tactics2d_b200 import BatchedWorld, synthetic
 
-    s = _scene(name)
+    s = scene(name)
     n, m = s.shape
     w = BatchedWorld(n, m, s.table)
     w.set_state(s.x, s.y, s.heading, s.speed, type_id=s.type_id)
     obs = torch.from_numpy(_duplicate_list(n, m)).to(w.device) if with_list else None
     rows = torch.from_numpy(synthetic.random_actions(1, (n, m))).to(w.device)
     act = torch.zeros((n, m, 2), dtype=torch.float32, device=w.device)
-
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        for _ in range(3):
-            w.scatter_agent_action(rows, act, obs)
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(reps):
-            w.scatter_agent_action(rows, act, obs)
-    for _ in range(5):
-        g.replay()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    calls, ms = 0, 0.0
-    t_end = time.perf_counter() + seconds
-    while time.perf_counter() < t_end:
-        e0.record()
-        for _ in range(10):
-            g.replay()
-        e1.record()
-        e1.synchronize()
-        ms += e0.elapsed_time(e1)
-        calls += 10 * reps
-    us = ms * 1e3 / calls
+    us, _ = time_graph(lambda: w.scatter_agent_action(rows, act, obs), seconds, per_graph=20)
     b = k11_bytes(n, m, m, with_list)
     w.close()
     return dict(us_per_call=round(us, 3), bytes_at_most=b, hbm_bound_us=round(b / PEAK_BYTES_PER_S * 1e6, 3),
@@ -226,41 +149,25 @@ def time_k11(name, seconds, with_list, reps=20):
 def time_env_actions(name, rounds, steps):
     import torch
     from tactics2d_b200 import synthetic
-    from tactics2d_b200.envs import BatchedTrafficEnv
 
-    s = _scene(name)
+    s = scene(name)
     n, m = s.shape
-    envs = {}
-    for scatter in (False, True):
-        cfg = dict(k_agents=16, k_segments=32, goals=_goals(s, "cuda:0"))
-        envs[scatter] = BatchedTrafficEnv(s, max_step=200, observation="agents", vector_obs=cfg, agent_rewards=True,
-                                          agent_actions=scatter)
-        envs[scatter].reset(seed=0)
+    envs = _envs(s, prescattered=dict(agent_rewards=True, agent_actions=False),
+                 agent_actions=dict(agent_rewards=True, agent_actions=True))
     rows = torch.from_numpy(synthetic.random_actions(2, (n, m), accel=(-0.1, 0.1), steer=(-0.05, 0.05))).cuda()
-    act = {True: rows, False: rows.clone()}   # Q = M without a list: the pre-scattered action is the same array
-    for scatter, env in envs.items():   # warm-up
-        for _ in range(3):
-            env.step(act[scatter])
-    torch.cuda.synchronize()
-    times = {False: [], True: []}
-    for _ in range(rounds):
-        for scatter, env in envs.items():
-            t0 = time.perf_counter()
-            for _ in range(steps):
-                env.step(act[scatter])
-            torch.cuda.synchronize()
-            times[scatter].append((time.perf_counter() - t0) * 1e6 / steps)
+    act = {"agent_actions": rows, "prescattered": rows.clone()}   # Q = M without a list: the pre-scattered action is the same
+    times = alternate({k: (lambda env=env, a=act[k]: env.step(a)) for k, env in envs.items()}, rounds, steps)
     for env in envs.values():
         env.close()
-    return dict(us_per_step_prescattered=[round(v, 1) for v in times[False]],
-                us_per_step_agent_actions=[round(v, 1) for v in times[True]], n=n, m=m, q=m)
+    return dict(us_per_step_prescattered=[round(v, 1) for v in times["prescattered"]],
+                us_per_step_agent_actions=[round(v, 1) for v in times["agent_actions"]], n=n, m=m, q=m)
 
 
 def time_host_step(rounds, steps):
     import torch
     from tactics2d_b200 import BatchedWorld, synthetic
 
-    s = _scene("c2")
+    s = scene("c2")
     n, m = s.shape
     worlds = {}
     for agents in (False, True):
@@ -271,17 +178,9 @@ def time_host_step(rounds, steps):
             w.set_agents()
         worlds[agents] = w
     host = torch.from_numpy(synthetic.random_actions(3, (n, m), accel=(-0.1, 0.1), steer=(-0.05, 0.05))).pin_memory()
-    run = {False: lambda: worlds[False].step_host(host), True: lambda: worlds[True].step_host_agents(host)}
-    for f in run.values():   # warm-up (and the staging allocations)
-        for _ in range(3):
-            f()
-    times = {False: [], True: []}
-    for _ in range(rounds):
-        for agents, f in run.items():
-            t0 = time.perf_counter()
-            for _ in range(steps):
-                f()
-            times[agents].append((time.perf_counter() - t0) * 1e6 / steps)
+    # the warm-up also makes the staging allocations
+    times = alternate({False: lambda: worlds[False].step_host(host), True: lambda: worlds[True].step_host_agents(host)},
+                      rounds, steps)
     for w in worlds.values():
         w.close()
     return dict(us_per_step_step_host=[round(v, 1) for v in times[False]],
@@ -297,25 +196,22 @@ def main():
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--actions", action="store_true", help="measure the per-agent action (K11) and the host step instead")
     args = ap.parse_args()
-    import torch
-
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_agents.py measures on a CUDA device; none is visible")
-    name, power = _gpu_info()
+    require_cuda("bench_agents.py")
+    name, power, _ = gpu_info()
     if args.actions:
-        for scene in args.scenes.split(","):
+        for key in args.scenes.split(","):
             for with_list in (False, True):
-                print(json.dumps(dict(what="k11", scene=scene, gpu=name, power_limit=power,
-                                      **time_k11(scene, args.seconds, with_list))), flush=True)
-            print(json.dumps(dict(what="env_step_actions", scene=scene, gpu=name, power_limit=power,
-                                  **time_env_actions(scene, args.rounds, args.steps))), flush=True)
+                print(json.dumps(dict(what="k11", scene=key, gpu=name, power_limit=power,
+                                      **time_k11(key, args.seconds, with_list))), flush=True)
+            print(json.dumps(dict(what="env_step_actions", scene=key, gpu=name, power_limit=power,
+                                  **time_env_actions(key, args.rounds, args.steps))), flush=True)
         print(json.dumps(dict(what="host_step", scene="c2", gpu=name, power_limit=power,
                               **time_host_step(args.rounds, args.steps))), flush=True)
         return
-    for scene in args.scenes.split(","):
-        print(json.dumps(dict(what="k10", scene=scene, gpu=name, power_limit=power, **time_k10(scene, args.seconds))), flush=True)
-        print(json.dumps(dict(what="env_step", scene=scene, gpu=name, power_limit=power,
-                              **time_env(scene, args.rounds, args.steps))), flush=True)
+    for key in args.scenes.split(","):
+        print(json.dumps(dict(what="k10", scene=key, gpu=name, power_limit=power, **time_k10(key, args.seconds))), flush=True)
+        print(json.dumps(dict(what="env_step", scene=key, gpu=name, power_limit=power,
+                              **time_env(key, args.rounds, args.steps))), flush=True)
 
 
 if __name__ == "__main__":

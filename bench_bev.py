@@ -12,30 +12,16 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
-import sys
 
 import numpy as np
 
-PEAK_BYTES_PER_S = 3.35e12
-
-
-def _gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = (v.strip() for v in out.split(","))
-        return name, power
-    except Exception:
-        import torch
-
-        return torch.cuda.get_device_name(0), "unknown"
+from benchlib import PEAK_BYTES_PER_S, gpu_info, require_cuda, scene, time_graph
 
 
 def _world(scene_name, n, m):
-    from tactics2d_b200 import BatchedWorld, synthetic
+    from tactics2d_b200 import BatchedWorld
 
-    s = synthetic.config2(n, m, seed=1)
+    s = scene("c2", n=n, m=m)
     w = BatchedWorld(n, m, s.table)
     x, y = s.x, s.y
     if scene_name == "c2":
@@ -55,38 +41,6 @@ def _world(scene_name, n, m):
     return w
 
 
-def _time(w, res, rgb, seconds):
-    import torch
-
-    out = w.bev(res, rgb=rgb)
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(3):
-            w.bev(res, rgb=rgb)
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        w.bev(res, rgb=rgb)
-    for _ in range(10):
-        g.replay()
-    torch.cuda.synchronize()
-    b, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    b.record()
-    for _ in range(20):
-        g.replay()
-    e.record()
-    e.synchronize()
-    per = b.elapsed_time(e) / 20 / 1e3
-    reps = max(20, int(seconds / max(per, 1e-7)))
-    b.record()
-    for _ in range(reps):
-        g.replay()
-    e.record()
-    e.synchronize()
-    return b.elapsed_time(e) / reps * 1e3, reps, out.numel()
-
-
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--n", type=int, default=4096)
@@ -94,17 +48,15 @@ def main(argv=None):
     ap.add_argument("--seconds", type=float, default=1.0)
     ap.add_argument("--scenes", default="c2,inD_1")
     a = ap.parse_args(argv)
-    import torch
-
-    if not torch.cuda.is_available():
-        sys.exit("bench_bev.py needs a CUDA device")
-    gpu, power = _gpu_info()
-    for scene in a.scenes.split(","):
-        w = _world(scene, a.n, a.m)
+    require_cuda("bench_bev.py")
+    gpu, power, _ = gpu_info()
+    for key in a.scenes.split(","):
+        w = _world(key, a.n, a.m)
         for rgb in (True, False):
-            us, reps, nbytes = _time(w, (200, 200), rgb, a.seconds)
+            nbytes = w.bev((200, 200), rgb=rgb).numel()
+            us, reps = time_graph(lambda: w.bev((200, 200), rgb=rgb), a.seconds)
             rate = nbytes / (us * 1e-6)
-            print(json.dumps(dict(metric="bev_render", scene=scene, n=a.n, m=a.m, resolution=[200, 200],
+            print(json.dumps(dict(metric="bev_render", scene=key, n=a.n, m=a.m, resolution=[200, 200],
                                   output="rgb" if rgb else "class", gpu=gpu, power_limit=power, us_per_call=round(us, 2),
                                   replays=reps, bytes_per_call=nbytes, achieved_gb_s=round(rate / 1e9, 1),
                                   share_of_store_bound=round(rate / PEAK_BYTES_PER_S, 3))), flush=True)

@@ -17,24 +17,12 @@ from __future__ import annotations
 
 import argparse
 import json
-import subprocess
 
 import numpy as np
 
-PEAK_BYTES_PER_S = 3.35e12
+from benchlib import PEAK_BYTES_PER_S, gpu_info, require_cuda
+
 N, M = 4096, 64
-
-
-def _gpu_info():
-    import torch
-
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = (v.strip() for v in out.split(","))
-        return name, power
-    except Exception:
-        return torch.cuda.get_device_name(0), "unknown"
 
 
 def _path(n_vert, k):
@@ -52,19 +40,18 @@ def _bytes(ctrl_id, kinds, is_pid):
 
 
 def main():
-    import torch
-
-    from tactics2d_b200 import BatchedWorld, synthetic
-    from tactics2d_b200.controller import AccelerationController, IDMController, PIDController, PurePursuitController
-
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=5)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_control.py needs a CUDA device")
-    name, power = _gpu_info()
+    require_cuda("bench_control.py")
+    import torch
+
+    from tactics2d_b200 import BatchedWorld, synthetic
+    from tactics2d_b200.controller import AccelerationController, IDMController, PIDController, PurePursuitController
+
+    name, power, _ = gpu_info()
     scene = synthetic.config4(N, M, seed=4)
     w = BatchedWorld(N, M, scene.table)
     w.set_state(scene.x, scene.y, scene.heading, scene.speed, vx=scene.vx, vy=scene.vy, type_id=scene.type_id)

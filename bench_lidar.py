@@ -22,36 +22,12 @@ from __future__ import annotations
 
 import argparse
 import json
-import time
 
 import numpy as np
 
-PEAK_BYTES_PER_S = 3.35e12
+from benchlib import PEAK_BYTES_PER_S, alternate, gpu_info, require_cuda, scene, time_graph
+
 SETTINGS = ((360, 20.0), (500, 12.0))
-
-
-def _gpu_info():
-    import subprocess
-
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = (v.strip() for v in out.split(","))
-        return name, power
-    except Exception:
-        import torch
-
-        return torch.cuda.get_device_name(0), "unknown"
-
-
-def _scene(name):
-    from tactics2d_b200 import synthetic
-    from tactics2d_b200.map import load_collidable_segments
-
-    if name == "c2":
-        return synthetic.config2(4096, 64, seed=1)
-    seg, b = load_collidable_segments("inD_1")
-    return synthetic.config4(16384, 32, seed=4, segments=seg, bounds=b)
 
 
 def lidar_bytes(n, m, q, n_beams, observers):
@@ -60,42 +36,12 @@ def lidar_bytes(n, m, q, n_beams, observers):
     return n * q * n_beams * 4 + (n * q * 2 if observers else 0) + n * m * (12 + 1) + n_beams * 16
 
 
-def _time_graph(launch, seconds, reps=20):
-    import torch
-
-    side = torch.cuda.Stream()
-    side.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(side):
-        for _ in range(3):
-            launch()
-    torch.cuda.current_stream().wait_stream(side)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(reps):
-            launch()
-    for _ in range(5):
-        g.replay()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    calls, ms = 0, 0.0
-    t_end = time.perf_counter() + seconds
-    while time.perf_counter() < t_end:
-        e0.record()
-        for _ in range(10):
-            g.replay()
-        e1.record()
-        e1.synchronize()
-        ms += e0.elapsed_time(e1)
-        calls += 10 * reps
-    return ms * 1e3 / calls
-
-
 def time_kernel(name, seconds, ego_only=False):
     """One dict per (setting, variant)."""
     import torch
     from tactics2d_b200 import BatchedWorld
 
-    s = _scene(name)
+    s = scene(name)
     n, m = s.shape
     w = BatchedWorld(n, m, s.table)
     w.set_map(s.segments, s.bounds)
@@ -109,7 +55,7 @@ def time_kernel(name, seconds, ego_only=False):
             variants += [("agents", 8, True, lambda: w.lidar_scan_agents(n_beams, max_range, observers=first8)),
                          ("agents", m, False, lambda: w.lidar_scan_agents(n_beams, max_range))]
         for call, q, with_list, launch in variants:
-            us = _time_graph(launch, seconds)
+            us, _ = time_graph(launch, seconds, per_graph=20)
             b = lidar_bytes(n, m, q, n_beams, with_list)
             out.append(dict(call=call, n_beams=n_beams, max_range=max_range, us_per_call=round(us, 2), bytes=b,
                             hbm_bound_us=round(b / PEAK_BYTES_PER_S * 1e6, 2),
@@ -124,7 +70,7 @@ def time_env(name, rounds, steps):
     import torch
     from tactics2d_b200.envs import BatchedTrafficEnv
 
-    s = _scene(name)
+    s = scene(name)
     n, m = s.shape
     envs = {}
     for lidar in (False, True):
@@ -132,18 +78,7 @@ def time_env(name, rounds, steps):
                                         lidar=dict(n_beams=360, max_range=20.0) if lidar else None)
         envs[lidar].reset(seed=0)
     act = torch.full((n, 2), 0.05, device="cuda:0")
-    for env in envs.values():   # warm-up
-        for _ in range(3):
-            env.step(act)
-    torch.cuda.synchronize()
-    times = {False: [], True: []}
-    for _ in range(rounds):
-        for lidar, env in envs.items():
-            t0 = time.perf_counter()
-            for _ in range(steps):
-                env.step(act)
-            torch.cuda.synchronize()
-            times[lidar].append((time.perf_counter() - t0) * 1e6 / steps)
+    times = alternate({lidar: (lambda env=env: env.step(act)) for lidar, env in envs.items()}, rounds, steps)
     for env in envs.values():
         env.close()
     return dict(us_per_step_without_lidar=[round(v, 1) for v in times[False]],
@@ -158,20 +93,17 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--ego-only", action="store_true", help="time the ego scan alone (no per-agent scan, no env step)")
     args = ap.parse_args()
-    import torch
-
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_lidar.py measures on a CUDA device; none is visible")
+    require_cuda("bench_lidar.py")
     from tactics2d_b200 import BatchedWorld
 
-    name, power = _gpu_info()
-    for scene in args.scenes.split(","):
-        for r in time_kernel(scene, args.seconds, args.ego_only):
-            print(json.dumps(dict(what="lidar", scene=scene, gpu=name, power_limit=power, **r)), flush=True)
+    name, power, _ = gpu_info()
+    for key in args.scenes.split(","):
+        for r in time_kernel(key, args.seconds, args.ego_only):
+            print(json.dumps(dict(what="lidar", scene=key, gpu=name, power_limit=power, **r)), flush=True)
     if hasattr(BatchedWorld, "lidar_scan_agents") and not args.ego_only:
-        for scene in args.scenes.split(","):
-            print(json.dumps(dict(what="env_step_lidar", scene=scene, gpu=name, power_limit=power,
-                                  **time_env(scene, args.rounds, args.steps))), flush=True)
+        for key in args.scenes.split(","):
+            print(json.dumps(dict(what="env_step_lidar", scene=key, gpu=name, power_limit=power,
+                                  **time_env(key, args.rounds, args.steps))), flush=True)
 
 
 if __name__ == "__main__":

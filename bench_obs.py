@@ -19,84 +19,29 @@ from __future__ import annotations
 
 import argparse
 import json
-import sys
-import time
 
 import numpy as np
 
-PEAK_BYTES_PER_S = 3.35e12
+from benchlib import PEAK_BYTES_PER_S, alternate, gpu_info, require_cuda, scene, time_graph
+
 K_AGENTS, K_SEGMENTS, AGENT_RANGE, SEGMENT_RANGE = 16, 32, 50.0, 30.0
+OBS_ARGS = (K_AGENTS, K_SEGMENTS, AGENT_RANGE, SEGMENT_RANGE)
 
 
-def _gpu_info():
-    import subprocess
-
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = (v.strip() for v in out.split(","))
-        return name, power
-    except Exception:
-        import torch
-
-        return torch.cuda.get_device_name(0), "unknown"
-
-
-def _world(scene):
+def _world(key):
     """(world, segments per scenario's tile, map table in use): C2 and C4 as ``bench.py`` builds them, C4's tile set through
     ``set_map_table``, and the C5 scene of ``bench.py`` at 8192 scenarios."""
-    from tactics2d_b200 import BatchedWorld, synthetic
-    from tactics2d_b200.map import load_collidable_segments
+    from tactics2d_b200 import BatchedWorld
 
-    if scene == "c2":
-        s = synthetic.config2(4096, 64, seed=1)
-    elif scene == "c4":
-        seg, b = load_collidable_segments("inD_1")
-        s = synthetic.config4(16384, 32, seed=4, segments=seg, bounds=b)
-    else:
-        seg, b = load_collidable_segments("rounD_0")
-        s = synthetic.config5(8192, 128, seed=5, segments=seg, bounds=b)
+    s = scene("c5", n=8192) if key == "round" else scene(key)
     n, m = s.shape
     w = BatchedWorld(n, m, s.table)
-    if scene == "c4":
+    if key == "c4":
         w.set_map_table([dict(segments=s.segments, bounds=s.bounds)], np.zeros(n, np.int64))
     else:
         w.set_map(s.segments, s.bounds)
     w.set_state(s.x, s.y, s.heading, s.speed, type_id=s.type_id)
-    return w, len(s.segments), scene == "c4"
-
-
-def _time_observe(w, seconds, call=None):
-    import torch
-
-    args = (K_AGENTS, K_SEGMENTS, AGENT_RANGE, SEGMENT_RANGE)
-    if call is None:
-        call = lambda: w.observe(*args)
-    st = torch.cuda.Stream()
-    st.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(st):
-        for _ in range(3):
-            call()
-    torch.cuda.current_stream().wait_stream(st)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        call()
-    for _ in range(20):
-        g.replay()
-    torch.cuda.synchronize()
-    b, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    b.record()
-    for _ in range(50):
-        g.replay()
-    e.record()
-    e.synchronize()
-    reps = max(100, int(seconds / max(b.elapsed_time(e) / 50 / 1e3, 1e-7)))
-    b.record()
-    for _ in range(reps):
-        g.replay()
-    e.record()
-    e.synchronize()
-    return b.elapsed_time(e) / reps * 1e3, reps
+    return w, len(s.segments), key == "c4"
 
 
 def _bytes(w, n_seg, map_table):
@@ -112,45 +57,24 @@ def _agents(a, gpu, power):
     """K9 with every slot and with observer 0 alone, each alternated with K8 on the same world."""
     import torch
 
-    args = (K_AGENTS, K_SEGMENTS, AGENT_RANGE, SEGMENT_RANGE)
-    for scene in a.scenes.split(","):
-        w, n_seg, map_table = _world(scene)
+    for key in a.scenes.split(","):
+        w, n_seg, map_table = _world(key)
         ego = torch.zeros((w.N, 1), dtype=torch.int16, device=w.device)
         k8_rd, k8_wr = _bytes(w, n_seg, map_table)
+        k8 = lambda: w.observe(*OBS_ARGS)
         for r in range(a.rounds):
-            for kernel, q, call in (("k9", w.M, lambda: w.observe_agents(*args)), ("k8", 1, None),
-                                    ("k9", 1, lambda: w.observe_agents(*args, observers=ego)), ("k8", 1, None)):
-                us, reps = _time_observe(w, a.seconds, call)
-                rd = k8_rd + (2 * w.N * q if call is not None and q == 1 else 0)   # the observer list
+            for kernel, q, call in (("k9", w.M, lambda: w.observe_agents(*OBS_ARGS)), ("k8", 1, k8),
+                                    ("k9", 1, lambda: w.observe_agents(*OBS_ARGS, observers=ego)), ("k8", 1, k8)):
+                us, reps = time_graph(call, a.seconds)
+                rd = k8_rd + (2 * w.N * q if kernel == "k9" and q == 1 else 0)   # the observer list
                 wr = k8_wr * q
-                print(json.dumps(dict(metric="observe_agents" if kernel == "k9" else "observe", kernel=kernel, scene=scene,
+                print(json.dumps(dict(metric="observe_agents" if kernel == "k9" else "observe", kernel=kernel, scene=key,
                                       round=r, n=w.N, m=w.M, q=q, segments_per_tile=n_seg, k_agents=K_AGENTS,
                                       k_segments=K_SEGMENTS, agent_range=AGENT_RANGE, segment_range=SEGMENT_RANGE, gpu=gpu,
                                       power_limit=power, us_per_call=round(us, 2), replays=reps, bytes_read=rd,
                                       bytes_written=wr, achieved_gb_s=round((rd + wr) / (us * 1e-6) / 1e9, 1),
                                       share_of_hbm=round((rd + wr) / (us * 1e-6) / PEAK_BYTES_PER_S, 3))), flush=True)
         w.close()
-
-
-def _time_env(observation, steps, warmup):
-    import torch
-    from tactics2d_b200 import synthetic
-    from tactics2d_b200.envs import BatchedTrafficEnv
-
-    s = synthetic.config2(4096, 64, seed=1)
-    env = BatchedTrafficEnv(s, max_step=200, observation=observation)
-    env.reset()
-    act = torch.zeros((4096, 2), device=env.world.device)
-    for _ in range(warmup):
-        env.step(act)
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    for _ in range(steps):
-        env.step(act)
-    torch.cuda.synchronize()
-    us = (time.perf_counter() - t) / steps * 1e6
-    env.close()
-    return us
 
 
 def main(argv=None):
@@ -162,33 +86,42 @@ def main(argv=None):
     ap.add_argument("--agents", action="store_true", help="time observe_agents (K9) against observe (K8) instead")
     ap.add_argument("--rounds", type=int, default=3, help="with --agents: alternating rounds per scene")
     a = ap.parse_args(argv)
-    import torch
-
-    if not torch.cuda.is_available():
-        sys.exit("bench_obs.py needs a CUDA device")
-    gpu, power = _gpu_info()
+    require_cuda("bench_obs.py")
+    gpu, power, _ = gpu_info()
     if a.agents:
         _agents(a, gpu, power)
         return
-    for scene in a.scenes.split(","):
-        w, n_seg, map_table = _world(scene)
-        us, reps = _time_observe(w, a.seconds)
+    for key in a.scenes.split(","):
+        w, n_seg, map_table = _world(key)
+        us, reps = time_graph(lambda: w.observe(*OBS_ARGS), a.seconds)
         rd, wr = _bytes(w, n_seg, map_table)
-        o = w.observe(K_AGENTS, K_SEGMENTS, AGENT_RANGE, SEGMENT_RANGE)
+        o = w.observe(*OBS_ARGS)
         rows_a = float((o.agent_index >= 0).sum(1).float().mean())
         rows_s = float((o.segment_index >= 0).sum(1).float().mean())
-        print(json.dumps(dict(metric="observe", scene=scene, n=w.N, m=w.M, segments_per_tile=n_seg, k_agents=K_AGENTS,
+        print(json.dumps(dict(metric="observe", scene=key, n=w.N, m=w.M, segments_per_tile=n_seg, k_agents=K_AGENTS,
                               k_segments=K_SEGMENTS, agent_range=AGENT_RANGE, segment_range=SEGMENT_RANGE, gpu=gpu,
                               power_limit=power, us_per_call=round(us, 2), replays=reps, bytes_read=rd, bytes_written=wr,
                               achieved_gb_s=round((rd + wr) / (us * 1e-6) / 1e9, 1),
                               share_of_hbm=round((rd + wr) / (us * 1e-6) / PEAK_BYTES_PER_S, 3),
                               mean_agent_rows=round(rows_a, 2), mean_segment_rows=round(rows_s, 2))), flush=True)
         w.close()
+    if a.env_rounds == 0:
+        return
+    import torch
+    from tactics2d_b200.envs import BatchedTrafficEnv
+
+    s = scene("c2")
+    envs = {observation: BatchedTrafficEnv(s, max_step=200, observation=observation) for observation in ("state", "vector")}
+    for env in envs.values():
+        env.reset()
+    act = torch.zeros((s.shape[0], 2), device="cuda:0")
+    times = alternate({k: (lambda env=env: env.step(act)) for k, env in envs.items()}, a.env_rounds, a.env_steps, warmup=50)
+    for env in envs.values():
+        env.close()
     for r in range(a.env_rounds):
-        for observation in ("state", "vector"):
-            us = _time_env(observation, a.env_steps, 50)
+        for observation, us in times.items():
             print(json.dumps(dict(metric="env_step", scene="c2", observation=observation, round=r, gpu=gpu, power_limit=power,
-                                  steps=a.env_steps, us_per_step=round(us, 2))), flush=True)
+                                  steps=a.env_steps, us_per_step=round(us[r], 2))), flush=True)
 
 
 if __name__ == "__main__":

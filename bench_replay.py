@@ -23,11 +23,10 @@ from __future__ import annotations
 
 import argparse
 import json
-import sys
 
 import numpy as np
 
-PEAK_BYTES_PER_S = 3.35e12
+from benchlib import PEAK_BYTES_PER_S, gpu_info, require_cuda, scene, time_graph
 
 
 def _worlds(n, m, n_tracks, seed):
@@ -35,7 +34,7 @@ def _worlds(n, m, n_tracks, seed):
     from tactics2d_b200 import BatchedWorld, synthetic
 
     ep = synthetic.replay_episodes(n, m, n_tracks, seed=seed)
-    c2 = synthetic.config2(8, 8, seed=1)   # only its map
+    c2 = scene("c2", n=8, m=8)   # only its map
     pool = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in ep.pool.items()}
     out = []
     for replay in (True, False):
@@ -55,52 +54,14 @@ def _worlds(n, m, n_tracks, seed):
     return ep, rep, plain
 
 
-def _restart(w, start):
+def _ticks(w, action, ticks, start=None):
+    """``ticks`` ticks, then every scenario back to its first step (``start`` None) or to ``start``: one graph replay."""
+    for _ in range(ticks):
+        w.step(action)
     if start is None:
         w.step_count.zero_()
     else:
         w.step_count.copy_(start)
-
-
-def _graph(w, action, ticks, start=None):
-    import torch
-
-    def body():
-        for _ in range(ticks):
-            w.step(action)
-        _restart(w, start)
-
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            body()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        body()
-    return g
-
-
-def _time(g, ticks, seconds):
-    import torch
-
-    for _ in range(10):
-        g.replay()
-    b, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    b.record()
-    for _ in range(20):
-        g.replay()
-    e.record()
-    e.synchronize()
-    per = b.elapsed_time(e) / 20 / 1e3
-    reps = max(20, int(seconds / max(per, 1e-7)))
-    b.record()
-    for _ in range(reps):
-        g.replay()
-    e.record()
-    e.synchronize()
-    return b.elapsed_time(e) / reps / ticks * 1e3, reps * ticks
 
 
 def _k7_bytes(ep, n, ticks, interval):
@@ -128,9 +89,7 @@ def _profile_k7(w, action, ticks, start=None):
 
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(4):
-            for _ in range(ticks):
-                w.step(action)
-            _restart(w, start)
+            _ticks(w, action, ticks, start)
         torch.cuda.synchronize()
     durs = [e for e in prof.key_averages() if "t2d_replay_kernel" in e.key]
     if not durs:
@@ -202,36 +161,6 @@ def _k7_schedule_bytes(ep, start, ticks, interval):
     return total / ticks, int((L > 0).sum()), switches, float(L[L > 0].mean()), int(L.max())
 
 
-def main_schedule(a):
-    import torch
-    from bench_bev import _gpu_info
-    from tactics2d_b200 import synthetic
-
-    gpu, power = _gpu_info()
-    ep, rep, plain, start = _schedule_worlds(a.n, a.m, a.seed)
-    action = torch.from_numpy(synthetic.random_actions(0, (a.n, a.m))).cuda()
-    graphs = {"replay": _graph(rep, action, a.ticks, start), "static": _graph(plain, action, a.ticks, start)}
-    us = {"replay": [], "static": []}
-    for _ in range(2):
-        for name in ("replay", "static"):
-            t, _ = _time(graphs[name], a.ticks, a.seconds)
-            us[name].append(round(t, 3))
-    k7_us, k7_launches = _profile_k7(rep, action, a.ticks, start)
-    nbytes, n_sched, switches, mean_l, max_l = _k7_schedule_bytes(ep, start.cpu().numpy().astype(np.int64), a.ticks, 100)
-    rate = None if not k7_us else nbytes / (k7_us * 1e-6)
-    print(json.dumps(dict(
-        metric="log_replay_schedule_tick", n=a.n, m=a.m, tracks=int(len(ep.log)), records=int(len(ep.log.records)),
-        scheduled_slots=n_sched, entries=int(len(ep.schedule[1])), mean_entries_per_slot=round(mean_l, 2), max_entries_per_slot=max_l,
-        dropped=int(ep.dropped.sum()), switches_per_graph=switches, gpu=gpu, power_limit=power, ticks_per_graph=a.ticks,
-        us_per_tick_replay=us["replay"], us_per_tick_static=us["static"],
-        replay_overhead_us=round(min(us["replay"]) - min(us["static"]), 3),
-        k7_us=None if k7_us is None else round(k7_us, 3), k7_profiled_launches=k7_launches,
-        k7_bytes_per_launch=int(nbytes), k7_bytes_per_scheduled_slot=round(nbytes / max(n_sched, 1), 1),
-        k7_achieved_gb_s=None if rate is None else round(rate / 1e9, 1),
-        k7_share_of_hbm_peak=None if rate is None else round(rate / PEAK_BYTES_PER_S, 3))), flush=True)
-    rep.close(); plain.close()
-
-
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--n", type=int, default=4096)
@@ -242,33 +171,39 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--schedule", action="store_true", help="time slot schedules on a highway-like recording instead")
     a = ap.parse_args(argv)
+    require_cuda("bench_replay.py")
     import torch
-    from bench_bev import _gpu_info
-
-    if not torch.cuda.is_available():
-        sys.exit("bench_replay.py needs a CUDA device")
-    if a.schedule:
-        return main_schedule(a)
-    gpu, power = _gpu_info()
-    ep, rep, plain = _worlds(a.n, a.m, a.tracks, a.seed)
     from tactics2d_b200 import synthetic
 
+    gpu, power, _ = gpu_info()
+    if a.schedule:
+        ep, rep, plain, start = _schedule_worlds(a.n, a.m, a.seed)
+    else:
+        (ep, rep, plain), start = _worlds(a.n, a.m, a.tracks, a.seed), None
     action = torch.from_numpy(synthetic.random_actions(0, (a.n, a.m))).cuda()
-    graphs = {"replay": _graph(rep, action, a.ticks), "static": _graph(plain, action, a.ticks)}
     us = {"replay": [], "static": []}
     for _ in range(2):
-        for name in ("replay", "static"):
-            t, _ = _time(graphs[name], a.ticks, a.seconds)
-            us[name].append(round(t, 3))
-    k7_us, k7_launches = _profile_k7(rep, action, a.ticks)
-    nbytes, n_bound = _k7_bytes(ep, a.n, a.ticks, 100)
+        for name, w in (("replay", rep), ("static", plain)):
+            t, _ = time_graph(lambda: _ticks(w, action, a.ticks, start), a.seconds)
+            us[name].append(round(t / a.ticks, 3))
+    k7_us, k7_launches = _profile_k7(rep, action, a.ticks, start)
+    if a.schedule:
+        nbytes, n_rows, switches, mean_l, max_l = _k7_schedule_bytes(ep, start.cpu().numpy().astype(np.int64), a.ticks, 100)
+        head = dict(metric="log_replay_schedule_tick", n=a.n, m=a.m, tracks=int(len(ep.log)), records=int(len(ep.log.records)),
+                    scheduled_slots=n_rows, entries=int(len(ep.schedule[1])), mean_entries_per_slot=round(mean_l, 2),
+                    max_entries_per_slot=max_l, dropped=int(ep.dropped.sum()), switches_per_graph=switches)
+        per_slot = "k7_bytes_per_scheduled_slot"
+    else:
+        nbytes, n_rows = _k7_bytes(ep, a.n, a.ticks, 100)
+        head = dict(metric="log_replay_tick", n=a.n, m=a.m, tracks=a.tracks, records=int(len(ep.log.records)),
+                    replayed_slots=n_rows)
+        per_slot = "k7_bytes_per_replayed_slot"
     rate = None if not k7_us else nbytes / (k7_us * 1e-6)
     print(json.dumps(dict(
-        metric="log_replay_tick", n=a.n, m=a.m, tracks=a.tracks, records=int(len(ep.log.records)), replayed_slots=n_bound,
-        gpu=gpu, power_limit=power, ticks_per_graph=a.ticks, us_per_tick_replay=us["replay"], us_per_tick_static=us["static"],
-        replay_overhead_us=round(min(us["replay"]) - min(us["static"]), 3),
+        **head, gpu=gpu, power_limit=power, ticks_per_graph=a.ticks, us_per_tick_replay=us["replay"],
+        us_per_tick_static=us["static"], replay_overhead_us=round(min(us["replay"]) - min(us["static"]), 3),
         k7_us=None if k7_us is None else round(k7_us, 3), k7_profiled_launches=k7_launches,
-        k7_bytes_per_launch=int(nbytes), k7_bytes_per_replayed_slot=round(nbytes / max(n_bound, 1), 1),
+        k7_bytes_per_launch=int(nbytes), **{per_slot: round(nbytes / max(n_rows, 1), 1)},
         k7_achieved_gb_s=None if rate is None else round(rate / 1e9, 1),
         k7_share_of_hbm_peak=None if rate is None else round(rate / PEAK_BYTES_PER_S, 3))), flush=True)
     rep.close(); plain.close()

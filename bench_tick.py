@@ -18,7 +18,6 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -28,6 +27,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 from bench import BYTES_PER_PARTICIPANT, BYTES_PER_SCENARIO, TICKS_PER_CHUNK, make_scene  # noqa: E402
+from benchlib import gpu_info  # noqa: E402
 
 
 def shuffled(scene, seed):
@@ -40,15 +40,6 @@ def shuffled(scene, seed):
     return dataclasses.replace(scene, x=take(scene.x), y=take(scene.y), heading=take(scene.heading), speed=take(scene.speed),
                                vx=take(scene.vx), vy=take(scene.vy), type_id=take(scene.type_id),
                                name=scene.name + ", slots shuffled"), perm
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else None
-    except Exception:
-        return None
 
 
 def time_scene(key, args, device):
@@ -129,7 +120,7 @@ def main():
     entry.build()
     device = torch.device("cuda", 0)
     torch.cuda.set_device(device)
-    print(json.dumps({"gpu": torch.cuda.get_device_name(device), "nvidia_smi": gpu_info(),
+    print(json.dumps({"gpu": torch.cuda.get_device_name(device), "nvidia_smi": gpu_info().nvidia_smi,
                       "lib": os.environ.get("T2D_B200_LIB", "in-tree")}), flush=True)
     for key in args.scenes.split(","):
         if key not in ("c2", "c2_shuffled", "c4", "c5"):

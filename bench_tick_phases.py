@@ -35,6 +35,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+from benchlib import gpu_info  # noqa: E402
+
 POINTS = ["entry", "wait", "loads", "physics", "sort", "sweep", "drain", "static", "exit"]
 TL_MAX_WARPS = 4096   # t2d_kernels.cu: TL_MAX_WARPS, TL_POINTS
 WPC = 8               # warps per CTA of the tick at C2 (2048 warp tiles: pick_wpc's largest CTA); a warp's slot is its tile
@@ -145,13 +147,8 @@ def main():
     if n_fixed != args.warmup + args.ticks:
         raise SystemExit(f"the C2-shaped instance ran {n_fixed} times, expected {args.warmup + args.ticks}")
 
-    props = torch.cuda.get_device_properties(device)
-    try:
-        smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception:
-        smi = None
-    print(json.dumps({"gpu": props.name, "nvidia_smi": smi, "scene": scene.name, "N": n, "M": m}), flush=True)
+    print(json.dumps({"gpu": torch.cuda.get_device_properties(device).name, "nvidia_smi": gpu_info().nvidia_smi,
+                      "scene": scene.name, "N": n, "M": m}), flush=True)
     slot = np.arange(TL_MAX_WARPS) % WPC
     for name in worlds:
         print(json.dumps({"instance": name, **summarise(records[name])}), flush=True)
