@@ -59,6 +59,10 @@
  *   t2d_scatter_agent_action
  *                        (no reference counterpart) one action per agent row, written into its slot of the action array
  *   t2d_step_host_agents (no reference counterpart) the multi-agent step for a caller whose buffers live in host memory
+ *   t2d_set_routes / t2d_bind_route_trackers
+ *                        OffRoute.reset / OffRoute.update   tactics2d/traffic/event_detection/off_route.py:24-51
+ *                        (+ a route-progress reward term, an extension)
+ *   t2d_route_observe    (no reference counterpart) the route of each observer row in its frame, with look-ahead points
  *
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types cross the ABI;
@@ -454,6 +458,49 @@ int t2d_set_controllers(t2d_ctx* ctx, const t2d_controller_params* table, int n_
  * owns vertices offsets[p] .. offsets[p + 1] - 1, at least 2).  n_paths == 0 or xy == NULL unbinds.  Rejected (the
  * previous paths stay bound): malformed offsets. */
 int t2d_set_paths(t2d_ctx* ctx, const float* xy, const int32_t* offsets, int n_paths);
+
+/* ---- route following: the OffRoute detector, route progress and the route observation --------------------------------
+ * DESIGN.md section 1 "Route following".  A route is a polyline of the t2d_set_paths table.  route_id: DEVICE int16 [N][M]
+ * owned by the caller (like tile_id; it may be rewritten between steps): the route of every slot, -1, or any id the table
+ * does not hold, for none; a route whose segments all have zero length is none too.  For a slot with a route, (x, y) its
+ * fp32 centre, the closest point is the first strict minimum of the squared distance over the route's segments of non-zero
+ * length (the projection clamped to the segment, as K5's PATH sources), d its distance, s its arc length (the lengths of
+ * the earlier segments of non-zero length summed in list order, plus t len), L the total length; fp64, one rounding per
+ * operation.
+ *   OffRoute (off_route.py:24-35, route.distance(centre) > threshold): a scored participant with a route whose status is
+ * NORMAL or COMPLETED is off route when d > threshold (status chain: time exceeded, no action, out of bound, collision,
+ * off route, completed).  t2d_env_epilogue: the ego's traffic status becomes T2D_TRAFFIC_OFF_ROUTE (the scenario status
+ * stays the tick's), the step is truncated and its reward is off_route_reward.  K10 (t2d_agents_epilogue): the row's
+ * status becomes FAILED, its slot's traffic status OFF_ROUTE, the row is truncated with reward off_route_reward and its
+ * slot retires.  t2d_step / t2d_step_host_ego leave status and done to the tick, unchanged.
+ *   Progress (an extension): a NORMAL row on its route adds fp32(progress_weight (s - s_best)) to its reward when
+ * s > s_best, then s_best = s.  s_best is an fp64 tracker per scored row (initialise to -inf: the first step only records
+ * s), reset where max_iou / min_dist are.
+ * route_id == NULL unbinds; with no routes bound (or all -1) every output of both epilogues is what it is without this
+ * call.  Rejected (the previous binding stays whole): a threshold that is negative or not finite, a progress_weight or
+ * off_route_reward that is not finite (T2D_E_INVALID).  The default off_route_reward of the Python layer is -5, the
+ * out-of-bound penalty. */
+int t2d_set_routes(t2d_ctx* ctx, const int16_t* route_id, double threshold, double progress_weight, float off_route_reward);
+/* The progress trackers, DEVICE fp64 and owned by the caller: s_best [N] for t2d_env_epilogue, agent_s_best [N][n_agent_rows]
+ * for t2d_agents_epilogue (n_agent_rows must equal the bound agents' Q when it runs, else T2D_E_STATE).  Either may be
+ * NULL: no progress term there.  They are read only while routes are bound.  Rejected: n_agent_rows outside 1..128 with
+ * an agent tracker, a tracker that is not 8-byte aligned (T2D_E_INVALID). */
+int t2d_bind_route_trackers(t2d_ctx* ctx, double* s_best, double* agent_s_best, int32_t n_agent_rows);
+
+#define T2D_TRAFFIC_OFF_ROUTE 5  /* TrafficStatus.OFF_ROUTE, status.py */
+#define T2D_ROUTE_OBS_FIELDS 5   /* has_route, lateral offset, heading error, s / L, L - s */
+#define T2D_ROUTE_MAX_POINTS 256 /* look-ahead points per row of t2d_route_observe */
+/* K12 (no reference counterpart): one fp32 row of T2D_ROUTE_OBS_FIELDS + 2 n_points per observer row, in the frame of the
+ * observer's slot (origin its centre, +x along its heading): has_route (1), the signed lateral offset u.x (c.y - y) -
+ * u.y (c.x - x) (positive when the route lies to the left), the heading error atan2(u.y, u.x) - heading wrapped to
+ * (-pi, pi], s / L, L - s, then n_points points (x, y) at arc length min(s + k spacing, L), k = 1..n_points.  observers
+ * DEVICE int16 [N][Q], Q = n_observers in 1..T2D_OBS_MAX_OBSERVERS, or NULL for slot q in row q (Q <= M).  Rows whose
+ * observer is outside [0, M), whose slot is empty or retired, or whose slot has no route are zeros.  out: DEVICE fp32
+ * [N][Q][T2D_ROUTE_OBS_FIELDS + 2 n_points].  Rejected without a launch: n_observers outside 1..128, observers == NULL
+ * with n_observers > M, n_points outside 0..T2D_ROUTE_MAX_POINTS, spacing not finite or <= 0, out == NULL
+ * (T2D_E_INVALID), state or type table not bound (T2D_E_STATE).  One launch, no allocation: capturable in a CUDA graph. */
+int t2d_route_observe(t2d_ctx* ctx, const int16_t* observers, int32_t n_observers, int n_points, float spacing, float* out,
+                      void* stream);
 
 /* Overwrites action[n][m] = (accel, steer) ((steer, accel) with T2D_CFG_STEER_FIRST) of every controlled participant from
  * the bound state, then stores |applied acceleration| of the WHOLE action buffer in last_accel (bicycles: the accel clipped

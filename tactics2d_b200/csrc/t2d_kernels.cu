@@ -13,6 +13,7 @@
 // K9  t2d_obs_agents_kernel the same observation from a list of observer slots per scenario (t2d_obs.cuh).
 // K10 t2d_agents_epilogue_kernel status, reward and retirement of every agent row of an observer list.
 // K11 t2d_agent_action_kernel    the action of every agent row of an observer list, scattered to its slot.
+// K12 t2d_route_obs_kernel       the route of every observer row in its frame, with look-ahead points.
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory.
 //
 // Work decomposition of K1: a scenario (M <= 128 participants) is owned by a group of G lanes of
@@ -1236,6 +1237,82 @@ __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
   }
 }
 
+// ---------------------------------------------------------------------------- route following
+// DESIGN.md section 1 "Route following": the polyline table (t2d_set_paths) read by K5's PATH sources, the OffRoute
+// detector and route progress of the epilogues, and K12.
+struct PathVertex { double x, y, cum, len; };   // vertex, arc length up to it, length of the segment that starts here
+
+// The closest point c of a polyline to (x, y): the first strict minimum of |p - c|^2 over the segments of non-zero
+// length, c the clamped projection, and that segment's unit tangent u.  ARC adds d2 = |p - c|^2, the arc length s of c
+// (the lengths of the earlier segments of non-zero length summed in list order, plus t len) and the total length L.
+// fp64, one rounding per operation, in this order (tests/pid_oracle.py, tests/route_oracle.py).  false: no segment.
+struct PathPoint { double cx, cy, ux, uy, d2, s, L; };
+
+template <bool ARC>
+__device__ __forceinline__ bool closest_on_path(const PathVertex* pv, int n_vert, double x, double y, PathPoint& c) {
+  double best = 0.0, acc = 0.0;
+  bool found = false;
+  for (int i = 0; i + 1 < n_vert; ++i) {
+    const double ax = pv[i].x, ay = pv[i].y;
+    const double dx = __dsub_rn(pv[i + 1].x, ax), dy = __dsub_rn(pv[i + 1].y, ay);
+    const double l2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
+    if (!(l2 > 0.0)) continue;
+    double t = __ddiv_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, ax), dx), __dmul_rn(__dsub_rn(y, ay), dy)), l2);
+    t = fmin(fmax(t, 0.0), 1.0);
+    const double qx = __dadd_rn(ax, __dmul_rn(t, dx)), qy = __dadd_rn(ay, __dmul_rn(t, dy));
+    const double ex = __dsub_rn(x, qx), ey = __dsub_rn(y, qy);
+    const double d2 = __dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey));
+    if constexpr (ARC) {
+      const double len = __dsqrt_rn(l2);
+      if (!found || d2 < best) {
+        best = d2; c.cx = qx; c.cy = qy; c.ux = __ddiv_rn(dx, len); c.uy = __ddiv_rn(dy, len);
+        c.s = __dadd_rn(acc, __dmul_rn(t, len));
+        found = true;
+      }
+      acc = __dadd_rn(acc, len);
+    } else {
+      if (!found || d2 < best) {
+        const double len = __dsqrt_rn(l2);
+        best = d2; c.cx = qx; c.cy = qy; c.ux = __ddiv_rn(dx, len); c.uy = __ddiv_rn(dy, len);
+        found = true;
+      }
+    }
+  }
+  if constexpr (ARC) { c.d2 = best; c.L = acc; }
+  return found;
+}
+
+// The bound routes (t2d_set_routes): route_id == nullptr when none are bound
+struct RouteArgs {
+  const int16_t* route_id;          // [N][M] path of every slot, -1 (or any id the table does not hold): none
+  const PathVertex* path_v;
+  const int* path_off;
+  int n_paths;
+  float off_reward;                 // the reward of an off-route step
+  double threshold, weight;         // OffRoute threshold (m), progress weight (per m)
+};
+
+// The polyline of slot i's route, or nullptr
+__device__ __forceinline__ const PathVertex* route_of(const RouteArgs& R, long long i, int& n_vert) {
+  const int rid = R.route_id[i];
+  if (rid < 0 || rid >= R.n_paths) return nullptr;
+  n_vert = R.path_off[rid + 1] - R.path_off[rid];
+  return R.path_v + R.path_off[rid];
+}
+
+enum : int { ROUTE_NONE = 0, ROUTE_ON = 1, ROUTE_OFF = 2 };
+struct RouteHit { double s; int state; };
+
+// OffRoute.update (off_route.py:24-35) for slot i at its fp32 centre: off when the distance to the route's closest point
+// exceeds the threshold; s is that point's arc length.  Out of line: both epilogues run this one compiled copy.
+__device__ __noinline__ RouteHit route_probe(const RouteArgs& R, long long i, float x, float y) {
+  int n_vert = 0;
+  const PathVertex* pv = route_of(R, i, n_vert);
+  PathPoint c;
+  if (pv == nullptr || !closest_on_path<true>(pv, n_vert, (double)x, (double)y, c)) return {0.0, ROUTE_NONE};
+  return {c.s, __dsqrt_rn(c.d2) > R.threshold ? ROUTE_OFF : ROUTE_ON};
+}
+
 // ---------------------------------------------------------------------------- env epilogue
 // What ParkingEnv.step does after check_status (envs/parking.py:240-256, _get_reward :148-190), for all N scenarios in
 // one launch: TrafficStatus per participant from the event byte (status.py:52-61), terminated / truncated
@@ -1253,18 +1330,23 @@ struct EnvArgs : WorldArgs {   // (the state after the tick: the ego's position 
   float* reward;               // [N]
   uint8_t *terminated, *truncated, *done;   // [N]
   uint8_t* traffic_status;     // [N][M]
+  RouteArgs route;
+  double* s_best;              // [N] best arc length of the episode, or nullptr: no progress term
   int max_step, reset_trackers;
 };
 
 // The reward chain of _get_reward (parking.py:148-190) for one scored participant: st its ScenarioStatus, ts its
-// TrafficStatus as check_status leaves it (only the collision detector sets it), step_count its scenario's tick count.
-// max_iou == nullptr skips the IoU term, min_dist == nullptr the progress term (target = the goal centre, (x, y) the
-// participant's position).  Out of line: the env epilogue and K10 run this one compiled copy, so that their rewards agree
-// bit for bit whatever the compiler would contract in an inlined copy.
+// TrafficStatus as check_status leaves it (only the collision and OffRoute detectors set it), step_count its scenario's
+// tick count.  max_iou == nullptr skips the IoU term, min_dist == nullptr the progress term (target = the goal centre,
+// (x, y) the participant's position), s_best == nullptr the route progress term (s the arc length on the route, weight
+// its factor; an extension).  Out of line: the env epilogue and K10 run this one compiled copy, so that their rewards
+// agree bit for bit whatever the compiler would contract in an inlined copy.
 __device__ __noinline__ float reward_chain(int st, int ts, int step_count, int max_step, float iou, float* max_iou,
-                                           const float* target, float* min_dist, float x, float y) {
+                                           const float* target, float* min_dist, float x, float y, float off_reward,
+                                           double weight, double s, double* s_best) {
   float r;
   if (ts == 3 || ts == 4) r = -5.0f;                                             // :151-152 (+ dynamic collision, an extension)
+  else if (ts == T2D_TRAFFIC_OFF_ROUTE) r = off_reward;                          // (an extension)
   else if (st == T2D_STATUS_TIME_EXCEEDED || st == T2D_STATUS_NO_ACTION) r = -1.0f;   // :153-157
   else if (st == T2D_STATUS_OUT_BOUND) r = -5.0f;                                // :158-159
   else if (st == T2D_STATUS_COMPLETED) r = 5.0f;                                 // :160-161
@@ -1283,6 +1365,13 @@ __device__ __noinline__ float reward_chain(int st, int ts, int step_count, int m
         *min_dist = d;
       }
     }
+    if (s_best != nullptr) {                                                       // route progress: weight (s - s_best)
+      const double best = *s_best;                                                 // in fp64, one rounding to fp32; the
+      if (s > best) {                                                              // first step only records s
+        if (best != -INFINITY) r += __double2float_rn(__dmul_rn(weight, __dsub_rn(s, best)));
+        *s_best = s;
+      }
+    }
   }
   return r;
 }
@@ -1297,14 +1386,24 @@ __global__ void __launch_bounds__(256) t2d_env_epilogue_kernel(const __grid_cons
     if (i - (long long)n * A.M != 0) continue;
     const int st = A.status[n];
     // check_status returns at the first detector that fires (parking.py:366-385): the ego's traffic status is only set
-    // by the collision detector, i.e. when the scenario status says FAILED
-    const int ego_ts = st == T2D_STATUS_FAILED ? ts : 1;
-    const bool term = st == T2D_STATUS_COMPLETED;                                  // :243-244
+    // by the collision detector, i.e. when the scenario status says FAILED, and by OffRoute, which ranks below collision
+    // and above completion
+    int ego_ts = st == T2D_STATUS_FAILED ? ts : 1;
+    RouteHit rh{0.0, ROUTE_NONE};
+    if (A.route.route_id != nullptr && (st == T2D_STATUS_NORMAL || st == T2D_STATUS_COMPLETED)) {
+      rh = route_probe(A.route, i, A.x[i], A.y[i]);
+      if (rh.state == ROUTE_OFF) {
+        ego_ts = T2D_TRAFFIC_OFF_ROUTE;
+        if (A.traffic_status) A.traffic_status[i] = T2D_TRAFFIC_OFF_ROUTE;
+      }
+    }
+    const bool term = st == T2D_STATUS_COMPLETED && ego_ts == 1;                   // :243-244
     const bool trunc = !term && (st != T2D_STATUS_NORMAL || ego_ts != 1);          // :245-248
     const bool scored_iou = A.iou != nullptr && A.max_iou != nullptr;
     const float r = reward_chain(st, ego_ts, A.step_count[n], A.max_step, scored_iou ? A.iou[n] : 0.0f,
                                  scored_iou ? A.max_iou + n : nullptr, A.target ? A.target + 5 * (long long)n : nullptr,
-                                 (A.target && A.min_dist) ? A.min_dist + n : nullptr, A.x[i], A.y[i]);
+                                 (A.target && A.min_dist) ? A.min_dist + n : nullptr, A.x[i], A.y[i], A.route.off_reward,
+                                 A.route.weight, rh.s, (rh.state == ROUTE_ON && A.s_best) ? A.s_best + n : nullptr);
     A.reward[n] = r;
     if (A.terminated) A.terminated[n] = term;
     if (A.truncated) A.truncated[n] = trunc;
@@ -1312,6 +1411,7 @@ __global__ void __launch_bounds__(256) t2d_env_epilogue_kernel(const __grid_cons
     if (A.reset_trackers && (term || trunc)) {   // the next episode starts fresh (ParkingEnv.reset, parking.py:276-277)
       if (A.max_iou) A.max_iou[n] = -INFINITY;
       if (A.min_dist) A.min_dist[n] = INFINITY;
+      if (A.s_best) A.s_best[n] = -INFINITY;
     }
   }
 }
@@ -1331,6 +1431,8 @@ struct AgentArgs : WorldArgs {
   uint8_t *terminated, *truncated, *status;   // [N][Q]
   uint8_t* done;                // [N]
   uint8_t* traffic_status;      // [N][M] or nullptr
+  RouteArgs route;
+  double* s_best;               // [N][Q] best arc length of the episode, or nullptr: no progress term
   int Q, max_step, reset_trackers;
 };
 
@@ -1347,6 +1449,7 @@ __global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(con
       const unsigned f = A.flags[s0 + m];
       A.traffic_status[s0 + m] = (f & T2D_F_STATIC) ? 3 : ((f & T2D_F_DYNAMIC) ? 4 : 1);
     }
+    if (A.route.route_id != nullptr) __syncwarp();   // before an off-route row overwrites its slot's code
   }
   const int cnt = A.step_count[n];
   const bool time_up = A.max_step > 0 && cnt > A.max_step;                     // parking.py:366-369
@@ -1385,11 +1488,20 @@ __global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(con
     if (f & T2D_F_OUTBOUND) st = T2D_STATUS_OUT_BOUND;
     if (ev & 2u) st = T2D_STATUS_NO_ACTION;
     if (time_up) st = T2D_STATUS_TIME_EXCEEDED;
-    const int ts = st == T2D_STATUS_FAILED ? ((f & T2D_F_STATIC) ? 3 : 4) : 1;
+    RouteHit rh{0.0, ROUTE_NONE};
+    if (A.route.route_id != nullptr && (st == T2D_STATUS_NORMAL || st == T2D_STATUS_COMPLETED)) {   // OffRoute: below
+      rh = route_probe(A.route, i, x, y);                                                            // collision, above
+      if (rh.state == ROUTE_OFF) {                                                                   // completion
+        st = T2D_STATUS_FAILED;
+        if (A.traffic_status) A.traffic_status[i] = T2D_TRAFFIC_OFF_ROUTE;
+      }
+    }
+    const int ts = st == T2D_STATUS_FAILED ? ((f & T2D_F_STATIC) ? 3 : ((f & T2D_F_DYNAMIC) ? 4 : T2D_TRAFFIC_OFF_ROUTE)) : 1;
     const bool term = st == T2D_STATUS_COMPLETED;
     const bool trunc = !term && st != T2D_STATUS_NORMAL;
     A.reward[r] = reward_chain(st, ts, cnt, A.max_step, iou, has_goal ? A.max_iou + r : nullptr, goal,
-                               has_goal ? A.min_dist + r : nullptr, x, y);
+                               has_goal ? A.min_dist + r : nullptr, x, y, A.route.off_reward, A.route.weight, rh.s,
+                               (rh.state == ROUTE_ON && A.s_best) ? A.s_best + r : nullptr);
     A.status[r] = (uint8_t)st; A.terminated[r] = term; A.truncated[r] = trunc;
     any_normal = any_normal || st == T2D_STATUS_NORMAL;
     if (st != T2D_STATUS_NORMAL) {   // retire the slot (duplicate rows store the same type)
@@ -1405,7 +1517,10 @@ __global__ void __launch_bounds__(K10_WARPS * 32) t2d_agents_epilogue_kernel(con
   for (int k = 0; k < K10_ROWS_PER_LANE; ++k) {
     const int q = lane + 32 * k;
     if (q >= A.Q) break;
-    if (A.reset_trackers && done) { A.max_iou[r0 + q] = -INFINITY; A.min_dist[r0 + q] = INFINITY; }
+    if (A.reset_trackers && done) {
+      A.max_iou[r0 + q] = -INFINITY; A.min_dist[r0 + q] = INFINITY;
+      if (A.s_best) A.s_best[r0 + q] = -INFINITY;
+    }
     if ((settle >> k) & 1u) const_cast<uint8_t*>(A.type_id)[s0 + (A.observers ? A.observers[r0 + q] : q)] = 0xff;
   }
 }
@@ -1463,6 +1578,78 @@ __global__ void __launch_bounds__(K11_WARPS * 32) t2d_agent_action_kernel(const 
 #pragma unroll
   for (int k = 0; k < K; ++k)
     if (put[k]) dst[lane + 32 * k] = val[k];
+}
+
+// ---------------------------------------------------------------------------- K12 route observation
+// DESIGN.md section 1 "Route following": row (n, q) describes the route of slot j = observers[n][q] (slot q without a
+// list) in the frame of that slot (origin its centre, +x along its heading): has_route, the signed lateral offset
+// (PATH_CROSS_TRACK's convention), the heading error to the closest segment's tangent in (-pi, pi], s / L, L - s, then P
+// look-ahead points (x, y) at arc length min(s + k spacing, L), k = 1..P.  Absent rows (observer outside [0, M), empty or
+// retired slot, no route) are zeros.  One warp per scenario; lane l takes rows l, l + 32, l + 64, l + 96.
+struct RouteObsArgs : WorldArgs {
+  RouteArgs route;              // route_id may be nullptr: every row is absent
+  const int16_t* observers;     // [N][Q] or nullptr: row q is slot q
+  float* out;                   // [N][Q][T2D_ROUTE_OBS_FIELDS + 2 P]
+  int Q, P;
+  double spacing;
+};
+
+constexpr int K12_WARPS = 8;
+
+__global__ void __launch_bounds__(K12_WARPS * 32) t2d_route_obs_kernel(const __grid_constant__ RouteObsArgs A) {
+  const int lane = threadIdx.x & 31;
+  const long long n = (long long)blockIdx.x * K12_WARPS + (threadIdx.x >> 5);
+  if (n >= A.N) return;   // whole warps
+  const int F = T2D_ROUTE_OBS_FIELDS + 2 * A.P;
+#pragma unroll 1
+  for (int q = lane; q < A.Q; q += 32) {
+    const long long r = n * A.Q + q;
+    float* o = A.out + r * F;
+    const int j = A.observers ? A.observers[r] : q;
+    const long long i = n * A.M + j;
+    int nv = 0;
+    const PathVertex* pv = nullptr;
+    PathPoint c;
+    if (A.route.route_id != nullptr && j >= 0 && j < A.M && A.type_id[i] < A.n_types) pv = route_of(A.route, i, nv);
+    if (pv == nullptr || !closest_on_path<true>(pv, nv, (double)A.x[i], (double)A.y[i], c)) {
+      for (int k = 0; k < F; ++k) o[k] = 0.0f;
+      continue;
+    }
+    const double x = A.x[i], y = A.y[i], h = A.h[i];
+    double sn, cs;
+    sincos(h, &sn, &cs);
+    const double d_h = __dsub_rn(atan2(c.uy, c.ux), h);
+    double err = atan2(sin(d_h), cos(d_h));
+    constexpr double PI_D = 3.141592653589793;
+    if (err == -PI_D) err = PI_D;   // (-pi, pi]
+    o[0] = 1.0f;
+    o[1] = (float)__dsub_rn(__dmul_rn(c.ux, __dsub_rn(c.cy, y)), __dmul_rn(c.uy, __dsub_rn(c.cx, x)));
+    o[2] = (float)err;
+    o[3] = (float)__ddiv_rn(c.s, c.L);
+    o[4] = (float)__dsub_rn(c.L, c.s);
+    int seg = 0;
+    double acc = 0.0;   // arc length at the start of segment seg
+    for (int k = 1; k <= A.P; ++k) {
+      const double sig = fmin(__dadd_rn(c.s, __dmul_rn((double)k, A.spacing)), c.L);
+      double px = pv[nv - 1].x, py = pv[nv - 1].y;
+      for (; seg + 1 < nv; ++seg) {   // the first segment of non-zero length that ends at or beyond sig
+        const double ax = pv[seg].x, ay = pv[seg].y;
+        const double dx = __dsub_rn(pv[seg + 1].x, ax), dy = __dsub_rn(pv[seg + 1].y, ay);
+        const double l2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
+        if (!(l2 > 0.0)) continue;
+        const double len = __dsqrt_rn(l2), end = __dadd_rn(acc, len);
+        if (sig <= end) {
+          const double t = __ddiv_rn(__dsub_rn(sig, acc), len);
+          px = __dadd_rn(ax, __dmul_rn(t, dx)); py = __dadd_rn(ay, __dmul_rn(t, dy));
+          break;
+        }
+        acc = end;
+      }
+      const double ex = __dsub_rn(px, x), ey = __dsub_rn(py, y);
+      o[T2D_ROUTE_OBS_FIELDS + 2 * (k - 1)] = (float)__dadd_rn(__dmul_rn(ex, cs), __dmul_rn(ey, sn));
+      o[T2D_ROUTE_OBS_FIELDS + 2 * (k - 1) + 1] = (float)__dsub_rn(__dmul_rn(ey, cs), __dmul_rn(ex, sn));
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------- K3
@@ -1896,7 +2083,6 @@ __global__ void __launch_bounds__(512) t2d_exchange_allgather_kernel(const __gri
 // One warp per scenario; lane l owns participants l, l + 32, ... .  fp64 on the fp32 state (a few dozen flops per
 // participant: the kernel is bound by its ~30 B / participant of HBM traffic).  All reads of last_accel (own and the
 // leader's, previous tick) happen before the warp barrier, all writes (this tick) after it.
-struct PathVertex { double x, y, cum, len; };   // vertex, arc length up to it, length of the segment that starts here
 
 // The leading fields of t2d_controller_params, the only ones the IDM / cruise / pure-pursuit laws read.  The row also
 // holds doubles (the PID part), so it is 8-byte aligned; read through this 4-byte-aligned view, those laws load their
@@ -2022,35 +2208,17 @@ __device__ double pid_channel(const t2d_controller_params& p, double e, double s
   return out;
 }
 
-// The lateral error of a PATH_* source (no reference counterpart): the closest point c of the polyline to (x, y) - the
-// first strict minimum of |p - c|^2 over the segments of non-zero length, c the clamped projection - and that segment's
-// unit tangent u.  PATH_CROSS_TRACK: e = u.x (c.y - y) - u.y (c.x - x), positive when the path lies to the left;
-// PATH_HEADING: target_heading = atan2(u.y, u.x).  fp64, one rounding per operation, in this order.  false: no segment.
+// The lateral error of a PATH_* source (no reference counterpart), from the closest point c and its tangent u:
+// PATH_CROSS_TRACK: e = u.x (c.y - y) - u.y (c.x - x), positive when the path lies to the left; PATH_HEADING:
+// target_heading = atan2(u.y, u.x).  false: no segment.
 __device__ bool path_lateral_error(const PathVertex* pv, int n_vert, double x, double y, double heading, bool cross,
                                    double& e) {
-  double best = 0.0, cx = 0.0, cy = 0.0, ux = 0.0, uy = 0.0;
-  bool found = false;
-  for (int i = 0; i + 1 < n_vert; ++i) {
-    const double ax = pv[i].x, ay = pv[i].y;
-    const double dx = __dsub_rn(pv[i + 1].x, ax), dy = __dsub_rn(pv[i + 1].y, ay);
-    const double l2 = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
-    if (!(l2 > 0.0)) continue;
-    double t = __ddiv_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, ax), dx), __dmul_rn(__dsub_rn(y, ay), dy)), l2);
-    t = fmin(fmax(t, 0.0), 1.0);
-    const double qx = __dadd_rn(ax, __dmul_rn(t, dx)), qy = __dadd_rn(ay, __dmul_rn(t, dy));
-    const double ex = __dsub_rn(x, qx), ey = __dsub_rn(y, qy);
-    const double d2 = __dadd_rn(__dmul_rn(ex, ex), __dmul_rn(ey, ey));
-    if (!found || d2 < best) {
-      const double len = __dsqrt_rn(l2);
-      best = d2; cx = qx; cy = qy; ux = __ddiv_rn(dx, len); uy = __ddiv_rn(dy, len);
-      found = true;
-    }
-  }
-  if (!found) return false;
+  PathPoint c;
+  if (!closest_on_path<false>(pv, n_vert, x, y, c)) return false;
   if (cross) {
-    e = __dsub_rn(__dmul_rn(ux, __dsub_rn(cy, y)), __dmul_rn(uy, __dsub_rn(cx, x)));
+    e = __dsub_rn(__dmul_rn(c.ux, __dsub_rn(c.cy, y)), __dmul_rn(c.uy, __dsub_rn(c.cx, x)));
   } else {
-    const double err = __dsub_rn(atan2(uy, ux), heading);
+    const double err = __dsub_rn(atan2(c.uy, c.ux), heading);
     e = atan2(sin(err), cos(err));
   }
   return true;
@@ -2352,6 +2520,13 @@ struct t2d_ctx {
   dev_ptr<PathVertex> d_path_v;
   dev_ptr<int> d_path_off;
   int n_paths = 0;
+  // routes (t2d_set_routes / t2d_bind_route_trackers); route_id == nullptr: none bound
+  const int16_t* route_id = nullptr;
+  double route_threshold = 0.0, route_weight = 0.0;
+  float route_off_reward = 0.0f;
+  double* route_s_best = nullptr;        // [N] or nullptr
+  double* route_agent_s_best = nullptr;  // [N][route_agent_rows] or nullptr
+  int route_agent_rows = 0;
   // host steps
   std::unique_ptr<ChunkedUpload> hs_upload;
   Mirror hs_out;                       // [2][N] status, done (t2d_step_host and t2d_step_host_ego)
@@ -2386,6 +2561,19 @@ static int require(const t2d_ctx* c, unsigned need) {
 
 static WorldArgs world_args(const t2d_ctx* c) {
   return {c->x, c->y, c->h, c->v, c->vx, c->vy, c->type_id, c->step_count, c->d_table.get(), c->n_types, c->N, c->M};
+}
+
+static RouteArgs route_args(const t2d_ctx* c) {
+  return {c->route_id, c->d_path_v.get(), c->d_path_off.get(), c->n_paths, c->route_off_reward, c->route_threshold,
+          c->route_weight};
+}
+
+// K10 reads its progress tracker by the bound agents' rows: a tracker bound for another Q is a call-order error
+static int check_route_trackers(const t2d_ctx* c, const char* fn) {
+  if (c->route_id && c->route_agent_s_best && c->route_agent_rows != c->agent_q)
+    return fail(T2D_E_STATE, std::string(fn) + ": the agents' route tracker has another row count than the bound agents: "
+                                               "call t2d_bind_route_trackers again");
+  return T2D_OK;
 }
 
 // from scenario `first` on (t2d_set_map_table keeps tile_id only with more than one tile)
@@ -3280,6 +3468,7 @@ int t2d_env_epilogue(t2d_ctx* c, const uint8_t* flags, const uint8_t* scn_status
   A.max_iou = max_iou; A.min_dist = min_dist;
   A.reward = reward; A.terminated = terminated; A.truncated = truncated; A.done = done; A.traffic_status = traffic_status;
   A.max_step = c->cfg.max_step; A.reset_trackers = reset_trackers_on_done ? 1 : 0;
+  A.route = route_args(c); A.s_best = c->route_id ? c->route_s_best : nullptr;
   t2d_env_epilogue_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(A);
   return launched();
 }
@@ -3308,8 +3497,10 @@ int t2d_agents_epilogue(t2d_ctx* c, const uint8_t* flags, float* reward, uint8_t
   if (c->agent_q == 0) return fail(T2D_E_STATE, "t2d_agents_epilogue: no agents bound: call t2d_set_agents first");
   if (!flags || !reward || !terminated || !truncated || !agent_status || !iou || !done || !max_iou || !min_dist)
     return fail(T2D_E_INVALID, "t2d_agents_epilogue: NULL array");
+  if (int r = check_route_trackers(c, "t2d_agents_epilogue")) return r;
   CUDA_TRY(cudaSetDevice(c->device));
   AgentArgs A{world_args(c)};
+  A.route = route_args(c); A.s_best = c->route_id ? c->route_agent_s_best : nullptr;
   A.goal = c->agent; A.goal.iou = iou;
   A.flags = flags; A.observers = c->agent_observers; A.retired = c->agent_retired;
   A.max_iou = max_iou; A.min_dist = min_dist; A.reward = reward; A.terminated = terminated; A.truncated = truncated;
@@ -3356,6 +3547,7 @@ int t2d_step_host_agents(t2d_ctx* c, const float* agent_action_host, float* acti
   if (!aligned8(action)) return fail(T2D_E_INVALID, "t2d_step_host_agents: action must be 8-byte aligned");
   if (int r = require(c, NEED_STATE | NEED_TABLE | NEED_TICK)) return r;
   if (c->agent_q == 0) return fail(T2D_E_STATE, "t2d_step_host_agents: no agents bound: call t2d_set_agents first");
+  if (int r = check_route_trackers(c, "t2d_step_host_agents")) return r;
   if (c->d_ctab)
     if (int r = check_pid_binding(c)) return r;
   CUDA_TRY(cudaSetDevice(c->device));
@@ -3682,6 +3874,52 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   if (int r = upload(d_off, offsets, (size_t)n_paths + 1)) return r;
   c->d_path_v = std::move(d_v); c->d_path_off = std::move(d_off); c->n_paths = n_paths;
   return T2D_OK;
+}
+
+int t2d_set_routes(t2d_ctx* c, const int16_t* route_id, double threshold, double progress_weight, float off_route_reward) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (route_id) {
+    if (!(std::isfinite(threshold) && threshold >= 0.0))
+      return fail(T2D_E_INVALID, "t2d_set_routes: threshold must be finite and >= 0");
+    if (!std::isfinite(progress_weight) || !std::isfinite(off_route_reward))
+      return fail(T2D_E_INVALID, "t2d_set_routes: progress_weight and off_route_reward must be finite");
+  }
+  c->route_id = route_id;
+  c->route_threshold = route_id ? threshold : 0.0;
+  c->route_weight = route_id ? progress_weight : 0.0;
+  c->route_off_reward = route_id ? off_route_reward : 0.0f;
+  return T2D_OK;
+}
+
+int t2d_bind_route_trackers(t2d_ctx* c, double* s_best, double* agent_s_best, int32_t n_agent_rows) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (agent_s_best && (n_agent_rows < 1 || n_agent_rows > T2D_OBS_MAX_OBSERVERS))
+    return fail(T2D_E_INVALID, "t2d_bind_route_trackers: n_agent_rows must be in 1..128");
+  if (!aligned8(s_best) || !aligned8(agent_s_best))
+    return fail(T2D_E_INVALID, "t2d_bind_route_trackers: the trackers must be 8-byte aligned");
+  c->route_s_best = s_best;
+  c->route_agent_s_best = agent_s_best;
+  c->route_agent_rows = agent_s_best ? n_agent_rows : 0;
+  return T2D_OK;
+}
+
+int t2d_route_observe(t2d_ctx* c, const int16_t* observers, int32_t n_observers, int n_points, float spacing, float* out,
+                      void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (n_observers < 1 || n_observers > T2D_OBS_MAX_OBSERVERS)
+    return fail(T2D_E_INVALID, "t2d_route_observe: n_observers must be in 1..128");
+  if (!observers && n_observers > c->M)
+    return fail(T2D_E_INVALID, "t2d_route_observe: without an observer list n_observers must not exceed the slots per scenario");
+  if (n_points < 0 || n_points > T2D_ROUTE_MAX_POINTS) return fail(T2D_E_INVALID, "t2d_route_observe: n_points must be in 0..256");
+  if (!(spacing > 0.0f) || !std::isfinite(spacing)) return fail(T2D_E_INVALID, "t2d_route_observe: spacing must be finite and > 0");
+  if (!out) return fail(T2D_E_INVALID, "t2d_route_observe: out is NULL");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  CUDA_TRY(cudaSetDevice(c->device));
+  RouteObsArgs A{world_args(c)};
+  A.route = route_args(c); A.observers = observers; A.out = out; A.Q = n_observers; A.P = n_points;
+  A.spacing = (double)spacing;
+  t2d_route_obs_kernel<<<(c->N + K12_WARPS - 1) / K12_WARPS, K12_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  return launched();
 }
 
 int t2d_control(t2d_ctx* c, float* action, void* stream) {

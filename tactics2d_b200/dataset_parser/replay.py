@@ -108,10 +108,33 @@ class ReplayEpisodes:
     t0: np.ndarray
     dropped: np.ndarray
     schedule: Optional[Tuple[np.ndarray, np.ndarray]] = None
+    ego_track: Optional[np.ndarray] = None   # int64 [P]: the log index of every row's ego track (build_replay_episodes)
 
     def binding(self) -> dict:
         """The slot binding as ``BatchedWorld.set_log`` keywords: ``row_track=`` or ``schedule=``."""
         return dict(row_track=self.row_track) if self.schedule is None else dict(schedule=self.schedule)
+
+    def ego_routes(self, horizon_ms: Optional[int] = None):
+        """Routes that make every row's ego follow its own logged track: ``(paths, route_id)`` for
+        ``BatchedWorld.set_paths`` / ``set_routes`` (or ``BatchedTrafficEnv(route=dict(paths=..., route_id=...))``).  Path p
+        is the ego track's recorded (x, y) every 40 ms from ``t0[p]`` on, to its end or to ``t0[p] + horizon_ms``;
+        ``route_id`` [P, M] int16 routes slot 0 of row p along path p and no other slot.  A track with a single frame left
+        gives a path of one repeated point, which has no segment of non-zero length: no route."""
+        if self.ego_track is None:
+            raise ValueError("these episodes do not know their ego tracks: build them with build_replay_episodes")
+        log = self.log
+        off, first, period, nf = log.rec_off, log.first_ms.astype(np.int64), log.period_ms.astype(np.int64), log.n_frames
+        paths = []
+        for p, k in enumerate(self.ego_track):
+            k = int(k)
+            j0 = (int(self.t0[p]) - int(first[k])) // int(period[k])
+            j1 = int(nf[k]) if horizon_ms is None else min(int(nf[k]), j0 + int(horizon_ms) // int(period[k]) + 1)
+            xy = np.ascontiguousarray(log.records[off[k] + j0:off[k] + j1, :2], dtype=np.float32)
+            paths.append(xy if len(xy) >= 2 else np.repeat(xy, 2, 0))
+        M = self.type_id.shape[1]
+        route_id = np.full((len(paths), M), -1, np.int16)
+        route_id[:, 0] = np.arange(len(paths))
+        return paths, route_id
 
     def scene(self, segments=None, bounds=None, name: str = "replay"):
         """A :class:`tactics2d_b200.synthetic.Scene` of the P rows (one scenario per row) on the given map."""
@@ -193,9 +216,12 @@ def build_replay_episodes(log: ReplayLog, m_participants: int, t0s: Sequence[int
             if first[k] <= t0 <= last[k]:
                 tid[p, m] = type_row[k]
     t0_arr = np.asarray(t0s, np.int32)
+    ego_track = np.asarray([log.index(e) for e in ego_tracks], np.int64)
     if not reuse_slots:
-        return ReplayEpisodes(replace(log, type_row=type_row), table, pool, tid, row_track, t0_arr, dropped)
+        return ReplayEpisodes(replace(log, type_row=type_row), table, pool, tid, row_track, t0_arr, dropped,
+                              ego_track=ego_track)
     flat = [s for row in slots for s in row]
     slot_off = np.concatenate([[0], np.cumsum([len(s) for s in flat])]).astype(np.int32)
     slot_track = np.asarray([k for s in flat for k in s], np.int32)
-    return ReplayEpisodes(replace(log, type_row=type_row), table, pool, tid, None, t0_arr, dropped, (slot_off, slot_track))
+    return ReplayEpisodes(replace(log, type_row=type_row), table, pool, tid, None, t0_arr, dropped, (slot_off, slot_track),
+                          ego_track)

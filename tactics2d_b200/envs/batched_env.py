@@ -49,7 +49,8 @@ class BatchedTrafficEnv:
                  any_participant: bool = False, auto_reset: bool = True, target=None, arrival_threshold: float = 0.95,
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
-                 agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None):
+                 agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
+                 route: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -78,7 +79,15 @@ class BatchedTrafficEnv:
         ``info["lidar"]`` to ``reset`` and ``step``, the reference env's ``infos["lidar"]`` (parking.py:206-217), scanned
         after the auto-reset like the observation: fp32 ``[N, n_beams]`` from every ego (``BatchedWorld.lidar_scan``), or
         with ``observation="agents"`` ``[N, Q, n_beams]`` from every observer row (``BatchedWorld.lidar_scan_agents`` on
-        ``vector_obs["observers"]``)."""
+        ``vector_obs["observers"]``);
+        ``route``: e.g. ``dict(paths=[...], route_id=..., threshold=3.0)`` gives participants a route to follow
+        (``BatchedWorld.set_paths`` + ``set_routes``; DESIGN.md section 1 "Route following"): ``route_id`` indexes ``paths``
+        per pool row, ``[P, M]`` or ``[P]`` for the ego only (-1: none); ``threshold`` is the ``OffRoute`` distance,
+        ``progress_weight`` (0.1) and ``off_route_reward`` (-5) the reward terms; an off-route ego or agent row is
+        truncated.  The routes follow their rows like the types do (an auto-reset keeps a scenario's route; a shuffle of a
+        replay deals them out with the rows).  ``info["route"]`` is the route observation after the auto-reset
+        (``BatchedWorld.route_observe`` with ``n_points`` (8) and ``spacing`` (2.0)): ``[N, F]`` from every ego, or with
+        ``observation="agents"`` ``[N, Q, F]`` from every observer row."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -104,6 +113,15 @@ class BatchedTrafficEnv:
             unknown = set(self.lidar) - {"n_beams", "max_range"}
             if unknown:
                 raise ValueError(f"lidar: unknown keys {sorted(unknown)}")
+        self.route = None if route is None else dict(route)
+        if self.route is not None:
+            unknown = set(self.route) - {"paths", "route_id", "threshold", "progress_weight", "off_route_reward", "n_points",
+                                         "spacing"}
+            if unknown:
+                raise ValueError(f"route: unknown keys {sorted(unknown)}")
+            missing = {"paths", "route_id", "threshold"} - set(self.route)
+            if missing:
+                raise ValueError(f"route: missing keys {sorted(missing)}")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -132,6 +150,23 @@ class BatchedTrafficEnv:
         if self.agent_rewards:
             self.world.set_agents(self.vector_obs.get("observers"), self.vector_obs.get("goals"), arrival_threshold,
                                   no_action_max_step)
+        self._route_pool = None
+        if self.route is not None:
+            rt = self.route
+            rid = np.asarray(rt["route_id"].cpu() if torch.is_tensor(rt["route_id"]) else rt["route_id"]).astype(np.int64)
+            if rid.shape == (n,):
+                rid = np.concatenate([rid[:, None], np.full((n, m - 1), -1, np.int64)], 1)
+            if rid.shape != (n, m):
+                raise ValueError(f"route['route_id'] must be [{n}, {m}] or [{n}] (one row per pool row)")
+            self.world.set_paths(rt["paths"])
+            self._route_pool = torch.from_numpy(rid.astype(np.int16)).to(dev)
+            self.world.set_routes(self._route_pool.clone(), rt["threshold"], rt.get("progress_weight", 0.1),
+                                  rt.get("off_route_reward", -5.0))
+            self._route_observers = None
+            if observation == "agents":
+                obs = self.vector_obs.get("observers")
+                self._route_observers = obs if obs is not None else \
+                    torch.arange(m, dtype=torch.int16, device=dev).expand(n, m).contiguous()
         if observation == "bev":
             w, h = self.bev_resolution
             self.observation_space = {"shape": (n, h, w, 3), "dtype": "uint8", "low": 0, "high": 255}
@@ -165,7 +200,11 @@ class BatchedTrafficEnv:
         return info
 
     def _add_lidar(self, info):
-        """``info["lidar"]`` when the env has a lidar; called after the auto-reset, so that the scan sees the new episodes."""
+        """``info["lidar"]`` / ``info["route"]`` when the env has a lidar / routes; called after the auto-reset, so that
+        the scan and the route rows see the new episodes."""
+        if self.route is not None:
+            info["route"] = self.world.route_observe(self.route.get("n_points", 8), self.route.get("spacing", 2.0),
+                                                     self._route_observers)
         if self.lidar is not None:
             if self.observation == "agents":
                 info["lidar"] = self.world.lidar_scan_agents(**self.lidar, observers=self.vector_obs.get("observers"))
@@ -187,8 +226,12 @@ class BatchedTrafficEnv:
             self.world.reset_agent_trackers()
         if self.replay is not None and perm is not None:   # the rows' own types (the replayed slots' are rewritten anyway)
             self.world.type_id.copy_(self._type_id[perm.long()])
+            if self._route_pool is not None:                # ... and routes
+                self.world.route_id.copy_(self._route_pool[perm.long()])
         else:
             self.world.type_id.copy_(self._type_id)
+            if self._route_pool is not None:
+                self.world.route_id.copy_(self._route_pool)
         self.scenario_manager.reset(pool_index=perm)
         self.world.reset_env_trackers()
         status = torch.full((self.num_envs,), int(ScenarioStatus.NORMAL), dtype=torch.uint8, device=self.world.device)

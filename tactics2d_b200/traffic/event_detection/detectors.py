@@ -18,7 +18,8 @@ Semantics kept from the reference:
   the reference method as written dereferences ``.geometry`` on shapely objects and cannot run - its intent,
   ego against every other pose with ``break``, is what is implemented, for every participant as the ego);
 * ``OutBound``         ``not box.contains(pose)`` with box = (xmin, xmax, ymin, ymax) (out_bound.py:28-48);
-* ``TimeExceed``       ``cnt_step += 1; cnt_step > max_step`` (time_exceed.py:26-33).
+* ``TimeExceed``       ``cnt_step += 1; cnt_step > max_step`` (time_exceed.py:26-33);
+* ``OffRoute``         ``route.distance(centre) > threshold`` (off_route.py:24-35), the route a polyline.
 """
 
 from __future__ import annotations
@@ -252,3 +253,79 @@ class NoAction(EventBase):
         if world is not None and world._goal is not None:
             world._goal["count"].zero_()
             world._goal["last_pose"].zero_()
+
+
+def _route_points(route):
+    """[V, 2] float64 vertices of a LineString-like route (anything with ``.coords``) or a list of points."""
+    import numpy as np
+
+    try:
+        pts = np.asarray(route.coords if hasattr(route, "coords") else route, dtype=np.float64)
+    except (TypeError, ValueError):
+        pts = None
+    if pts is None or pts.ndim != 2 or pts.shape[1] != 2 or pts.shape[0] < 2:
+        raise TypeError("The route should be a LineString or a list of points.")
+    return pts
+
+
+class OffRoute(EventBase):
+    """``OffRoute`` (reference off_route.py:12-51): off when the distance from the agent's centre to the route exceeds
+    ``threshold``.  Batched: ``world.set_routes(route_id, threshold)`` binds one route per slot and the epilogues apply
+    the detector (DESIGN.md section 1 "Route following"); ``update(world)`` returns their flags.  ``reset(route)`` /
+    ``update(location)`` keep the reference's single-agent form: the location goes through a one-scenario world."""
+
+    def __init__(self, threshold):
+        self.threshold = threshold
+        self.route = None
+
+    def update(self, location):
+        """``update(world)`` -> bool [N, M]: the slots the last epilogue found off route (``agents_epilogue``'s traffic
+        status when agents are bound, else ``env_epilogue``'s, which scores the ego); ``update(location)``
+        (off_route.py:24-35, a shapely Point or an (x, y) pair) -> bool against the route of ``reset``."""
+        if _is_world(location):
+            from ..status import TrafficStatus
+
+            w = location
+            traffic = w._agents["traffic"] if w._agents is not None else (None if w._env is None else w._env["traffic"])
+            if traffic is None:
+                raise RuntimeError("no epilogue has run: call env_epilogue or agents_epilogue first")
+            return traffic == int(TrafficStatus.OFF_ROUTE)
+        if self.route is None:
+            raise ValueError("The route should be set before the event detection.")
+        import numpy as np
+
+        xy = np.asarray(location.coords[0] if hasattr(location, "coords") else location, dtype=np.float64).reshape(-1)[:2]
+        if not hasattr(self, "_probe"):
+            self._probe = _RouteProbe()
+        return self._probe.run(self.route, float(self.threshold), float(xy[0]), float(xy[1]))
+
+    def reset(self, route):
+        """``route``: a LineString-like object or a list of points (off_route.py:37-51); TypeError otherwise."""
+        self.route = _route_points(route)
+
+
+class _RouteProbe:
+    """One scenario with one static participant at the location, its route bound: the single-location call form."""
+
+    def __init__(self, device="cuda:0"):
+        self.device = device
+        self._world = None
+
+    def run(self, route, threshold, x, y):
+        import numpy as np
+
+        from ...types import MODEL_STATIC, SHAPE_NONE, TypeParams, TypeTable
+        from ...world import BatchedWorld
+
+        if self._world is None:
+            table = TypeTable([TypeParams(half_len=0.5, half_wid=0.5, model=MODEL_STATIC, shape=SHAPE_NONE)])
+            self._world = BatchedWorld(1, 1, table, device=self.device)
+        w = self._world
+        w.set_paths([route])
+        w.set_routes(np.zeros((1, 1), np.int16), threshold, 0.0, 0.0)
+        z = np.zeros((1, 1), np.float32)
+        w.set_state(np.full((1, 1), x, np.float32), np.full((1, 1), y, np.float32), z, z, type_id=np.zeros((1, 1), np.uint8))
+        w.check_events()
+        w._out.status.fill_(1)   # NORMAL: the probe never ticks
+        e = w.env_epilogue()
+        return bool(e.truncated[0].item())

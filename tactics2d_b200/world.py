@@ -70,6 +70,10 @@ EGO_FIELDS = ("valid", "speed", "v_long", "v_lat", "half_len", "half_wid", "is_d
 GOAL_FIELDS = ("valid", "ex", "ey", "cos_dh", "sin_dh", "half_len", "half_wid", "dist")
 AGENT_FIELDS = ("valid", "ex", "ey", "cos_dh", "sin_dh", "v_x", "v_y", "half_len", "half_wid", "is_disc", "dist")
 SEGMENT_FIELDS = ("valid", "ex1", "ey1", "ex2", "ey2", "ecx", "ecy", "dist", "in_ring")
+# Leading columns of a row of the route observation (``BatchedWorld.route_observe``; DESIGN.md section 1 "Route
+# following"), followed by the look-ahead points (x, y) in the observer's frame.
+ROUTE_FIELDS = ("has_route", "lateral", "heading_error", "s_frac", "remaining")
+ROUTE_MAX_POINTS = 256
 
 
 def vector_obs_width(k_agents: int, k_segments: int) -> int:
@@ -162,7 +166,8 @@ class BatchedWorld:
         self.bounds = None
         self.paths = None
         # what the setters bind (None until they are called) and the output buffers made on first use
-        self._goal = self._ctrl = self._log = self._agents = self._ego_action = None
+        self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = None
+        self._route_out = {}
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
         self._agent_lidar, self._obs_out, self._agent_obs_out = {}, {}, {}
         self._seg_style_keys = []
@@ -401,6 +406,82 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_control(self._ctx, _ptr(action), self._stream()))
         return action
 
+    # ------------------------------------------------------------------ route following
+    def set_routes(self, route_id, threshold: float = None, progress_weight: float = 0.1, off_route_reward: float = -5.0):
+        """Give slots a route to follow (``t2d_set_routes``; DESIGN.md section 1 "Route following"): ``route_id`` [N, M]
+        indexes the ``set_paths`` table (the one the controllers' ``path_id`` indexes), -1 for none; it is kept as the int16
+        device tensor :attr:`route_id`, which may be rewritten between steps.  Every scored participant with a route - the
+        ego in ``env_epilogue``, every agent row in ``agents_epilogue`` - is off route (``OffRoute``, off_route.py:24-35)
+        when its centre is more than ``threshold`` metres from the route: traffic status OFF_ROUTE, truncated, reward
+        ``off_route_reward`` (an extension; default -5, the out-of-bound penalty).  A NORMAL step on the route adds
+        ``progress_weight`` x the gain of arc length over the episode's best (default 0.1, the weight of the progress
+        towards a target; :attr:`route_s_best` / :attr:`agent_route_s_best` hold the best, fp64).  None unbinds."""
+        if route_id is None:
+            _lib.check(self.lib.t2d_set_routes(self._ctx, _ptr(None), 0.0, 0.0, 0.0))
+            _lib.check(self.lib.t2d_bind_route_trackers(self._ctx, _ptr(None), _ptr(None), 0))
+            self._routes = None
+            return
+        if threshold is None:
+            raise ValueError("set_routes needs the OffRoute threshold (metres)")
+        if (route_id.numel() if torch.is_tensor(route_id) else np.size(route_id)) != self.N * self.M:
+            raise ValueError(f"route_id must hold [{self.N}, {self.M}] path indices")
+        rid = self._to_device(route_id, torch.int16, (self.N, self.M))
+        # the library keeps the previous routes until a call succeeds: replace the tensors only then
+        _lib.check(self.lib.t2d_set_routes(self._ctx, _ptr(rid), float(threshold), float(progress_weight),
+                                           float(off_route_reward)))
+        self._routes = dict(route_id=rid, threshold=float(threshold), progress_weight=float(progress_weight),
+                            off_route_reward=float(off_route_reward),
+                            s_best=torch.full((self.N,), -float("inf"), dtype=torch.float64, device=self.device),
+                            agent_s_best=None)
+        self._bind_route_trackers()
+
+    def _bind_route_trackers(self):
+        """(Re)bind the progress trackers: [N] for the ego, [N, Q] for the bound agents' rows."""
+        r = self._routes
+        if r is None:
+            return
+        Q = 0 if self._agents is None else self._agents["Q"]
+        if Q and (r["agent_s_best"] is None or r["agent_s_best"].shape[1] != Q):
+            r["agent_s_best"] = torch.full((self.N, Q), -float("inf"), dtype=torch.float64, device=self.device)
+        if not Q:
+            r["agent_s_best"] = None
+        _lib.check(self.lib.t2d_bind_route_trackers(self._ctx, _ptr(r["s_best"]), _ptr(r["agent_s_best"]), Q))
+
+    @property
+    def route_id(self) -> Optional[torch.Tensor]:
+        """int16 [N, M] device tensor: the route of every slot (None without routes)."""
+        return None if self._routes is None else self._routes["route_id"]
+
+    @property
+    def route_s_best(self) -> Optional[torch.Tensor]:
+        """fp64 [N] device tensor: the ego's best arc length on its route this episode (-inf before its first step)."""
+        return None if self._routes is None else self._routes["s_best"]
+
+    @property
+    def agent_route_s_best(self) -> Optional[torch.Tensor]:
+        """fp64 [N, Q] device tensor: every agent row's best arc length on its slot's route (None without agents)."""
+        return None if self._routes is None else self._routes["agent_s_best"]
+
+    def route_observe(self, n_points: int = 8, spacing: float = 2.0, observers: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The route of each observer in its own frame, in one launch (``t2d_route_observe``, K12): fp32 rows of
+        :data:`ROUTE_FIELDS` (has_route, signed lateral offset - positive when the route lies to the left -, heading error
+        to the closest segment in (-pi, pi], s / L, L - s) followed by ``n_points`` look-ahead points (x, y) at arc length
+        ``min(s + k spacing, L)``, k = 1..n_points.  ``observers=None``: the ego of every scenario, ``[N, F]``; an int16
+        ``[N, Q]`` device tensor as in ``observe_agents``: ``[N, Q, F]``.  Rows without a route, or whose observer is out
+        of range, empty or retired, are zeros.  The tensor is a buffer the next call with the same shape reuses."""
+        P = int(n_points)
+        if not 0 <= P <= ROUTE_MAX_POINTS:
+            raise ValueError(f"n_points must be in 0..{ROUTE_MAX_POINTS}")
+        F = len(ROUTE_FIELDS) + 2 * P
+        Q = 1 if observers is None else self._agent_rows(observers, None)
+        key = (F, None if observers is None else Q)
+        out = self._route_out.get(key)
+        if out is None:
+            out = self._route_out[key] = torch.empty((self.N, F) if observers is None else (self.N, Q, F),
+                                                     dtype=torch.float32, device=self.device)
+        _lib.check(self.lib.t2d_route_observe(self._ctx, _ptr(observers), Q, P, float(spacing), _ptr(out), self._stream()))
+        return out
+
     # ------------------------------------------------------------------ log replay
     def set_log(self, log, t0=None, row_track=None, schedule=None):
         """Replay recorded tracks in the slots bound to them (``t2d_set_log``; DESIGN.md section 1 "Log replay").  ``log``:
@@ -603,6 +684,8 @@ class BatchedWorld:
         if self._env is not None:
             self._env["max_iou"].fill_(-float("inf"))
             self._env["min_dist"].fill_(float("inf"))
+        if self._routes is not None:
+            self._routes["s_best"].fill_(-float("inf"))
 
     # ------------------------------------------------------------------ per-agent status and reward
     def set_agents(self, observers: Optional[torch.Tensor] = None, goals: Optional[torch.Tensor] = None,
@@ -633,6 +716,9 @@ class BatchedWorld:
                                            int(no_action_max_step), _ptr(a["last_pose"]), _ptr(a["noact_count"]),
                                            _ptr(a["retired_type"])))
         self._agents = a
+        if self._routes is not None:   # the agents' progress tracker follows their rows
+            self._routes["agent_s_best"] = None
+            self._bind_route_trackers()
 
     @property
     def retired_type(self) -> Optional[torch.Tensor]:
@@ -657,6 +743,8 @@ class BatchedWorld:
         if self._agents is not None:
             self._agents["max_iou"].fill_(-float("inf"))
             self._agents["min_dist"].fill_(float("inf"))
+        if self._routes is not None and self._routes["agent_s_best"] is not None:
+            self._routes["agent_s_best"].fill_(-float("inf"))
 
     # ------------------------------------------------------------------ per-agent action
     def scatter_agent_action(self, agent_action: torch.Tensor, action: torch.Tensor,
