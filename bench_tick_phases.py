@@ -1,21 +1,26 @@
 #!/usr/bin/env python
 """bench_tick_phases.py - where one tick's time goes, phase by phase, at C2 (4096 x 64, kinematics, grid map).
 
-    python bench_tick_phases.py [--ticks K] [--warmup W] [--lib PATH] [--cohorts C]
+    python bench_tick_phases.py [--ticks K] [--warmup W] [--lib PATH] [--cohorts C] [--restore-every R]
 
 Compiles `t2d_kernels.cu` with -DT2D_TICK_TIMELINE into a temporary directory (or takes a library built that way from
 --lib) and loads it in place of the in-tree build.  In that build lane 0 of every warp of the tick records %globaltimer
 and %clock64 at nine points of its first tile: entry, after griddepcontrol.wait, loads consumed, physics done, sort
 done, sweep done, drain done, static done, exit.  Two worlds hold the same C2 scene: one runs the tick's C2-shaped
 instance, the other is kept on the generic instance (T2D_TICK_GENERIC=1 at its creation).  They tick in alternation,
-each tick on its own with the L2 flushed before it, and after each tick the timeline is read back.
+each tick on its own with the L2 flushed before it, and after each tick the timeline is read back.  Before every R-th
+tick both worlds are restored to the configured scene, as bench.py restores its replicas every 8 ticks: the C2-shaped
+instance starts its x sort from the order the previous tick left (the order hint), so after a restore that order is
+stale and most warps fall back to the sort network.
 
 Printed, one JSON line per instance: per phase the median and p99 over all warps and ticks of its duration in SM
 cycles and in ns (cycles converted at the clock measured over the warps' lifetimes), the spread of the warps' entry,
 post-wait and loads-consumed times relative to the first warp of the tick, the median warp lifetime and the median
 tick span (first entry to last exit).  Then the same once per cohort: the warps of every CTA split into C equal groups
 by their index in the CTA (default 2: the C2-shaped instance's cohorts A and B, which issue their first loads one after
-the other), with times still taken from the tick's first entry.  The timeline build is a measurement build: the
+the other), with times still taken from the tick's first entry.  Last, the C2-shaped instance once per sort path: its
+ticks where most warps kept the repaired order ("hint") and those where most fell back ("network"), by
+t2d_tick_order_fallback_count, each also per cohort.  The timeline build is a measurement build: the
 recording itself costs time, so its spans are longer than the shipped tick's.  Nothing is written to the tree.
 """
 
@@ -96,6 +101,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--lib", default=None, help="a library built with -DT2D_TICK_TIMELINE (default: build one in a temp dir)")
     ap.add_argument("--cohorts", type=int, default=2, help="also summarise the warps of each CTA in this many equal groups")
+    ap.add_argument("--restore-every", type=int, default=8, help="restore the configured scene before every R-th tick (0: never)")
     args = ap.parse_args()
 
     tmp = tempfile.mkdtemp(prefix="t2d_timeline_")
@@ -130,19 +136,29 @@ def main():
         worlds[name] = w
     flush = torch.empty(2 * torch.cuda.get_device_properties(device).L2_cache_size // 4, dtype=torch.float32, device=device)
 
+    pools = {name: {k: getattr(w, k).clone() for k in ("x", "y", "heading", "speed", "vx", "vy")} for name, w in worlds.items()}
+    ones = torch.ones(n, dtype=torch.uint8, device=device)
     records = {k: [] for k in worlds}
+    network = []   # per timed tick of the C2-shaped instance: did most of its warps fall back to the sort network?
     fixed0 = lib.t2d_tick_fixed_count()
     _lib.check(read(buf.ctypes.data, buf.nbytes, 1))
     for t in range(args.warmup + args.ticks):
+        if args.restore_every and t % args.restore_every == 0:
+            for name, w in worlds.items():
+                w.reset(ones, pools[name])
         act = torch.from_numpy(synthetic.random_actions(7000 + t, (n, m))).to(device)
         for name, w in worlds.items():
             flush.zero_()
             torch.cuda.synchronize()
+            f0 = lib.t2d_tick_order_fallback_count()
             w.step(act)
             torch.cuda.synchronize()
+            fell = lib.t2d_tick_order_fallback_count() - f0
             _lib.check(read(buf.ctypes.data, buf.nbytes, 1))
             if t >= args.warmup:
                 records[name].append(buf.copy())
+                if name == "fixed":
+                    network.append(2 * fell > (n + 1) // 2)
     n_fixed = lib.t2d_tick_fixed_count() - fixed0
     if n_fixed != args.warmup + args.ticks:
         raise SystemExit(f"the C2-shaped instance ran {n_fixed} times, expected {args.warmup + args.ticks}")
@@ -156,6 +172,15 @@ def main():
             sel = slot * args.cohorts // WPC == k
             print(json.dumps({"instance": name, "cohort": k, "warps": f"{k * WPC // args.cohorts}-{(k + 1) * WPC // args.cohorts - 1}",
                               **summarise(records[name], sel)}), flush=True)
+    for path, sel_ticks in (("hint", [not f for f in network]), ("network", network)):
+        recs = [r for r, keep in zip(records["fixed"], sel_ticks) if keep]
+        if not recs:
+            continue
+        print(json.dumps({"instance": "fixed", "sort_path": path, **summarise(recs)}), flush=True)
+        for k in range(args.cohorts):
+            sel = slot * args.cohorts // WPC == k
+            print(json.dumps({"instance": "fixed", "sort_path": path, "cohort": k,
+                              "warps": f"{k * WPC // args.cohorts}-{(k + 1) * WPC // args.cohorts - 1}", **summarise(recs, sel)}), flush=True)
     for w in worlds.values():
         w.close()
 

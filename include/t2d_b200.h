@@ -649,6 +649,17 @@ int64_t t2d_launch_count(void);
    The environment variable T2D_TICK_GENERIC=1, read at t2d_create, keeps a world on the generic instance. */
 int64_t t2d_tick_fixed_count(void);
 
+/* Number of warp tiles of that instance, on the current device, whose x sort fell back to the sort network.  The
+   instance starts every scenario's sort from the slot order it left after the scenario's previous tick (an [N][64] hint
+   the world holds, the identity at t2d_create; set_state, reset and the other kernels leave it alone) and falls back
+   when two repair passes do not sort it.  Returns -1 when the counters cannot be read. */
+int64_t t2d_tick_order_fallback_count(void);
+
+/* The order hint of t2d_tick_order_fallback_count: copies its N x 64 bytes to the HOST buffer read_to (unless NULL),
+   then overwrites it with the N x 64 bytes at the HOST buffer write_from (unless NULL).  Whatever the hint holds, every
+   tick computes the same results; only the time the sort takes depends on it.  For tests and diagnostics. */
+int t2d_order_hint(t2d_ctx* ctx, void* read_to, const void* write_from);
+
 /* Number of launches of the tick kernel (t2d_step and every call that ticks or checks events) since load that the CUDA
    runtime accepted (a fault while the kernel runs is not seen here), per instance:
    k = 0 / 1: fp64 models compiled in (the table holds a type that is neither kinematic nor static), one map tile / a map

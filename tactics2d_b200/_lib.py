@@ -115,6 +115,8 @@ SYMBOLS = {
     "t2d_set_prefetch": (C.c_int, [_P, C.c_int]),
     "t2d_launch_count": (C.c_int64, []),
     "t2d_tick_fixed_count": (C.c_int64, []),
+    "t2d_tick_order_fallback_count": (C.c_int64, []),
+    "t2d_order_hint": (C.c_int, [_P, _P, _P]),
     "t2d_tick_instance_count": (C.c_int64, [C.c_int]),
 }
 

@@ -139,6 +139,8 @@ struct StepArgs {
   float rb_max;                    // largest bounding radius in the type table (broadphase threshold)
   GoalArgs goal;                   // the ego's; goal.target == nullptr: no goal
   float *wheel_f, *wheel_r;        // [N][M] wheel angular speeds of the SingleTrackDrift participants, or nullptr
+  uint8_t* order;                  // [N][64] the world's x-order hint (FIXED instance only; see the sort)
+  unsigned long long* order_fallbacks;   // the device's fallback counters (FIXED instance only)
 };
 
 // ---------------------------------------------------------------------------- PTX helpers
@@ -609,7 +611,18 @@ __device__ __forceinline__ void cohort_wait(int threads) {
   asm volatile("barrier.sync %0, %1;" ::"n"(COHORT_BAR), "r"(threads) : "memory");
 }
 
-// L2 prefetch of the lines a lane's PPL participants will load (state, action, type ids).
+// The FIXED instance's x sort starts from the order the scenario's slots had after the previous tick (the world's
+// [N][64] order hint) and repairs it with T2D_ORDER_PASSES odd-even transposition passes; a warp whose order is still not
+// strictly ascending falls back to the sort network (see the sort).  At C2 a participant moves at most about 1.5 m per
+// tick, and two passes sort nearly every warp from the previous tick's order.  A warp that falls back counts itself in
+// StepArgs::order_fallbacks, spread over ORDER_COUNTERS 128-byte lines (by CTA) so that a tick where every warp falls
+// back does not queue its atomics on one address; t2d_tick_order_fallback_count sums them.
+#ifndef T2D_ORDER_PASSES
+#define T2D_ORDER_PASSES 2
+#endif
+constexpr int ORDER_COUNTERS = 64, ORDER_COUNTER_STRIDE = 16;   // (16 counters of 8 bytes: one per 128-byte line)
+
+// L2 prefetch of the lines a lane's PPL participants will load (state, action, type ids; order hint in FIXED).
 template <bool FIXED>
 __device__ __forceinline__ void prefetch_tile_l2(const StepArgs& A, long long i) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.x + i));
@@ -618,6 +631,7 @@ __device__ __forceinline__ void prefetch_tile_l2(const StepArgs& A, long long i)
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.v + i));
   if (FIXED || A.action) asm volatile("prefetch.global.L2 [%0];" ::"l"(A.action + 2 * i));
   asm volatile("prefetch.global.L2 [%0];" ::"l"(A.type_id + i));
+  if (FIXED) asm volatile("prefetch.global.L2 [%0];" ::"l"(A.order + i));   // (M = 64: the hint's index is the state's)
   if (!FIXED && A.needs_vel_in) {
     asm volatile("prefetch.global.L2 [%0];" ::"l"(A.vx + i));
     asm volatile("prefetch.global.L2 [%0];" ::"l"(A.vy + i));
@@ -757,6 +771,8 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       sx[i] = sy[i] = shd[i] = sv[i] = svx[i] = svy[i] = a0[i] = a1[i] = 0.0f;
       tidv[i] = T2D_TYPE_INACTIVE;
     }
+    // FIXED: the order hint of entries 4 gl .. 4 gl + 3, one byte each (the identity outside the batch)
+    uint32_t hint = 0x03020100u + 0x04040404u * (uint32_t)gl;
     if (nvalid == PPL && K1_SHAPE(vec_ok, 1)) {
       ld_vec<float, PPL>(A.x + idx0, sx);
       ld_vec<float, PPL>(A.y + idx0, sy);
@@ -764,6 +780,7 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
       ld_vec<float, PPL>(A.v + idx0, sv);
       uint8_t tb8[PPL];
       ld_vec<uint8_t, PPL>(A.type_id + idx0, tb8);
+      if constexpr (FIXED) hint = *reinterpret_cast<const uint32_t*>(A.order + idx0);   // (M = 64: the state's index)
 #pragma unroll
       for (int i = 0; i < PPL; ++i) tidv[i] = tb8[i];
       if (K1_SHAPE(do_physics, 1)) {
@@ -965,18 +982,71 @@ __global__ void __launch_bounds__(CTA_THREADS, 2) t2d_step_kernel(const __grid_c
         key[a] = desc ? hi : lo;
         key[b] = desc ? lo : hi;
       };
-      cx(0, 1, false); cx(2, 3, true);   // sorted runs of 2, alternating in direction (element bit 1)
-      for (int S = PPL; S <= MP; S <<= 1) {           // merge into sorted runs of S (the last one, S = MP, ascending)
-        const bool desc = (gl & (S >> 2)) != 0;       // element bit log2(S) = lane bit log2(S / 4)
-        for (int j = S >> 3; j > 0; j >>= 1) {        // element stride 4 j = lane stride j
-          const bool keep_max = ((gl & j) != 0) != desc;
+      // FIXED: start from the previous tick's order instead.  Entry e = 4 gl + k takes the slot s = hint byte k & 63 and
+      // its key is built as above, from the x in the pose tile; T2D_ORDER_PASSES odd-even transposition passes (an even
+      // phase: pairs (4 gl, 4 gl + 1), (4 gl + 2, 4 gl + 3); an odd phase: (4 gl + 1, 4 gl + 2) and, across lanes,
+      // (4 gl + 3, 4 gl + 4)) repair it, and the result is kept if every key is strictly below its successor in every
+      // scenario of the warp.  Otherwise the whole warp runs the network on the keys above (one decision per warp, so the
+      // network's shuffles see every lane).
+      //
+      // Why the kept list is the network's output, bit for bit.  A key is a function of its slot alone, so keys of
+      // distinct slots differ in their low bits and keys of equal slots are equal: 64 strictly ascending keys therefore
+      // name 64 distinct slots of 0..63, every slot once, whatever the hint held (a stale, duplicated or corrupt hint
+      // cannot pass).  The passes only compare-exchange, so the list is a permutation of the key set the network sorts;
+      // a strictly ascending arrangement of a set is unique, and the network's output is one.  From (2) on the tick
+      // sees the same keys in the same entries, so the scan, the queue, the drain and every output are unchanged.  A
+      // stale hint costs time, never a result; it is stored back only where the sorted slots differ from it.
+      bool hinted = false;
+      if constexpr (FIXED) {
+        unsigned hk[PPL];
 #pragma unroll
-          for (int i = 0; i < PPL; ++i) {
-            const unsigned o = __shfl_xor_sync(0xffffffffu, key[i], j);
-            key[i] = keep_max ? max(key[i], o) : min(key[i], o);
-          }
+        for (int i = 0; i < PPL; ++i) {
+          const unsigned s = (hint >> (8 * i)) & 63u;
+          const float x = poseA[pslot(tb + (int)s)].x;
+          hk[i] = (x == x ? (f2ord(x) & ~127u) : 0xffffff80u) | s;
         }
-        cx(0, 2, desc); cx(1, 3, desc); cx(0, 1, desc); cx(2, 3, desc);
+        auto up = [&](int a, int b) {
+          const unsigned lo = min(hk[a], hk[b]), hi = max(hk[a], hk[b]);
+          hk[a] = lo;
+          hk[b] = hi;
+        };
+#pragma unroll
+        for (int pass = 0; pass < T2D_ORDER_PASSES; ++pass) {
+          up(0, 1); up(2, 3);
+          up(1, 2);
+          const unsigned next = __shfl_down_sync(0xffffffffu, hk[0], 1);
+          const unsigned prev = __shfl_up_sync(0xffffffffu, hk[PPL - 1], 1);
+          if (gl != G - 1) hk[PPL - 1] = min(hk[PPL - 1], next);
+          if (gl != 0) hk[0] = max(hk[0], prev);
+        }
+        const unsigned next = __shfl_down_sync(0xffffffffu, hk[0], 1);
+        const bool ascending = hk[0] < hk[1] && hk[1] < hk[2] && hk[2] < hk[3] && (gl == G - 1 || hk[3] < next);
+        hinted = __all_sync(0xffffffffu, ascending);
+        if (hinted) {
+#pragma unroll
+          for (int i = 0; i < PPL; ++i) key[i] = hk[i];
+        } else if (lane == 0) {
+          atomicAdd(&A.order_fallbacks[(blockIdx.x & (ORDER_COUNTERS - 1)) * ORDER_COUNTER_STRIDE], 1ull);
+        }
+      }
+      if (!hinted) {
+        cx(0, 1, false); cx(2, 3, true);   // sorted runs of 2, alternating in direction (element bit 1)
+        for (int S = PPL; S <= MP; S <<= 1) {           // merge into sorted runs of S (the last one, S = MP, ascending)
+          const bool desc = (gl & (S >> 2)) != 0;       // element bit log2(S) = lane bit log2(S / 4)
+          for (int j = S >> 3; j > 0; j >>= 1) {        // element stride 4 j = lane stride j
+            const bool keep_max = ((gl & j) != 0) != desc;
+#pragma unroll
+            for (int i = 0; i < PPL; ++i) {
+              const unsigned o = __shfl_xor_sync(0xffffffffu, key[i], j);
+              key[i] = keep_max ? max(key[i], o) : min(key[i], o);
+            }
+          }
+          cx(0, 2, desc); cx(1, 3, desc); cx(0, 1, desc); cx(2, 3, desc);
+        }
+      }
+      if constexpr (FIXED) {
+        const uint32_t sorted_slots = (key[0] & 127u) | (key[1] & 127u) << 8 | (key[2] & 127u) << 16 | (key[3] & 127u) << 24;
+        if (scn_ok && sorted_slots != hint) *reinterpret_cast<uint32_t*>(A.order + idx0) = sorted_slots;
       }
       T2D_TL(4, tl_on, tl_slot, __uint_as_float(key[0] ^ key[PPL - 1]));
       // (2) Stage the sorted list: entry 4 gl + k = (x, y, -thr, key) of the slot the key names, from the pose tile.
@@ -2351,6 +2421,10 @@ static std::atomic<long long> g_launches{0};
 static std::atomic<long long> g_tick_instances[7] = {};
 static std::atomic<int> g_exchanges_alive{0};   // peer-memory done exchanges in this process (see StepArgs::prefetch)
 static std::mutex g_smem_mutex;
+// [device]: the fallback counters of K1's FIXED instance (ORDER_COUNTERS x ORDER_COUNTER_STRIDE, zeroed), allocated by
+// the first t2d_create on the device and kept for the life of the process, as a __device__ variable would be
+static unsigned long long* g_order_fallbacks[64] = {};
+static std::mutex g_order_mutex;
 static int g_smem_configured[64][6];   // [device][kernel variant]: dynamic shared memory opted in so far (process-wide)
 
 static int fail(int code, const std::string& msg) {
@@ -2541,6 +2615,7 @@ struct t2d_ctx {
   int bev_target_style = bev::NO_STYLE;
   std::unique_ptr<DeviceLog> log;      // nullptr: no log bound
   std::vector<int> type_model;         // host copy of the current type table's model ids
+  dev_ptr<uint8_t> order;              // [N][64] x-order hint of K1's FIXED instance (t2d_create: the identity)
 };
 
 enum : unsigned { NEED_STATE = 1, NEED_TABLE = 2, NEED_TICK = 4 };
@@ -2610,6 +2685,17 @@ int t2d_version(void) { return T2D_VERSION; }
 const char* t2d_last_error(void) { return g_err.c_str(); }
 int64_t t2d_launch_count(void) { return (int64_t)g_launches.load(); }
 int64_t t2d_tick_fixed_count(void) { return (int64_t)(g_tick_instances[4].load() + g_tick_instances[5].load()); }
+int64_t t2d_tick_order_fallback_count(void) {
+  std::lock_guard<std::mutex> lock(g_order_mutex);
+  int64_t sum = 0;
+  for (unsigned long long* d : g_order_fallbacks) {
+    if (!d) continue;
+    unsigned long long n[ORDER_COUNTERS * ORDER_COUNTER_STRIDE];
+    if (cudaMemcpy(n, d, sizeof(n), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+    for (int i = 0; i < ORDER_COUNTERS; ++i) sum += (int64_t)n[i * ORDER_COUNTER_STRIDE];
+  }
+  return sum;
+}
 int64_t t2d_tick_instance_count(int k) { return k >= 0 && k < 7 ? (int64_t)g_tick_instances[k].load() : -1; }
 
 #ifdef T2D_TICK_TIMELINE
@@ -2666,7 +2752,35 @@ int t2d_create(t2d_ctx** out, int device, int n_scenarios, int m_participants, c
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
   c->sm_count = prop.multiProcessorCount;
   c->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
+  {
+    std::lock_guard<std::mutex> lock(g_order_mutex);
+    unsigned long long*& counters = g_order_fallbacks[device % 64];
+    const size_t bytes = ORDER_COUNTERS * ORDER_COUNTER_STRIDE * sizeof(unsigned long long);
+    if (!counters && (cudaMalloc(&counters, bytes) != cudaSuccess || cudaMemset(counters, 0, bytes) != cudaSuccess)) {
+      cudaFree(counters);
+      counters = nullptr;
+      delete c;
+      return fail(T2D_E_CUDA, "t2d_create: cannot allocate the order fallback counters");
+    }
+  }
+  {
+    std::vector<uint8_t> identity((size_t)n_scenarios * FIX_M);
+    for (size_t i = 0; i < identity.size(); ++i) identity[i] = (uint8_t)(i % FIX_M);
+    if (int r = upload(c->order, identity.data(), identity.size())) {
+      delete c;
+      return r;
+    }
+  }
   *out = c;
+  return T2D_OK;
+}
+
+int t2d_order_hint(t2d_ctx* c, void* read_to, const void* write_from) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  CUDA_TRY(cudaSetDevice(c->device));
+  const size_t bytes = (size_t)c->N * FIX_M;
+  if (read_to) CUDA_TRY(cudaMemcpy(read_to, c->order.get(), bytes, cudaMemcpyDeviceToHost));
+  if (write_from) CUDA_TRY(cudaMemcpy(c->order.get(), write_from, bytes, cudaMemcpyHostToDevice));
   return T2D_OK;
 }
 
@@ -3185,6 +3299,8 @@ static int launch_step(t2d_ctx* c, const float* action, const float* ego, uint8_
   A.wheel_f = c->wheel_f ? c->wheel_f + p0 : nullptr; A.wheel_r = c->wheel_r ? c->wheel_r + p0 : nullptr;
   A.action = action; A.ego_action = ego ? ego + 2 * (size_t)first : nullptr; A.flags = flags; A.hit_index = hit_index; A.hit_segment = hit_segment;
   A.scn_status = scn_status; A.done = done;
+  A.order = c->order.get() + (size_t)first * FIX_M;
+  A.order_fallbacks = g_order_fallbacks[c->device % 64];
   const bool map_table = map.n_tiles > 1;
   const MapArgs mp = map_args(map, first);
   A.map_blob = mp.map_blob; A.tile_off = mp.tile_off; A.tile_id = mp.tile_id; A.map_bytes = map.smem_bytes; A.mh = map.mh;
