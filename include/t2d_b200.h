@@ -254,6 +254,56 @@ int t2d_reset(t2d_ctx* ctx, const uint8_t* mask, const int32_t* pool_index, int 
 /* Optional initial wheel speeds for t2d_reset: DEVICE arrays [n_pool][M] indexed like the other pool columns (NULL, NULL unbinds). */
 int t2d_bind_reset_wheel_pool(t2d_ctx* ctx, const float* pool_omega_front, const float* pool_omega_rear);
 
+/* ---- sampled resets: a seeded pool-row draw and collision-checked random start states -------------------------------
+ * ParkingEnv.reset draws a new start state on every reset (envs/parking.py:397-441) and keeps a draw only when the
+ * vehicle's box meets no obstacle and not the target area (ParkingLotGenerator._verify_start_state,
+ * map/generator/generate_parking_lot.py:231-237).  The contract is DESIGN.md section 1 "Sampled resets":
+ *   draws      Philox4x32-10, key (seed low, seed high), counter (d, n, episode[n], 0);
+ *   row        d = 0: row = (u0 * P) >> 32 over the P pool rows (sample_rows; else row n), written to pool_row[n];
+ *   columns    the optional DEVICE pools are copied from the row into what they belong to: pool_type_id [n_rows][M] into
+ *              the bound type_id (with agents bound the scenario's retired list is cleared), pool_target [n_rows][5] into
+ *              the t2d_set_goal target, pool_tile_id [n_rows] into the map table's tile_id (ids < n_tiles at every
+ *              sampled reset: the library does not read the device pool to check them),
+ *              pool_route_id [n_rows][M] into the t2d_set_routes route_id;
+ *   jitter     after K2 (and K7) slot m = 0 .. M-1 of every masked scenario, unless inactive or retired or its jitter row
+ *              is all zero, tries t < tries with draw d = 1 + 32 m + t: (x + dx, y + dy, wrap(h + dh), v + dv), dx ... from
+ *              the (lo, hi) ranges of jitter[m] (HOST fp32 [M][4][2], copied; NULL: none).  The lowest t whose pose is
+ *              inside its tile's box, meets no collidable segment or Area of its tile and no other active slot at its
+ *              current state (and, for slot 0 with avoid_target, not the goal target) wins; reset_try[n][m] = t, or -1
+ *              when no try is accepted (the pool state is kept) or the slot is not jittered.  A moved slot's vx, vy are
+ *              v (cos h, sin h); a moved SingleTrackDrift slot rolls freely (v / wheel_radius), or keeps the wheel speeds
+ *              of a bound t2d_bind_reset_wheel_pool;
+ *   episode    [N] uint32, zeroed when a sampler is bound; each sampled reset of scenario n draws with e = episode[n]
+ *              and then increments it.
+ * episode [N], pool_row [N] int32 and reset_try [N][M] int8 are caller-owned DEVICE buffers that must stay alive while
+ * bound.  NULL unbinds.  Rejected (the previous sampler stays bound): tries outside 1..32, a NULL episode / pool_row /
+ * reset_try, row pools with n_rows <= 0, a jitter range that is not finite or has lo > hi (T2D_E_INVALID); a pool whose
+ * destination is not bound (T2D_E_STATE). */
+typedef struct t2d_reset_sampler {
+  uint64_t seed;
+  int32_t sample_rows;            /* 1: draw the row; 0: scenario n runs pool row n */
+  int32_t tries;                  /* 1..32 */
+  int32_t avoid_target;           /* slot 0 must not meet its goal target */
+  int32_t n_rows;                 /* rows of the pools below (the reset's n_pool must match) */
+  const float* jitter;            /* HOST [M][4][2] or NULL */
+  const uint8_t* pool_type_id;    /* DEVICE [n_rows][M] or NULL */
+  const float* pool_target;       /* DEVICE [n_rows][5] or NULL */
+  const uint16_t* pool_tile_id;   /* DEVICE [n_rows] or NULL */
+  const int16_t* pool_route_id;   /* DEVICE [n_rows][M] or NULL */
+  uint32_t* episode;              /* DEVICE [N] */
+  int32_t* pool_row;              /* DEVICE [N] */
+  int8_t* reset_try;              /* DEVICE [N][M] */
+} t2d_reset_sampler;
+int t2d_set_reset_sampler(t2d_ctx* ctx, const t2d_reset_sampler* sampler);
+/* A sampled reset of the scenarios with mask[n] != 0 (envs/parking.py:397-441, generate_parking_lot.py:231-237): K13
+ * (row draw, row-owned columns), t2d_reset with pool_index = pool_row (K2, then K7 with a log: the drawn row is the
+ * replayed one), K14 (jitter).  Pool arguments as t2d_reset's.  Rejected without a launch: whatever t2d_reset rejects,
+ * no sampler bound or a pool destination no longer bound (T2D_E_STATE), row pools with n_pool != n_rows, no row draws
+ * with n_pool < N (T2D_E_INVALID). */
+int t2d_reset_sampled(t2d_ctx* ctx, const uint8_t* mask, int n_pool, const float* pool_x, const float* pool_y,
+                      const float* pool_heading, const float* pool_speed, const float* pool_vx, const float* pool_vy,
+                      void* stream);
+
 /* ---- log replay: recorded tracks drive participants around a simulated ego ------------------------------------------
  * Trajectory.get_state(frame) / Vehicle.get_pose(frame) (participant/trajectory/trajectory.py:97-113,
  * participant/element/vehicle.py:263-281) for every replayed slot of every scenario, on the device.  The contract

@@ -58,6 +58,15 @@ class LogC(C.Structure):
                 ("row_track", C.c_void_p), ("log_row", C.c_void_p), ("type_id", C.c_void_p)]
 
 
+class ResetSamplerC(C.Structure):
+    """``t2d_reset_sampler``: the seed and options of the sampled resets, the host jitter table, the device row pools and
+    the world-owned episode / pool_row / reset_try buffers."""
+    _fields_ = [("seed", C.c_uint64), ("sample_rows", C.c_int32), ("tries", C.c_int32), ("avoid_target", C.c_int32),
+                ("n_rows", C.c_int32), ("jitter", C.c_void_p), ("pool_type_id", C.c_void_p), ("pool_target", C.c_void_p),
+                ("pool_tile_id", C.c_void_p), ("pool_route_id", C.c_void_p), ("episode", C.c_void_p),
+                ("pool_row", C.c_void_p), ("reset_try", C.c_void_p)]
+
+
 class ObsConfigC(C.Structure):
     """``t2d_obs_config``: rows and ranges of the vector observation."""
     _fields_ = [("k_agents", C.c_int32), ("k_segments", C.c_int32), ("agent_range", C.c_float), ("segment_range", C.c_float)]
@@ -88,6 +97,8 @@ SYMBOLS = {
     "t2d_scatter_agent_action": (C.c_int, [_P, _P, C.c_int32, _P, _P, _P]),
     "t2d_step_host_agents": (C.c_int, [_P] + [_P] * 7 + [C.c_int] + [_P] * 6),
     "t2d_reset": (C.c_int, [_P, _P, _P, C.c_int] + [_P] * 7),
+    "t2d_set_reset_sampler": (C.c_int, [_P, C.POINTER(ResetSamplerC)]),
+    "t2d_reset_sampled": (C.c_int, [_P, _P, C.c_int] + [_P] * 7),
     "t2d_lidar_scan": (C.c_int, [_P, C.c_int, C.c_float, _P, _P, _P]),
     "t2d_lidar_scan_agents": (C.c_int, [_P, _P, C.c_int32, C.c_int, C.c_float, _P, _P, _P]),
     "t2d_set_bev_styles": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int]),

@@ -14,6 +14,8 @@
 // K10 t2d_agents_epilogue_kernel status, reward and retirement of every agent row of an observer list.
 // K11 t2d_agent_action_kernel    the action of every agent row of an observer list, scattered to its slot.
 // K12 t2d_route_obs_kernel       the route of every observer row in its frame, with look-ahead points.
+// K13 t2d_episode_draw_kernel    sampled resets: the seeded pool-row draw and the row-owned columns.
+// K14 t2d_episode_place_kernel   sampled resets: collision-checked jitter of the start states, one warp per scenario.
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory.
 //
 // Work decomposition of K1: a scenario (M <= 128 participants) is owned by a group of G lanes of
@@ -1307,6 +1309,173 @@ __global__ void t2d_reset_kernel(const __grid_constant__ ResetArgs A) {
   }
 }
 
+// ---------------------------------------------------------------------------- K13 / K14: sampled resets
+// DESIGN.md section 1 "Sampled resets" (envs/parking.py:397-441, map/generator/generate_parking_lot.py:231-237).
+// K13 draws the pool row of every masked scenario and copies the columns that belong to the row; K2 (and K7) then run
+// with pool_index = pool_row; K14 moves the start states by seeded jitter, checked by the tick's own predicates.
+struct DrawArgs {
+  const uint8_t* mask;
+  const uint32_t* episode;             // [N]
+  int32_t* pool_row;                   // [N]
+  uint64_t seed;
+  int sample_rows, N, M, P;
+  const uint8_t* pool_type;  uint8_t* type_id;  uint8_t* retired;   // [P][M] -> [N][M]; retired: [N][M] or nullptr
+  const float* pool_target;  float* target;                         // [P][5] -> [N][5]
+  const uint16_t* pool_tile; uint16_t* tile_id;                     // [P] -> [N]
+  const int16_t* pool_route; int16_t* route_id;                     // [P][M] -> [N][M]
+};
+
+__global__ void __launch_bounds__(256) t2d_episode_draw_kernel(const __grid_constant__ DrawArgs A) {
+  const long long total = (long long)A.N * A.M;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int n = (int)(i / A.M), m = (int)(i - (long long)n * A.M);
+    if (!A.mask[n]) continue;
+    const int r = A.sample_rows ? draw_row(episode_draw(A.seed, 0u, (uint32_t)n, A.episode[n]).x, A.P) : min(n, A.P - 1);
+    const long long s = (long long)r * A.M + m;
+    if (A.pool_type) {
+      A.type_id[i] = A.pool_type[s];
+      if (A.retired) A.retired[i] = 0xff;   // K2 would restore a retired type of the old episode over the new one
+    }
+    if (A.pool_route) A.route_id[i] = A.pool_route[s];
+    if (m == 0) {
+      A.pool_row[n] = r;
+      if (A.pool_tile) A.tile_id[n] = A.pool_tile[r];
+      if (A.pool_target)
+        for (int k = 0; k < 5; ++k) A.target[5 * (long long)n + k] = A.pool_target[5 * (long long)r + k];
+    }
+  }
+}
+
+struct PlaceArgs : WorldArgs {
+  const uint8_t* mask;
+  uint32_t* episode;                   // [N]
+  int8_t* reset_try;                   // [N][M]
+  uint64_t seed;
+  const float* jitter;                 // [M][8] (lo, hi) of dx, dy, dheading, dspeed, or nullptr: no slot is jittered
+  int tries, avoid_target;
+  const float* target;                 // [N][5] the t2d_set_goal target (avoid_target), or nullptr
+  MapArgs map;
+  MapHeader mh;                        // the single tile's header (its bounds also when no tile has segments)
+  int has_bounds;
+  float *wheel_f, *wheel_r;            // [N][M] or nullptr
+  int pool_wheels;                     // t2d_bind_reset_wheel_pool is bound: K2's wheel speeds stay
+};
+
+// The tick's pose of a slot at (x, y, heading) with its type's shape (K1's pose tile: sincos_fast, pose_l, pose_w)
+__device__ __forceinline__ Pose slot_pose(const Params& p, float x, float y, float h) {
+  Pose a;
+  a.x = x; a.y = y; a.h = h; a.l = p.pose_l; a.w = p.pose_w;
+  sincos_fast(h, &a.s, &a.c);
+  return a;
+}
+
+// Would check_events flag slot m of scenario n at pose a?  The same filtered predicates as K1: out of its tile's box,
+// a collidable segment or Area of its tile, any other active slot at its current state; with avoid, the target box too.
+__device__ __forceinline__ bool place_blocked(const PlaceArgs& A, long long n, int m, const Pose a, float rb, bool avoid,
+                                              const float4* sa, const float4* sb) {
+  const unsigned char* blob = tile_blob(A.map, n);
+  const MapHeader* mh = (A.map.tile_id && blob) ? reinterpret_cast<const MapHeader*>(blob) : &A.mh;
+  const bool bounded = A.map.tile_id && blob ? mh->has_bounds != 0 : A.has_bounds != 0;
+  if (bounded) {
+    int r = out_of_bound_f32(a.x, a.y, a.c, a.s, a.l, a.w, a.w < 0.0f, mh->bxmin, mh->bxmax, mh->bymin, mh->bymax);
+    if (r < 0) r = out_of_bound_f64(a.x, a.y, a.h, a.l, a.w, a.w < 0.0f, mh->bxmin, mh->bxmax, mh->bymin, mh->bymax) ? 1 : 0;
+    if (r) return true;
+  }
+  if (blob && mh->n_seg > 0) {
+    // (the blob and its header as global addresses: the out-of-line walks K1 shares keep their global loads)
+    const unsigned char* g = reinterpret_cast<const unsigned char*>(__cvta_global_to_generic(__cvta_generic_to_global(blob)));
+    const MapHeader& gh = *reinterpret_cast<const MapHeader*>(g);   // (tile 0's header starts the blob)
+    const MapView mv = map_view(g, gh);
+    int best = static_walk_exact(a, rb, gh, mv.seg, mv.cell_start, mv.items);
+    if (gh.n_poly > 0) best = static_objects(best, a.x, a.y, gh, g);
+    if (best != 0x7fffffff) return true;
+  }
+  for (int j = 0; j < A.M; ++j) {   // the scenario's slots as K14 staged them (rb < 0: inactive, retired or no shape)
+    const float4 pa = sa[j];
+    if (j == m || !(pa.z >= 0.0f)) continue;
+    const float dx = pa.x - a.x, dy = pa.y - a.y, rr = rb + pa.z;
+    if (dx * dx + dy * dy > fmaf(rr * rr, 1.00001f, 1e-12f)) continue;   // bounding circles apart (conservative, as K1)
+    const float4 pb = sb[j];
+    Pose b;
+    b.x = pa.x; b.y = pa.y; b.h = pa.w; b.c = pb.x; b.s = pb.y; b.l = pb.z; b.w = pb.w;
+    if (pair_hit(a, b)) return true;
+  }
+  if (avoid) {
+    const float* tg = A.target + 5 * n;
+    Pose t;
+    t.x = tg[0]; t.y = tg[1]; t.h = tg[2]; t.l = tg[3]; t.w = tg[4];
+    sincos_fast(t.h, &t.s, &t.c);
+    if (pair_hit(a, t)) return true;
+  }
+  return false;
+}
+
+// One warp per scenario: slots in order 0 .. M-1, lane t tries draw 1 + 32 m + t, the lowest accepted lane wins.  The
+// scenario's poses are staged in the warp's shared memory (K1's pose tile layout, slot-major), so the partner loop of
+// every try reads them there; the winner of a slot writes its new pose to both copies.
+constexpr int K14_WARPS = 4;
+__device__ __forceinline__ void stage_pose(const PlaceArgs& A, long long i, int tid, float x, float y, float h, float4* sa,
+                                           float4* sb, int j) {
+  const bool solid = tid < A.n_types && A.table[tid].shape() != SHAPE_NONE;
+  const Params& p = A.table[solid ? tid : 0];
+  float sn, cs;
+  sincos_fast(h, &sn, &cs);
+  sa[j] = make_float4(x, y, solid ? p.rbound : -1.0f, h);
+  sb[j] = make_float4(cs, sn, p.pose_l, p.pose_w);
+}
+
+__global__ void __launch_bounds__(K14_WARPS * 32) t2d_episode_place_kernel(const __grid_constant__ PlaceArgs A) {
+  __shared__ float4 s_pose[K14_WARPS][2][T2D_MAX_PARTICIPANTS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long n = (long long)blockIdx.x * K14_WARPS + warp;
+  if (n >= A.N || !A.mask[n]) return;
+  float4* sa = s_pose[warp][0];
+  float4* sb = s_pose[warp][1];
+  const uint32_t e = A.episode[n];
+  const long long base = n * A.M;
+  if (A.jitter != nullptr)
+    for (int j = lane; j < A.M; j += 32) stage_pose(A, base + j, A.type_id[base + j], A.x[base + j], A.y[base + j], A.h[base + j], sa, sb, j);
+  __syncwarp();
+  for (int m = 0; m < A.M; ++m) {
+    const long long i = base + m;
+    const int tid = A.type_id[i];
+    bool jittered = A.jitter != nullptr && tid < A.n_types;
+    if (jittered) {
+      bool any = false;
+      for (int k = 0; k < 8; ++k) any = any || A.jitter[8 * m + k] != 0.0f;
+      jittered = any;
+    }
+    if (!jittered) {
+      if (lane == 0) A.reset_try[i] = -1;
+      continue;
+    }
+    const Params& p = A.table[tid];
+    bool ok = false;
+    Cand cd{};
+    if (lane < A.tries) {
+      cd = jitter_candidate(episode_draw(A.seed, 1u + 32u * (uint32_t)m + (uint32_t)lane, (uint32_t)n, e), A.jitter + 8 * m,
+                            A.x[i], A.y[i], A.h[i], A.v[i]);
+      ok = p.shape() == SHAPE_NONE ||
+           !place_blocked(A, n, m, slot_pose(p, cd.x, cd.y, cd.h), p.rbound, A.avoid_target && m == 0 && A.target != nullptr,
+                          sa, sb);
+    }
+    const unsigned acc = __ballot_sync(0xffffffffu, ok);
+    const int win = acc ? __ffs(acc) - 1 : -1;
+    if (lane == (win < 0 ? 0 : win)) {
+      if (win >= 0) {
+        A.x[i] = cd.x; A.y[i] = cd.y; A.h[i] = cd.h; A.v[i] = cd.v;
+        A.vx[i] = cd.v * cosf(cd.h); A.vy[i] = cd.v * sinf(cd.h);   // as K2 for a pool without velocities
+        // free rolling, as K2 sets it without a wheel pool; with one, the slot keeps the pool's wheel speeds
+        if (A.wheel_f != nullptr && !A.pool_wheels && p.model() == MODEL_DRIFT) A.wheel_f[i] = A.wheel_r[i] = cd.v / p.wheel_radius;
+        stage_pose(A, i, tid, cd.x, cd.y, cd.h, sa, sb, m);
+      }
+      A.reset_try[i] = (int8_t)win;
+    }
+    __syncwarp();   // the next slot's tries read this one's placed pose
+  }
+  if (lane == 0) A.episode[n] = e + 1u;
+}
+
 // ---------------------------------------------------------------------------- route following
 // DESIGN.md section 1 "Route following": the polyline table (t2d_set_paths) read by K5's PATH sources, the OffRoute
 // detector and route progress of the epilogues, and K12.
@@ -2515,6 +2684,13 @@ struct DeviceLog {
   std::vector<uint8_t> track_type_host;   // host copy: t2d_set_type_table keeps these rows static
 };
 
+// The bound reset sampler (t2d_set_reset_sampler), replaced as a whole: the caller's struct with the jitter table moved
+// into the library's own device copy
+struct DeviceSampler {
+  t2d_reset_sampler s{};               // s.jitter: jitter.get() or nullptr
+  dev_ptr<float> jitter;               // [M][8]
+};
+
 // Staging of the host steps (t2d_step_host, t2d_step_host_ego, t2d_step_host_agents); every piece is created whole the
 // first time a step needs it.
 static constexpr int MAX_HOST_CHUNKS = 8;
@@ -2616,6 +2792,7 @@ struct t2d_ctx {
   std::unique_ptr<DeviceLog> log;      // nullptr: no log bound
   std::vector<int> type_model;         // host copy of the current type table's model ids
   dev_ptr<uint8_t> order;              // [N][64] x-order hint of K1's FIXED instance (t2d_create: the identity)
+  std::unique_ptr<DeviceSampler> sampler;   // t2d_set_reset_sampler; nullptr: none bound
 };
 
 enum : unsigned { NEED_STATE = 1, NEED_TABLE = 2, NEED_TICK = 4 };
@@ -3709,14 +3886,21 @@ int t2d_check_events(t2d_ctx* c, uint8_t* flags, int16_t* hit_index, int16_t* hi
   return launch_step(c, nullptr, c ? c->ego_action : nullptr, flags, hit_index, hit_segment, nullptr, nullptr, stream, 0);
 }
 
-int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x, const float* pool_y,
-              const float* pool_heading, const float* pool_speed, const float* pool_vx, const float* pool_vy, void* stream) {
+// The arguments t2d_reset and t2d_reset_sampled share
+static int check_reset(t2d_ctx* c, const uint8_t* mask, int n_pool, const float* pool_x, const float* pool_y,
+                       const float* pool_heading, const float* pool_speed) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (int r = require(c, NEED_STATE)) return r;
   if (!mask || !pool_x || !pool_y || !pool_heading || !pool_speed) return fail(T2D_E_INVALID, "t2d_reset: NULL array");
   if (n_pool <= 0) return fail(T2D_E_INVALID, "n_pool must be > 0");
   if (c->log && n_pool != c->log->n_rows) return fail(T2D_E_INVALID, "t2d_reset: with a log bound, pool row p is episode row p (n_pool == n_rows)");
   if (c->log && c->log->type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+  return T2D_OK;
+}
+
+int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x, const float* pool_y,
+              const float* pool_heading, const float* pool_speed, const float* pool_vx, const float* pool_vy, void* stream) {
+  if (int r = check_reset(c, mask, n_pool, pool_x, pool_y, pool_heading, pool_speed)) return r;
   CUDA_TRY(cudaSetDevice(c->device));
   ResetArgs A{world_args(c)};
   A.mask = mask; A.pool_index = pool_index;
@@ -3732,6 +3916,79 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   if (int r = launched()) return r;
   if (c->log) return launch_replay(c, stream, 0, c->N, 0, mask, pool_index);   // the new episode's traffic at t0
   return T2D_OK;
+}
+
+// A row-owned pool needs what it writes into: checked when the sampler is bound and before every sampled reset (the
+// goal, the map table or the routes may have been unbound since)
+static int check_sampler_targets(const t2d_ctx* c, const t2d_reset_sampler& s) {
+  if (s.pool_target && !c->goal.target) return fail(T2D_E_STATE, "reset sampler: a target pool needs a t2d_set_goal target");
+  if (s.pool_tile_id && !c->map.tile_id) return fail(T2D_E_STATE, "reset sampler: a tile pool needs a map table of more than one tile");
+  if (s.pool_route_id && !c->route_id) return fail(T2D_E_STATE, "reset sampler: a route pool needs t2d_set_routes");
+  return T2D_OK;
+}
+
+int t2d_set_reset_sampler(t2d_ctx* c, const t2d_reset_sampler* s) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!s) {
+    c->sampler.reset();
+    return T2D_OK;
+  }
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (s->tries < 1 || s->tries > 32) return fail(T2D_E_INVALID, "reset sampler: tries must be in 1..32");
+  if (!s->episode || !s->pool_row || !s->reset_try) return fail(T2D_E_INVALID, "reset sampler: NULL episode / pool_row / reset_try");
+  const bool pools = s->pool_type_id || s->pool_target || s->pool_tile_id || s->pool_route_id;
+  if (pools && s->n_rows <= 0) return fail(T2D_E_INVALID, "reset sampler: row pools need n_rows > 0");
+  if (s->jitter)
+    for (int k = 0; k < c->M * 4; ++k) {
+      const float lo = s->jitter[2 * k], hi = s->jitter[2 * k + 1];
+      if (!(std::isfinite(lo) && std::isfinite(hi) && lo <= hi))
+        return fail(T2D_E_INVALID, "reset sampler: every jitter range must be finite with lo <= hi");
+    }
+  if (int r = check_sampler_targets(c, *s)) return r;
+  CUDA_TRY(cudaSetDevice(c->device));
+  auto d = std::make_unique<DeviceSampler>();
+  d->s = *s;
+  if (s->jitter) {
+    if (int r = upload(d->jitter, s->jitter, (size_t)c->M * 8)) return r;
+    d->s.jitter = d->jitter.get();
+  }
+  CUDA_TRY(cudaMemset(s->episode, 0, sizeof(uint32_t) * c->N));
+  c->sampler = std::move(d);
+  return T2D_OK;
+}
+
+int t2d_reset_sampled(t2d_ctx* c, const uint8_t* mask, int n_pool, const float* pool_x, const float* pool_y,
+                      const float* pool_heading, const float* pool_speed, const float* pool_vx, const float* pool_vy,
+                      void* stream) {
+  if (int r = check_reset(c, mask, n_pool, pool_x, pool_y, pool_heading, pool_speed)) return r;
+  if (!c->sampler) return fail(T2D_E_STATE, "t2d_reset_sampled: no reset sampler bound");
+  if (int r = require(c, NEED_TABLE)) return r;
+  const t2d_reset_sampler& s = c->sampler->s;
+  if (int r = check_sampler_targets(c, s)) return r;
+  if ((s.pool_type_id || s.pool_target || s.pool_tile_id || s.pool_route_id) && n_pool != s.n_rows)
+    return fail(T2D_E_INVALID, "t2d_reset_sampled: the pool must have the sampler's n_rows rows");
+  if (!s.sample_rows && n_pool < c->N) return fail(T2D_E_INVALID, "t2d_reset_sampled: without row draws the pool needs one row per scenario");
+  CUDA_TRY(cudaSetDevice(c->device));
+  DrawArgs D{};
+  D.mask = mask; D.episode = s.episode; D.pool_row = s.pool_row; D.seed = s.seed; D.sample_rows = s.sample_rows;
+  D.N = c->N; D.M = c->M; D.P = n_pool;
+  // the row-owned columns are written into the caller's bound arrays (type_id, the goal target, the map table's tile_id,
+  // the route ids), which the library documents as rewritable between ticks
+  D.pool_type = s.pool_type_id; D.type_id = const_cast<uint8_t*>(c->type_id);
+  D.retired = c->agent_q > 0 ? c->agent_retired : nullptr;
+  D.pool_target = s.pool_target; D.target = const_cast<float*>(c->goal.target);
+  D.pool_tile = s.pool_tile_id; D.tile_id = const_cast<uint16_t*>(c->map.tile_id);
+  D.pool_route = s.pool_route_id; D.route_id = const_cast<int16_t*>(c->route_id);
+  t2d_episode_draw_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(D);
+  if (int r = launched()) return r;
+  if (int r = t2d_reset(c, mask, s.pool_row, n_pool, pool_x, pool_y, pool_heading, pool_speed, pool_vx, pool_vy, stream)) return r;
+  PlaceArgs P{world_args(c)};
+  P.mask = mask; P.episode = s.episode; P.reset_try = s.reset_try; P.seed = s.seed;
+  P.jitter = s.jitter; P.tries = s.tries; P.avoid_target = s.avoid_target; P.target = c->goal.target;
+  P.map = map_args(c->map); P.mh = c->map.mh; P.has_bounds = c->map.has_bounds ? 1 : 0;
+  P.wheel_f = c->wheel_f; P.wheel_r = c->wheel_r; P.pool_wheels = c->reset_pool_wf != nullptr;
+  t2d_episode_place_kernel<<<(unsigned)((c->N + K14_WARPS - 1) / K14_WARPS), K14_WARPS * 32, 0, (cudaStream_t)stream>>>(P);
+  return launched();
 }
 
 // K4 over the rows of an observer list (observers == nullptr: row q is slot q); the callers have checked their arguments

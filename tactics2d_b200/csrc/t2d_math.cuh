@@ -699,6 +699,67 @@ T2D_HD void pointmass_euler_step(OneIO& io, const Params& p, int n_steps, double
 }
 
 // ------------------------------------------------------------------------------------------
+// Sampled resets (K13 / K14; DESIGN.md section 1 "Sampled resets")
+// ------------------------------------------------------------------------------------------
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11): stateless and counter-based, so
+// every thread that needs a draw recomputes it from (key, counter).  Counter 0 with key 0 gives 6627e8d5 e169c58d
+// bc57ac4c 9b00dbd8 (Random123's known-answer vector; cuRAND's Philox4_32_10 at seed 0, offset 0 gives the same words).
+struct U4 { uint32_t x, y, z, w; };
+
+T2D_HD uint32_t mulhi32(uint32_t a, uint32_t b) {
+#if defined(__CUDA_ARCH__)
+  return __umulhi(a, b);
+#else
+  return (uint32_t)(((uint64_t)a * b) >> 32);
+#endif
+}
+
+T2D_HD U4 philox4x32_10(U4 c, uint32_t k0, uint32_t k1) {
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = mulhi32(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = mulhi32(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = U4{hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0};
+    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// Draw d of scenario n in its episode e under a 64-bit seed: key (seed low, seed high), counter (d, n, e, 0).
+T2D_HD U4 episode_draw(uint64_t seed, uint32_t d, uint32_t n, uint32_t e) {
+  return philox4x32_10(U4{d, n, e, 0u}, (uint32_t)seed, (uint32_t)(seed >> 32));
+}
+
+// The pool row of a draw word over P rows: multiply-high, bias below P / 2^32.
+T2D_HD int draw_row(uint32_t u, int P) { return (int)(((uint64_t)u * (uint32_t)P) >> 32); }
+
+// (u >> 8) 2^-24: exact in fp32, in [0, 1).  Then lo + f (hi - lo), each operation rounded on its own (no FMA), in [lo, hi].
+T2D_HD float draw_unit(uint32_t u) { return (float)(u >> 8) * 5.9604644775390625e-8f; }
+#if defined(__CUDA_ARCH__)
+#define T2D_FADD_RN(a, b) __fadd_rn((a), (b))
+#define T2D_FSUB_RN(a, b) __fsub_rn((a), (b))
+#define T2D_FMUL_RN(a, b) __fmul_rn((a), (b))
+#else
+#define T2D_FADD_RN(a, b) ((a) + (b))   // (host builds use -ffp-contract=off)
+#define T2D_FSUB_RN(a, b) ((a) - (b))
+#define T2D_FMUL_RN(a, b) ((a) * (b))
+#endif
+T2D_HD float draw_range(uint32_t u, float lo, float hi) {
+  return T2D_FADD_RN(lo, T2D_FMUL_RN(draw_unit(u), T2D_FSUB_RN(hi, lo)));
+}
+
+// Try t of a slot: the candidate (x, y, heading, speed) from the four words of its draw and the slot's jitter row
+// jit[8] = (lo, hi) of dx, dy, dheading, dspeed.
+struct Cand { float x, y, h, v; };
+T2D_HD Cand jitter_candidate(U4 u, const float* jit, float x, float y, float h, float v) {
+  Cand c;
+  c.x = T2D_FADD_RN(x, draw_range(u.x, jit[0], jit[1]));
+  c.y = T2D_FADD_RN(y, draw_range(u.y, jit[2], jit[3]));
+  c.h = wrap_two_pi(T2D_FADD_RN(h, draw_range(u.z, jit[4], jit[5])));
+  c.v = T2D_FADD_RN(v, draw_range(u.w, jit[6], jit[7]));
+  return c;
+}
+
+// ------------------------------------------------------------------------------------------
 // Lidar (K4)
 // ------------------------------------------------------------------------------------------
 struct BeamWindow { int x, y; };   // first beam, number of beams (wraps modulo n_beams)

@@ -50,7 +50,7 @@ class BatchedTrafficEnv:
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
                  agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
-                 route: Optional[dict] = None):
+                 route: Optional[dict] = None, sampler: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -87,7 +87,14 @@ class BatchedTrafficEnv:
         truncated.  The routes follow their rows like the types do (an auto-reset keeps a scenario's route; a shuffle of a
         replay deals them out with the rows).  ``info["route"]`` is the route observation after the auto-reset
         (``BatchedWorld.route_observe`` with ``n_points`` (8) and ``spacing`` (2.0)): ``[N, F]`` from every ego, or with
-        ``observation="agents"`` ``[N, Q, F]`` from every observer row."""
+        ``observation="agents"`` ``[N, Q, F]`` from every observer row;
+        ``sampler``: e.g. ``dict(seed=0, jitter=..., tries=8, sample_rows=True, avoid_target=False)`` draws every episode
+        (``BatchedWorld.set_reset_sampler``; DESIGN.md section 1 "Sampled resets"; envs/parking.py:397-441): every reset
+        and auto-reset runs a pool row drawn from a seeded stream and moves the start states by ``jitter`` ([M, 4, 2]
+        ranges) where the move is collision-free; the row's types, ``target`` and routes follow it.  ``reset(seed=s)``
+        re-keys the stream and restarts the episode counters, ``reset()`` keeps drawing; ``info["pool_row"]`` is the row
+        each scenario runs after the step's auto-reset.  A shuffle is then rejected, as are jitter on the replayed slots
+        (with ``replay``, only slot 0 may move) and per-row goals with ``sample_rows`` (they belong to scenarios, not rows)."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -122,6 +129,16 @@ class BatchedTrafficEnv:
             missing = {"paths", "route_id", "threshold"} - set(self.route)
             if missing:
                 raise ValueError(f"route: missing keys {sorted(missing)}")
+        self.sampler = None if sampler is None else dict(sampler)
+        if self.sampler is not None:
+            unknown = set(self.sampler) - {"seed", "jitter", "tries", "sample_rows", "avoid_target"}
+            if unknown:
+                raise ValueError(f"sampler: unknown keys {sorted(unknown)}")
+            jit = self.sampler.get("jitter")
+            if replay is not None and jit is not None and np.any(np.asarray(jit)[1:] != 0):
+                raise ValueError("sampler: with replay only slot 0 may have jitter (the log drives the others)")
+            if agent_rewards and self.vector_obs.get("goals") is not None and self.sampler.get("sample_rows", True):
+                raise ValueError("sampler: per-row goals belong to scenarios, not pool rows: use sample_rows=False")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -167,6 +184,9 @@ class BatchedTrafficEnv:
                 obs = self.vector_obs.get("observers")
                 self._route_observers = obs if obs is not None else \
                     torch.arange(m, dtype=torch.int16, device=dev).expand(n, m).contiguous()
+        self._target_pool = None if target is None else self.world._goal["target"].clone()
+        if self.sampler is not None:
+            self._bind_sampler(self.sampler.get("seed", 0))
         if observation == "bev":
             w, h = self.bev_resolution
             self.observation_space = {"shape": (n, h, w, 3), "dtype": "uint8", "low": 0, "high": 255}
@@ -183,6 +203,13 @@ class BatchedTrafficEnv:
             self.action_space["shape"] = (n, m if obs is None else int(obs.shape[1]), 2)
 
     # ------------------------------------------------------------------ helpers
+    def _bind_sampler(self, seed):
+        """(Re)key the reset sampler (zeroes the episode counters); the pool rows' types, targets and routes follow them."""
+        sp = self.sampler
+        self.world.set_reset_sampler(seed, jitter=sp.get("jitter"), tries=sp.get("tries", 8),
+                                     sample_rows=sp.get("sample_rows", True), avoid_target=sp.get("avoid_target", False),
+                                     type_id=self._type_id, target=self._target_pool, route_id=self._route_pool)
+
     def _obs(self):
         if self.observation == "bev":
             return self.world.bev(self.bev_resolution, self.bev_range, rgb=True)
@@ -197,6 +224,8 @@ class BatchedTrafficEnv:
                 "hit_segment": hit_segment, "step_count": self.world.step_count}
         if self.world.replay_track is not None:   # scheduled replay: the track each slot shows (-1: none)
             info["track"] = self.world.replay_track
+        if self.sampler is not None:
+            info["pool_row"] = self.world.pool_row
         return info
 
     def _add_lidar(self, info):
@@ -216,15 +245,21 @@ class BatchedTrafficEnv:
     def reset(self, seed: int = None, options: dict = None):
         import torch
 
+        if self.sampler is not None and options and options.get("shuffle"):
+            raise ValueError("a sampled env draws its rows: options={'shuffle': True} is not taken")
         if seed is not None:
             self._rng = np.random.default_rng(seed)
+            if self.sampler is not None:
+                self._bind_sampler(seed)
         perm = None
         if options and options.get("shuffle"):
             perm = torch.from_numpy(self._rng.permutation(self.num_envs).astype(np.int32)).to(self.world.device)
         if self.agent_rewards:   # every slot takes its pool row's type below; no retired type of the old episodes survives
             self.world.retired_type.fill_(255)
             self.world.reset_agent_trackers()
-        if self.replay is not None and perm is not None:   # the rows' own types (the replayed slots' are rewritten anyway)
+        if self.sampler is not None:                        # K13 copies the drawn rows' types and routes
+            self.scenario_manager.reset(sample=True)
+        elif self.replay is not None and perm is not None:   # the rows' own types (the replayed slots' are rewritten anyway)
             self.world.type_id.copy_(self._type_id[perm.long()])
             if self._route_pool is not None:                # ... and routes
                 self.world.route_id.copy_(self._route_pool[perm.long()])
@@ -232,7 +267,8 @@ class BatchedTrafficEnv:
             self.world.type_id.copy_(self._type_id)
             if self._route_pool is not None:
                 self.world.route_id.copy_(self._route_pool)
-        self.scenario_manager.reset(pool_index=perm)
+        if self.sampler is None:
+            self.scenario_manager.reset(pool_index=perm)
         self.world.reset_env_trackers()
         status = torch.full((self.num_envs,), int(ScenarioStatus.NORMAL), dtype=torch.uint8, device=self.world.device)
         traffic = torch.full((self.num_envs, self.num_participants), int(TrafficStatus.NORMAL), dtype=torch.uint8,
@@ -286,7 +322,7 @@ class BatchedTrafficEnv:
             info = self._info(r.status, a.traffic, r.flags, r.hit_index, r.hit_segment)
             info["agent_status"], info["agent_iou"] = a.status, a.iou
             if self.auto_reset:
-                self.scenario_manager.reset(mask=a.done, pool_index=w.log_row)
+                self._auto_reset(a.done)
             obs = self._obs()
             return obs, a.reward, a.terminated, a.truncated, self._add_lidar(info)
         status, traffic = self.scenario_manager.check_status()
@@ -296,9 +332,17 @@ class BatchedTrafficEnv:
         if r.iou is not None:
             info["iou"] = r.iou
         if self.auto_reset:
-            self.scenario_manager.reset(mask=e.done, pool_index=w.log_row)   # (a log: restart the scenario's row)
+            self._auto_reset(e.done)
         obs = self._obs()
         return obs, e.reward, e.terminated, e.truncated, self._add_lidar(info)
+
+    def _auto_reset(self, done):
+        """The masked reset of the finished scenarios: a new draw with a sampler, else the scenario's row again (with a
+        log: its episode row)."""
+        if self.sampler is not None:
+            self.scenario_manager.reset(mask=done, sample=True)
+        else:
+            self.scenario_manager.reset(mask=done, pool_index=self.world.log_row)
 
     def render(self):
         raise NotImplementedError("rendering is outside this hot path")

@@ -89,14 +89,21 @@ class BatchedScenarioManager(ScenarioManager):
     def render(self):
         raise NotImplementedError("rendering is outside this hot path (SURVEY.md section 2, row 13)")
 
-    def reset(self, mask=None, pool_index=None):
-        """Masked reset (all scenarios when ``mask`` is None) from the initial-state pool."""
+    def reset(self, mask=None, pool_index=None, sample=False):
+        """Masked reset (all scenarios when ``mask`` is None) from the initial-state pool.  ``sample``: draw the episodes
+        through the world's reset sampler (``BatchedWorld.reset_sampled``: the rows come from its seeded stream, so
+        ``pool_index`` is not taken)."""
         import torch
 
         if self._initial is None:
             raise RuntimeError("call set_initial_state(pool) before reset()")
+        if sample and pool_index is not None:
+            raise ValueError("a sampled reset draws its rows: pool_index is not taken")
         if mask is None:
             mask = torch.ones(self.world.N, dtype=torch.uint8, device=self.world.device)
             self.cnt_step = 0
-        self.world.reset(mask, self._initial, pool_index)
+        if sample:
+            self.world.reset_sampled(mask, self._initial)
+        else:
+            self.world.reset(mask, self._initial, pool_index)
         self._last = None

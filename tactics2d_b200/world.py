@@ -166,7 +166,7 @@ class BatchedWorld:
         self.bounds = None
         self.paths = None
         # what the setters bind (None until they are called) and the output buffers made on first use
-        self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = None
+        self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = self._sampler = None
         self._route_out = {}
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
         self._agent_lidar, self._obs_out, self._agent_obs_out = {}, {}, {}
@@ -995,32 +995,142 @@ class BatchedWorld:
                                                _ptr(obs.agent_index), _ptr(obs.segment_index), self._stream()))
         return obs
 
-    def reset(self, mask: torch.Tensor, pool: dict, pool_index: Optional[torch.Tensor] = None):
-        """Re-initialise the scenarios with ``mask[n] != 0`` from row ``pool_index[n]`` (default n)
-        of the pool arrays ``x, y, heading, speed[, vx, vy]`` [P, M] (``ScenarioManager.reset``,
-        parking.py:397-441; ``ParticipantBase.reset``, participant_base.py:236-246)."""
-        px = pool["x"]
-        n_pool = px.shape[0]
+    def _reset_args(self, mask, pool):
+        """The checks ``reset`` and ``reset_sampled`` share: the pool columns (fp32 [P, M] on the device, vx / vy and the
+        wheel columns in pairs) and the mask; returns (mask as a uint8 [N] device tensor, P)."""
+        n_pool = pool["x"].shape[0]
         cols = ["x", "y", "heading", "speed"] + [k for k in ("vx", "vy", "omega_wf", "omega_wr") if pool.get(k) is not None]
         for k in cols:
             self._device_tensor(f"pool[{k!r}]", pool[k], torch.float32, (n_pool, self.M))
         if (pool.get("vx") is None) != (pool.get("vy") is None):
             raise ValueError("give both pool['vx'] and pool['vy'], or neither")
+        if self.omega_front is not None and (pool.get("omega_wf") is None) != (pool.get("omega_wr") is None):
+            raise ValueError("give both pool['omega_wf'] and pool['omega_wr'], or neither")
         # mask / pool_index reach the kernel as raw pointers: a wrong length would be an illegal address
         if not torch.is_tensor(mask) or mask.numel() != self.N:
             raise ValueError(f"mask must be a tensor of {self.N} scenarios")
-        mask = self._to_device(mask, torch.uint8, (self.N,))
+        return self._to_device(mask, torch.uint8, (self.N,)), n_pool
+
+    def _bind_wheel_pool(self, pool):
+        if self.omega_front is not None:
+            _lib.check(self.lib.t2d_bind_reset_wheel_pool(self._ctx, _ptr(pool.get("omega_wf")), _ptr(pool.get("omega_wr"))))
+
+    def reset(self, mask: torch.Tensor, pool: dict, pool_index: Optional[torch.Tensor] = None):
+        """Re-initialise the scenarios with ``mask[n] != 0`` from row ``pool_index[n]`` (default n)
+        of the pool arrays ``x, y, heading, speed[, vx, vy]`` [P, M] (``ScenarioManager.reset``,
+        parking.py:397-441; ``ParticipantBase.reset``, participant_base.py:236-246)."""
+        mask, n_pool = self._reset_args(mask, pool)
         if pool_index is not None:
             if not torch.is_tensor(pool_index) or pool_index.numel() != self.N:
                 raise ValueError(f"pool_index must be a tensor of {self.N} scenarios")
             pool_index = self._to_device(pool_index, torch.int32, (self.N,))
         if pool_index is None and n_pool < self.N:
             raise ValueError("without pool_index the pool needs one row per scenario")
-        if self.omega_front is not None:
-            wf, wr = pool.get("omega_wf"), pool.get("omega_wr")
-            if (wf is None) != (wr is None):
-                raise ValueError("give both pool['omega_wf'] and pool['omega_wr'], or neither")
-            _lib.check(self.lib.t2d_bind_reset_wheel_pool(self._ctx, _ptr(wf), _ptr(wr)))
+        self._bind_wheel_pool(pool)
         _lib.check(self.lib.t2d_reset(self._ctx, _ptr(mask), _ptr(pool_index), n_pool, _ptr(pool["x"]), _ptr(pool["y"]),
                                       _ptr(pool["heading"]), _ptr(pool["speed"]), _ptr(pool.get("vx")),
                                       _ptr(pool.get("vy")), self._stream()))
+
+    # ------------------------------------------------------------------ sampled resets
+    def set_reset_sampler(self, seed: Optional[int], jitter=None, tries: int = 8, sample_rows: bool = True,
+                          avoid_target: bool = False, type_id=None, target=None, tile_id=None, route_id=None):
+        """Draw every episode that ``reset_sampled`` starts (``t2d_set_reset_sampler``; DESIGN.md section 1 "Sampled
+        resets"; envs/parking.py:397-441, generate_parking_lot.py:231-237).  ``seed`` keys a Philox4x32-10 stream (None
+        unbinds); with ``sample_rows`` each reset scenario runs a pool row drawn from it, else its own row n.
+        ``jitter`` [M, 4, 2]: the (lo, hi) of dx, dy, dheading, dspeed per slot (a slot of zeros is not moved); up to
+        ``tries`` (1..32) drawn start states per slot are checked in slot order with the tick's predicates, and the first
+        one that is inside the bounds and meets no map object, no other slot (and, for the ego with ``avoid_target``, not
+        the ``set_goal`` target) is taken.  The optional row pools follow the drawn row: ``type_id`` [P, M] into the
+        world's type ids, ``target`` [P, 5] into the ``set_goal`` target, ``tile_id`` [P] into the map table's tile ids,
+        ``route_id`` [P, M] into ``set_routes``' route ids.  Binding zeroes :attr:`episode_count`."""
+        if seed is None:
+            _lib.check(self.lib.t2d_set_reset_sampler(self._ctx, None))
+            self._sampler = None
+            return
+        tries = int(tries)
+        if not 1 <= tries <= 32:
+            raise ValueError("tries must be in 1..32")
+        jit = None
+        if jitter is not None:
+            jit = np.ascontiguousarray(np.asarray(jitter, dtype=np.float32))
+            if jit.shape != (self.M, 4, 2):
+                raise ValueError(f"jitter must be [{self.M}, 4, 2] (lo, hi) ranges")
+            if not (np.isfinite(jit).all() and (jit[..., 0] <= jit[..., 1]).all()):
+                raise ValueError("every jitter range must be finite with lo <= hi")
+        rows = {}
+        for name, a, dtype, tail in (("type_id", type_id, torch.uint8, (self.M,)), ("target", target, torch.float32, (5,)),
+                                     ("tile_id", tile_id, torch.int16, ()), ("route_id", route_id, torch.int16, (self.M,))):
+            if a is None:
+                continue
+            t = a if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))
+            if t.dim() != 1 + len(tail) or tuple(t.shape[1:]) != tail or t.shape[0] < 1:
+                raise ValueError(f"the {name} pool must be [P{''.join(', ' + str(d) for d in tail)}]")
+            rows[name] = self._to_device(t, dtype, tuple(t.shape))
+        n_rows = {t.shape[0] for t in rows.values()}
+        if len(n_rows) > 1:
+            raise ValueError("the row pools must have the same number of rows")
+        if "type_id" in rows:
+            tv = rows["type_id"]
+            if bool(((tv >= len(self.type_table)) & (tv != TYPE_INACTIVE)).any()):
+                raise ValueError("the type_id pool holds ids outside the type table")
+        if "target" in rows and self._goal is None:
+            raise ValueError("a target pool needs set_goal")
+        if "tile_id" in rows:
+            if self.tiles is None or len(self.tiles) < 2:
+                raise ValueError("a tile_id pool needs a map table of more than one tile")
+            tv = rows["tile_id"].to(torch.int64)
+            tile_max = int(tv.max())
+            if int(tv.min()) < 0 or tile_max >= len(self.tiles):
+                raise ValueError(f"the tile_id pool must index the {len(self.tiles)} tiles")
+        if "route_id" in rows and self._routes is None:
+            raise ValueError("a route_id pool needs set_routes")
+        dev = self.device
+        s = dict(rows=rows, jitter=jit, tile_max=tile_max if "tile_id" in rows else -1,
+                 seed=int(seed) & 0xFFFFFFFFFFFFFFFF, tries=tries, sample_rows=bool(sample_rows),
+                 avoid_target=bool(avoid_target), n_rows=n_rows.pop() if n_rows else 0,
+                 episode=torch.zeros(self.N, dtype=torch.int32, device=dev),
+                 pool_row=torch.arange(self.N, dtype=torch.int32, device=dev),
+                 reset_try=torch.full((self.N, self.M), -1, dtype=torch.int8, device=dev))
+        c = _lib.ResetSamplerC(s["seed"], int(s["sample_rows"]), tries, int(s["avoid_target"]), s["n_rows"],
+                               None if jit is None else jit.ctypes.data, _ptr(rows.get("type_id")),
+                               _ptr(rows.get("target")), _ptr(rows.get("tile_id")), _ptr(rows.get("route_id")),
+                               _ptr(s["episode"]), _ptr(s["pool_row"]), _ptr(s["reset_try"]))
+        # the library keeps the previous sampler until a call succeeds: replace the tensors only then
+        _lib.check(self.lib.t2d_set_reset_sampler(self._ctx, C.byref(c)))
+        self._sampler = s
+
+    def reset_sampled(self, mask: torch.Tensor, pool: dict):
+        """``reset`` of the scenarios with ``mask[n] != 0`` through the bound sampler (``t2d_reset_sampled``): each takes
+        the pool row it draws (:attr:`pool_row`), the row-owned columns follow it, then its start states are jittered
+        (:attr:`reset_try`) and its :attr:`episode_count` advances.  ``pool`` as ``reset``'s."""
+        if self._sampler is None:
+            raise RuntimeError("call set_reset_sampler before reset_sampled")
+        mask, n_pool = self._reset_args(mask, pool)
+        s = self._sampler
+        if s["n_rows"] and n_pool != s["n_rows"]:
+            raise ValueError(f"the pool must have the row pools' {s['n_rows']} rows")
+        if not s["sample_rows"] and n_pool < self.N:
+            raise ValueError("without row draws the pool needs one row per scenario")
+        # the tile pool was checked against the map bound then; a map table rebound since may hold fewer tiles
+        if s["tile_max"] >= 0 and (self.tiles is None or s["tile_max"] >= len(self.tiles)):
+            raise ValueError(f"the tile_id pool names tile {s['tile_max']}, beyond the bound map's tiles")
+        self._bind_wheel_pool(pool)
+        _lib.check(self.lib.t2d_reset_sampled(self._ctx, _ptr(mask), n_pool, _ptr(pool["x"]), _ptr(pool["y"]),
+                                              _ptr(pool["heading"]), _ptr(pool["speed"]), _ptr(pool.get("vx")),
+                                              _ptr(pool.get("vy")), self._stream()))
+
+    @property
+    def pool_row(self) -> Optional[torch.Tensor]:
+        """int32 [N] device tensor: the pool row every scenario started its episode from (None without a sampler)."""
+        return None if self._sampler is None else self._sampler["pool_row"]
+
+    @property
+    def episode_count(self) -> Optional[torch.Tensor]:
+        """int32 [N] device tensor holding the uint32 episode counters of the sampler (None without one)."""
+        return None if self._sampler is None else self._sampler["episode"]
+
+    @property
+    def reset_try(self) -> Optional[torch.Tensor]:
+        """int8 [N, M] device tensor: the try that placed each slot at the last sampled reset, -1 where the pool state
+        was kept or the slot is not jittered (None without a sampler)."""
+        return None if self._sampler is None else self._sampler["reset_try"]
