@@ -63,6 +63,9 @@
  *                        OffRoute.reset / OffRoute.update   tactics2d/traffic/event_detection/off_route.py:24-51
  *                        (+ a route-progress reward term, an extension)
  *   t2d_route_observe    (no reference counterpart) the route of each observer row in its frame, with look-ahead points
+ *   t2d_set_history      Trajectory.add_state / Trajectory.reset(state) / history_states of every participant slot
+ *                                                         tactics2d/participant/trajectory/trajectory.py:115-149,170-188
+ *   t2d_observe_history  (no reference counterpart) the recent past of an observer and its agents in its current frame
  *
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types cross the ABI;
@@ -551,6 +554,50 @@ int t2d_bind_route_trackers(t2d_ctx* ctx, double* s_best, double* agent_s_best, 
  * (T2D_E_INVALID), state or type table not bound (T2D_E_STATE).  One launch, no allocation: capturable in a CUDA graph. */
 int t2d_route_observe(t2d_ctx* ctx, const int16_t* observers, int32_t n_observers, int n_points, float spacing, float* out,
                       void* stream);
+
+/* ---- trajectory history: the recent states of every participant slot, and past poses in an observer's frame ------------
+ * Trajectory.add_state appends every tick's State and Trajectory.reset(state) starts the history again from that state
+ * (participant/trajectory/trajectory.py:115-149,170-188).  The contract is DESIGN.md section 1 "Trajectory history".
+ * t2d_set_history(ctx, H), H in 1..T2D_HISTORY_MAX, allocates the library's ring (N M H 25 bytes, plus 4 bytes per entry
+ * while a log schedule with a track_out is bound) and H = 0 frees it.  A new binding is empty (every count 0).  Rejected
+ * (the previous ring stays bound, entries and all): H outside 0..64 (T2D_E_INVALID), an allocation that fails (T2D_E_CUDA).
+ *   append   t2d_step, t2d_step_host (after its last chunk), t2d_step_host_ego and t2d_step_host_agents (before K10)
+ *            append the post-tick state of every scenario: entry e = count[n] goes to ring index e % H, count[n] + 1;
+ *   restart  t2d_reset and t2d_reset_sampled restart every masked scenario: entry 0 = the state after the whole reset (the
+ *            log replay and the sampled placement included), count = 1; the other scenarios keep their history;
+ *   alone    t2d_set_state-style writes, t2d_check_events and every observation leave the ring untouched;
+ *   valid    entry e of slot m counts for the slot's current occupant iff it is one of the last min(count, H) entries, its
+ *            recorded type id is < n_types and equals the slot's current one, and - with a schedule's track_out bound - its
+ *            recorded track equals the slot's current track_out value.  Binding a log drops the recorded tracks (they
+ *            read -1 afterwards: not replayed).
+ * With no ring bound nothing of this launches. */
+#define T2D_HISTORY_MAX 64
+#define T2D_HISTORY_FIELDS 7 /* valid, ex, ey, cos dh, sin dh, v_x, v_y */
+int t2d_set_history(t2d_ctx* ctx, int32_t length);
+/* K16: for every observer row, its own past (block 0) and the past of K agent slots (block 1 + k), lag 0 (the newest entry)
+ * first, T2D_HISTORY_FIELDS values per lag in the observer's CURRENT frame, with the arithmetic of t2d_observe's agent rows
+ * applied to the recorded pose and velocity.  n_observers == 0 (observers NULL): one row per scenario, observed by slot 0
+ * (t2d_observe's rows); n_observers = Q in 1..T2D_OBS_MAX_OBSERVERS: the rows of observers DEVICE int16 [N][Q], or NULL for
+ * slot q in row q (Q <= M), as t2d_observe_agents.  agent_index: DEVICE int16 [rows][k_agents] as t2d_observe /
+ * t2d_observe_agents return it (-1: none), k_agents in 0..T2D_OBS_MAX_AGENTS, NULL when k_agents == 0.  out: DEVICE fp32
+ * [rows][1 + k_agents][H][T2D_HISTORY_FIELDS] (64-bit offsets).  An observer outside [0, M) or whose slot is empty gives a
+ * zero row; an agent slot outside [0, M) and an entry that is not valid give zero lags.  When the newest entry is the
+ * current state, block 1 + k at lag 0, fields 1..6, equals fields 1..6 of t2d_observe's agent row k bit for bit.
+ * Rejected without a launch: n_observers outside 0..128, observers with n_observers == 0, observers == NULL with
+ * n_observers > M, k_agents outside 0..127, agent_index NULL with k_agents > 0, out NULL (T2D_E_INVALID), state or type table
+ * not bound, no ring bound (T2D_E_STATE).  One launch, no allocation, no synchronisation: capturable in a CUDA graph. */
+int t2d_observe_history(t2d_ctx* ctx, const int16_t* observers, int32_t n_observers, const int16_t* agent_index,
+                        int32_t k_agents, float* out, void* stream);
+/* The bound ring's DEVICE arrays, for read-back utilities and tests (length 0 and NULL pointers without a ring).  They belong
+ * to the library and live until the next t2d_set_history or t2d_destroy; track is NULL unless tracks are recorded. */
+typedef struct t2d_history_ring {
+  int32_t length;                                 /* H */
+  float *x, *y, *heading, *speed, *vx, *vy;       /* [N][H][M] */
+  uint8_t* type_id;                               /* [N][H][M] */
+  int32_t* track;                                 /* [N][H][M] or NULL */
+  int64_t* count;                                 /* [N] entries since the scenario's episode began */
+} t2d_history_ring;
+int t2d_history_view(t2d_ctx* ctx, t2d_history_ring* out);
 
 /* Overwrites action[n][m] = (accel, steer) ((steer, accel) with T2D_CFG_STEER_FIRST) of every controlled participant from
  * the bound state, then stores |applied acceleration| of the WHOLE action buffer in last_accel (bicycles: the accel clipped

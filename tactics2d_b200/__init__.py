@@ -14,5 +14,5 @@ from .types import (  # noqa: F401
     MODEL_DYNAMICS, MODEL_KINEMATICS, MODEL_POINTMASS_EULER, MODEL_POINTMASS_NEWTON, MODEL_STATIC,
     SHAPE_CIRCLE, SHAPE_NONE, SHAPE_OBB, TYPE_INACTIVE, TypeParams, TypeTable)
 from .world import (  # noqa: F401
-    AGENT_FIELDS, EGO_FIELDS, GOAL_FIELDS, SEGMENT_FIELDS, AgentEnvResult, AgentObservation, BatchedWorld, StepResult,
+    AGENT_FIELDS, EGO_FIELDS, GOAL_FIELDS, HIST_FIELDS, SEGMENT_FIELDS, AgentEnvResult, AgentObservation, BatchedWorld, StepResult,
     VectorObservation, vector_obs_width)

@@ -72,6 +72,12 @@ class ObsConfigC(C.Structure):
     _fields_ = [("k_agents", C.c_int32), ("k_segments", C.c_int32), ("agent_range", C.c_float), ("segment_range", C.c_float)]
 
 
+class HistoryRingC(C.Structure):
+    """``t2d_history_ring``: the device arrays of the bound trajectory-history ring."""
+    _fields_ = [("length", C.c_int32)] + [(n, C.c_void_p) for n in (
+        "x", "y", "heading", "speed", "vx", "vy", "type_id", "track", "count")]
+
+
 # name -> (restype, argtypes); every symbol include/t2d_b200.h declares
 _P = C.c_void_p
 SYMBOLS = {
@@ -112,6 +118,9 @@ SYMBOLS = {
     "t2d_set_routes": (C.c_int, [_P, _P, C.c_double, C.c_double, C.c_float]),
     "t2d_bind_route_trackers": (C.c_int, [_P, _P, _P, C.c_int32]),
     "t2d_route_observe": (C.c_int, [_P, _P, C.c_int32, C.c_int, C.c_float, _P, _P]),
+    "t2d_set_history": (C.c_int, [_P, C.c_int32]),
+    "t2d_observe_history": (C.c_int, [_P, _P, C.c_int32, _P, C.c_int32, _P, _P]),
+    "t2d_history_view": (C.c_int, [_P, C.POINTER(HistoryRingC)]),
     "t2d_exchange_create": (C.c_int, [C.POINTER(_P), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "t2d_exchange_connect": (C.c_int, [_P, _P]),
     "t2d_exchange_allgather": (C.c_int, [_P, _P, _P, _P]),

@@ -16,6 +16,8 @@
 // K12 t2d_route_obs_kernel       the route of every observer row in its frame, with look-ahead points.
 // K13 t2d_episode_draw_kernel    sampled resets: the seeded pool-row draw and the row-owned columns.
 // K14 t2d_episode_place_kernel   sampled resets: collision-checked jitter of the start states, one warp per scenario.
+// K15 t2d_history_append_kernel  trajectory history: append the state after a tick, restart it after a reset (t2d_history.cuh).
+// K16 t2d_history_obs_kernel     trajectory history: past poses of an observer and its agents in its current frame.
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory.
 //
 // Work decomposition of K1: a scenario (M <= 128 participants) is owned by a group of G lanes of
@@ -2578,6 +2580,7 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
 
 #include "t2d_bev.cuh"
 #include "t2d_obs.cuh"
+#include "t2d_history.cuh"
 
 // =============================================================================================
 // C ABI
@@ -2691,6 +2694,16 @@ struct DeviceSampler {
   dev_ptr<float> jitter;               // [M][8]
 };
 
+// The trajectory history ring (t2d_set_history), replaced as a whole; the track ring exists exactly while a log schedule
+// with a track output is bound (history_tracks)
+struct DeviceHistory {
+  int H = 0;
+  dev_ptr<float> f;                    // [6][N][H][M]: x, y, heading, speed, vx, vy
+  dev_ptr<uint8_t> type;               // [N][H][M]
+  dev_ptr<int32_t> track;              // [N][H][M] or nullptr
+  dev_ptr<long long> count;            // [N]
+};
+
 // Staging of the host steps (t2d_step_host, t2d_step_host_ego, t2d_step_host_agents); every piece is created whole the
 // first time a step needs it.
 static constexpr int MAX_HOST_CHUNKS = 8;
@@ -2793,6 +2806,7 @@ struct t2d_ctx {
   std::vector<int> type_model;         // host copy of the current type table's model ids
   dev_ptr<uint8_t> order;              // [N][64] x-order hint of K1's FIXED instance (t2d_create: the identity)
   std::unique_ptr<DeviceSampler> sampler;   // t2d_set_reset_sampler; nullptr: none bound
+  std::unique_ptr<DeviceHistory> hist;      // t2d_set_history; nullptr: none bound
 };
 
 enum : unsigned { NEED_STATE = 1, NEED_TABLE = 2, NEED_TICK = 4 };
@@ -2828,6 +2842,32 @@ static int check_route_trackers(const t2d_ctx* c, const char* fn) {
   return T2D_OK;
 }
 
+// ---- trajectory history (t2d_set_history; K15 / K16)
+static hist::Ring history_ring(const t2d_ctx* c) {
+  const DeviceHistory& g = *c->hist;
+  const size_t plane = (size_t)c->N * g.H * c->M;
+  float* f = g.f.get();
+  return {f, f + plane, f + 2 * plane, f + 3 * plane, f + 4 * plane, f + 5 * plane, g.type.get(), g.track.get(), g.count.get(), g.H};
+}
+
+// the track every slot shows now, when the ring records tracks
+static const int32_t* history_track_now(const t2d_ctx* c) { return c->hist->track ? c->log->track_out : nullptr; }
+
+// Gives `g` a fresh track ring filled with -1 (an entry recorded before the schedule counts as showing no track) when
+// `track_out`, the bound schedule's track output, is set, and drops it otherwise
+static int history_tracks(const t2d_ctx* c, DeviceHistory& g, const int32_t* track_out) {
+  if (!track_out) {
+    g.track.reset();
+    return T2D_OK;
+  }
+  const size_t n = (size_t)c->N * g.H * c->M;
+  dev_ptr<int32_t> t;
+  if (int r = dev_alloc(t, n)) return r;
+  CUDA_TRY(cudaMemset(t.get(), 0xff, n * sizeof(int32_t)));
+  g.track = std::move(t);
+  return T2D_OK;
+}
+
 // from scenario `first` on (t2d_set_map_table keeps tile_id only with more than one tile)
 static MapArgs map_args(const DeviceMap& map, int first = 0) {
   return {map.blob.get(), map.tile_off.get(), map.tile_id ? map.tile_id + first : nullptr};
@@ -2843,6 +2883,15 @@ static int launched() {
 // grid of a grid-stride kernel: one CTA per `per_cta` items, at most `per_sm` CTAs per SM
 static int capped_grid(long long items, int per_cta, int sm_count, int per_sm) {
   return (int)std::max(1LL, std::min((items + per_cta - 1) / per_cta, (long long)sm_count * per_sm));
+}
+
+// K15 after a tick (mask == nullptr: every scenario appends) or a reset (the masked scenarios restart); no ring, no launch
+static int launch_history(t2d_ctx* c, const uint8_t* mask, void* stream) {
+  if (!c->hist) return T2D_OK;
+  hist::AppendArgs A{world_args(c)};
+  A.ring = history_ring(c); A.track_now = history_track_now(c); A.mask = mask;
+  hist::t2d_history_append_kernel<<<(c->N + hist::K15_WARPS - 1) / hist::K15_WARPS, hist::K15_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  return launched();
 }
 
 // the integration steps of one interval, for the tick and t2d_physics_step
@@ -3389,6 +3438,12 @@ static int set_log(t2d_ctx* c, const t2d_log* L, const char* who, const int32_t*
   g->track_type_host.assign(L->type_row, L->type_row + K);
   g->n_tracks = K; g->n_rows = L->n_rows;
   g->row = L->log_row; g->type_id = L->type_id; g->track_out = track_out;
+  if (c->hist) {   // the ring's tracks restart with the log (a rejected call keeps both as they were)
+    DeviceHistory tracks;
+    tracks.H = c->hist->H;
+    if (int r = history_tracks(c, tracks, track_out)) return r;
+    c->hist->track = std::move(tracks.track);
+  }
   c->log = std::move(g);
   return T2D_OK;
 }
@@ -3398,6 +3453,7 @@ int t2d_set_log(t2d_ctx* c, const t2d_log* L) {
   if (!L) {
     CUDA_TRY(cudaSetDevice(c->device));
     c->log.reset();
+    if (c->hist) c->hist->track.reset();
     return T2D_OK;
   }
   return set_log(c, L, "t2d_set_log", nullptr, nullptr, 0, nullptr);
@@ -3649,7 +3705,9 @@ int t2d_set_goal(t2d_ctx* c, const float* target, float arrival_threshold, int n
 
 int t2d_step(t2d_ctx* c, const float* action, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment, uint8_t* scn_status,
              uint8_t* done, void* stream) {
-  return launch_step(c, action, c ? c->ego_action : nullptr, flags, hit_index, hit_segment, scn_status, done, stream, 1);
+  if (int r = launch_step(c, action, c ? c->ego_action : nullptr, flags, hit_index, hit_segment, scn_status, done, stream, 1))
+    return r;
+  return launch_history(c, nullptr, stream);
 }
 
 int t2d_step_host(t2d_ctx* c, const float* action_host, uint8_t* flags, int16_t* hit_index, int16_t* hit_segment,
@@ -3698,6 +3756,7 @@ int t2d_step_host(t2d_ctx* c, const float* action_host, uint8_t* flags, int16_t*
                             hit_segment ? hit_segment + p0 : nullptr, out + first, out + N + first, stream, 1, first, count))
       return r;
   }
+  if (int r = launch_history(c, nullptr, stream)) return r;   // after the last chunk
   return read_back(c->hs_out, 2 * (size_t)N, s, {{scn_status_host, 0, (size_t)N}, {done_host, (size_t)N, (size_t)N}});
 }
 
@@ -3744,6 +3803,7 @@ int t2d_step_host_ego(t2d_ctx* c, const float* ego_action_host, float* action, u
   }
   uint8_t* out = c->hs_out.dev.get();
   if (int r = launch_step(c, action, ego, flags, hit_index, hit_segment, out, out + N, stream, 1)) return r;
+  if (int r = launch_history(c, nullptr, stream)) return r;
   return read_back(c->hs_out, 2 * (size_t)N, (cudaStream_t)stream,
                    {{scn_status_host, 0, (size_t)N}, {done_host, (size_t)N, (size_t)N}});
 }
@@ -3874,6 +3934,7 @@ int t2d_step_host_agents(t2d_ctx* c, const float* agent_action_host, float* acti
   if (c->d_ctab)
     if (int r = launch_control(c, action, c->ego_action, stream)) return r;
   if (int r = launch_step(c, action, c->ego_action, fl, hit_index, hit_segment, nullptr, nullptr, stream, 1)) return r;
+  if (int r = launch_history(c, nullptr, stream)) return r;   // the post-tick state, before K10 retires slots
   if (int r = t2d_agents_epilogue(c, fl, d_reward, d_term, d_trunc, d_status, d_iou, d_done, max_iou, min_dist, nullptr,
                                   reset_trackers_on_done, stream))
     return r;
@@ -3898,9 +3959,10 @@ static int check_reset(t2d_ctx* c, const uint8_t* mask, int n_pool, const float*
   return T2D_OK;
 }
 
-int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x, const float* pool_y,
-              const float* pool_heading, const float* pool_speed, const float* pool_vx, const float* pool_vy, void* stream) {
-  if (int r = check_reset(c, mask, n_pool, pool_x, pool_y, pool_heading, pool_speed)) return r;
+// K2 (and K7) of t2d_reset, after check_reset; t2d_reset_sampled runs it between K13 and K14
+static int launch_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x,
+                        const float* pool_y, const float* pool_heading, const float* pool_speed, const float* pool_vx,
+                        const float* pool_vy, void* stream) {
   CUDA_TRY(cudaSetDevice(c->device));
   ResetArgs A{world_args(c)};
   A.mask = mask; A.pool_index = pool_index;
@@ -3916,6 +3978,14 @@ int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_
   if (int r = launched()) return r;
   if (c->log) return launch_replay(c, stream, 0, c->N, 0, mask, pool_index);   // the new episode's traffic at t0
   return T2D_OK;
+}
+
+int t2d_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_index, int n_pool, const float* pool_x, const float* pool_y,
+              const float* pool_heading, const float* pool_speed, const float* pool_vx, const float* pool_vy, void* stream) {
+  if (int r = check_reset(c, mask, n_pool, pool_x, pool_y, pool_heading, pool_speed)) return r;
+  if (int r = launch_reset(c, mask, pool_index, n_pool, pool_x, pool_y, pool_heading, pool_speed, pool_vx, pool_vy, stream))
+    return r;
+  return launch_history(c, mask, stream);   // entry 0 of the new episode: the state after the whole reset
 }
 
 // A row-owned pool needs what it writes into: checked when the sampler is bound and before every sampled reset (the
@@ -3981,14 +4051,16 @@ int t2d_reset_sampled(t2d_ctx* c, const uint8_t* mask, int n_pool, const float* 
   D.pool_route = s.pool_route_id; D.route_id = const_cast<int16_t*>(c->route_id);
   t2d_episode_draw_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(D);
   if (int r = launched()) return r;
-  if (int r = t2d_reset(c, mask, s.pool_row, n_pool, pool_x, pool_y, pool_heading, pool_speed, pool_vx, pool_vy, stream)) return r;
+  if (int r = launch_reset(c, mask, s.pool_row, n_pool, pool_x, pool_y, pool_heading, pool_speed, pool_vx, pool_vy, stream))
+    return r;
   PlaceArgs P{world_args(c)};
   P.mask = mask; P.episode = s.episode; P.reset_try = s.reset_try; P.seed = s.seed;
   P.jitter = s.jitter; P.tries = s.tries; P.avoid_target = s.avoid_target; P.target = c->goal.target;
   P.map = map_args(c->map); P.mh = c->map.mh; P.has_bounds = c->map.has_bounds ? 1 : 0;
   P.wheel_f = c->wheel_f; P.wheel_r = c->wheel_r; P.pool_wheels = c->reset_pool_wf != nullptr;
   t2d_episode_place_kernel<<<(unsigned)((c->N + K14_WARPS - 1) / K14_WARPS), K14_WARPS * 32, 0, (cudaStream_t)stream>>>(P);
-  return launched();
+  if (int r = launched()) return r;
+  return launch_history(c, mask, stream);   // entry 0 of the new episode: the placed state
 }
 
 // K4 over the rows of an observer list (observers == nullptr: row q is slot q); the callers have checked their arguments
@@ -4154,6 +4226,63 @@ int t2d_observe_agents(t2d_ctx* c, const t2d_obs_config* cfg, const int16_t* obs
   const long long rows = (long long)c->N * n_observers;
   const int grid = (int)std::min<long long>((rows + obs::WARPS - 1) / obs::WARPS, 1ll << 30);   // the kernel strides past 2^32 rows
   obs::t2d_obs_agents_kernel<<<grid, obs::WARPS * 32, 0, (cudaStream_t)stream>>>(G);
+  return launched();
+}
+
+int t2d_set_history(t2d_ctx* c, int32_t length) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (length < 0 || length > T2D_HISTORY_MAX) return fail(T2D_E_INVALID, "t2d_set_history: length must be in 0..64");
+  CUDA_TRY(cudaSetDevice(c->device));
+  if (length == 0) {
+    c->hist.reset();
+    return T2D_OK;
+  }
+  static_assert(T2D_HISTORY_MAX == hist::MAX_H && T2D_HISTORY_FIELDS == hist::HIST_F, "K16's stage holds the ABI's limits");
+  auto g = std::make_unique<DeviceHistory>();
+  g->H = length;
+  const size_t plane = (size_t)c->N * length * c->M;
+  if (int r = dev_alloc(g->f, 6 * plane)) return r;
+  if (int r = dev_alloc(g->type, plane)) return r;
+  if (int r = dev_alloc(g->count, (size_t)c->N)) return r;
+  CUDA_TRY(cudaMemset(g->f.get(), 0, 6 * plane * sizeof(float)));
+  CUDA_TRY(cudaMemset(g->type.get(), 0xff, plane));
+  CUDA_TRY(cudaMemset(g->count.get(), 0, (size_t)c->N * sizeof(long long)));
+  if (int r = history_tracks(c, *g, c->log ? c->log->track_out : nullptr)) return r;
+  c->hist = std::move(g);
+  return T2D_OK;
+}
+
+int t2d_history_view(t2d_ctx* c, t2d_history_ring* out) {
+  if (!c || !out) return fail(T2D_E_INVALID, "t2d_history_view: ctx / out is NULL");
+  *out = t2d_history_ring{};
+  if (!c->hist) return T2D_OK;
+  const hist::Ring R = history_ring(c);
+  out->length = R.H;
+  out->x = R.x; out->y = R.y; out->heading = R.h; out->speed = R.v; out->vx = R.vx; out->vy = R.vy;
+  out->type_id = R.type; out->track = R.track; out->count = reinterpret_cast<int64_t*>(R.count);
+  return T2D_OK;
+}
+
+int t2d_observe_history(t2d_ctx* c, const int16_t* observers, int32_t n_observers, const int16_t* agent_index, int32_t k_agents,
+                        float* out, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (n_observers < 0 || n_observers > T2D_OBS_MAX_OBSERVERS)
+    return fail(T2D_E_INVALID, "t2d_observe_history: n_observers must be in 0..128");
+  if (n_observers == 0 && observers) return fail(T2D_E_INVALID, "t2d_observe_history: an observer list needs n_observers >= 1");
+  if (!observers && n_observers > c->M)
+    return fail(T2D_E_INVALID, "t2d_observe_history: without an observer list n_observers must not exceed the slots per scenario");
+  if (k_agents < 0 || k_agents > T2D_OBS_MAX_AGENTS) return fail(T2D_E_INVALID, "t2d_observe_history: k_agents must be in 0..127");
+  if (k_agents > 0 && !agent_index) return fail(T2D_E_INVALID, "t2d_observe_history: agent_index is NULL");
+  if (!out) return fail(T2D_E_INVALID, "t2d_observe_history: out is NULL");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (!c->hist) return fail(T2D_E_STATE, "t2d_observe_history: no history bound: call t2d_set_history first");
+  CUDA_TRY(cudaSetDevice(c->device));
+  hist::ObsArgs A{world_args(c)};
+  A.ring = history_ring(c); A.track_now = history_track_now(c);
+  A.observers = observers; A.Q = n_observers; A.agent_index = agent_index; A.K = k_agents; A.out = out;
+  const long long rows = (long long)c->N * std::max(1, n_observers);
+  const int grid = (int)std::min<long long>((rows + hist::K16_WARPS - 1) / hist::K16_WARPS, 1ll << 30);   // the kernel strides
+  hist::t2d_history_obs_kernel<<<grid, hist::K16_WARPS * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
 }
 

@@ -87,6 +87,26 @@ struct Frame {   // the ego: origin and (cos, sin) of its heading
   __device__ __forceinline__ double ey(double dx, double dy) const { return dadd(dmul(-s, dx), dmul(c, dy)); }
 };
 
+// Fields 1..6 of an agent row - ex, ey, cos dh, sin dh, v_x, v_y - of the participant at index p of the arrays (x, y, h, vx,
+// vy), in the frame f of an observer whose heading is h0: frame_vals computes them in fp64 ((dx, dy) is the participant's
+// offset from the observer's centre), frame_put rounds them into o[0..5].  K8 / K9's agent rows and K16's history rows
+// (t2d_history.cuh) both run them, so a history row of the current state is an agent row bit for bit.
+struct FrameVals {
+  double dx, dy, vx, vy, sd, cd;
+};
+__device__ __forceinline__ FrameVals frame_vals(const Frame& f, double h0, const float* x, const float* y, const float* h,
+                                                const float* vx, const float* vy, long long p) {
+  FrameVals r;
+  r.dx = dsub(x[p], f.x0); r.dy = dsub(y[p], f.y0);
+  r.vx = vx[p]; r.vy = vy[p];
+  sincos_angle(dsub(h[p], h0), &r.sd, &r.cd);
+  return r;
+}
+__device__ __forceinline__ void frame_put(const Frame& f, const FrameVals& r, float* o) {
+  o[0] = f32(f.ex(r.dx, r.dy)); o[1] = f32(f.ey(r.dx, r.dy)); o[2] = f32(r.cd); o[3] = f32(r.sd);
+  o[4] = f32(f.ex(r.vx, r.vy)); o[5] = f32(f.ey(r.vx, r.vy));
+}
+
 __device__ __forceinline__ void extents(const Params& p, float& hl, float& hw, float& disc) {
   const int sh = p.shape();
   if (sh == SHAPE_CIRCLE) { hl = hw = p.radius; disc = 1.0f; }
@@ -278,15 +298,12 @@ __device__ __forceinline__ void observe_row(const Args& A, Smem& sm, int lane, l
     if (r < na) {
       j = sm.asel[r];
       const long long pj = base + j;
-      const double dx = dsub(A.x[pj], f.x0), dy = dsub(A.y[pj], f.y0);
-      const double vx = A.vx[pj], vy = A.vy[pj];
-      double sd, cd;
-      sincos_angle(dsub(A.h[pj], h0), &sd, &cd);
+      const FrameVals fv = frame_vals(f, h0, A.x, A.y, A.h, A.vx, A.vy, pj);
       float hl, hw, disc;
       extents(A.table[A.type_id[pj]], hl, hw, disc);
-      o[0] = 1.0f; o[1] = f32(f.ex(dx, dy)); o[2] = f32(f.ey(dx, dy)); o[3] = f32(cd); o[4] = f32(sd);
-      o[5] = f32(f.ex(vx, vy)); o[6] = f32(f.ey(vx, vy)); o[7] = hl; o[8] = hw; o[9] = disc;
-      o[10] = f32(__dsqrt_rn(dadd(dmul(dx, dx), dmul(dy, dy))));
+      o[0] = 1.0f; frame_put(f, fv, o + 1);
+      o[7] = hl; o[8] = hw; o[9] = disc;
+      o[10] = f32(__dsqrt_rn(dadd(dmul(fv.dx, fv.dx), dmul(fv.dy, fv.dy))));
     } else if (r < K) {
       for (int k = 0; k < AGENT_F; ++k) o[k] = 0.0f;
     }

@@ -50,7 +50,7 @@ class BatchedTrafficEnv:
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
                  agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
-                 route: Optional[dict] = None, sampler: Optional[dict] = None):
+                 route: Optional[dict] = None, sampler: Optional[dict] = None, history: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -94,7 +94,13 @@ class BatchedTrafficEnv:
         ranges) where the move is collision-free; the row's types, ``target`` and routes follow it.  ``reset(seed=s)``
         re-keys the stream and restarts the episode counters, ``reset()`` keeps drawing; ``info["pool_row"]`` is the row
         each scenario runs after the step's auto-reset.  A shuffle is then rejected, as are jitter on the replayed slots
-        (with ``replay``, only slot 0 may move) and per-row goals with ``sample_rows`` (they belong to scenarios, not rows)."""
+        (with ``replay``, only slot 0 may move) and per-row goals with ``sample_rows`` (they belong to scenarios, not rows);
+        ``history``: e.g. ``dict(length=16)`` keeps the last ``length`` states of every slot on the device
+        (``BatchedWorld.set_history``; DESIGN.md section 1 "Trajectory history") and adds ``info["history"]`` to ``reset``
+        and ``step``, computed after the auto-reset like the observation (``BatchedWorld.observe_history``): with
+        ``observation="vector"`` the ego's past and that of the agents of its observation (``[N, 1 + K, H, 7]``), with
+        ``"agents"`` every observer row's and its agents' (``[N, Q, 1 + K, H, 7]``), else the ego's own past
+        (``[N, 1, H, 7]``).  A scenario that auto-reset shows one valid entry per present slot, its new start state."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -139,6 +145,13 @@ class BatchedTrafficEnv:
                 raise ValueError("sampler: with replay only slot 0 may have jitter (the log drives the others)")
             if agent_rewards and self.vector_obs.get("goals") is not None and self.sampler.get("sample_rows", True):
                 raise ValueError("sampler: per-row goals belong to scenarios, not pool rows: use sample_rows=False")
+        self.history = None if history is None else dict(history)
+        if self.history is not None:
+            unknown = set(self.history) - {"length"}
+            if unknown:
+                raise ValueError(f"history: unknown keys {sorted(unknown)}")
+            if "length" not in self.history:
+                raise ValueError("history: missing key 'length'")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -187,6 +200,9 @@ class BatchedTrafficEnv:
         self._target_pool = None if target is None else self.world._goal["target"].clone()
         if self.sampler is not None:
             self._bind_sampler(self.sampler.get("seed", 0))
+        if self.history is not None:
+            self.world.set_history(self.history["length"])
+        self._last_obs = None
         if observation == "bev":
             w, h = self.bev_resolution
             self.observation_space = {"shape": (n, h, w, 3), "dtype": "uint8", "low": 0, "high": 255}
@@ -214,9 +230,11 @@ class BatchedTrafficEnv:
         if self.observation == "bev":
             return self.world.bev(self.bev_resolution, self.bev_range, rgb=True)
         if self.observation == "vector":
-            return self.world.observe(**self.vector_obs).flat
+            self._last_obs = self.world.observe(**self.vector_obs)
+            return self._last_obs.flat
         if self.observation == "agents":
-            return self.world.observe_agents(**self.vector_obs).flat
+            self._last_obs = self.world.observe_agents(**self.vector_obs)
+            return self._last_obs.flat
         return self.scenario_manager.get_observation()
 
     def _info(self, status, traffic, flags, hit_index, hit_segment):
@@ -229,8 +247,8 @@ class BatchedTrafficEnv:
         return info
 
     def _add_lidar(self, info):
-        """``info["lidar"]`` / ``info["route"]`` when the env has a lidar / routes; called after the auto-reset, so that
-        the scan and the route rows see the new episodes."""
+        """``info["lidar"]`` / ``info["route"]`` / ``info["history"]`` when the env has a lidar / routes / a history; called
+        after the auto-reset and the observation, so that they see the new episodes and the observation's agents."""
         if self.route is not None:
             info["route"] = self.world.route_observe(self.route.get("n_points", 8), self.route.get("spacing", 2.0),
                                                      self._route_observers)
@@ -239,6 +257,13 @@ class BatchedTrafficEnv:
                 info["lidar"] = self.world.lidar_scan_agents(**self.lidar, observers=self.vector_obs.get("observers"))
             else:
                 info["lidar"] = self.world.lidar_scan(**self.lidar)
+        if self.history is not None:
+            if self.observation == "vector":
+                info["history"] = self.world.observe_history(self._last_obs.agent_index)
+            elif self.observation == "agents":
+                info["history"] = self.world.observe_history(self._last_obs.agent_index, self.vector_obs.get("observers"))
+            else:
+                info["history"] = self.world.observe_history()
         return info
 
     # ------------------------------------------------------------------ gym surface

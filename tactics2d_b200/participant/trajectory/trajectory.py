@@ -6,8 +6,10 @@ warns and overwrites when the frame already exists, flips ``stable_freq`` when t
 changes (:139-144); ``reset(state, keep_history)`` as :170-188.  (One deliberate deviation: overwriting an
 existing frame does not append the frame a second time to ``frames``.)
 
-The batched engine keeps only the *current* state of every participant in HBM; a Trajectory is the
-optional host-side history for the reference-shaped participant objects.
+The batched engine keeps the current state of every participant in HBM and, with ``BatchedWorld.set_history``, a
+ring of its last H states on the device (DESIGN.md section 1 "Trajectory history"); ``BatchedWorld.trajectory(n, m)``
+reads a slot's valid entries back as a Trajectory.  A Trajectory is also the host-side history of the
+reference-shaped participant objects.
 """
 
 from __future__ import annotations

@@ -74,6 +74,10 @@ SEGMENT_FIELDS = ("valid", "ex1", "ey1", "ex2", "ey2", "ecx", "ecy", "dist", "in
 # following"), followed by the look-ahead points (x, y) in the observer's frame.
 ROUTE_FIELDS = ("has_route", "lateral", "heading_error", "s_frac", "remaining")
 ROUTE_MAX_POINTS = 256
+# Columns of every lag of the history observation (``BatchedWorld.observe_history``; DESIGN.md section 1 "Trajectory
+# history"): a recorded pose and velocity in the observer's current frame, as an agent row's fields 1..6 put them.
+HIST_FIELDS = ("valid", "ex", "ey", "cos_dh", "sin_dh", "v_x", "v_y")
+HISTORY_MAX = 64
 
 
 def vector_obs_width(k_agents: int, k_segments: int) -> int:
@@ -111,6 +115,13 @@ class AgentObservation:
 
 def _ptr(t: Optional[torch.Tensor]):
     return C.c_void_p(0 if t is None else t.data_ptr())
+
+
+class _DeviceArray:
+    """A device array the library owns, seen by ``torch.as_tensor`` through the CUDA array interface (no copy)."""
+
+    def __init__(self, ptr: int, shape, typestr: str):
+        self.__cuda_array_interface__ = dict(shape=tuple(shape), typestr=typestr, data=(int(ptr), False), version=2)
 
 
 class BatchedWorld:
@@ -167,6 +178,7 @@ class BatchedWorld:
         self.paths = None
         # what the setters bind (None until they are called) and the output buffers made on first use
         self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = self._sampler = None
+        self._history, self._hist_out = 0, {}
         self._route_out = {}
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
         self._agent_lidar, self._obs_out, self._agent_obs_out = {}, {}, {}
@@ -481,6 +493,122 @@ class BatchedWorld:
                                                      dtype=torch.float32, device=self.device)
         _lib.check(self.lib.t2d_route_observe(self._ctx, _ptr(observers), Q, P, float(spacing), _ptr(out), self._stream()))
         return out
+
+    # ------------------------------------------------------------------ trajectory history
+    def set_history(self, length: int):
+        """Keep the last ``length`` (1..64) states of every slot on the device (``t2d_set_history``; DESIGN.md section 1
+        "Trajectory history"; ``Trajectory.add_state`` / ``Trajectory.reset(state)``, trajectory.py:115-149,170-188): every
+        step appends the state after its tick, every ``reset`` / ``reset_sampled`` starts the reset scenarios' histories
+        again from the state it leaves.  ``set_state``, ``check_events`` and the observations leave the ring alone.  A new
+        binding is empty; 0 frees the ring.  A rejected call keeps the previous ring.  It costs N M length 25 bytes (4 more
+        per entry with a log schedule)."""
+        n = int(length)
+        if not 0 <= n <= HISTORY_MAX:
+            raise ValueError(f"history length must be in 0..{HISTORY_MAX}")
+        _lib.check(self.lib.t2d_set_history(self._ctx, n))
+        self._history, self._hist_out = n, {}
+
+    @property
+    def history_length(self) -> int:
+        """H of the bound history ring, 0 without one."""
+        return self._history
+
+    def observe_history(self, agent_index: Optional[torch.Tensor] = None,
+                        observers: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The recent past of each observer and of its agents in the observer's CURRENT frame, in one launch
+        (``t2d_observe_history``, K16): fp32 ``[..., 1 + K, H, 7]`` of :data:`HIST_FIELDS`, block 0 the observer itself and
+        block 1 + k the slot ``agent_index[..., k]``, lag 0 (the newest entry) first; an invalid entry, an absent agent and
+        an absent observer give zeros.  Without ``observers`` and with ``agent_index`` None or int16 ``[N, K]`` (what
+        ``observe`` returns) the rows are the egos': ``[N, 1 + K, H, 7]``.  With ``observers`` (int16 ``[N, Q]``, as in
+        ``observe_agents``) or an ``agent_index`` of ``[N, Q, K]`` (what ``observe_agents`` returns; without ``observers``
+        row q is slot q) there is a row per observer: ``[N, Q, 1 + K, H, 7]``.  ``agent_index=None`` is K = 0.  At lag 0,
+        while the newest entry is the current state, block 1 + k equals fields 1..6 of the observation's agent row k.  The
+        tensor is a buffer the next call with the same shape reuses."""
+        if not self._history:
+            raise RuntimeError("call set_history before observe_history")
+        per_row = observers is not None or (agent_index is not None and torch.is_tensor(agent_index) and agent_index.dim() == 3)
+        if per_row:
+            if observers is not None:
+                Q = self._agent_rows(observers, None)
+            else:
+                Q = int(agent_index.shape[1])
+                if not 1 <= Q <= min(128, self.M):
+                    raise ValueError("without observers the agent_index rows are slots: Q must be in 1..min(128, M)")
+            lead = (self.N, Q)
+        else:
+            Q, lead = 0, (self.N,)
+        K = 0
+        if agent_index is not None:
+            if not (torch.is_tensor(agent_index) and agent_index.dim() == len(lead) + 1):
+                raise ValueError(f"agent_index must be a contiguous int16 {list(lead) + ['K']} tensor on {self.device}")
+            K = int(agent_index.shape[-1])
+            if not 0 <= K <= 127:
+                raise ValueError("agent_index may name 0..127 agents per row")
+            self._device_tensor("agent_index", agent_index, torch.int16, lead + (K,))
+        shape = lead + (1 + K, self._history, len(HIST_FIELDS))
+        out = self._hist_out.get(shape)
+        if out is None:
+            out = self._hist_out[shape] = torch.empty(shape, dtype=torch.float32, device=self.device)
+        _lib.check(self.lib.t2d_observe_history(self._ctx, _ptr(observers), Q, _ptr(agent_index if K else None), K, _ptr(out),
+                                                self._stream()))
+        return out
+
+    def _history_ring(self) -> dict:
+        """The library's ring as device tensors (views, no copy): x ... vy [N, H, M], type_id, track (or None), count [N]."""
+        v = _lib.HistoryRingC()
+        _lib.check(self.lib.t2d_history_view(self._ctx, C.byref(v)))
+        if v.length == 0:
+            raise RuntimeError("no history bound: call set_history first")
+        shape = (self.N, v.length, self.M)
+        view = lambda ptr, typestr, shp=shape: torch.as_tensor(_DeviceArray(ptr, shp, typestr), device=self.device)
+        ring = {k: view(getattr(v, k), "<f4") for k in ("x", "y", "heading", "speed", "vx", "vy")}
+        ring["type_id"] = view(v.type_id, "|u1")
+        ring["track"] = None if not v.track else view(v.track, "<i4")
+        ring["count"] = view(v.count, "<i8", (self.N,))
+        return ring
+
+    def history(self) -> dict:
+        """Read back the ring (a utility; eager torch): ``x, y, heading, speed, vx, vy`` fp32 and ``type_id`` uint8, each
+        ``[N, M, H]`` with lag 0 (the newest entry) first, ``valid`` bool ``[N, M, H]`` (DESIGN.md section 1 "Trajectory
+        history": one of the last min(count, H) entries, recorded with the slot's current type - and, with a schedule, its
+        current track), zeros (type 255) where not valid, and ``count`` int64 ``[N]``, the entries since each scenario's
+        episode began.  Every tensor is a copy."""
+        ring = self._history_ring()
+        N, M, H = self.N, self.M, self._history
+        count = ring["count"].clone()
+        lag = torch.arange(H, device=self.device)
+        idx = torch.remainder(count[:, None] - 1 - lag[None, :], H)                 # [N, H] ring index of every lag
+        recent = lag[None, :] < torch.clamp(count, max=H)[:, None]                  # [N, H]
+        pick = lambda a: torch.gather(a, 1, idx[:, :, None].expand(N, H, M)).permute(0, 2, 1).contiguous()
+        tid = pick(ring["type_id"])
+        valid = recent[:, None, :] & (tid == self.type_id[:, :, None]) & (tid.to(torch.int64) < len(self.type_table))
+        if ring["track"] is not None:
+            valid &= pick(ring["track"]) == self.replay_track[:, :, None]
+        out = {k: torch.where(valid, pick(ring[k]), torch.zeros((), device=self.device))
+               for k in ("x", "y", "heading", "speed", "vx", "vy")}
+        out["type_id"] = torch.where(valid, tid, torch.full((), TYPE_INACTIVE, dtype=torch.uint8, device=self.device))
+        out["valid"], out["count"] = valid, count
+        return out
+
+    def trajectory(self, n: int, m: int):
+        """Slot m of scenario n's valid history as the reference's ``Trajectory`` of ``State`` objects, oldest first; the
+        frame of entry e (counted from the episode's first state) is e x ``interval``."""
+        from .participant.trajectory import State, Trajectory
+
+        h = self.history()
+        n, m = int(n), int(m)
+        if not (0 <= n < self.N and 0 <= m < self.M):
+            raise IndexError(f"slot ({n}, {m}) outside the [{self.N}, {self.M}] world")
+        cols = {k: h[k][n, m].cpu().numpy() for k in ("x", "y", "heading", "speed", "vx", "vy")}
+        valid = h["valid"][n, m].cpu().numpy()
+        count = int(h["count"][n])
+        traj = Trajectory((n, m), fps=1000.0 / self.interval)
+        for lag in range(self._history - 1, -1, -1):
+            if valid[lag]:
+                c = {k: float(v[lag]) for k, v in cols.items()}
+                traj.add_state(State(frame=(count - 1 - lag) * self.interval, x=c["x"], y=c["y"], heading=c["heading"],
+                                     vx=c["vx"], vy=c["vy"], speed=c["speed"]))
+        return traj
 
     # ------------------------------------------------------------------ log replay
     def set_log(self, log, t0=None, row_track=None, schedule=None):
