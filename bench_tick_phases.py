@@ -43,7 +43,7 @@ if ROOT not in sys.path:
 from benchlib import gpu_info  # noqa: E402
 
 POINTS = ["entry", "wait", "loads", "physics", "sort", "sweep", "drain", "static", "exit"]
-TL_MAX_WARPS = 4096   # t2d_kernels.cu: TL_MAX_WARPS, TL_POINTS
+TL_MAX_WARPS = 4096   # t2d_tick.cuh: TL_MAX_WARPS, TL_POINTS
 WPC = 8               # warps per CTA of the tick at C2 (2048 warp tiles: pick_wpc's largest CTA); a warp's slot is its tile
 
 

@@ -15,7 +15,7 @@
 
 #include <stdint.h>
 
-#include "t2d_math.cuh"
+#include "t2d_world.cuh"
 
 namespace t2d {
 namespace bev {

@@ -19,6 +19,7 @@
 #include <stdint.h>
 
 #include "t2d_obs.cuh"
+#include "t2d_world.cuh"
 
 namespace t2d {
 namespace hist {
