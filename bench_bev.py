@@ -6,6 +6,9 @@ renders 200 x 200 images, as RGB (the reference's observation) and as style indi
 over CUDA-graph replays of one render each, for at least ``--seconds`` after warm-up; the output holds the GPU name and
 power limit, microseconds per call, bytes written per call, the achieved store rate and its share of the H100 SXM data
 sheet's 3.35 TB/s HBM3 bandwidth (the kernel reads little: its lower bound is the image stores).
+
+``--agents`` times the per-agent view (``BatchedWorld.bev_agents``) instead, on the same scenes: ``--q`` observer rows per
+scenario, slots 0 .. q-1, one 200 x 200 image each.
 """
 
 from __future__ import annotations
@@ -47,11 +50,17 @@ def main(argv=None):
     ap.add_argument("--m", type=int, default=64)
     ap.add_argument("--seconds", type=float, default=1.0)
     ap.add_argument("--scenes", default="c2,inD_1")
+    ap.add_argument("--agents", action="store_true", help="time bev_agents (one image per observer row) instead of bev")
+    ap.add_argument("--q", type=int, default=8, help="observer rows per scenario with --agents")
     a = ap.parse_args(argv)
     require_cuda("bench_bev.py")
     gpu, power, _ = gpu_info()
     for key in a.scenes.split(","):
         w = _world(key, a.n, a.m)
+        if a.agents:
+            _bench_agents(w, key, a, gpu, power)
+            w.close()
+            continue
         for rgb in (True, False):
             nbytes = w.bev((200, 200), rgb=rgb).numel()
             us, reps = time_graph(lambda: w.bev((200, 200), rgb=rgb), a.seconds)
@@ -61,6 +70,22 @@ def main(argv=None):
                                   replays=reps, bytes_per_call=nbytes, achieved_gb_s=round(rate / 1e9, 1),
                                   share_of_store_bound=round(rate / PEAK_BYTES_PER_S, 3))), flush=True)
         w.close()
+
+
+def _bench_agents(w, key, a, gpu, power):
+    import torch
+
+    obs = torch.arange(a.q, dtype=torch.int16, device=w.device).expand(a.n, a.q).contiguous()
+    for rgb in (True, False):
+        nbytes = w.bev_agents((200, 200), 20.0, rgb=rgb, observers=obs).numel()
+        us, reps = time_graph(lambda: w.bev_agents((200, 200), 20.0, rgb=rgb, observers=obs), a.seconds)
+        rate = nbytes / (us * 1e-6)
+        print(json.dumps(dict(metric="bev_render_agents", scene=key, n=a.n, m=a.m, q=a.q, resolution=[200, 200],
+                              output="rgb" if rgb else "class", gpu=gpu, power_limit=power, us_per_call=round(us, 2),
+                              us_per_row=round(us / a.q, 2), replays=reps, bytes_per_call=nbytes,
+                              achieved_gb_s=round(rate / 1e9, 1), share_of_store_bound=round(rate / PEAK_BYTES_PER_S, 3))),
+              flush=True)
+        w._agent_bev.clear()   # the next output's buffer is allocated afresh
 
 
 if __name__ == "__main__":

@@ -35,6 +35,8 @@
  *   t2d_bev_render       BEVCamera.update + MatplotlibRenderer.update / save_single_frame(return_array=True)
  *                                                         tactics2d/sensor/camera.py:333-386,
  *                                                         renderer/matplotlib_renderer.py:542-768
+ *   t2d_bev_render_agents
+ *                        (no reference counterpart: the reference's BEVCamera bound to each row's slot)
  *   t2d_set_controllers  IDMController / AccelerationController / PurePursuitController / PIDController objects
  *                                                         tactics2d/controller/idm_controller.py:33-58,
  *                                                         acceleration_controller.py:33-80, pure_pursuit_controller.py:26-49,
@@ -406,6 +408,23 @@ int t2d_set_bev_styles(t2d_ctx* ctx, const t2d_bev_style* table, int n_styles, c
  * style indices (RGB = the style's colour).  range: HOST float [4] = (left, right, front, back) in metres, each in
  * (0, 1e5]; width, height in 1..1024.  One launch, no allocation, no synchronisation: capturable in a CUDA graph. */
 int t2d_bev_render(t2d_ctx* ctx, int width, int height, const float* range, int rgb, uint8_t* out, void* stream);
+/* Per-agent BEV: t2d_bev_render seen from any list of observer slots per scenario (no reference counterpart: the
+ * reference's BEVCamera bound to each row's slot, sensor_base.py:89-95; DESIGN.md section 1 "Per-agent BEV").  Row (n, q),
+ * q < Q = n_observers (1..T2D_OBS_MAX_OBSERVERS), is the view centred on slot j = observers[n][q] at its fp32 (x, y,
+ * heading), +x along its heading, whatever j's shape; it draws what t2d_bev_render draws for the scenario, j's own body
+ * included.  observers: DEVICE int16 [N][Q], or NULL for slot q in row q (needs Q <= M).  A value outside [0, M) or an
+ * empty slot (type_id >= n_types, a retired one included) gives an absent row: every pixel the background (style 0); it
+ * does not take t2d_bev_render's no-ego view.  goals: DEVICE float [N][Q][5] (cx, cy, heading, half_len, half_wid), the
+ * goal rectangle of every row (NaN cx: none), or NULL: the rows observed by slot 0 draw the t2d_set_goal target, the
+ * others none; drawn in the target style either way.  out: DEVICE uint8 [N][Q][height][width][3] RGB, or
+ * [N][Q][height][width] style indices (64-bit offsets).  A row observed by slot 0 without goals equals t2d_bev_render's
+ * image whenever slot 0 is present.  Rejected without a launch: what t2d_bev_render rejects, n_observers outside
+ * 1..128, observers == NULL with n_observers > M (T2D_E_INVALID), N·Q above 2^31 - 1 (T2D_E_UNSUPPORTED).  One launch, no
+ * allocation, no synchronisation: capturable in a CUDA graph. */
+int t2d_bev_render_agents(t2d_ctx* ctx, const int16_t* observers /* DEVICE [N][Q] or NULL */, int32_t n_observers /* Q */,
+                          const float* goals /* DEVICE [N][Q][5] or NULL */, int width, int height,
+                          const float* range /* HOST [4] */, int rgb, uint8_t* out /* DEVICE [N][Q][H][W](3) */,
+                          void* stream);
 
 /* ---- vector observation of the ego of every scenario -----------------------------------------------------------------
  * One fp32 row of F = 16 + 11 k_agents + 9 k_segments values per scenario, everything in the frame of participant 0 (origin

@@ -109,6 +109,7 @@ SYMBOLS = {
     "t2d_lidar_scan_agents": (C.c_int, [_P, _P, C.c_int32, C.c_int, C.c_float, _P, _P, _P]),
     "t2d_set_bev_styles": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.c_int]),
     "t2d_bev_render": (C.c_int, [_P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
+    "t2d_bev_render_agents": (C.c_int, [_P, _P, C.c_int32, _P, C.c_int, C.c_int, _P, C.c_int, _P, _P]),
     "t2d_observe": (C.c_int, [_P, C.POINTER(ObsConfigC), _P, _P, _P, _P]),
     "t2d_observe_agents": (C.c_int, [_P, C.POINTER(ObsConfigC), _P, C.c_int32, _P, _P, _P, _P, _P]),
     "t2d_set_controllers": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P]),

@@ -10,6 +10,11 @@
 // coordinates, in the order the float64 oracle evaluates them: the class image is bit-exact against it.  On H100 fp64
 // runs at half the fp32 rate, and the kernel is bound by its image stores, so no fp32 pre-filter is used.
 //
+// The same kernel renders the view of any list of observer slots per scenario (t2d_bev_render_agents, DESIGN.md section 1
+// "Per-agent BEV"; the reference's BEVCamera bound to each row's slot): one CTA per row n·Q + q, centred on the row's slot,
+// which draws the scenario's primitives exactly as the ego's view does.  A row differs from the ego's image only in its
+// view, its goal rectangle and where it is stored; an absent row stages no primitive, so every pixel is the background.
+//
 // The predicates are __host__ __device__ so that a g++ build can check them against the oracle.
 #pragma once
 
@@ -134,7 +139,11 @@ struct Args : WorldArgs {
   uint8_t type_style[T2D_MAX_TYPES];
   uint8_t style_rgb[MAX_STYLES][3];
   int8_t style_z[MAX_STYLES];
-  uint8_t* out;
+  uint8_t* out;                    // [N][Q][H][W](3)
+  // the rows of t2d_bev_render_agents (the ego's view reads none of these)
+  const int16_t* observers;        // [N][Q] the slot observing row n·Q + q, or nullptr: row q is slot q
+  const float* goals;              // [N][Q][5] the goal rectangle of every row (NaN cx: none), or nullptr
+  int Q;                           // rows per scenario (1 for the ego's view)
 };
 
 struct Prim {
@@ -145,7 +154,7 @@ struct Prim {
   double g[8];                // K_POLY: nv vertices (x[0..nv), then y at +4); K_DISC: cx, cy, r2; K_STROKE: x1, y1, x2, y2
 };
 
-struct Scene {   // per scenario, shared
+struct Scene {   // per row, shared
   View view;
   const unsigned char* blob;
   const float4* seg;
@@ -168,8 +177,10 @@ __device__ __forceinline__ void to_pixel(const Args& A, const View& v, double X,
 }
 
 // Candidate i of the scenario in draw order: 0 the goal rectangle, then the rings, then the open segments, then per
-// participant its body and heading arrow.  Returns false when the candidate draws nothing or misses the image.
-__device__ bool make_prim(const Args& A, const Scene& S, long long n, int i, Prim& p) {
+// participant its body and heading arrow.  Returns false when the candidate draws nothing or misses the image.  The goal
+// is the scenario's target, or with ROWS the row's goal `goal` (nullptr: none).
+template <bool ROWS>
+__device__ bool make_prim(const Args& A, const Scene& S, const float* goal, long long n, int i, Prim& p) {
   double bx0 = INFINITY, bx1 = -INFINITY, by0 = INFINITY, by1 = -INFINITY, grow = 0.0;
   auto pt = [&](double X, double Y) {
     double fc, fr;
@@ -178,8 +189,8 @@ __device__ bool make_prim(const Args& A, const Scene& S, long long n, int i, Pri
   };
   int z, draw;
   if (i == 0) {   // the goal rectangle
-    if (!A.target || A.target_style == NO_STYLE) return false;
-    const float* t = A.target + n * 5;
+    if (!(ROWS ? goal : A.target) || A.target_style == NO_STYLE) return false;
+    const float* t = ROWS ? goal : A.target + n * 5;
     double s, c;
     sincos((double)t[2], &s, &c);
     box_ring(t[0], t[1], c, s, t[3], t[4], p.g, p.g + 4);
@@ -269,11 +280,12 @@ struct Smem {
   uint16_t order[MAX_PRIMS];    // rank (0 = top-most) -> staged slot
   uint32_t mask[BINS_X][WORDS]; // this band's bins: bit r = the primitive of rank r may cover a centre of the bin
   Prim prim[MAX_PRIMS];
+  const float* goal;            // ROWS: the row's goal rectangle (cx, cy, heading, half_len, half_wid), or nullptr
 };
 
-__device__ __forceinline__ void store_run(const Args& A, long long n, long long off, int len, const uint8_t (&cls)[16]) {
+__device__ __forceinline__ void store_run(const Args& A, long long row, long long off, int len, const uint8_t (&cls)[16]) {
   if (!A.rgb) {
-    uint8_t* dst = A.out + n * (long long)A.W * A.H + off;
+    uint8_t* dst = A.out + row * (long long)A.W * A.H + off;
     if (len == 16 && ((uintptr_t)dst & 15) == 0) {
       uint4 v;
       memcpy(&v, cls, 16);
@@ -283,7 +295,7 @@ __device__ __forceinline__ void store_run(const Args& A, long long n, long long 
     }
     return;
   }
-  uint8_t* dst = A.out + (n * (long long)A.W * A.H + off) * 3;
+  uint8_t* dst = A.out + (row * (long long)A.W * A.H + off) * 3;
   uint8_t px[48];
 #pragma unroll
   for (int k = 0; k < 16; ++k) {
@@ -301,11 +313,24 @@ __device__ __forceinline__ void store_run(const Args& A, long long n, long long 
   }
 }
 
+// View centred on slot pj (a global slot index), +x along its heading
+__device__ __forceinline__ View slot_view(const Args& A, long long pj) {
+  View v;
+  v.ex = A.x[pj]; v.ey = A.y[pj];
+  sincos((double)A.h[pj], &v.sn, &v.cs);
+  return v;
+}
+
+// ROWS = false: the ego's view (t2d_bev_render), one CTA per scenario.  ROWS = true: one CTA per observer row n·Q + q
+// (t2d_bev_render_agents); with Q = 1 and no list that is slot 0's view, except that a scenario without slot 0 gives an
+// absent row instead of the no-ego view.
+template <bool ROWS>
 __global__ void __launch_bounds__(CTA) t2d_bev_kernel(const __grid_constant__ Args A) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
   Scene& S = sm.S;
-  const long long n = blockIdx.x;
+  const long long row = blockIdx.x;
+  const long long n = ROWS ? row / A.Q : row;
   const int tid = threadIdx.x;
   if (tid == 0) {
     const unsigned char* blob = tile_blob(A.map, n);
@@ -321,10 +346,17 @@ __global__ void __launch_bounds__(CTA) t2d_bev_kernel(const __grid_constant__ Ar
     S.sstyle = A.seg_style ? A.seg_style + A.seg_base[A.map.tile_id ? A.map.tile_id[n] : 0] : nullptr;
     S.n_cand = 1 + S.n_poly + S.n_seg + 2 * A.M;
     View v;
-    const int t0 = A.type_id[n * A.M];
-    if (t0 < A.n_types) {   // the ego: centred, +x along its heading
-      v.ex = A.x[n * A.M]; v.ey = A.y[n * A.M];
-      sincos((double)A.h[n * A.M], &v.sn, &v.cs);
+    if (ROWS) {
+      const int q = (int)(row - n * A.Q);
+      const int j = A.observers ? (int)A.observers[row] : q;   // the observing slot
+      v = View{0.0, 0.0, 1.0, 0.0};
+      if (j >= 0 && j < A.M && A.type_id[n * A.M + j] < A.n_types) v = slot_view(A, n * A.M + j);
+      else S.n_cand = 0;   // not a slot, an empty or a retired one: an absent row, all background
+      // the goal (observe_agents' rule): the row's own (NaN cx: none), or without goals the target for slot 0 only
+      if (A.goals) sm.goal = isnan(A.goals[row * 5]) ? nullptr : A.goals + row * 5;
+      else sm.goal = j == 0 && A.target ? A.target + n * 5 : nullptr;
+    } else if (A.type_id[n * A.M] < A.n_types) {   // the ego: centred, +x along its heading
+      v = slot_view(A, n * A.M);
     } else {   // no ego (sensor_base.py:185-191): the tile's bounds box centre, or the origin; yaw 0
       v.ex = v.ey = 0.0;
       if (blob && mh->has_bounds) {
@@ -338,9 +370,10 @@ __global__ void __launch_bounds__(CTA) t2d_bev_kernel(const __grid_constant__ Ar
   }
   __syncthreads();
   // ---- stage the visible primitives
+  const float* goal = ROWS ? sm.goal : nullptr;
   for (int i = tid; i < S.n_cand; i += CTA) {
     Prim p;
-    if (make_prim(A, S, n, i, p)) {
+    if (make_prim<ROWS>(A, S, goal, n, i, p)) {
       const int slot = atomicAdd(&sm.count, 1);
       if (slot < MAX_PRIMS) { sm.prim[slot] = p; sm.key[slot] = p.key; }
     }
@@ -400,13 +433,13 @@ __global__ void __launch_bounds__(CTA) t2d_bev_kernel(const __grid_constant__ Ar
           uint32_t best = 0;
           for (int i = 0; i < S.n_cand; ++i) {
             Prim p;
-            if (!make_prim(A, S, n, i, p) || p.key <= best) continue;
+            if (!make_prim<ROWS>(A, S, goal, n, i, p) || p.key <= best) continue;
             if (r < p.r0 || r > p.r1 || c < p.c0 || c > p.c1) continue;
             if (covers(p, S, A, X, Y)) { best = p.key; cls[k] = p.style; }
           }
         }
       }
-      store_run(A, n, off, len, cls);
+      store_run(A, row, off, len, cls);
     }
   }
 }

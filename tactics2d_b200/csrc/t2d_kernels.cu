@@ -11,7 +11,7 @@
 // K3  t2d_physics_kernel   flat batch through one physics model (PhysicsModelBase.step) (t2d_tick.cuh).
 // K4  t2d_lidar_kernel     single-line lidar of every scenario's ego (per-edge beam windows) (t2d_lidar.cuh).
 // K5  t2d_control_kernel   NPC controllers: IDM, cruise / adaptive cruise, pure pursuit, PID (t2d_control.cuh).
-// K6  t2d_bev_kernel       the bird's-eye-view observation of every scenario's ego (t2d_bev.cuh).
+// K6  t2d_bev_kernel       the bird's-eye-view observation of every scenario's ego, or of every observer row (t2d_bev.cuh).
 // K7  t2d_replay_kernel    log replay: recorded tracks pose the replayed slots before K1 / after K2 (t2d_replay.cuh).
 // K8  t2d_obs_kernel       the ego-frame vector observation (t2d_obs.cuh).
 // K9  t2d_obs_agents_kernel the same observation from a list of observer slots per scenario (t2d_obs.cuh).
@@ -1606,7 +1606,8 @@ int t2d_set_bev_styles(t2d_ctx* c, const t2d_bev_style* table, int n_styles, con
     if (int r = upload(d_base, base.data(), base.size())) return r;
   }
   // opt in to the kernel's shared memory here: t2d_bev_render must stay free of anything a graph capture rejects
-  CUDA_TRY(cudaFuncSetAttribute(bev::t2d_bev_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(bev::Smem)));
+  CUDA_TRY(cudaFuncSetAttribute(bev::t2d_bev_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(bev::Smem)));
+  CUDA_TRY(cudaFuncSetAttribute(bev::t2d_bev_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(bev::Smem)));
   c->map.seg_style = std::move(d_style);
   c->map.seg_base = std::move(d_base);
   memcpy(c->bev_style, table, sizeof(t2d_bev_style) * (size_t)n_styles);
@@ -1617,15 +1618,19 @@ int t2d_set_bev_styles(t2d_ctx* c, const t2d_bev_style* table, int n_styles, con
   return T2D_OK;
 }
 
-int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rgb, uint8_t* out, void* stream) {
-  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+// K6 over the rows of an observer list (rows: t2d_bev_render_agents) or over the egos (t2d_bev_render); the arguments
+// both entries take are checked here, with messages prefixed by fn
+static int launch_bev(t2d_ctx* c, const std::string& fn, bool rows, const int16_t* observers, int Q, const float* goals,
+                      int width, int height, const float* range, int rgb, uint8_t* out, void* stream) {
   if (int r = require(c, NEED_STATE)) return r;
   if (c->n_bev_styles == 0) return fail(T2D_E_STATE, "BEV styles not set: call t2d_set_bev_styles first");
-  if (!range || !out) return fail(T2D_E_INVALID, "t2d_bev_render: range / out is NULL");
+  if (!range || !out) return fail(T2D_E_INVALID, fn + ": range / out is NULL");
   if (width < 1 || height < 1 || width > bev::MAX_SIDE || height > bev::MAX_SIDE)
-    return fail(T2D_E_INVALID, "t2d_bev_render: width and height must be in 1..1024");
+    return fail(T2D_E_INVALID, fn + ": width and height must be in 1..1024");
   for (int k = 0; k < 4; ++k)
-    if (!(range[k] > 0.0f && range[k] <= 1.0e5f)) return fail(T2D_E_INVALID, "t2d_bev_render: every range must be in (0, 1e5] m");
+    if (!(range[k] > 0.0f && range[k] <= 1.0e5f)) return fail(T2D_E_INVALID, fn + ": every range must be in (0, 1e5] m");
+  const long long grid = (long long)c->N * Q;   // one CTA per row
+  if (grid > INT32_MAX) return fail(T2D_E_UNSUPPORTED, fn + ": more than 2^31 - 1 rows (one CTA per row)");
   // the window (matplotlib_renderer.py:152-164, auto_scale :200-224), in the float64 oracle's operation order
   const double L = range[0], R = range[1], F = range[2], B = range[3];
   const double x_min = -L, x_max = R, y_min = -B, y_max = F;
@@ -1650,10 +1655,24 @@ int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rg
   A.map = map_args(c->map); A.seg_style = c->map.seg_style.get(); A.seg_base = c->map.seg_base.get();
   A.target = c->goal.target; A.target_style = c->bev_target_style;
   A.ring_style = T2D_BEV_STYLE_RING; A.open_style = T2D_BEV_STYLE_OPEN;
+  A.observers = observers; A.goals = goals; A.Q = Q;
   A.W = width; A.H = height; A.rgb = rgb ? 1 : 0; A.out = out;
   CUDA_TRY(cudaSetDevice(c->device));
-  bev::t2d_bev_kernel<<<c->N, bev::CTA, sizeof(bev::Smem), (cudaStream_t)stream>>>(A);
+  if (rows) bev::t2d_bev_kernel<true><<<(unsigned)grid, bev::CTA, sizeof(bev::Smem), (cudaStream_t)stream>>>(A);
+  else bev::t2d_bev_kernel<false><<<(unsigned)grid, bev::CTA, sizeof(bev::Smem), (cudaStream_t)stream>>>(A);
   return launched();
+}
+
+int t2d_bev_render(t2d_ctx* c, int width, int height, const float* range, int rgb, uint8_t* out, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  return launch_bev(c, "t2d_bev_render", false, nullptr, 1, nullptr, width, height, range, rgb, out, stream);
+}
+
+int t2d_bev_render_agents(t2d_ctx* c, const int16_t* observers, int32_t n_observers, const float* goals, int width, int height,
+                          const float* range, int rgb, uint8_t* out, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (int r = check_rows(c, "t2d_bev_render_agents", observers, n_observers, 1)) return r;
+  return launch_bev(c, "t2d_bev_render_agents", true, observers, n_observers, goals, width, height, range, rgb, out, stream);
 }
 
 // What t2d_observe and t2d_observe_agents share: the checks of cfg and out (messages prefixed with fn) and K8's arguments

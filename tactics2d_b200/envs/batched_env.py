@@ -50,7 +50,8 @@ class BatchedTrafficEnv:
                  no_action_max_step: int = 100, observation: str = "state", bev_resolution=(200, 200),
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
                  agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
-                 route: Optional[dict] = None, sampler: Optional[dict] = None, history: Optional[dict] = None):
+                 route: Optional[dict] = None, sampler: Optional[dict] = None, history: Optional[dict] = None,
+                 camera: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -100,7 +101,12 @@ class BatchedTrafficEnv:
         and ``step``, computed after the auto-reset like the observation (``BatchedWorld.observe_history``): with
         ``observation="vector"`` the ego's past and that of the agents of its observation (``[N, 1 + K, H, 7]``), with
         ``"agents"`` every observer row's and its agents' (``[N, Q, 1 + K, H, 7]``), else the ego's own past
-        (``[N, 1, H, 7]``).  A scenario that auto-reset shows one valid entry per present slot, its new start state."""
+        (``[N, 1, H, 7]``).  A scenario that auto-reset shows one valid entry per present slot, its new start state;
+        ``camera``: e.g. ``dict(resolution=(200, 200), perception_range=20.0, rgb=True)`` adds ``info["bev"]`` to ``reset``
+        and ``step``, rendered after the auto-reset like the lidar: with ``observation="agents"`` ``uint8 [N, Q, H, W(,
+        3)]`` from every observer row (``BatchedWorld.bev_agents`` on ``vector_obs["observers"]`` and ``["goals"]``;
+        DESIGN.md section 1 "Per-agent BEV"), else ``[N, H, W(, 3)]`` from every ego (``BatchedWorld.bev``).  It is
+        rejected with ``observation="bev"``, whose observation already is that image."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -152,6 +158,13 @@ class BatchedTrafficEnv:
                 raise ValueError(f"history: unknown keys {sorted(unknown)}")
             if "length" not in self.history:
                 raise ValueError("history: missing key 'length'")
+        self.camera = None if camera is None else dict(camera)
+        if self.camera is not None:
+            if observation == "bev":
+                raise ValueError("camera: the 'bev' observation already is the ego's image; use bev_resolution / bev_range")
+            unknown = set(self.camera) - {"resolution", "perception_range", "rgb"}
+            if unknown:
+                raise ValueError(f"camera: unknown keys {sorted(unknown)}")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -247,8 +260,9 @@ class BatchedTrafficEnv:
         return info
 
     def _add_lidar(self, info):
-        """``info["lidar"]`` / ``info["route"]`` / ``info["history"]`` when the env has a lidar / routes / a history; called
-        after the auto-reset and the observation, so that they see the new episodes and the observation's agents."""
+        """``info["lidar"]`` / ``info["bev"]`` / ``info["route"]`` / ``info["history"]`` when the env has a lidar / a camera
+        / routes / a history; called after the auto-reset and the observation, so that they see the new episodes and the
+        observation's agents."""
         if self.route is not None:
             info["route"] = self.world.route_observe(self.route.get("n_points", 8), self.route.get("spacing", 2.0),
                                                      self._route_observers)
@@ -257,6 +271,14 @@ class BatchedTrafficEnv:
                 info["lidar"] = self.world.lidar_scan_agents(**self.lidar, observers=self.vector_obs.get("observers"))
             else:
                 info["lidar"] = self.world.lidar_scan(**self.lidar)
+        if self.camera is not None:
+            cam = dict(resolution=self.camera.get("resolution", (200, 200)),
+                       perception_range=self.camera.get("perception_range", 20.0), rgb=self.camera.get("rgb", True))
+            if self.observation == "agents":
+                info["bev"] = self.world.bev_agents(**cam, observers=self.vector_obs.get("observers"),
+                                                    goals=self.vector_obs.get("goals"))
+            else:
+                info["bev"] = self.world.bev(**cam)
         if self.history is not None:
             if self.observation == "vector":
                 info["history"] = self.world.observe_history(self._last_obs.agent_index)

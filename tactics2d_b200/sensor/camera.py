@@ -3,7 +3,8 @@
 The reference's ``BEVCamera.update`` (``tactics2d/sensor/camera.py:333-386``) returns geometry dicts that a
 ``MatplotlibRenderer`` then draws into the 200 x 200 x 3 ``uint8`` observation of ``ParkingEnv`` / ``RacingEnv``
 (``envs/parking.py:130``).  This class returns the rendered batch instead: ``render(world)`` is one launch of the
-K6 kernel (``t2d_bev_render``) and yields ``uint8 [N, H, W, 3]``.  The drawing contract, and where it deliberately
+K6 kernel (``t2d_bev_render``) and yields ``uint8 [N, H, W, 3]``; ``render_agents(world, observers)`` renders the same view
+from every observer row (``t2d_bev_render_agents``) as ``uint8 [N, Q, H, W, 3]``.  The drawing contract, and where it deliberately
 differs from the reference's renderer, is DESIGN.md section 1 "BEV observation".
 
 ``BEV_STYLES`` restates the rows of the reference's style tables that this renderer uses, as
@@ -88,4 +89,13 @@ class BEVCamera:
         """``uint8 [N, H, W, 3]`` (``rgb``) or the style indices ``uint8 [N, H, W]``; a view of a buffer the world
         reuses on the next render of the same shape."""
         self.observation = world.bev(self.resolution, self.perception_range, rgb=rgb)
+        return self.observation
+
+    def render_agents(self, world, observers=None, goals=None, rgb: bool = True):
+        """This camera's view bound to every observer row's slot (``BatchedWorld.bev_agents``; DESIGN.md section 1
+        "Per-agent BEV"): ``uint8 [N, Q, H, W, 3]`` (``rgb``) or ``[N, Q, H, W]`` style indices.  ``observers`` int16
+        ``[N, Q]`` and ``goals`` fp32 ``[N, Q, 5]`` as in ``BatchedWorld.observe_agents``; an absent row is all
+        background.  A view of a buffer the world reuses on the next call with the same shape."""
+        self.observation = world.bev_agents(self.resolution, self.perception_range, rgb=rgb, observers=observers,
+                                            goals=goals)
         return self.observation

@@ -181,7 +181,7 @@ class BatchedWorld:
         self._history, self._hist_out = 0, {}
         self._route_out = {}
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
-        self._agent_lidar, self._obs_out, self._agent_obs_out = {}, {}, {}
+        self._agent_lidar, self._obs_out, self._agent_obs_out, self._agent_bev = {}, {}, {}, {}
         self._seg_style_keys = []
         self._bev_cfg = None
 
@@ -1055,6 +1055,34 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_bev_render(self._ctx, w, h, C.c_void_p(rng.ctypes.data), 1 if rgb else 0, _ptr(cache[1]),
                                            self._stream()))
         return cache[1]
+
+    def bev_agents(self, resolution=(200, 200), perception_range=20.0, rgb: bool = True,
+                   observers: Optional[torch.Tensor] = None, goals: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``bev`` seen from a list of observer slots per scenario, in one launch (``t2d_bev_render_agents``; DESIGN.md
+        section 1 "Per-agent BEV"): the reference's ``BEVCamera`` bound to each row's slot, centred on it with +x along its
+        heading, drawing every participant, its own body included.  ``observers``: int16 ``[N, Q]`` device tensor as in
+        ``observe_agents`` (None: every slot, Q = M); a value outside ``[0, M)``, an empty or a retired slot gives an
+        absent row, all background.  ``goals``: fp32 ``[N, Q, 5]`` per-row goal rectangles (a NaN cx for none); without it
+        the rows observed by slot 0 draw the ``set_goal`` target and the others none.  Returns ``uint8 [N, Q, H, W, 3]``, or
+        with ``rgb=False`` the style indices ``[N, Q, H, W]``: a buffer per ``(width, height, rgb, Q)`` that the next call
+        with those values reuses.  A row observed by slot 0 without ``goals`` equals ``bev``'s image when slot 0 is
+        present."""
+        Q = self._agent_rows(observers, goals)
+        if self._bev_cfg is None:
+            self.set_bev_styles()
+        w, h = int(resolution[0]), int(resolution[1])
+        pr = perception_range
+        rng = np.ascontiguousarray(np.asarray([pr] * 4 if np.ndim(pr) == 0 else pr, dtype=np.float32).reshape(4))
+        key = (w, h, bool(rgb), Q)
+        out = self._agent_bev.get(key)
+        if out is None:
+            if not (1 <= w <= 1024 and 1 <= h <= 1024):
+                raise ValueError("resolution: width and height must be in 1..1024")
+            shape = (self.N, Q, h, w, 3) if rgb else (self.N, Q, h, w)
+            out = self._agent_bev[key] = torch.empty(shape, dtype=torch.uint8, device=self.device)
+        _lib.check(self.lib.t2d_bev_render_agents(self._ctx, _ptr(observers), Q, _ptr(goals), w, h, C.c_void_p(rng.ctypes.data),
+                                                  1 if rgb else 0, _ptr(out), self._stream()))
+        return out
 
     # ------------------------------------------------------------------ vector observation
     def observe(self, k_agents: int = 16, k_segments: int = 32, agent_range: float = 50.0,
