@@ -46,6 +46,9 @@
  *   t2d_control          ControllerBase.step for every controlled participant
  *                                                         idm_controller.py:59-141, acceleration_controller.py:82-145,
  *                                                         pure_pursuit_controller.py:51-98, pid_controller.py:159-406
+ *   t2d_set_leader_search / t2d_find_leaders
+ *                        (no reference counterpart) the leader of every slot in its corridor, for the controllers'
+ *                        `leading_state` / `front_state`
  *   t2d_check_events     the same detectors on caller-supplied poses (no physics)
  *   t2d_reset            ScenarioManager.reset / ParticipantBase.reset
  *                                                         tactics2d/envs/parking.py:397-441, participant_base.py:236-246
@@ -517,7 +520,8 @@ typedef struct t2d_controller_params {
 /* table: HOST array of n_rows (<= T2D_MAX_CONTROLLERS) rows, copied.  The rest are DEVICE arrays owned by the caller:
  * ctrl_id [N, M] uint8 = row of the participant's controller (255, or a row of kind EXTERNAL: not controlled);
  * lead_index [N, M] int16 = the participant's leading vehicle inside its scenario (`leading_state` / `front_state`),
- * -1 for none (NULL: nobody has one); path_id [N, M] int16 = the pure-pursuit path, -1 for none (NULL allowed);
+ * -1 for none (NULL: nobody has one); while a leader search is bound (t2d_set_leader_search) t2d_control ignores it and
+ * takes every leader from the search, found on the same state in the same call; path_id [N, M] int16 = the pure-pursuit path, -1 for none (NULL allowed);
  * last_accel [N, M] float = |acceleration| each participant applied on the previous tick (State.accel,
  * participant/trajectory/state.py:171-185), read and rewritten by t2d_control; zero it before the first tick.
  * table == NULL removes the controllers.  Rejected (the previous binding stays whole): an unknown kind, and a PID row with
@@ -623,6 +627,30 @@ int t2d_history_view(t2d_ctx* ctx, t2d_history_ring* out);
  * to the type's range; point masses: |(ax, ay)|).  Call it after the external actions are in the buffer and before
  * t2d_step.  action: DEVICE [N, M, 2] fp32. */
 int t2d_control(t2d_ctx* ctx, float* action, void* stream);
+
+/* ---- leader search (K17, no reference counterpart: the reference's controllers take the leader from their caller) ------
+ * DESIGN.md section 1 "Leader search".  fp64, one rounding per operation.  A follower is every slot with type_id < n_types
+ * (controlled or not) at a position that is not NaN; a candidate is every other slot with type_id < n_types and a shape
+ * other than T2D_SHAPE_NONE at a position that is not NaN (replayed slots and discs count, empty and retired slots do not).
+ *   path frame     the follower's path_id of the bound controllers is in [0, n_paths) and that path has a segment of
+ *                  non-zero length: follower and candidates are projected onto it as t2d_set_routes' closest point (arc
+ *                  length s, distance d); a candidate qualifies when d <= half_width and 0 < gap = s_j - s_i <= max_range;
+ *   heading frame  every other follower (all of them without controllers or paths): with (c, s) the sine and cosine of
+ *                  its fp32 heading as t2d_observe computes them, ex = c dx + s dy and ey = -s dx + c dy of the candidate's
+ *                  offset; it qualifies when ex > 0, |ey| <= half_width and ex <= max_range, and gap = ex (bit for bit
+ *                  the ex of the t2d_observe_agents row for the same pair).
+ * The leader is the qualifying candidate of smallest (gap, slot).  lead: DEVICE int16 [N][M], -1 for none; gap: DEVICE
+ * fp32 [N][M], the gap rounded once, +inf for none.  half_width in (0, 100] m, max_range in (0, 1e5] m, both finite.
+ *   t2d_set_leader_search binds a search: every t2d_control, t2d_step_host_ego and t2d_step_host_agents then launches K17
+ * in front of the controllers, into the caller-owned lead / gap (gap may be NULL), and the controllers follow `lead`
+ * instead of set_controllers' lead_index (the laws themselves, and their centre distance, are unchanged).  lead == NULL
+ * unbinds; with no search bound nothing of this launches.  The search keeps no state: resets need nothing.
+ *   t2d_find_leaders writes the leaders of the bound state into lead / gap once: one launch, no allocation, capturable.
+ * Rejected without a launch (a rejected set keeps the previous binding whole): half_width or max_range outside its range
+ * or not finite, lead NULL for find, lead not 2-byte or gap not 4-byte aligned (T2D_E_INVALID), state or type table not
+ * bound (T2D_E_STATE). */
+int t2d_set_leader_search(t2d_ctx* ctx, double half_width, double max_range, int16_t* lead, float* gap);
+int t2d_find_leaders(t2d_ctx* ctx, double half_width, double max_range, int16_t* lead, float* gap, void* stream);
 
 /* Inputs and memory of the PID rows: DEVICE arrays owned by the caller.  target [N][M][2] fp32 = (target_speed, lateral
  * target: target_heading in rad for HEADING rows, cross_track_error in m for CROSS_TRACK rows; PATH rows ignore it);

@@ -116,6 +116,8 @@ SYMBOLS = {
     "t2d_set_paths": (C.c_int, [_P, _P, _P, C.c_int]),
     "t2d_control": (C.c_int, [_P, _P, _P]),
     "t2d_set_pid": (C.c_int, [_P, _P, _P]),
+    "t2d_set_leader_search": (C.c_int, [_P, C.c_double, C.c_double, _P, _P]),
+    "t2d_find_leaders": (C.c_int, [_P, C.c_double, C.c_double, _P, _P, _P]),
     "t2d_set_routes": (C.c_int, [_P, _P, C.c_double, C.c_double, C.c_float]),
     "t2d_bind_route_trackers": (C.c_int, [_P, _P, _P, C.c_int32]),
     "t2d_route_observe": (C.c_int, [_P, _P, C.c_int32, C.c_int, C.c_float, _P, _P]),

@@ -25,6 +25,8 @@
 // K15 t2d_history_append_kernel  trajectory history: append the state after a tick, restart it after a reset (t2d_history.cuh).
 // K16 t2d_history_obs_kernel     trajectory history: past poses of an observer and its agents in its current frame
 //                                (t2d_history.cuh).
+// K17 t2d_leader_kernel          the leader of every slot in its corridor, which K5 follows while a search is bound
+//                                (t2d_leader.cuh).
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory (t2d_exchange.cuh).
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -54,6 +56,7 @@
 #include "t2d_bev.cuh"
 #include "t2d_obs.cuh"
 #include "t2d_history.cuh"
+#include "t2d_leader.cuh"
 
 // =============================================================================================
 // C ABI
@@ -256,6 +259,10 @@ struct t2d_ctx {
   dev_ptr<PathVertex> d_path_v;
   dev_ptr<int> d_path_off;
   int n_paths = 0;
+  // leader search (t2d_set_leader_search / K17); leader_lead == nullptr: none bound, K5 reads ctrl_lead
+  int16_t* leader_lead = nullptr;
+  float* leader_gap = nullptr;
+  double leader_half_width = 0.0, leader_max_range = 0.0;
   // routes (t2d_set_routes / t2d_bind_route_trackers); route_id == nullptr: none bound
   const int16_t* route_id = nullptr;
   double route_threshold = 0.0, route_weight = 0.0;
@@ -327,6 +334,7 @@ static int check_rows(const t2d_ctx* c, const char* fn, const int16_t* observers
 }
 
 // Pointer alignment (nullptr counts as aligned)
+static bool aligned2(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 1) == 0; }
 static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
@@ -1134,6 +1142,27 @@ static int check_pid_binding(const t2d_ctx* c) {
   return T2D_OK;
 }
 
+// ---- leader search (t2d_set_leader_search / t2d_find_leaders; K17)
+static int check_leader_args(const char* fn, double half_width, double max_range, const int16_t* lead, const float* gap) {
+  if (!(std::isfinite(half_width) && half_width > 0.0 && half_width <= 100.0))
+    return fail(T2D_E_INVALID, std::string(fn) + ": half_width must be finite and in (0, 100] m");
+  if (!(std::isfinite(max_range) && max_range > 0.0 && max_range <= 1.0e5))
+    return fail(T2D_E_INVALID, std::string(fn) + ": max_range must be finite and in (0, 1e5] m");
+  if (!aligned2(lead) || !aligned4(gap))
+    return fail(T2D_E_INVALID, std::string(fn) + ": lead must be 2-byte and gap 4-byte aligned");
+  return T2D_OK;
+}
+
+// K17 on the bound state and the controllers' paths; the caller has checked the arguments and the bindings
+static int launch_leaders(t2d_ctx* c, double half_width, double max_range, int16_t* lead, float* gap, void* stream) {
+  CUDA_TRY(cudaSetDevice(c->device));
+  leader::Args A{world_args(c)};
+  A.path_id = c->ctrl_path; A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.half_width = half_width; A.max_range = max_range; A.lead = lead; A.gap = gap;
+  leader::t2d_leader_kernel<<<(c->N + leader::WARPS - 1) / leader::WARPS, leader::WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  return launched();
+}
+
 static int launch_control(t2d_ctx* c, float* action, const float* ego, void* stream) {
   if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   if (!c->d_ctab) return fail(T2D_E_STATE, "controllers not set: call t2d_set_controllers first");
@@ -1141,8 +1170,12 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
   if (!action) return fail(T2D_E_INVALID, "action is NULL");
   if (!aligned8(action)) return fail(T2D_E_INVALID, "action must be 8-byte aligned");
   CUDA_TRY(cudaSetDevice(c->device));
+  // a bound search finds the leaders on the state K5 reads next, and K5 follows them instead of the controllers' lead_index
+  if (c->leader_lead)
+    if (int r = launch_leaders(c, c->leader_half_width, c->leader_max_range, c->leader_lead, c->leader_gap, stream)) return r;
   CtrlArgs A{world_args(c)};
-  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.lead = c->ctrl_lead; A.path_id = c->ctrl_path;
+  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.path_id = c->ctrl_path;
+  A.lead = c->leader_lead ? c->leader_lead : c->ctrl_lead;
   A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
   A.last_accel = c->ctrl_last_accel; A.action = action; A.ego_action = ego;
   A.steer_first = (c->cfg.flags & T2D_CFG_STEER_FIRST) ? 1 : 0;
@@ -1914,6 +1947,26 @@ int t2d_route_observe(t2d_ctx* c, const int16_t* observers, int32_t n_observers,
 int t2d_control(t2d_ctx* c, float* action, void* stream) {
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   return launch_control(c, action, c->ego_action, stream);
+}
+
+int t2d_set_leader_search(t2d_ctx* c, double half_width, double max_range, int16_t* lead, float* gap) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!lead) {   // unbind
+    c->leader_lead = nullptr; c->leader_gap = nullptr; c->leader_half_width = c->leader_max_range = 0.0;
+    return T2D_OK;
+  }
+  if (int r = check_leader_args("t2d_set_leader_search", half_width, max_range, lead, gap)) return r;
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  c->leader_lead = lead; c->leader_gap = gap; c->leader_half_width = half_width; c->leader_max_range = max_range;
+  return T2D_OK;
+}
+
+int t2d_find_leaders(t2d_ctx* c, double half_width, double max_range, int16_t* lead, float* gap, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!lead) return fail(T2D_E_INVALID, "t2d_find_leaders: lead is NULL");
+  if (int r = check_leader_args("t2d_find_leaders", half_width, max_range, lead, gap)) return r;
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  return launch_leaders(c, half_width, max_range, lead, gap, stream);
 }
 int t2d_exchange_create(t2d_exchange** out, int device, int world, int rank, int n_local, int slots, void* ipc_handle_out) {
   if (!out || !ipc_handle_out) return fail(T2D_E_INVALID, "out / ipc_handle_out is NULL");

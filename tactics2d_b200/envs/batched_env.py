@@ -51,7 +51,7 @@ class BatchedTrafficEnv:
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
                  agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
                  route: Optional[dict] = None, sampler: Optional[dict] = None, history: Optional[dict] = None,
-                 camera: Optional[dict] = None):
+                 camera: Optional[dict] = None, leaders: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -106,7 +106,12 @@ class BatchedTrafficEnv:
         and ``step``, rendered after the auto-reset like the lidar: with ``observation="agents"`` ``uint8 [N, Q, H, W(,
         3)]`` from every observer row (``BatchedWorld.bev_agents`` on ``vector_obs["observers"]`` and ``["goals"]``;
         DESIGN.md section 1 "Per-agent BEV"), else ``[N, H, W(, 3)]`` from every ego (``BatchedWorld.bev``).  It is
-        rejected with ``observation="bev"``, whose observation already is that image."""
+        rejected with ``observation="bev"``, whose observation already is that image;
+        ``leaders``: e.g. ``dict(half_width=1.8, max_range=100.0)`` binds a leader search (``BatchedWorld.set_leader_search``;
+        DESIGN.md section 1 "Leader search"), so the controllers set on ``env.world`` follow the participant ahead of them
+        every step instead of a fixed ``lead_index``, and adds ``info["leader"]`` (int16 [N, M], -1 for none) and
+        ``info["leader_gap"]`` (fp32 [N, M], +inf for none) to ``reset`` and ``step``: the leaders of the state after the
+        auto-reset (``BatchedWorld.find_leaders``)."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -165,6 +170,13 @@ class BatchedTrafficEnv:
             unknown = set(self.camera) - {"resolution", "perception_range", "rgb"}
             if unknown:
                 raise ValueError(f"camera: unknown keys {sorted(unknown)}")
+        self.leaders = None if leaders is None else dict(leaders)
+        if self.leaders is not None:
+            unknown = set(self.leaders) - {"half_width", "max_range"}
+            if unknown:
+                raise ValueError(f"leaders: unknown keys {sorted(unknown)}")
+            self.leaders = dict(half_width=float(self.leaders.get("half_width", 1.8)),
+                                max_range=float(self.leaders.get("max_range", 100.0)))
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -215,6 +227,8 @@ class BatchedTrafficEnv:
             self._bind_sampler(self.sampler.get("seed", 0))
         if self.history is not None:
             self.world.set_history(self.history["length"])
+        if self.leaders is not None:
+            self.world.set_leader_search(**self.leaders)
         self._last_obs = None
         if observation == "bev":
             w, h = self.bev_resolution
@@ -260,9 +274,9 @@ class BatchedTrafficEnv:
         return info
 
     def _add_lidar(self, info):
-        """``info["lidar"]`` / ``info["bev"]`` / ``info["route"]`` / ``info["history"]`` when the env has a lidar / a camera
-        / routes / a history; called after the auto-reset and the observation, so that they see the new episodes and the
-        observation's agents."""
+        """``info["lidar"]`` / ``info["bev"]`` / ``info["route"]`` / ``info["history"]`` / ``info["leader"]`` and
+        ``info["leader_gap"]`` when the env has a lidar / a camera / routes / a history / a leader search; called after the
+        auto-reset and the observation, so that they see the new episodes and the observation's agents."""
         if self.route is not None:
             info["route"] = self.world.route_observe(self.route.get("n_points", 8), self.route.get("spacing", 2.0),
                                                      self._route_observers)
@@ -286,6 +300,8 @@ class BatchedTrafficEnv:
                 info["history"] = self.world.observe_history(self._last_obs.agent_index, self.vector_obs.get("observers"))
             else:
                 info["history"] = self.world.observe_history()
+        if self.leaders is not None:
+            info["leader"], info["leader_gap"] = self.world.find_leaders(**self.leaders)
         return info
 
     # ------------------------------------------------------------------ gym surface

@@ -180,6 +180,7 @@ class BatchedWorld:
         self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = self._sampler = None
         self._history, self._hist_out = 0, {}
         self._route_out = {}
+        self._leader = self._leader_out = None
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
         self._agent_lidar, self._obs_out, self._agent_obs_out, self._agent_bev = {}, {}, {}, {}
         self._seg_style_keys = []
@@ -363,7 +364,8 @@ class BatchedWorld:
         from the caller"; ``lead_index`` [N, M] int16: its leading vehicle (``leading_state`` / ``front_state``), -1 for
         none; ``path_id`` [N, M] int16: its pure-pursuit path or the PID rows' path (``set_paths``), -1 for none;
         ``last_accel`` [N, M]: ``State.accel`` of the previous tick (default zeros).  ``None`` for ``controllers``
-        removes them.
+        removes them.  While a leader search is bound (``set_leader_search``), ``control`` ignores ``lead_index`` and
+        every controller follows the leader the search finds on the same state in the same call.
 
         PID rows (``PIDController``): ``pid_target`` [N, M, 2] = (target_speed, target_heading or cross_track_error),
         fp32, read every tick (write new targets into ``self.pid_target`` in place).  Their memory is ``self.pid_state``,
@@ -417,6 +419,46 @@ class BatchedWorld:
         self._device_tensor("action", action, torch.float32, (self.N, self.M, 2))
         _lib.check(self.lib.t2d_control(self._ctx, _ptr(action), self._stream()))
         return action
+
+    # ------------------------------------------------------------------ leader search
+    def set_leader_search(self, half_width: Optional[float] = 1.8, max_range: float = 100.0):
+        """Find every slot's leader on the device in front of every ``control`` (``t2d_set_leader_search``, K17; DESIGN.md
+        section 1 "Leader search"): the nearest participant ahead within ``half_width`` metres of the slot's corridor and
+        at most ``max_range`` metres ahead - along the slot's controller path when it has one, else along its heading.
+        The controllers then follow these leaders instead of ``lead_index``, so the traffic reacts to every cut-in, reset,
+        replayed track and retirement.  The leaders of the last ``control`` are in :attr:`leader` (int16 [N, M], -1 for
+        none) and :attr:`leader_gap` (fp32 [N, M], +inf for none).  ``half_width=None`` unbinds.  A rejected call keeps the
+        previous search."""
+        if half_width is None:
+            _lib.check(self.lib.t2d_set_leader_search(self._ctx, 0.0, 0.0, _ptr(None), _ptr(None)))
+            self._leader = None
+            return
+        lead = torch.full((self.N, self.M), -1, dtype=torch.int16, device=self.device)
+        gap = torch.full((self.N, self.M), float("inf"), dtype=torch.float32, device=self.device)
+        _lib.check(self.lib.t2d_set_leader_search(self._ctx, float(half_width), float(max_range), _ptr(lead), _ptr(gap)))
+        self._leader = dict(lead=lead, gap=gap, half_width=float(half_width), max_range=float(max_range))
+
+    @property
+    def leader(self) -> Optional[torch.Tensor]:
+        """int16 [N, M] device tensor: the leaders the bound search found in the last ``control`` (None without one)."""
+        return None if self._leader is None else self._leader["lead"]
+
+    @property
+    def leader_gap(self) -> Optional[torch.Tensor]:
+        """fp32 [N, M] device tensor: the gap to each of those leaders, +inf where there is none."""
+        return None if self._leader is None else self._leader["gap"]
+
+    def find_leaders(self, half_width: float = 1.8, max_range: float = 100.0):
+        """The leaders of the current state in one launch (``t2d_find_leaders``, K17), with or without a bound search:
+        ``(lead, gap)``, int16 and fp32 [N, M] as :attr:`leader` / :attr:`leader_gap`.  The tensors are buffers the next
+        call reuses."""
+        if self._leader_out is None:
+            self._leader_out = (torch.empty((self.N, self.M), dtype=torch.int16, device=self.device),
+                                torch.empty((self.N, self.M), dtype=torch.float32, device=self.device))
+        lead, gap = self._leader_out
+        _lib.check(self.lib.t2d_find_leaders(self._ctx, float(half_width), float(max_range), _ptr(lead), _ptr(gap),
+                                             self._stream()))
+        return lead, gap
 
     # ------------------------------------------------------------------ route following
     def set_routes(self, route_id, threshold: float = None, progress_weight: float = 0.1, off_route_reward: float = -5.0):
