@@ -49,6 +49,8 @@
  *   t2d_set_leader_search / t2d_find_leaders
  *                        (no reference counterpart) the leader of every slot in its corridor, for the controllers'
  *                        `leading_state` / `front_state`
+ *   t2d_set_lane_change  (no reference counterpart) MOBIL lane changes (Kesting, Treiber and Helbing 2007) for the IDM
+ *                        rows with a lateral channel, decided on the device before every t2d_control
  *   t2d_check_events     the same detectors on caller-supplied poses (no physics)
  *   t2d_reset            ScenarioManager.reset / ParticipantBase.reset
  *                                                         tactics2d/envs/parking.py:397-441, participant_base.py:236-246
@@ -477,7 +479,9 @@ int t2d_observe_agents(t2d_ctx* ctx, const t2d_obs_config* cfg, const int16_t* o
 
 /* On-device NPC controllers (tactics2d/controller).  A controller row is one configured controller object; the fields
  * are the reference's attribute names.  kind selects the law:
- *   T2D_CTRL_IDM           IDMController.step               (steering 0; free flow, or car following when a leader is set)
+ *   T2D_CTRL_IDM           IDMController.step               (steering 0; free flow, or car following when a leader is set;
+ *                                                            with pid_lateral PATH_HEADING / PATH_CROSS_TRACK the steering
+ *                                                            is a PID row's lateral channel on the slot's path, see below)
  *   T2D_CTRL_CRUISE        AccelerationController.step      (steering 0; cruise, or adaptive cruise with a leader)
  *   T2D_CTRL_PURE_PURSUIT  PurePursuitController.step       (pure-pursuit steering on a path + the cruise laws)
  *   T2D_CTRL_PID           PIDController.step               (PID steering and acceleration with per-slot state, t2d_set_pid) */
@@ -524,15 +528,24 @@ typedef struct t2d_controller_params {
  * takes every leader from the search, found on the same state in the same call; path_id [N, M] int16 = the pure-pursuit path, -1 for none (NULL allowed);
  * last_accel [N, M] float = |acceleration| each participant applied on the previous tick (State.accel,
  * participant/trajectory/state.py:171-185), read and rewritten by t2d_control; zero it before the first tick.
- * table == NULL removes the controllers.  Rejected (the previous binding stays whole): an unknown kind, and a PID row with
+ * Lane keeping (an extension, DESIGN.md section 1 "Lane keeping for IDM rows"): an IDM row whose pid_lateral is
+ * T2D_PID_LAT_PATH_HEADING or T2D_PID_LAT_PATH_CROSS_TRACK keeps its IDM acceleration and steers with the lateral half of
+ * the PID law on the slot's path (kp_lat / ki_lat / kd_lat, dt, derivative_filter_alpha, max_steering, wheel_base; the
+ * same code and rounding as a PID row with pid_longitudinal NONE, the same state[..., 0:3] of t2d_set_pid, never the
+ * target).  Such a row needs t2d_set_pid's state like a PID row; its pid_longitudinal is not read.  An IDM row with
+ * pid_lateral NONE is the reference's IDM.
+ * table == NULL removes the controllers.  Every call that is not rejected drops a bound lane change
+ * (t2d_set_lane_change).  Rejected (the previous binding stays whole): an unknown kind, a PID row with
  * dt <= 0, max_steering <= 0, max_accel <= 0, min_accel >= 0, max_accel <= min_accel, derivative_filter_alpha outside
- * (0, 1], an unknown source, or wheel_base <= 0 with a cross-track source. */
+ * (0, 1], an unknown source, or wheel_base <= 0 with a cross-track source, and an IDM row whose pid_lateral is neither
+ * NONE nor a PATH source, or that has one with dt <= 0, max_steering <= 0, derivative_filter_alpha outside (0, 1], or
+ * wheel_base <= 0 with PATH_CROSS_TRACK. */
 int t2d_set_controllers(t2d_ctx* ctx, const t2d_controller_params* table, int n_rows, const uint8_t* ctrl_id,
                         const int16_t* lead_index, const int16_t* path_id, float* last_accel);
 
 /* Pure-pursuit paths: HOST arrays, copied.  xy [V][2] vertices of all paths back to back, offsets [n_paths + 1] (path p
  * owns vertices offsets[p] .. offsets[p + 1] - 1, at least 2).  n_paths == 0 or xy == NULL unbinds.  Rejected (the
- * previous paths stay bound): malformed offsets. */
+ * previous paths stay bound): malformed offsets.  Every call that is not rejected drops a bound lane change. */
 int t2d_set_paths(t2d_ctx* ctx, const float* xy, const int32_t* offsets, int n_paths);
 
 /* ---- route following: the OffRoute detector, route progress and the route observation --------------------------------
@@ -651,6 +664,45 @@ int t2d_control(t2d_ctx* ctx, float* action, void* stream);
  * bound (T2D_E_STATE). */
 int t2d_set_leader_search(t2d_ctx* ctx, double half_width, double max_range, int16_t* lead, float* gap);
 int t2d_find_leaders(t2d_ctx* ctx, double half_width, double max_range, int16_t* lead, float* gap, void* stream);
+/* Unbinding the search (lead == NULL) also drops a bound lane change. */
+
+/* ---- lane changes (K18, no reference counterpart): MOBIL (Kesting, Treiber and Helbing 2007) ---------------------------
+ * DESIGN.md section 1 "Lane changes".  Evaluated on the state K5 reads next, fp64 with one rounding per operation except
+ * the IDM accelerations, which are K5's own idm_law.  Candidates are the leader search's; a candidate is on path r when
+ * its distance to r (t2d_set_routes' closest point) is <= the bound search's half_width, s^r is its arc length there.
+ *   A lane changer is a slot whose controller row is an IDM row with a lateral channel, whose current path
+ * p = lane_path[n][m] has a segment of non-zero length, whose cooldown is 0 and which is itself on p.  Its target lanes
+ * are left[p] and right[p] when >= 0.  On a target q: blocked when a candidate on q has |s^q_j - s^q_c| < min_gap; the new
+ * leader l' is the candidate on q of smallest gap s^q_j - s^q_c in (0, max_range] (ties: lower slot), the new follower n
+ * the same behind; the old leader l and follower o are the same on p.  a(f | L) is idm_law with f's own IDM row (the
+ * changer's row when f has none); a missing leader is free flow, a missing follower gives 0 to both its terms.
+ *   safe       a(n | c) >= -b_safe, or no new follower;
+ *   incentive  (a(c | l') - a(c | l)) + politeness ((a(n | c) - a(n | l')) + (a(o | l) - a(o | c))).
+ * Among the unblocked safe sides with incentive > threshold the larger incentive wins (a tie goes left): lane_path = q,
+ * cooldown = params.cooldown, change = +1 (left) / -1 (right).  Every other slot: change = 0 and a positive cooldown
+ * counts down by 1.  All decisions of a scenario are made on the same state (two cars may take the same gap).
+ *   t2d_set_lane_change binds it: left / right HOST int16 [n_paths] (-1: none), copied; lane_path, cooldown DEVICE int16
+ * [N][M] and change DEVICE int8 [N][M] (may be NULL) owned by the caller.  The call copies the controllers' path_id into
+ * lane_path and zeroes cooldown (and change).  While bound, t2d_control, t2d_step_host_ego and t2d_step_host_agents launch
+ * K18, then K17, then K5; K17 (also under t2d_find_leaders) and K5's path reads take lane_path instead of path_id, which is
+ * never written (it stays the episode's starting lane).  t2d_reset / t2d_reset_sampled copy path_id into lane_path and
+ * zero cooldown and change for the reset scenarios.  p == NULL unbinds; with nothing bound nothing of this launches.
+ * t2d_set_controllers, t2d_set_paths and unbinding the leader search drop the binding.
+ * Rejected (a rejected call keeps the previous binding whole): politeness < 0 or not finite, threshold not finite,
+ * b_safe <= 0 or not finite, min_gap <= 0, min_gap > max_range or not finite, cooldown outside 0..32767, NULL left / right
+ * / lane_path / cooldown, a left / right entry outside [-1, n_paths) or naming its own path, lane_path or cooldown not
+ * 2-byte aligned (T2D_E_INVALID); state, type table, controllers, their path_id, paths or the leader search not bound
+ * (T2D_E_STATE). */
+typedef struct t2d_lane_change_params {
+  double politeness; /* p: weight of the followers' accelerations */
+  double threshold;  /* a_th (m/s^2): the incentive must exceed it */
+  double b_safe;     /* (m/s^2): the new follower's predicted deceleration limit */
+  double min_gap;    /* (m): the blocking distance along the target lane, in (0, max_range] */
+  int32_t cooldown;  /* ticks without a decision after a change, 0..32767 */
+  int32_t reserved;  /* 0 */
+} t2d_lane_change_params; /* 40 bytes */
+int t2d_set_lane_change(t2d_ctx* ctx, const t2d_lane_change_params* p, const int16_t* left, const int16_t* right,
+                        int16_t* lane_path, int16_t* cooldown, int8_t* change);
 
 /* Inputs and memory of the PID rows: DEVICE arrays owned by the caller.  target [N][M][2] fp32 = (target_speed, lateral
  * target: target_heading in rad for HEADING rows, cross_track_error in m for CROSS_TRACK rows; PATH rows ignore it);

@@ -46,6 +46,12 @@ class ControllerParamsC(C.Structure):
         "dt", "kp_lat", "ki_lat", "kd_lat", "max_steering", "kp_lon", "ki_lon", "kd_lon", "derivative_filter_alpha")]
 
 
+class LaneChangeParamsC(C.Structure):
+    """``t2d_lane_change_params``: the MOBIL parameters of a bound lane change."""
+    _fields_ = [(n, C.c_double) for n in ("politeness", "threshold", "b_safe", "min_gap")] + [
+        ("cooldown", C.c_int32), ("reserved", C.c_int32)]
+
+
 class BevStyleC(C.Structure):
     """``t2d_bev_style``: colour, z order and stroke width (points) of one BEV style row."""
     _fields_ = [("r", C.c_uint8), ("g", C.c_uint8), ("b", C.c_uint8), ("z", C.c_int8), ("line_width_pt", C.c_float)]
@@ -118,6 +124,7 @@ SYMBOLS = {
     "t2d_set_pid": (C.c_int, [_P, _P, _P]),
     "t2d_set_leader_search": (C.c_int, [_P, C.c_double, C.c_double, _P, _P]),
     "t2d_find_leaders": (C.c_int, [_P, C.c_double, C.c_double, _P, _P, _P]),
+    "t2d_set_lane_change": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
     "t2d_set_routes": (C.c_int, [_P, _P, C.c_double, C.c_double, C.c_float]),
     "t2d_bind_route_trackers": (C.c_int, [_P, _P, _P, C.c_int32]),
     "t2d_route_observe": (C.c_int, [_P, _P, C.c_int32, C.c_int, C.c_float, _P, _P]),

@@ -151,14 +151,13 @@ __device__ bool path_lateral_error(const PathVertex* pv, int n_vert, double x, d
   return true;
 }
 
-// pid_controller.py:309-406 for slot i: (steering, acceleration) into steer / acc; the slot's state row is rewritten
-// for each channel that runs.  A channel whose source is NONE, or whose error is missing (a PATH source without a usable
-// path: the combined mode's missing keyword), gives 0 and leaves its half of the row alone.
-__device__ void pid_law(const t2d_controller_params& p, const CtrlArgs& A, size_t i, double x, double y, double v,
-                        double heading, double& steer, double& acc) {
+// The lateral channel of pid_controller.py:309-406 for slot i: the steering, 0 when the source is NONE or its error is
+// missing (a PATH source without a usable path: the combined mode's missing keyword); the lateral half of the slot's state
+// row is rewritten when the channel runs.  PID rows and IDM rows with a lateral channel (lane keeping) share it.
+__device__ __forceinline__ double pid_lateral_law(const t2d_controller_params& p, const CtrlArgs& A, size_t i, double x,
+                                                  double y, double heading) {
   double* st = A.pid_state + 6 * i;
-  steer = 0.0;
-  acc = 0.0;
+  double steer = 0.0;
   const int lat = p.pid_lateral;
   if (lat != T2D_PID_LAT_NONE) {
     double e = 0.0;
@@ -183,6 +182,17 @@ __device__ void pid_law(const t2d_controller_params& p, const CtrlArgs& A, size_
       st[0] = s[0]; st[1] = s[1]; st[2] = s[2];
     }
   }
+  return steer;
+}
+
+// pid_controller.py:309-406 for slot i: (steering, acceleration) into steer / acc; the slot's state row is rewritten
+// for each channel that runs.  A channel whose source is NONE, or whose error is missing, gives 0 and leaves its half of
+// the row alone.
+__device__ void pid_law(const t2d_controller_params& p, const CtrlArgs& A, size_t i, double x, double y, double v,
+                        double heading, double& steer, double& acc) {
+  double* st = A.pid_state + 6 * i;
+  steer = pid_lateral_law(p, A, i, x, y, heading);
+  acc = 0.0;
   if (p.pid_longitudinal == T2D_PID_LON_TARGET) {
     const double e = __dsub_rn((double)A.pid_target[2 * i], v);                              // :306-307
     double s[3] = {st[3], st[4], st[5]};
@@ -196,7 +206,8 @@ __device__ __forceinline__ const CtrlLawRow& law_row(const t2d_controller_params
   return *reinterpret_cast<const CtrlLawRow*>(reinterpret_cast<const char*>(ctab) + (size_t)cid * sizeof(t2d_controller_params));
 }
 
-// HAS_PID: the instance with the PID law, launched when the bound table holds a PID row; the other one is today's K5.
+// HAS_PID: the instance with the PID law, launched when the bound table holds a PID row or an IDM row with a lateral
+// channel; the other one is the plain K5.
 template <bool HAS_PID>
 __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant__ CtrlArgs A) {
   const int lane = threadIdx.x & 31;
@@ -233,6 +244,9 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
           pid_law(A.ctab[cid], A, base + m, x, y, v, (double)A.h[base + m], steer, acc);
         } else if (p.kind == T2D_CTRL_IDM) {
           acc = idm_law(p, v, x, y, has, vl, xl, yl);
+          // lane keeping: an IDM row with a lateral channel (only a PATH source passes t2d_set_controllers)
+          if (HAS_PID && A.ctab[cid].pid_lateral != T2D_PID_LAT_NONE)
+            steer = pid_lateral_law(A.ctab[cid], A, base + m, x, y, (double)A.h[base + m]);
         } else {
           acc = longitudinal_law(p, v, x, y, (double)A.last_accel[base + m], has, vl, xl, yl, al);
           if (p.kind == T2D_CTRL_PURE_PURSUIT) {

@@ -27,6 +27,9 @@
 //                                (t2d_history.cuh).
 // K17 t2d_leader_kernel          the leader of every slot in its corridor, which K5 follows while a search is bound
 //                                (t2d_leader.cuh).
+// K18 t2d_lane_change_kernel     MOBIL lane changes of the IDM rows with a lateral channel, in front of K17 and K5 while
+//                                a lane change is bound; t2d_lane_reset_kernel restarts the reset scenarios' lanes
+//                                (t2d_lane.cuh).
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory (t2d_exchange.cuh).
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -57,6 +60,7 @@
 #include "t2d_obs.cuh"
 #include "t2d_history.cuh"
 #include "t2d_leader.cuh"
+#include "t2d_lane.cuh"
 
 // =============================================================================================
 // C ABI
@@ -213,6 +217,15 @@ struct AgentStaging {   // t2d_step_host_agents, sized for q rows per scenario
                                        // host: the part up to done
 };
 
+// A bound lane change: the parameters, the neighbour table on the device and the caller's per-slot arrays
+struct LaneChange {
+  t2d_lane_change_params p;
+  dev_ptr<int16_t> left, right;
+  int16_t* lane_path;
+  int16_t* cooldown;
+  int8_t* change;
+};
+
 struct t2d_ctx {
   int device = 0, N = 0, M = 0, G = 0;
   t2d_config cfg{};
@@ -263,6 +276,8 @@ struct t2d_ctx {
   int16_t* leader_lead = nullptr;
   float* leader_gap = nullptr;
   double leader_half_width = 0.0, leader_max_range = 0.0;
+  // lane change (t2d_set_lane_change / K18); lane == nullptr: none bound, K17 and K5 read ctrl_path
+  std::unique_ptr<LaneChange> lane;
   // routes (t2d_set_routes / t2d_bind_route_trackers); route_id == nullptr: none bound
   const int16_t* route_id = nullptr;
   double route_threshold = 0.0, route_weight = 0.0;
@@ -1153,13 +1168,31 @@ static int check_leader_args(const char* fn, double half_width, double max_range
   return T2D_OK;
 }
 
+// The slots' current paths: a bound lane change's lane_path, else the controllers' path_id
+static const int16_t* current_path(const t2d_ctx* c) { return c->lane ? c->lane->lane_path : c->ctrl_path; }
+
 // K17 on the bound state and the controllers' paths; the caller has checked the arguments and the bindings
 static int launch_leaders(t2d_ctx* c, double half_width, double max_range, int16_t* lead, float* gap, void* stream) {
   CUDA_TRY(cudaSetDevice(c->device));
   leader::Args A{world_args(c)};
-  A.path_id = c->ctrl_path; A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.path_id = current_path(c); A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
   A.half_width = half_width; A.max_range = max_range; A.lead = lead; A.gap = gap;
   leader::t2d_leader_kernel<<<(c->N + leader::WARPS - 1) / leader::WARPS, leader::WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  return launched();
+}
+
+// K18 on the bound state with the bound lane change and search; the caller has checked the bindings
+static int launch_lane_change(t2d_ctx* c, void* stream) {
+  const LaneChange& L = *c->lane;
+  lane::Args A{world_args(c)};
+  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id;
+  A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.left = L.left.get(); A.right = L.right.get();
+  A.half_width = c->leader_half_width; A.max_range = c->leader_max_range;
+  A.politeness = L.p.politeness; A.threshold = L.p.threshold; A.b_safe = L.p.b_safe; A.min_gap = L.p.min_gap;
+  A.cooldown = L.p.cooldown;
+  A.lane_path = L.lane_path; A.cool = L.cooldown; A.change = L.change;
+  lane::t2d_lane_change_kernel<<<(c->N + lane::WARPS - 1) / lane::WARPS, lane::WARPS * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
 }
 
@@ -1170,11 +1203,14 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
   if (!action) return fail(T2D_E_INVALID, "action is NULL");
   if (!aligned8(action)) return fail(T2D_E_INVALID, "action must be 8-byte aligned");
   CUDA_TRY(cudaSetDevice(c->device));
+  // a bound lane change decides first (it is only bound with a search), on the state K17 and K5 read next
+  if (c->lane)
+    if (int r = launch_lane_change(c, stream)) return r;
   // a bound search finds the leaders on the state K5 reads next, and K5 follows them instead of the controllers' lead_index
   if (c->leader_lead)
     if (int r = launch_leaders(c, c->leader_half_width, c->leader_max_range, c->leader_lead, c->leader_gap, stream)) return r;
   CtrlArgs A{world_args(c)};
-  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.path_id = c->ctrl_path;
+  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.path_id = current_path(c);
   A.lead = c->leader_lead ? c->leader_lead : c->ctrl_lead;
   A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
   A.last_accel = c->ctrl_last_accel; A.action = action; A.ego_action = ego;
@@ -1489,6 +1525,11 @@ static int launch_reset(t2d_ctx* c, const uint8_t* mask, const int32_t* pool_ind
   }
   t2d_reset_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(A);
   if (int r = launched()) return r;
+  if (c->lane) {   // the new episodes start from their starting lanes
+    lane::ResetArgs R{mask, c->ctrl_path, c->lane->lane_path, c->lane->cooldown, c->lane->change, (long long)c->N, c->M};
+    lane::t2d_lane_reset_kernel<<<capped_grid((long long)c->N * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(R);
+    if (int r = launched()) return r;
+  }
   if (c->log) return launch_replay(c, stream, 0, c->N, 0, mask, pool_index);   // the new episode's traffic at t0
   return T2D_OK;
 }
@@ -1818,6 +1859,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
     c->n_ctrl = 0; c->ctrl_id = nullptr; c->ctrl_lead = nullptr; c->ctrl_path = nullptr;
     c->ctrl_last_accel = nullptr;
     c->ctrl_has_pid = c->ctrl_pid_reads_target = false;
+    c->lane.reset();
     return T2D_OK;
   }
   if (n_rows <= 0 || n_rows > T2D_MAX_CONTROLLERS) return fail(T2D_E_INVALID, "n_rows must be in 1..T2D_MAX_CONTROLLERS");
@@ -1844,6 +1886,17 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
       reads_target = reads_target || p.pid_longitudinal == T2D_PID_LON_TARGET || p.pid_lateral == T2D_PID_LAT_HEADING ||
                      p.pid_lateral == T2D_PID_LAT_CROSS_TRACK;
     }
+    if (p.kind == T2D_CTRL_IDM && p.pid_lateral != T2D_PID_LAT_NONE) {   // lane keeping: the PID row's lateral checks
+      if (p.pid_lateral != T2D_PID_LAT_PATH_HEADING && p.pid_lateral != T2D_PID_LAT_PATH_CROSS_TRACK)
+        return fail(T2D_E_INVALID, "IDM row: the lateral channel must be a PATH source");
+      if (!(p.dt > 0.0)) return fail(T2D_E_INVALID, "IDM row with a lateral channel: dt must be positive");
+      if (!(p.max_steering > 0.0)) return fail(T2D_E_INVALID, "IDM row with a lateral channel: max_steering must be positive");
+      if (!(p.derivative_filter_alpha > 0.0 && p.derivative_filter_alpha <= 1.0))
+        return fail(T2D_E_INVALID, "IDM row with a lateral channel: derivative_filter_alpha must be in range (0, 1]");
+      if (p.pid_lateral == T2D_PID_LAT_PATH_CROSS_TRACK && !(p.wheel_base > 0.0f))
+        return fail(T2D_E_INVALID, "IDM row with a lateral channel: wheel_base must be positive");
+      has_pid = true;   // K5's PID instance runs the channel, on t2d_set_pid's state
+    }
     if (p.kind == T2D_CTRL_PURE_PURSUIT && !(p.min_pre_aiming_distance > 0.0f))
       return fail(T2D_E_INVALID, "min_pre_aiming_distance must be positive");   // pure_pursuit_controller.py:30-31
     if (p.kind >= T2D_CTRL_CRUISE && p.target_speed < 0.0f)
@@ -1852,6 +1905,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
   if (int r = upload(c->d_ctab, table, (size_t)n_rows)) return r;
   c->n_ctrl = n_rows; c->ctrl_id = ctrl_id; c->ctrl_lead = lead_index; c->ctrl_path = path_id; c->ctrl_last_accel = last_accel;
   c->ctrl_has_pid = has_pid; c->ctrl_pid_reads_target = reads_target;
+  c->lane.reset();   // its lane_path was copied from the old path_id
   return T2D_OK;
 }
 
@@ -1873,6 +1927,7 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   CUDA_TRY(cudaSetDevice(c->device));
   if (n_paths == 0 || !xy) {   // unbind
     c->d_path_v.reset(); c->d_path_off.reset(); c->n_paths = 0;
+    c->lane.reset();
     return T2D_OK;
   }
   if (n_paths < 0 || !offsets) return fail(T2D_E_INVALID, "t2d_set_paths: bad argument");
@@ -1898,6 +1953,7 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   if (int r = upload(d_v, pv.data(), pv.size())) return r;
   if (int r = upload(d_off, offsets, (size_t)n_paths + 1)) return r;
   c->d_path_v = std::move(d_v); c->d_path_off = std::move(d_off); c->n_paths = n_paths;
+  c->lane.reset();   // its neighbour table named the old paths
   return T2D_OK;
 }
 
@@ -1953,6 +2009,7 @@ int t2d_set_leader_search(t2d_ctx* c, double half_width, double max_range, int16
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (!lead) {   // unbind
     c->leader_lead = nullptr; c->leader_gap = nullptr; c->leader_half_width = c->leader_max_range = 0.0;
+    c->lane.reset();   // a lane change reads the search's corridor
     return T2D_OK;
   }
   if (int r = check_leader_args("t2d_set_leader_search", half_width, max_range, lead, gap)) return r;
@@ -1968,6 +2025,52 @@ int t2d_find_leaders(t2d_ctx* c, double half_width, double max_range, int16_t* l
   if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   return launch_leaders(c, half_width, max_range, lead, gap, stream);
 }
+
+int t2d_set_lane_change(t2d_ctx* c, const t2d_lane_change_params* p, const int16_t* left, const int16_t* right,
+                        int16_t* lane_path, int16_t* cooldown, int8_t* change) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!p) {   // unbind
+    c->lane.reset();
+    return T2D_OK;
+  }
+  if (!(std::isfinite(p->politeness) && p->politeness >= 0.0))
+    return fail(T2D_E_INVALID, "t2d_set_lane_change: politeness must be finite and >= 0");
+  if (!std::isfinite(p->threshold)) return fail(T2D_E_INVALID, "t2d_set_lane_change: threshold must be finite");
+  if (!(std::isfinite(p->b_safe) && p->b_safe > 0.0))
+    return fail(T2D_E_INVALID, "t2d_set_lane_change: b_safe must be finite and > 0");
+  if (!(std::isfinite(p->min_gap) && p->min_gap > 0.0))
+    return fail(T2D_E_INVALID, "t2d_set_lane_change: min_gap must be finite and > 0");
+  if (p->cooldown < 0 || p->cooldown > 32767) return fail(T2D_E_INVALID, "t2d_set_lane_change: cooldown must be in 0..32767");
+  if (!left || !right || !lane_path || !cooldown)
+    return fail(T2D_E_INVALID, "t2d_set_lane_change: left / right / lane_path / cooldown is NULL");
+  if (!aligned2(lane_path) || !aligned2(cooldown))
+    return fail(T2D_E_INVALID, "t2d_set_lane_change: lane_path and cooldown must be 2-byte aligned");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (!c->d_ctab) return fail(T2D_E_STATE, "t2d_set_lane_change: controllers not set: call t2d_set_controllers first");
+  if (!c->ctrl_path) return fail(T2D_E_STATE, "t2d_set_lane_change: the controllers have no path_id");
+  if (c->n_paths == 0) return fail(T2D_E_STATE, "t2d_set_lane_change: no paths bound: call t2d_set_paths first");
+  if (!c->leader_lead) return fail(T2D_E_STATE, "t2d_set_lane_change: no leader search bound: call t2d_set_leader_search first");
+  if (p->min_gap > c->leader_max_range)
+    return fail(T2D_E_INVALID, "t2d_set_lane_change: min_gap must not exceed the search's max_range");
+  for (int q = 0; q < c->n_paths; ++q) {
+    if (left[q] < -1 || left[q] >= c->n_paths || right[q] < -1 || right[q] >= c->n_paths)
+      return fail(T2D_E_INVALID, "t2d_set_lane_change: a neighbour must be -1 or a path of the table");
+    if (left[q] == q || right[q] == q) return fail(T2D_E_INVALID, "t2d_set_lane_change: a path cannot be its own neighbour");
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  auto L = std::make_unique<LaneChange>();
+  L->p = *p;
+  if (int r = upload(L->left, left, (size_t)c->n_paths)) return r;
+  if (int r = upload(L->right, right, (size_t)c->n_paths)) return r;
+  L->lane_path = lane_path; L->cooldown = cooldown; L->change = change;
+  const size_t nm = (size_t)c->N * c->M;
+  CUDA_TRY(cudaMemcpy(lane_path, c->ctrl_path, nm * sizeof(int16_t), cudaMemcpyDeviceToDevice));
+  CUDA_TRY(cudaMemset(cooldown, 0, nm * sizeof(int16_t)));
+  if (change) CUDA_TRY(cudaMemset(change, 0, nm));
+  c->lane = std::move(L);
+  return T2D_OK;
+}
+
 int t2d_exchange_create(t2d_exchange** out, int device, int world, int rank, int n_local, int slots, void* ipc_handle_out) {
   if (!out || !ipc_handle_out) return fail(T2D_E_INVALID, "out / ipc_handle_out is NULL");
   *out = nullptr;

@@ -51,7 +51,7 @@ class BatchedTrafficEnv:
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
                  agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
                  route: Optional[dict] = None, sampler: Optional[dict] = None, history: Optional[dict] = None,
-                 camera: Optional[dict] = None, leaders: Optional[dict] = None):
+                 camera: Optional[dict] = None, leaders: Optional[dict] = None, lane_change: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -111,7 +111,14 @@ class BatchedTrafficEnv:
         DESIGN.md section 1 "Leader search"), so the controllers set on ``env.world`` follow the participant ahead of them
         every step instead of a fixed ``lead_index``, and adds ``info["leader"]`` (int16 [N, M], -1 for none) and
         ``info["leader_gap"]`` (fp32 [N, M], +inf for none) to ``reset`` and ``step``: the leaders of the state after the
-        auto-reset (``BatchedWorld.find_leaders``)."""
+        auto-reset (``BatchedWorld.find_leaders``);
+        ``lane_change``: e.g. ``dict(left=[1, -1], right=[-1, 0], politeness=0.0)`` (the keywords of
+        ``BatchedWorld.set_lane_change``; needs ``leaders``) lets the IDM rows with a lateral channel change lanes with
+        MOBIL (DESIGN.md section 1 "Lane changes").  It is bound after the search, at ``reset`` - set the paths and the
+        controllers (with ``path_id``) on ``env.world`` first - and bound again there whenever ``set_controllers`` or
+        ``set_paths`` dropped it.  It adds ``info["lane_path"]`` (int16 [N, M], every slot's current lane) and
+        ``info["lane_change"]`` (int8 [N, M], the decisions of the step) to ``reset`` and ``step``, after the auto-reset,
+        which restarts the reset scenarios from their ``path_id``."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -177,6 +184,15 @@ class BatchedTrafficEnv:
                 raise ValueError(f"leaders: unknown keys {sorted(unknown)}")
             self.leaders = dict(half_width=float(self.leaders.get("half_width", 1.8)),
                                 max_range=float(self.leaders.get("max_range", 100.0)))
+        self.lane_change = None if lane_change is None else dict(lane_change)
+        if self.lane_change is not None:
+            if self.leaders is None:
+                raise ValueError("lane_change needs a leader search: pass leaders=dict(...)")
+            unknown = set(self.lane_change) - {"left", "right", "politeness", "threshold", "b_safe", "min_gap", "cooldown"}
+            if unknown:
+                raise ValueError(f"lane_change: unknown keys {sorted(unknown)}")
+            if "left" not in self.lane_change or "right" not in self.lane_change:
+                raise ValueError("lane_change needs the 'left' and 'right' neighbour tables")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -302,6 +318,8 @@ class BatchedTrafficEnv:
                 info["history"] = self.world.observe_history()
         if self.leaders is not None:
             info["leader"], info["leader_gap"] = self.world.find_leaders(**self.leaders)
+        if self.lane_change is not None:
+            info["lane_path"], info["lane_change"] = self.world.lane_path, self.world.lane_change
         return info
 
     # ------------------------------------------------------------------ gym surface
@@ -317,6 +335,8 @@ class BatchedTrafficEnv:
         perm = None
         if options and options.get("shuffle"):
             perm = torch.from_numpy(self._rng.permutation(self.num_envs).astype(np.int32)).to(self.world.device)
+        if self.lane_change is not None and self.world.lane_path is None:   # bound after the search, on the set controllers
+            self.world.set_lane_change(**self.lane_change)
         if self.agent_rewards:   # every slot takes its pool row's type below; no retired type of the old episodes survives
             self.world.retired_type.fill_(255)
             self.world.reset_agent_trackers()

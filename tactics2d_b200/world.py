@@ -180,7 +180,7 @@ class BatchedWorld:
         self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = self._sampler = None
         self._history, self._hist_out = 0, {}
         self._route_out = {}
-        self._leader = self._leader_out = None
+        self._leader = self._leader_out = self._lane = None
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
         self._agent_lidar, self._obs_out, self._agent_obs_out, self._agent_bev = {}, {}, {}, {}
         self._seg_style_keys = []
@@ -356,6 +356,7 @@ class BatchedWorld:
             off[1:] = np.cumsum([len(p) for p in paths])
             _lib.check(self.lib.t2d_set_paths(self._ctx, C.c_void_p(xy.ctypes.data), C.c_void_p(off.ctypes.data), len(paths)))
         self.paths = paths
+        self._lane = None   # the library dropped a bound lane change
 
     def set_controllers(self, controllers, ctrl_id, lead_index=None, path_id=None, last_accel=None, pid_target=None,
                         pid_state=None):
@@ -364,7 +365,8 @@ class BatchedWorld:
         from the caller"; ``lead_index`` [N, M] int16: its leading vehicle (``leading_state`` / ``front_state``), -1 for
         none; ``path_id`` [N, M] int16: its pure-pursuit path or the PID rows' path (``set_paths``), -1 for none;
         ``last_accel`` [N, M]: ``State.accel`` of the previous tick (default zeros).  ``None`` for ``controllers``
-        removes them.  While a leader search is bound (``set_leader_search``), ``control`` ignores ``lead_index`` and
+        removes them, and any call drops a bound lane change (``set_lane_change``).  An ``IDMController(lateral=...)``
+        row keeps its lane: it steers along its path with a PID lateral channel, on ``pid_state``.  While a leader search is bound (``set_leader_search``), ``control`` ignores ``lead_index`` and
         every controller follows the leader the search finds on the same state in the same call.
 
         PID rows (``PIDController``): ``pid_target`` [N, M, 2] = (target_speed, target_heading or cross_track_error),
@@ -375,7 +377,7 @@ class BatchedWorld:
         if controllers is None:
             _lib.check(self.lib.t2d_set_controllers(self._ctx, _ptr(None), 0, _ptr(None), _ptr(None), _ptr(None), _ptr(None)))
             _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(None), _ptr(None)))
-            self._ctrl = None
+            self._ctrl = self._lane = None
             return
         rows = [c if isinstance(c, _lib.ControllerParamsC) else c.params() for c in controllers]
         arr = (_lib.ControllerParamsC * len(rows))(*rows)
@@ -385,10 +387,11 @@ class BatchedWorld:
         la = dev(last_accel, torch.float32)
         if la is None:
             la = torch.zeros(NM, dtype=torch.float32, device=self.device)
-        from .controller.controller_base import CTRL_PID
+        from .controller.controller_base import CTRL_IDM, CTRL_PID, PID_LAT_NONE
 
         tgt, st = None, None
-        if any(r.kind == CTRL_PID for r in rows):
+        # PID rows and IDM rows with a lateral channel (lane keeping) keep their PID memory in pid_state
+        if any(r.kind == CTRL_PID or (r.kind == CTRL_IDM and r.pid_lateral != PID_LAT_NONE) for r in rows):
             if pid_target is not None:
                 tgt = self._to_device(pid_target, torch.float32, NM + (2,))
             if pid_state is None:
@@ -399,6 +402,7 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_set_controllers(self._ctx, arr, len(rows), _ptr(cid), _ptr(lead), _ptr(pid), _ptr(la)))
         _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(tgt), _ptr(st)))
         self._ctrl = dict(rows=arr, ctrl_id=cid, lead_index=lead, path_id=pid, last_accel=la, pid_target=tgt, pid_state=st)
+        self._lane = None   # the library dropped a bound lane change
 
     @property
     def last_accel(self) -> Optional[torch.Tensor]:
@@ -427,11 +431,11 @@ class BatchedWorld:
         at most ``max_range`` metres ahead - along the slot's controller path when it has one, else along its heading.
         The controllers then follow these leaders instead of ``lead_index``, so the traffic reacts to every cut-in, reset,
         replayed track and retirement.  The leaders of the last ``control`` are in :attr:`leader` (int16 [N, M], -1 for
-        none) and :attr:`leader_gap` (fp32 [N, M], +inf for none).  ``half_width=None`` unbinds.  A rejected call keeps the
-        previous search."""
+        none) and :attr:`leader_gap` (fp32 [N, M], +inf for none).  ``half_width=None`` unbinds, and drops a bound lane
+        change.  A rejected call keeps the previous search."""
         if half_width is None:
             _lib.check(self.lib.t2d_set_leader_search(self._ctx, 0.0, 0.0, _ptr(None), _ptr(None)))
-            self._leader = None
+            self._leader = self._lane = None   # unbinding the search drops a bound lane change
             return
         lead = torch.full((self.N, self.M), -1, dtype=torch.int16, device=self.device)
         gap = torch.full((self.N, self.M), float("inf"), dtype=torch.float32, device=self.device)
@@ -459,6 +463,55 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_find_leaders(self._ctx, float(half_width), float(max_range), _ptr(lead), _ptr(gap),
                                              self._stream()))
         return lead, gap
+
+    # ------------------------------------------------------------------ lane changes
+    def set_lane_change(self, left, right=None, politeness: float = 0.0, threshold: float = 0.2, b_safe: float = 2.0,
+                        min_gap: float = 6.0, cooldown: int = 10):
+        """MOBIL lane changes on the device in front of every ``control`` (``t2d_set_lane_change``, K18; DESIGN.md section 1
+        "Lane changes").  ``left`` / ``right``: the left and right neighbour of every path of ``set_paths``, -1 for none.
+        Every IDM row with a lateral channel (``IDMController(lateral=...)``) that is on its current lane and out of its
+        cooldown moves to a neighbour when that gains it more than ``threshold`` m/s^2 (its followers' gains weighted by
+        ``politeness``), no car is within ``min_gap`` metres along the target lane, and the new follower brakes no harder
+        than ``b_safe``; it then waits ``cooldown`` ticks.  Needs the controllers (with ``path_id``), the paths and a
+        leader search, whose corridor it uses.  The current lanes are in :attr:`lane_path` (from ``path_id`` at binding and
+        at every reset), the last decisions in :attr:`lane_change` (+1 left, -1 right, 0) and the cooldowns in
+        :attr:`lane_cooldown`.  ``left=None`` unbinds; ``set_controllers``, ``set_paths`` and unbinding the search drop it.
+        A rejected call keeps the previous binding."""
+        if left is None:
+            _lib.check(self.lib.t2d_set_lane_change(self._ctx, None, None, None, None, None, None))
+            self._lane = None
+            return
+        n_paths = 0 if self.paths is None else len(self.paths)
+        nb = []
+        for name, a in (("left", left), ("right", right)):
+            a = np.ascontiguousarray(np.asarray(a, dtype=np.int64).reshape(-1))
+            if a.shape != (n_paths,) or (a < -32768).any() or (a > 32767).any():   # the library checks the entries
+                raise ValueError(f"{name} must hold one int16 neighbour per path of set_paths ({n_paths})")
+            nb.append(np.ascontiguousarray(a.astype(np.int16)))
+        p = _lib.LaneChangeParamsC(politeness=float(politeness), threshold=float(threshold), b_safe=float(b_safe),
+                                   min_gap=float(min_gap), cooldown=int(cooldown))
+        NM = (self.N, self.M)
+        lane_path = torch.full(NM, -1, dtype=torch.int16, device=self.device)
+        cool = torch.zeros(NM, dtype=torch.int16, device=self.device)
+        change = torch.zeros(NM, dtype=torch.int8, device=self.device)
+        _lib.check(self.lib.t2d_set_lane_change(self._ctx, C.byref(p), C.c_void_p(nb[0].ctypes.data),
+                                                C.c_void_p(nb[1].ctypes.data), _ptr(lane_path), _ptr(cool), _ptr(change)))
+        self._lane = dict(params=p, left=nb[0], right=nb[1], lane_path=lane_path, cooldown=cool, change=change)
+
+    @property
+    def lane_path(self) -> Optional[torch.Tensor]:
+        """int16 [N, M] device tensor: every slot's current path while a lane change is bound (None without one)."""
+        return None if self._lane is None else self._lane["lane_path"]
+
+    @property
+    def lane_change(self) -> Optional[torch.Tensor]:
+        """int8 [N, M] device tensor: the decisions of the last ``control``, +1 left, -1 right, 0 none."""
+        return None if self._lane is None else self._lane["change"]
+
+    @property
+    def lane_cooldown(self) -> Optional[torch.Tensor]:
+        """int16 [N, M] device tensor: the ticks each slot still waits before it may change lanes again."""
+        return None if self._lane is None else self._lane["cooldown"]
 
     # ------------------------------------------------------------------ route following
     def set_routes(self, route_id, threshold: float = None, progress_weight: float = 0.1, off_route_reward: float = -5.0):
