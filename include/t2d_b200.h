@@ -57,6 +57,8 @@
  *   t2d_set_log          Trajectory.get_state / Vehicle.get_pose of logged participants at a frame
  *                                                         participant/trajectory/trajectory.py:97-113, vehicle.py:263-281
  *   t2d_set_log_schedule the same, with several tracks replayed one after the other in a slot
+ *   t2d_set_log_reactive (no reference counterpart) reactive log agents: a track handed over to path-following IDM after
+ *                        its first sample
  *   t2d_observe          (no reference counterpart) the ego-frame vector observation: ego motion, goal, nearest
  *                        participants and nearest map segments of every scenario's ego
  *   t2d_observe_agents   (no reference counterpart) the same observation seen from a list of observer slots per scenario,
@@ -358,6 +360,41 @@ int t2d_set_log(t2d_ctx* ctx, const t2d_log* log);
  * Host arrays are copied.  Rejected (the previous log stays bound): any malformed field. */
 int t2d_set_log_schedule(t2d_ctx* ctx, const t2d_log* log, const int32_t* slot_off, const int32_t* slot_track,
                          int32_t n_entries, int32_t* track_out);
+/* Reactive replay (DESIGN.md section 1 "Reactive replay"): a track k with track_path[k] >= 0 is reactive.  At every
+ * replay launch that samples a slot showing a reactive track k at time t (the sample time above):
+ *   handover   (reset mode, or t - interval_ms < first_ms[k] <= t in tick mode): the slot is posed from the log and takes
+ *              type_row[k] exactly as plain replay does, and drive_path[n][m] = track_path[k],
+ *              slot_desired_speed[n][m] = desired_speed[k], the lateral PID state pid_state[n][m][0:3] (t2d_set_pid) and
+ *              last_accel[n][m] (t2d_set_controllers) are zeroed.  The tick does not integrate this static row.
+ *   simulated  (every later sample up to the track's last stamp): the state is left alone, type_id = drive_row[k] (the
+ *              tick integrates it with K5's action), drive_path and slot_desired_speed as at the handover.
+ * After the last stamp the slot is T2D_TYPE_INACTIVE as in plain replay.  Every other slot the launch samples (plain
+ * tracks, absent tracks, slots without a track, the ego) gets drive_path = -1.  K17 and K5 read drive_path instead of the
+ * controllers' path_id, and K5's IDM rows take slot_desired_speed instead of the row's desired_speed where drive_path >=
+ * 0; the caller gives those slots an IDM row with a PATH lateral channel.
+ *   track_path          HOST int16 [n_tracks] a path of t2d_set_paths, -1: plain replay
+ *   drive_row           HOST uint8 [n_tracks] for a reactive track a row of the type table that is not
+ *                       T2D_MODEL_STATIC, with type_row[k]'s shape, half_len, half_wid and radius (not read otherwise)
+ *   desired_speed       HOST float [n_tracks] finite and > 0 on a reactive track (m/s; not read otherwise)
+ *   drive_path          DEVICE int16 [N][M], caller-owned, 2-byte aligned; set to -1 by the call
+ *   slot_desired_speed  DEVICE float [N][M], caller-owned, 4-byte aligned; set to 0 by the call
+ * Host arrays are copied.  NULL unbinds; with nothing bound every launch is the plain one.  t2d_set_log,
+ * t2d_set_log_schedule, t2d_set_paths, t2d_set_controllers, t2d_set_type_table and unbinding the leader search drop the
+ * binding; t2d_set_lane_change is rejected while it is bound.  Rejected (the previous binding stays whole): n_tracks
+ * other than the log's, a NULL array, a track_path entry outside [-1, n_paths), a drive_row of a reactive track outside
+ * the table, static or of another shape or extents, a desired speed that is not finite and > 0, misaligned device arrays
+ * (T2D_E_INVALID); state, type table, log, controllers, paths, PID state or leader search not bound, or a lane change
+ * bound (T2D_E_STATE).  The history ring (t2d_set_history) does not keep a reactive slot's handover entry: its type id
+ * changes on the next tick. */
+typedef struct t2d_reactive_replay {
+  int32_t n_tracks;               /* the bound log's n_tracks */
+  const int16_t* track_path;      /* HOST [n_tracks] */
+  const uint8_t* drive_row;       /* HOST [n_tracks] */
+  const float* desired_speed;     /* HOST [n_tracks] */
+  int16_t* drive_path;            /* DEVICE [N][M] */
+  float* slot_desired_speed;      /* DEVICE [N][M] */
+} t2d_reactive_replay;
+int t2d_set_log_reactive(t2d_ctx* ctx, const t2d_reactive_replay* replay);
 
 /* Single-line lidar of the ego (participant 0) of every scenario: SingleLineLidar._scan_obstacles
  * (tactics2d/sensor/lidar.py:128-221).  n_beams = point_density (lidar.py:49), max_range = perception range;

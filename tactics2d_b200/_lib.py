@@ -64,6 +64,12 @@ class LogC(C.Structure):
                 ("row_track", C.c_void_p), ("log_row", C.c_void_p), ("type_id", C.c_void_p)]
 
 
+class ReactiveReplayC(C.Structure):
+    """``t2d_reactive_replay``: the per-track tables (host pointers) and the per-slot device arrays of a reactive replay."""
+    _fields_ = [("n_tracks", C.c_int32), ("track_path", C.c_void_p), ("drive_row", C.c_void_p),
+                ("desired_speed", C.c_void_p), ("drive_path", C.c_void_p), ("slot_desired_speed", C.c_void_p)]
+
+
 class ResetSamplerC(C.Structure):
     """``t2d_reset_sampler``: the seed and options of the sampled resets, the host jitter table, the device row pools and
     the world-owned episode / pool_row / reset_try buffers."""
@@ -142,6 +148,7 @@ SYMBOLS = {
     "t2d_bind_reset_wheel_pool": (C.c_int, [_P, _P, _P]),
     "t2d_set_log": (C.c_int, [_P, C.POINTER(LogC)]),
     "t2d_set_log_schedule": (C.c_int, [_P, C.POINTER(LogC), _P, _P, C.c_int32, _P]),
+    "t2d_set_log_reactive": (C.c_int, [_P, C.POINTER(ReactiveReplayC)]),
     "t2d_set_prefetch": (C.c_int, [_P, C.c_int]),
     "t2d_launch_count": (C.c_int64, []),
     "t2d_tick_fixed_count": (C.c_int64, []),

@@ -38,6 +38,7 @@ struct CtrlArgs : WorldArgs {
   int steer_first;
   const float* pid_target;   // [N][M][2] (target_speed, lateral target) or nullptr; read by the HAS_PID instance only
   double* pid_state;         // [N][M][6] or nullptr; read and written by the HAS_PID instance only
+  const float* slot_desired_speed;   // [N][M]: the reactive instance's IDM desired speed of every slot with a path
 };
 
 __device__ __forceinline__ double clip_np(double v, double lo, double hi) {   // np.clip: NaN propagates
@@ -207,9 +208,11 @@ __device__ __forceinline__ const CtrlLawRow& law_row(const t2d_controller_params
 }
 
 // HAS_PID: the instance with the PID law, launched when the bound table holds a PID row or an IDM row with a lateral
-// channel; the other one is the plain K5.
-template <bool HAS_PID>
-__global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant__ CtrlArgs A) {
+// channel; the other one is the plain K5.  SLOT_SPEED: the reactive-replay instance (t2d_reactive_control_kernel, with
+// the PID law), whose IDM rows take slot_desired_speed in place of the row's desired_speed on every slot whose path_id
+// (there: the replay's drive_path) is >= 0.
+template <bool HAS_PID, bool SLOT_SPEED>
+__device__ __forceinline__ void control_body(const CtrlArgs& A) {
   const int lane = threadIdx.x & 31;
   const int warps = (gridDim.x * blockDim.x) >> 5;
   for (int n = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; n < A.N; n += warps) {
@@ -243,7 +246,13 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
         if (HAS_PID && p.kind == T2D_CTRL_PID) {
           pid_law(A.ctab[cid], A, base + m, x, y, v, (double)A.h[base + m], steer, acc);
         } else if (p.kind == T2D_CTRL_IDM) {
-          acc = idm_law(p, v, x, y, has, vl, xl, yl);
+          if (SLOT_SPEED && A.path_id[base + m] >= 0) {   // a reactive slot: its track's desired speed
+            CtrlLawRow q = p;
+            q.desired_speed = A.slot_desired_speed[base + m];
+            acc = idm_law(q, v, x, y, has, vl, xl, yl);
+          } else {
+            acc = idm_law(p, v, x, y, has, vl, xl, yl);
+          }
           // lane keeping: an IDM row with a lateral channel (only a PATH source passes t2d_set_controllers)
           if (HAS_PID && A.ctab[cid].pid_lateral != T2D_PID_LAT_NONE)
             steer = pid_lateral_law(A.ctab[cid], A, base + m, x, y, (double)A.h[base + m]);
@@ -274,6 +283,15 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
       A.last_accel[base + m] = mag[j];
     }
   }
+}
+
+template <bool HAS_PID>
+__global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant__ CtrlArgs A) {
+  control_body<HAS_PID, false>(A);
+}
+
+__global__ void __launch_bounds__(128) t2d_reactive_control_kernel(const __grid_constant__ CtrlArgs A) {
+  control_body<true, true>(A);
 }
 
 }  // namespace t2d

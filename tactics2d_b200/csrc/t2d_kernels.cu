@@ -10,9 +10,11 @@
 // K2  t2d_reset_kernel     masked re-initialisation from a pool of initial states (t2d_reset.cuh).
 // K3  t2d_physics_kernel   flat batch through one physics model (PhysicsModelBase.step) (t2d_tick.cuh).
 // K4  t2d_lidar_kernel     single-line lidar of every scenario's ego (per-edge beam windows) (t2d_lidar.cuh).
-// K5  t2d_control_kernel   NPC controllers: IDM, cruise / adaptive cruise, pure pursuit, PID (t2d_control.cuh).
+// K5  t2d_control_kernel   NPC controllers: IDM, cruise / adaptive cruise, pure pursuit, PID (t2d_control.cuh);
+//                         t2d_reactive_control_kernel adds the reactive slots' own IDM desired speeds.
 // K6  t2d_bev_kernel       the bird's-eye-view observation of every scenario's ego, or of every observer row (t2d_bev.cuh).
-// K7  t2d_replay_kernel    log replay: recorded tracks pose the replayed slots before K1 / after K2 (t2d_replay.cuh).
+// K7  t2d_replay_kernel    log replay: recorded tracks pose the replayed slots before K1 / after K2 (t2d_replay.cuh);
+//                         t2d_reactive_replay_kernel hands reactive tracks over to K5 while a reactive replay is bound.
 // K8  t2d_obs_kernel       the ego-frame vector observation (t2d_obs.cuh).
 // K9  t2d_obs_agents_kernel the same observation from a list of observer slots per scenario (t2d_obs.cuh).
 //     t2d_env_epilogue_kernel    status, reward and done mask of every scenario's ego (t2d_agents.cuh).
@@ -226,6 +228,15 @@ struct LaneChange {
   int8_t* change;
 };
 
+// A bound reactive replay: the per-track tables on the device and the caller's per-slot arrays
+struct ReactiveReplay {
+  dev_ptr<int16_t> track_path;
+  dev_ptr<uint8_t> drive_row;
+  dev_ptr<float> desired_speed;
+  int16_t* drive_path;
+  float* slot_desired_speed;
+};
+
 struct t2d_ctx {
   int device = 0, N = 0, M = 0, G = 0;
   t2d_config cfg{};
@@ -278,6 +289,8 @@ struct t2d_ctx {
   double leader_half_width = 0.0, leader_max_range = 0.0;
   // lane change (t2d_set_lane_change / K18); lane == nullptr: none bound, K17 and K5 read ctrl_path
   std::unique_ptr<LaneChange> lane;
+  // reactive replay (t2d_set_log_reactive); nullptr: none bound, K7 and K5 run their plain instances
+  std::unique_ptr<ReactiveReplay> reactive;
   // routes (t2d_set_routes / t2d_bind_route_trackers); route_id == nullptr: none bound
   const int16_t* route_id = nullptr;
   double route_threshold = 0.0, route_weight = 0.0;
@@ -299,6 +312,7 @@ struct t2d_ctx {
   int bev_target_style = bev::NO_STYLE;
   std::unique_ptr<DeviceLog> log;      // nullptr: no log bound
   std::vector<int> type_model;         // host copy of the current type table's model ids
+  std::vector<t2d_type_params> type_rows;   // ... and of its rows (t2d_set_log_reactive compares shapes)
   dev_ptr<uint8_t> order;              // [N][64] x-order hint of K1's FIXED instance (t2d_create: the identity)
   std::unique_ptr<DeviceSampler> sampler;   // t2d_set_reset_sampler; nullptr: none bound
   std::unique_ptr<DeviceHistory> hist;      // t2d_set_history; nullptr: none bound
@@ -586,6 +600,8 @@ int t2d_set_type_table(t2d_ctx* c, const t2d_type_params* table, int n_types) {
   c->n_types = n_types;
   c->type_model.resize(n_types);
   for (int i = 0; i < n_types; ++i) c->type_model[i] = table[i].model;
+  c->type_rows.assign(table, table + n_types);
+  c->reactive.reset();   // its driving rows named the old table
   c->has_pointmass = has_pointmass;
   c->has_drift = has_drift;
   c->rb_max = rb_max;
@@ -957,6 +973,7 @@ static int set_log(t2d_ctx* c, const t2d_log* L, const char* who, const int32_t*
     c->hist->track = std::move(tracks.track);
   }
   c->log = std::move(g);
+  c->reactive.reset();   // its tables described the old log's tracks
   return T2D_OK;
 }
 
@@ -965,6 +982,7 @@ int t2d_set_log(t2d_ctx* c, const t2d_log* L) {
   if (!L) {
     CUDA_TRY(cudaSetDevice(c->device));
     c->log.reset();
+    c->reactive.reset();
     if (c->hist) c->hist->track.reset();
     return T2D_OK;
   }
@@ -996,7 +1014,19 @@ static int launch_replay(t2d_ctx* c, void* stream, int first, int count, int off
   R.t0 = g.t0.get(); R.slot_off = g.slot_off.get(); R.entries = g.entries.get(); R.slot_track1 = g.slot_track1.get();
   R.track_out = g.track_out ? g.track_out + p0 : nullptr;
   R.N = count; R.M = c->M; R.n_rows = g.n_rows; R.offset = offset; R.interval_ms = c->cfg.interval_ms;
-  t2d_replay_kernel<<<capped_grid((long long)count * c->M, 256, c->sm_count, 8), 256, 0, (cudaStream_t)stream>>>(R);
+  const int grid = capped_grid((long long)count * c->M, 256, c->sm_count, 8);
+  if (c->reactive) {   // the reactive instance: handovers to K5, and the driving rows after them
+    const ReactiveReplay& rr = *c->reactive;
+    ReactiveReplayArgs X{};
+    static_cast<ReplayArgs&>(X) = R;
+    X.track_path = rr.track_path.get(); X.drive_row = rr.drive_row.get(); X.desired_speed = rr.desired_speed.get();
+    X.drive_path = rr.drive_path + p0; X.slot_desired_speed = rr.slot_desired_speed + p0;
+    X.pid_state = c->pid_state ? c->pid_state + 6 * p0 : nullptr;
+    X.last_accel = c->ctrl_last_accel ? c->ctrl_last_accel + p0 : nullptr;
+    t2d_reactive_replay_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(X);
+    return launched();
+  }
+  t2d_replay_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(R);
   return launched();
 }
 
@@ -1168,8 +1198,11 @@ static int check_leader_args(const char* fn, double half_width, double max_range
   return T2D_OK;
 }
 
-// The slots' current paths: a bound lane change's lane_path, else the controllers' path_id
-static const int16_t* current_path(const t2d_ctx* c) { return c->lane ? c->lane->lane_path : c->ctrl_path; }
+// The slots' current paths: a bound reactive replay's drive_path, a bound lane change's lane_path (never both), else the
+// controllers' path_id
+static const int16_t* current_path(const t2d_ctx* c) {
+  return c->reactive ? c->reactive->drive_path : c->lane ? c->lane->lane_path : c->ctrl_path;
+}
 
 // K17 on the bound state and the controllers' paths; the caller has checked the arguments and the bindings
 static int launch_leaders(t2d_ctx* c, double half_width, double max_range, int16_t* lead, float* gap, void* stream) {
@@ -1218,6 +1251,10 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
   A.pid_target = c->pid_target; A.pid_state = c->pid_state;
   const int warps_per_cta = 4;
   auto kern = c->ctrl_has_pid ? t2d_control_kernel<true> : t2d_control_kernel<false>;
+  if (c->reactive) {   // the reactive slots' own desired speeds (only bound with a PID state)
+    A.slot_desired_speed = c->reactive->slot_desired_speed;
+    kern = t2d_reactive_control_kernel;
+  }
   kern<<<capped_grid(c->N, warps_per_cta, c->sm_count, 16), warps_per_cta * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
 }
@@ -1860,6 +1897,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
     c->ctrl_last_accel = nullptr;
     c->ctrl_has_pid = c->ctrl_pid_reads_target = false;
     c->lane.reset();
+    c->reactive.reset();
     return T2D_OK;
   }
   if (n_rows <= 0 || n_rows > T2D_MAX_CONTROLLERS) return fail(T2D_E_INVALID, "n_rows must be in 1..T2D_MAX_CONTROLLERS");
@@ -1906,6 +1944,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
   c->n_ctrl = n_rows; c->ctrl_id = ctrl_id; c->ctrl_lead = lead_index; c->ctrl_path = path_id; c->ctrl_last_accel = last_accel;
   c->ctrl_has_pid = has_pid; c->ctrl_pid_reads_target = reads_target;
   c->lane.reset();   // its lane_path was copied from the old path_id
+  c->reactive.reset();   // its slots needed the old table's rows
   return T2D_OK;
 }
 
@@ -1928,6 +1967,7 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   if (n_paths == 0 || !xy) {   // unbind
     c->d_path_v.reset(); c->d_path_off.reset(); c->n_paths = 0;
     c->lane.reset();
+    c->reactive.reset();
     return T2D_OK;
   }
   if (n_paths < 0 || !offsets) return fail(T2D_E_INVALID, "t2d_set_paths: bad argument");
@@ -1954,6 +1994,7 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   if (int r = upload(d_off, offsets, (size_t)n_paths + 1)) return r;
   c->d_path_v = std::move(d_v); c->d_path_off = std::move(d_off); c->n_paths = n_paths;
   c->lane.reset();   // its neighbour table named the old paths
+  c->reactive.reset();   // its track paths named them too
   return T2D_OK;
 }
 
@@ -2010,6 +2051,7 @@ int t2d_set_leader_search(t2d_ctx* c, double half_width, double max_range, int16
   if (!lead) {   // unbind
     c->leader_lead = nullptr; c->leader_gap = nullptr; c->leader_half_width = c->leader_max_range = 0.0;
     c->lane.reset();   // a lane change reads the search's corridor
+    c->reactive.reset();   // reactive slots brake for the search's leaders
     return T2D_OK;
   }
   if (int r = check_leader_args("t2d_set_leader_search", half_width, max_range, lead, gap)) return r;
@@ -2050,6 +2092,7 @@ int t2d_set_lane_change(t2d_ctx* c, const t2d_lane_change_params* p, const int16
   if (!c->ctrl_path) return fail(T2D_E_STATE, "t2d_set_lane_change: the controllers have no path_id");
   if (c->n_paths == 0) return fail(T2D_E_STATE, "t2d_set_lane_change: no paths bound: call t2d_set_paths first");
   if (!c->leader_lead) return fail(T2D_E_STATE, "t2d_set_lane_change: no leader search bound: call t2d_set_leader_search first");
+  if (c->reactive) return fail(T2D_E_STATE, "t2d_set_lane_change: a reactive replay is bound (lane changes on track paths are not supported)");
   if (p->min_gap > c->leader_max_range)
     return fail(T2D_E_INVALID, "t2d_set_lane_change: min_gap must not exceed the search's max_range");
   for (int q = 0; q < c->n_paths; ++q) {
@@ -2068,6 +2111,54 @@ int t2d_set_lane_change(t2d_ctx* c, const t2d_lane_change_params* p, const int16
   CUDA_TRY(cudaMemset(cooldown, 0, nm * sizeof(int16_t)));
   if (change) CUDA_TRY(cudaMemset(change, 0, nm));
   c->lane = std::move(L);
+  return T2D_OK;
+}
+
+int t2d_set_log_reactive(t2d_ctx* c, const t2d_reactive_replay* r) {
+  const std::string fn = "t2d_set_log_reactive";
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!r) {   // unbind
+    c->reactive.reset();
+    return T2D_OK;
+  }
+  if (!r->track_path || !r->drive_row || !r->desired_speed || !r->drive_path || !r->slot_desired_speed)
+    return fail(T2D_E_INVALID, fn + ": NULL array");
+  if (!aligned2(r->drive_path) || !aligned4(r->slot_desired_speed))
+    return fail(T2D_E_INVALID, fn + ": drive_path must be 2-byte and slot_desired_speed 4-byte aligned");
+  if (int e = require(c, NEED_STATE | NEED_TABLE)) return e;
+  if (!c->log) return fail(T2D_E_STATE, fn + ": no log bound: call t2d_set_log or t2d_set_log_schedule first");
+  if (!c->d_ctab) return fail(T2D_E_STATE, fn + ": controllers not set: call t2d_set_controllers first");
+  if (c->n_paths == 0) return fail(T2D_E_STATE, fn + ": no paths bound: call t2d_set_paths first");
+  if (!c->pid_state) return fail(T2D_E_STATE, fn + ": no PID state bound: call t2d_set_pid first");
+  if (!c->leader_lead) return fail(T2D_E_STATE, fn + ": no leader search bound: call t2d_set_leader_search first");
+  if (c->lane) return fail(T2D_E_STATE, fn + ": a lane change is bound (lane changes on track paths are not supported)");
+  if (r->n_tracks != c->log->n_tracks)
+    return fail(T2D_E_INVALID, fn + ": n_tracks must be the bound log's (" + std::to_string(c->log->n_tracks) + ")");
+  for (int k = 0; k < r->n_tracks; ++k) {
+    const std::string at = fn + ": track " + std::to_string(k) + ": ";
+    const int p = r->track_path[k];
+    if (p < -1 || p >= c->n_paths) return fail(T2D_E_INVALID, at + "track_path outside [-1, n_paths)");
+    if (p < 0) continue;   // plain replay: its drive row and desired speed are not read
+    const int row = r->drive_row[k];
+    if (row >= c->n_types) return fail(T2D_E_INVALID, at + "drive_row outside the type table");
+    const t2d_type_params& d = c->type_rows[row];
+    const t2d_type_params& s = c->type_rows[c->log->track_type_host[k]];
+    if (d.model == T2D_MODEL_STATIC) return fail(T2D_E_INVALID, at + "drive_row is a T2D_MODEL_STATIC row");
+    if (d.shape != s.shape || d.half_len != s.half_len || d.half_wid != s.half_wid || d.radius != s.radius)
+      return fail(T2D_E_INVALID, at + "drive_row has another shape or other extents than the track's row");
+    if (!(std::isfinite(r->desired_speed[k]) && r->desired_speed[k] > 0.0f))
+      return fail(T2D_E_INVALID, at + "desired_speed must be finite and > 0");
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  auto g = std::make_unique<ReactiveReplay>();
+  if (int e = upload(g->track_path, r->track_path, (size_t)r->n_tracks)) return e;
+  if (int e = upload(g->drive_row, r->drive_row, (size_t)r->n_tracks)) return e;
+  if (int e = upload(g->desired_speed, r->desired_speed, (size_t)r->n_tracks)) return e;
+  g->drive_path = r->drive_path; g->slot_desired_speed = r->slot_desired_speed;
+  const size_t nm = (size_t)c->N * c->M;
+  CUDA_TRY(cudaMemset(r->drive_path, 0xff, nm * sizeof(int16_t)));   // -1: no slot is reactive before a reset
+  CUDA_TRY(cudaMemset(r->slot_desired_speed, 0, nm * sizeof(float)));
+  c->reactive = std::move(g);
   return T2D_OK;
 }
 

@@ -43,7 +43,25 @@ __device__ __forceinline__ float replay_lerp(float a, float b, double w) {   // 
   return __double2float_rn(__dadd_rn((double)a, __dmul_rn(w, __dsub_rn((double)b, (double)a))));
 }
 
-__global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__ ReplayArgs A) {
+// Reactive replay (t2d_set_log_reactive): the per-track tables and the per-slot arrays a handover writes.  The base part
+// is the plain kernel's; pid_state / last_accel address the first scenario of the launch like the state does.
+struct ReactiveReplayArgs : ReplayArgs {
+  const int16_t* track_path;       // [n_tracks] the path of a reactive track, -1: plain replay
+  const uint8_t* drive_row;        // [n_tracks] the non-static row that drives a reactive track after its handover
+  const float* desired_speed;      // [n_tracks] its IDM desired speed
+  int16_t* drive_path;             // [N][M] the path K17 and K5 read, -1 unless the slot shows a reactive track
+  float* slot_desired_speed;       // [N][M]
+  double* pid_state;               // [N][M][6] or nullptr: the lateral half is zeroed on handover
+  float* last_accel;               // [N][M] or nullptr: zeroed on handover
+};
+
+// REACTIVE: the reactive instance (t2d_reactive_replay_kernel).  A slot that shows a reactive track k is posed from the
+// log only at its handover - reset mode, or the first sample with first_k <= t, i.e. t - first_k < interval_ms - where
+// it also takes the track's path and desired speed and a cleared controller state; at every later sample it keeps its
+// state and takes the driving row drive_row[k], which the tick integrates.  Every other slot the launch visits gets
+// drive_path = -1 and is replayed exactly as by the plain instance.
+template <bool REACTIVE, class Args>
+__device__ __forceinline__ void replay_body(const Args& A) {
   constexpr double PI_D = 3.141592653589793, TWO_PI_D = 6.283185307179586;
   const long long total = (long long)A.N * A.M;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -64,6 +82,7 @@ __global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__
       k = __ldg(A.slot_track1 + s);
       if (k < 0) {
         if (A.track_out) A.track_out[i] = -1;
+        if constexpr (REACTIVE) A.drive_path[i] = -1;
         continue;
       }
       t = (long long)A.t0[row] + ((long long)A.step_count[n] + A.offset) * A.interval_ms;
@@ -71,6 +90,7 @@ __global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__
       int lo = __ldg(A.slot_off + s), hi = __ldg(A.slot_off + s + 1) - 1;
       if (hi < lo) {   // an empty schedule: the slot is not replayed
         if (A.track_out) A.track_out[i] = -1;
+        if constexpr (REACTIVE) A.drive_path[i] = -1;
         continue;
       }
       t = (long long)A.t0[row] + ((long long)A.step_count[n] + A.offset) * A.interval_ms;
@@ -87,9 +107,26 @@ __global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__
     if (d < 0 || d > (long long)(n_frames - 1) * period) {   // the track is not in the scene at t
       A.type_id[i] = T2D_TYPE_INACTIVE;
       if (A.track_out) A.track_out[i] = -1;
+      if constexpr (REACTIVE) A.drive_path[i] = -1;
       continue;
     }
     if (A.track_out) A.track_out[i] = k;
+    if constexpr (REACTIVE) {
+      const int16_t path = __ldg(A.track_path + k);
+      A.drive_path[i] = path;
+      if (path >= 0) {
+        A.slot_desired_speed[i] = __ldg(A.desired_speed + k);
+        if (A.mask == nullptr && d >= (long long)A.interval_ms) {   // simulated: K5 drives it, K1 integrates it
+          A.type_id[i] = __ldg(A.drive_row + k);
+          continue;
+        }
+        if (A.pid_state) {   // handover: a fresh controller on the log's state
+          double* st = A.pid_state + 6 * i;
+          st[0] = 0.0; st[1] = 0.0; st[2] = 0.0;
+        }
+        if (A.last_accel) A.last_accel[i] = 0.0f;
+      }
+    }
     const long long j = d / period;
     const int r = (int)(d - j * period);
     const float* a = A.rec + 5 * ((long long)rec_off + j);
@@ -118,6 +155,12 @@ __global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__
     A.x[i] = x; A.y[i] = y; A.h[i] = h; A.v[i] = v; A.vx[i] = vx; A.vy[i] = vy;
     A.type_id[i] = A.track_type[k];
   }
+}
+
+__global__ void __launch_bounds__(256) t2d_replay_kernel(const __grid_constant__ ReplayArgs A) { replay_body<false>(A); }
+
+__global__ void __launch_bounds__(256) t2d_reactive_replay_kernel(const __grid_constant__ ReactiveReplayArgs A) {
+  replay_body<true>(A);
 }
 
 }  // namespace t2d

@@ -60,6 +60,34 @@ class ReplayLog:
             raise KeyError(f"track {int(self.ids[k])} has no frame at {t_ms} ms")
         return self.records[self.rec_off[k] + j]
 
+    def track_paths(self, tolerance: float = 0.1, extend: float = 30.0):
+        """Paths for reactive replay (``BatchedWorld.set_reactive_replay``; DESIGN.md section 1 "Reactive replay"):
+        ``(paths, track_path, desired_speed)``.  Track k's path is its logged (x, y) without repeated points, simplified
+        with Douglas-Peucker at ``tolerance`` metres and extended straight by ``extend`` metres along its last segment
+        (so that the lateral controller does not turn back at its end), all in float64, then fp32; ``track_path[k]``
+        (int16 [K]) indexes ``paths``.  ``desired_speed[k]`` (fp32 [K]) is the track's highest logged speed.  A track
+        whose path has no segment of non-zero length, or whose highest speed is not > 0 (a parked car), stays plain
+        replay: ``track_path[k] = -1``.  A logged stop (at a signal, say) is not reproduced: the IDM only stops behind a
+        leader."""
+        if not tolerance >= 0.0 or not extend >= 0.0:
+            raise ValueError("tolerance and extend must be >= 0")
+        rec = np.asarray(self.records, np.float32).astype(np.float64)
+        speed = np.sqrt(rec[:, 3] * rec[:, 3] + rec[:, 4] * rec[:, 4])
+        paths, track_path = [], np.full(len(self), -1, np.int16)
+        desired = np.zeros(len(self), np.float32)
+        for k, (a, n) in enumerate(zip(self.rec_off, self.n_frames)):
+            desired[k] = np.float32(speed[a:a + n].max())
+            xy = rec[a:a + n, :2]
+            keep = np.concatenate([[True], np.any(xy[1:] != xy[:-1], axis=1)])
+            xy = douglas_peucker(xy[keep], tolerance)
+            if len(xy) < 2 or not desired[k] > 0.0:
+                continue
+            d = xy[-1] - xy[-2]
+            end = xy[-1] + float(extend) * d / np.hypot(d[0], d[1])
+            track_path[k] = len(paths)
+            paths.append(np.concatenate([xy, end[None]], 0).astype(np.float32))
+        return paths, track_path, desired
+
     @classmethod
     def from_levelx(cls, parser: LevelXParser, file, folder: str, time_range=None, ids=None) -> "ReplayLog":
         """The tracks of a LevelX recording (``LevelXParser._frames``: highD's box centres and (-pi, pi] headings, the degree
@@ -144,6 +172,32 @@ class ReplayEpisodes:
         seg = None if segments is None else np.ascontiguousarray(segments, dtype=np.float32).reshape(-1, 4)
         return Scene(self.table, p["x"], p["y"], p["heading"], p["speed"], p["vx"], p["vy"], self.type_id, seg, bounds, name,
                      dict(replay=True))
+
+
+def douglas_peucker(xy, tolerance: float):
+    """The Douglas-Peucker simplification of the polyline ``xy`` [V, 2] (float64): the end points, and recursively the
+    vertex farthest from the chord between two kept ones (the first of equals) while that distance exceeds
+    ``tolerance``.  Distances are to the chord segment."""
+    xy = np.asarray(xy, np.float64)
+    if len(xy) < 3:
+        return xy.copy()
+    keep = np.zeros(len(xy), bool)
+    keep[0] = keep[-1] = True
+    stack = [(0, len(xy) - 1)]
+    while stack:
+        i, j = stack.pop()
+        if j - i < 2:
+            continue
+        a, b, p = xy[i], xy[j], xy[i + 1:j]
+        ab = b - a
+        L2 = ab[0] * ab[0] + ab[1] * ab[1]
+        t = np.zeros(len(p)) if L2 == 0.0 else np.clip(((p - a) @ ab) / L2, 0.0, 1.0)
+        d = np.hypot(*(p - (a + t[:, None] * ab)).T)
+        f = int(np.argmax(d))
+        if d[f] > tolerance:
+            keep[i + 1 + f] = True
+            stack += [(i, i + 1 + f), (i + 1 + f, j)]
+    return xy[keep]
 
 
 def _speed(vx, vy):

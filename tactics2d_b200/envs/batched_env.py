@@ -51,7 +51,8 @@ class BatchedTrafficEnv:
                  bev_range=(20.0, 20.0, 20.0, 20.0), replay=None, vector_obs: Optional[dict] = None,
                  agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
                  route: Optional[dict] = None, sampler: Optional[dict] = None, history: Optional[dict] = None,
-                 camera: Optional[dict] = None, leaders: Optional[dict] = None, lane_change: Optional[dict] = None):
+                 camera: Optional[dict] = None, leaders: Optional[dict] = None, lane_change: Optional[dict] = None,
+                 reactive: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -118,7 +119,15 @@ class BatchedTrafficEnv:
         controllers (with ``path_id``) on ``env.world`` first - and bound again there whenever ``set_controllers`` or
         ``set_paths`` dropped it.  It adds ``info["lane_path"]`` (int16 [N, M], every slot's current lane) and
         ``info["lane_change"]`` (int8 [N, M], the decisions of the step) to ``reset`` and ``step``, after the auto-reset,
-        which restarts the reset scenarios from their ``path_id``."""
+        which restarts the reset scenarios from their ``path_id``;
+        ``reactive``: e.g. ``dict(controller=IDMController(..., lateral=PIDController(lateral_error="path_cross_track")),
+        tolerance=0.1, extend=30.0)`` (needs ``replay`` and ``leaders``) makes the replayed traffic react (DESIGN.md
+        section 1 "Reactive replay"): every moving track follows its own logged path (``ReplayLog.track_paths``, appended
+        to the ``route`` paths) with the controller from its first sample on, braking for whatever the leader search finds
+        ahead of it, the ego included.  Every slot but the ego's gets the controller row (``world.set_controllers``); the
+        reactive replay is bound at ``reset``, and bound again there whenever a later setter dropped it.  It adds
+        ``info["reactive"]`` (bool [N, M], the slots that show a reactive track, ``BatchedWorld.reactive``) to ``reset``
+        and ``step``, after the auto-reset."""
         import torch
 
         if observation not in ("state", "bev", "vector", "agents"):
@@ -193,6 +202,17 @@ class BatchedTrafficEnv:
                 raise ValueError(f"lane_change: unknown keys {sorted(unknown)}")
             if "left" not in self.lane_change or "right" not in self.lane_change:
                 raise ValueError("lane_change needs the 'left' and 'right' neighbour tables")
+        self.reactive = None if reactive is None else dict(reactive)
+        if self.reactive is not None:
+            if replay is None or leaders is None:
+                raise ValueError("reactive needs a log and a leader search: pass replay=... and leaders=dict(...)")
+            if lane_change is not None:
+                raise ValueError("reactive does not take lane changes (lane_change)")
+            unknown = set(self.reactive) - {"controller", "tolerance", "extend"}
+            if unknown:
+                raise ValueError(f"reactive: unknown keys {sorted(unknown)}")
+            if "controller" not in self.reactive:
+                raise ValueError("reactive needs the 'controller' its tracks drive with")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -245,6 +265,16 @@ class BatchedTrafficEnv:
             self.world.set_history(self.history["length"])
         if self.leaders is not None:
             self.world.set_leader_search(**self.leaders)
+        self._reactive_tracks = None
+        if self.reactive is not None:
+            rc = self.reactive
+            paths, track_path, speed = replay.log.track_paths(rc.get("tolerance", 0.1), rc.get("extend", 30.0))
+            base = [] if self.route is None else list(self.route["paths"])
+            self.world.set_paths(base + paths)
+            ctrl = np.zeros((n, m), np.uint8)
+            ctrl[:, 0] = 255                                   # the ego is the policy's
+            self.world.set_controllers([rc["controller"]], ctrl)
+            self._reactive_tracks = dict(track_path=track_path, desired_speed=speed, path_base=len(base))
         self._last_obs = None
         if observation == "bev":
             w, h = self.bev_resolution
@@ -320,6 +350,8 @@ class BatchedTrafficEnv:
             info["leader"], info["leader_gap"] = self.world.find_leaders(**self.leaders)
         if self.lane_change is not None:
             info["lane_path"], info["lane_change"] = self.world.lane_path, self.world.lane_change
+        if self.reactive is not None:
+            info["reactive"] = self.world.reactive
         return info
 
     # ------------------------------------------------------------------ gym surface
@@ -337,6 +369,8 @@ class BatchedTrafficEnv:
             perm = torch.from_numpy(self._rng.permutation(self.num_envs).astype(np.int32)).to(self.world.device)
         if self.lane_change is not None and self.world.lane_path is None:   # bound after the search, on the set controllers
             self.world.set_lane_change(**self.lane_change)
+        if self.reactive is not None and self.world.drive_path is None:   # the reset below hands the present tracks over
+            self.world.set_reactive_replay(**self._reactive_tracks)
         if self.agent_rewards:   # every slot takes its pool row's type below; no retired type of the old episodes survives
             self.world.retired_type.fill_(255)
             self.world.reset_agent_trackers()

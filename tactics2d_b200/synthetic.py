@@ -278,3 +278,59 @@ def highway_episodes(n_rows: int, m: int, seed: int = 0, duration_ms: int = 2000
     ego = rng.choice(ok, int(n_rows))
     t0 = log.first_ms[ego] + rng.integers(0, (log.n_frames[ego] + 1) // 2) * log.period_ms[ego]
     return build_replay_episodes(log, m, t0.tolist(), log.ids[ego].tolist(), horizon_ms=horizon_ms, reuse_slots=reuse_slots)
+
+
+def idm_highway_log(duration_ms: int = 60000, seed: int = 0, lanes: int = 3, lane_width: float = 3.5,
+                    length_m: float = 800.0, period_ms: int = 100, desired=(24.0, 28.0, 32.0), headway_s: float = 3.0):
+    """A seeded one-way highway recording made by car following (a :class:`tactics2d_b200.dataset_parser.ReplayLog`, type
+    rows unassigned): lane l runs along y = l * ``lane_width`` in +x.  At t = 0 the road holds a car every
+    ``headway_s * desired[l]`` metres of lane l, and a new car enters x = 0 about every ``headway_s`` seconds (+-30 %),
+    at its own desired speed (the lane's +-10 %).  Every car follows the one ahead in its lane with the IDM (headway
+    1.2 s, min spacing 4 m, acceleration 1.5, deceleration 3 m/s^2), integrated in float64 every ``period_ms``, and
+    leaves past x = ``length_m``.  Cars are 4.5 m x 1.9 m; heading 0, vy 0."""
+    from .dataset_parser.replay import ReplayLog
+    from .participant.element import Vehicle
+
+    rng = np.random.default_rng(seed)
+    dt = period_ms / 1000.0
+    tracks = []                                    # [first_ms, records]
+    road = [[] for _ in range(lanes)]              # per lane, front first: [x, v, vd, track]
+
+    def new(l, x, t_ms):
+        vd = desired[l] * rng.uniform(0.9, 1.1)
+        tracks.append([t_ms, []])
+        return [x, vd, vd, len(tracks) - 1]
+
+    for l in range(lanes):
+        gap = headway_s * desired[l]
+        road[l] = [new(l, x, 0) for x in np.arange(length_m - gap * rng.uniform(0.2, 1.0), 0.0, -gap)]
+    due = [rng.uniform(0.0, headway_s) for _ in range(lanes)]
+    for step in range(duration_ms // period_ms + 1):
+        t_ms = step * period_ms
+        for l in range(lanes):
+            if t_ms / 1000.0 >= due[l] and (not road[l] or road[l][-1][0] > 30.0):
+                road[l].append(new(l, 0.0, t_ms))
+                due[l] = t_ms / 1000.0 + headway_s * rng.uniform(0.7, 1.3)
+            for c in road[l]:
+                tracks[c[3]][1].append((c[0], l * lane_width, 0.0, c[1], 0.0))
+            acc = []
+            for i, c in enumerate(road[l]):
+                x, v, vd = c[0], c[1], c[2]
+                a = 1.5 * (1.0 - (v / vd) ** 4)
+                if i > 0:
+                    lead = road[l][i - 1]
+                    s = lead[0] - x - 4.5
+                    s_star = 4.0 + v * 1.2 + v * (v - lead[1]) / (2.0 * np.sqrt(1.5 * 3.0))
+                    a -= 1.5 * (max(s_star, 4.0) / max(s, 0.1)) ** 2
+                acc.append(max(a, -8.0))
+            for c, a in zip(road[l], acc):
+                v_new = max(c[1] + a * dt, 0.0)
+                c[0] += 0.5 * (c[1] + v_new) * dt
+                c[1] = v_new
+            road[l] = [c for c in road[l] if c[0] <= length_m]
+    K = len(tracks)
+    recs = [np.asarray(r, np.float32) for _, r in tracks]
+    return ReplayLog(ids=np.arange(K, dtype=np.int64), first_ms=np.asarray([f for f, _ in tracks], np.int32),
+                     n_frames=np.asarray([len(r) for r in recs], np.int32), period_ms=np.full(K, period_ms, np.int32),
+                     records=np.ascontiguousarray(np.concatenate(recs)), type_row=np.full(K, TYPE_INACTIVE, np.uint8),
+                     cls=[Vehicle] * K, length=np.full(K, 4.5), width=np.full(K, 1.9))

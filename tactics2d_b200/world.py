@@ -12,14 +12,14 @@ Replaces the per-object loop of the reference tick: ``ScenarioManager.update`` -
 from __future__ import annotations
 
 import ctypes as C
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 from typing import Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _lib
-from .types import MODEL_DRIFT, TYPE_INACTIVE, TypeTable
+from .types import MODEL_DRIFT, MODEL_STATIC, TYPE_INACTIVE, TypeTable
 
 CFG_ANY_PARTICIPANT = 1
 CFG_STEER_FIRST = 2
@@ -180,7 +180,7 @@ class BatchedWorld:
         self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = self._sampler = None
         self._history, self._hist_out = 0, {}
         self._route_out = {}
-        self._leader = self._leader_out = self._lane = None
+        self._leader = self._leader_out = self._lane = self._reactive = None
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
         self._agent_lidar, self._obs_out, self._agent_obs_out, self._agent_bev = {}, {}, {}, {}
         self._seg_style_keys = []
@@ -256,6 +256,7 @@ class BatchedWorld:
             raise ValueError("a SingleTrackDrift row needs a world created with one (its wheel speeds are allocated there)")
         _lib.check(self.lib.t2d_set_type_table(self._ctx, type_table.to_c_array(), len(type_table)))
         self.type_table = type_table
+        self._reactive = None   # the library dropped a bound reactive replay
         if self._bev_cfg is not None:
             type_styles, target = self._bev_cfg
             if len(type_styles) != len(type_table):
@@ -356,7 +357,7 @@ class BatchedWorld:
             off[1:] = np.cumsum([len(p) for p in paths])
             _lib.check(self.lib.t2d_set_paths(self._ctx, C.c_void_p(xy.ctypes.data), C.c_void_p(off.ctypes.data), len(paths)))
         self.paths = paths
-        self._lane = None   # the library dropped a bound lane change
+        self._lane = self._reactive = None   # the library dropped a bound lane change and reactive replay
 
     def set_controllers(self, controllers, ctrl_id, lead_index=None, path_id=None, last_accel=None, pid_target=None,
                         pid_state=None):
@@ -377,7 +378,7 @@ class BatchedWorld:
         if controllers is None:
             _lib.check(self.lib.t2d_set_controllers(self._ctx, _ptr(None), 0, _ptr(None), _ptr(None), _ptr(None), _ptr(None)))
             _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(None), _ptr(None)))
-            self._ctrl = self._lane = None
+            self._ctrl = self._lane = self._reactive = None
             return
         rows = [c if isinstance(c, _lib.ControllerParamsC) else c.params() for c in controllers]
         arr = (_lib.ControllerParamsC * len(rows))(*rows)
@@ -402,7 +403,7 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_set_controllers(self._ctx, arr, len(rows), _ptr(cid), _ptr(lead), _ptr(pid), _ptr(la)))
         _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(tgt), _ptr(st)))
         self._ctrl = dict(rows=arr, ctrl_id=cid, lead_index=lead, path_id=pid, last_accel=la, pid_target=tgt, pid_state=st)
-        self._lane = None   # the library dropped a bound lane change
+        self._lane = self._reactive = None   # the library dropped a bound lane change and reactive replay
 
     @property
     def last_accel(self) -> Optional[torch.Tensor]:
@@ -435,7 +436,7 @@ class BatchedWorld:
         change.  A rejected call keeps the previous search."""
         if half_width is None:
             _lib.check(self.lib.t2d_set_leader_search(self._ctx, 0.0, 0.0, _ptr(None), _ptr(None)))
-            self._leader = self._lane = None   # unbinding the search drops a bound lane change
+            self._leader = self._lane = self._reactive = None   # unbinding the search drops a bound lane change and reactive replay
             return
         lead = torch.full((self.N, self.M), -1, dtype=torch.int16, device=self.device)
         gap = torch.full((self.N, self.M), float("inf"), dtype=torch.float32, device=self.device)
@@ -720,7 +721,7 @@ class BatchedWorld:
         status (``any_participant=False``)."""
         if log is None:
             _lib.check(self.lib.t2d_set_log(self._ctx, None))
-            self._log = None
+            self._log = self._reactive = None
             return
         if (row_track is None) == (schedule is None):
             raise ValueError("give exactly one of row_track and schedule")
@@ -752,6 +753,84 @@ class BatchedWorld:
             _lib.check(self.lib.t2d_set_log_schedule(self._ctx, C.byref(c), p(keep["slot_off"]), p(keep["slot_track"]),
                                                      int(keep["slot_track"].shape[0]), _ptr(track)))
         self._log = dict(keep, log_row=log_row, track=track)
+        self._reactive = None   # the library dropped a bound reactive replay
+
+    def set_reactive_replay(self, track_path, drive_row=None, desired_speed=None, path_base: int = 0):
+        """Let the bound log's reactive tracks react (``t2d_set_log_reactive``; DESIGN.md section 1 "Reactive replay").
+        ``track_path`` [K]: the path of every track of the log, -1 for plain replay (``ReplayLog.track_paths``); an entry
+        p >= 0 names path ``path_base + p`` of ``set_paths``.  A reactive track is posed from its log at its first sample
+        (its handover: the first one after it enters, or the reset), and from then on drives: its slot takes
+        ``drive_row[k]`` (default: the non-static row whose static twin is the track's row, ``TypeTable.with_static_twins``),
+        the controllers follow :attr:`drive_path` instead of ``path_id``, and the IDM rows take ``desired_speed[k]``
+        (default: the track's highest logged speed) from :attr:`slot_desired_speed`.  It leaves at its last stamp, wherever
+        it is.  Give the replayed slots an ``IDMController(lateral=PIDController(lateral_error="path_cross_track"))`` row
+        first; a leader search, the paths and the log must be bound, no lane change.  The binding takes effect at the next
+        ``reset``.  ``track_path=None`` unbinds; ``set_log``, ``set_paths``, ``set_controllers``, ``set_type_table`` and
+        unbinding the search drop it.  A rejected call keeps the previous binding."""
+        if track_path is None:
+            _lib.check(self.lib.t2d_set_log_reactive(self._ctx, None))
+            self._reactive = None
+            return
+        if self._log is None:
+            raise ValueError("set_reactive_replay needs a log: call set_log first")
+        K = self._log["first"].shape[0]
+        tp = np.asarray(track_path, np.int64).reshape(-1)
+        if tp.shape != (K,):
+            raise ValueError(f"track_path must hold one entry per track of the log ({K})")
+        tp = np.where(tp >= 0, tp + int(path_base), -1)
+        if (tp > 32767).any():
+            raise ValueError("track_path + path_base must fit int16")
+        tp = np.ascontiguousarray(tp.astype(np.int16))
+        if drive_row is None:
+            drive_row = self._class_rows(self._log["type_row"])
+        dr = np.asarray(drive_row, np.int64).reshape(-1)
+        if dr.shape != (K,) or (dr < 0).any() or (dr > 255).any():
+            raise ValueError(f"drive_row must hold one uint8 type row per track ({K})")
+        dr = np.ascontiguousarray(dr.astype(np.uint8))
+        if desired_speed is None:
+            v = self._log["records"].astype(np.float64)
+            speed = np.sqrt(v[:, 3] * v[:, 3] + v[:, 4] * v[:, 4])
+            bounds = np.concatenate([[0], np.cumsum(self._log["n_frames"].astype(np.int64))])
+            desired_speed = [speed[a:b].max() for a, b in zip(bounds[:-1], bounds[1:])]
+        ds = np.ascontiguousarray(np.asarray(desired_speed, np.float32).reshape(-1))
+        if ds.shape != (K,):
+            raise ValueError(f"desired_speed must hold one entry per track ({K})")
+        NM = (self.N, self.M)
+        drive_path = torch.full(NM, -1, dtype=torch.int16, device=self.device)
+        sds = torch.zeros(NM, dtype=torch.float32, device=self.device)
+        p = lambda a: C.c_void_p(a.ctypes.data)
+        c = _lib.ReactiveReplayC(K, p(tp), p(dr), p(ds), _ptr(drive_path), _ptr(sds))
+        _lib.check(self.lib.t2d_set_log_reactive(self._ctx, C.byref(c)))
+        self._reactive = dict(track_path=tp, drive_row=dr, desired_speed=ds, drive_path=drive_path,
+                              slot_desired_speed=sds)
+
+    def _class_rows(self, type_row):
+        """For every static row of ``type_row``, the non-static row it is the twin of (``TypeTable.with_static_twins``)."""
+        rows = self.type_table.rows
+        out = []
+        for r in np.asarray(type_row, np.int64):
+            hit = [i for i, q in enumerate(rows) if q.model != MODEL_STATIC and replace(q, model=MODEL_STATIC) == rows[r]]
+            if not hit:
+                raise ValueError(f"type row {int(r)} is the static twin of no row of the table: pass drive_row")
+            out.append(hit[0])
+        return out
+
+    @property
+    def drive_path(self) -> Optional[torch.Tensor]:
+        """int16 [N, M] device tensor: the path every slot showing a reactive track drives along, -1 elsewhere (None
+        without a reactive replay).  Every replay rewrites the slots it samples."""
+        return None if self._reactive is None else self._reactive["drive_path"]
+
+    @property
+    def slot_desired_speed(self) -> Optional[torch.Tensor]:
+        """fp32 [N, M] device tensor: the IDM desired speed of every slot showing a reactive track."""
+        return None if self._reactive is None else self._reactive["slot_desired_speed"]
+
+    @property
+    def reactive(self) -> Optional[torch.Tensor]:
+        """bool [N, M] device tensor: the slots that show a reactive track, from its handover to its exit (None without
+        a reactive replay)."""
+        return None if self._reactive is None else self._reactive["drive_path"] >= 0
 
     def _log_struct(self, keep, log_row, type_id):
         p = lambda a: C.c_void_p(a.ctypes.data)
