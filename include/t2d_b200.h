@@ -51,6 +51,9 @@
  *                        `leading_state` / `front_state`
  *   t2d_set_lane_change  (no reference counterpart) MOBIL lane changes (Kesting, Treiber and Helbing 2007) for the IDM
  *                        rows with a lateral channel, decided on the device before every t2d_control
+ *   t2d_set_yielding / t2d_find_yields
+ *                        (no reference counterpart) yielding at the conflict zones of crossing and merging paths for
+ *                        path-following IDM traffic, decided on the device before every t2d_control
  *   t2d_check_events     the same detectors on caller-supplied poses (no physics)
  *   t2d_reset            ScenarioManager.reset / ParticipantBase.reset
  *                                                         tactics2d/envs/parking.py:397-441, participant_base.py:236-246
@@ -740,6 +743,50 @@ typedef struct t2d_lane_change_params {
 } t2d_lane_change_params; /* 40 bytes */
 int t2d_set_lane_change(t2d_ctx* ctx, const t2d_lane_change_params* p, const int16_t* left, const int16_t* right,
                         int16_t* lane_path, int16_t* cooldown, int8_t* change);
+
+/* ---- yielding at conflict zones (K19, no reference counterpart) --------------------------------------------------------
+ * DESIGN.md section 1 "Yielding at conflict zones".  fp64 with one rounding per operation, on the state K5 reads next.
+ * The zone table is built on the host from the bound path table (tactics2d_b200.traffic.conflict_zones): for path p,
+ * rows zone_off[p] .. zone_off[p + 1] - 1, sorted by s_in_p, each naming the other path q and the arc intervals
+ * [s_in_p, s_out_p] on p and [s_in_q, s_out_q] on q where the two come within the zone width (widened by a margin).
+ *   A slot's path is its current path (K17's: drive_path, lane_path or path_id) when that has a segment of non-zero length,
+ * else its route (t2d_set_routes, read at every launch) when that has one, which makes it a partner only.  s_k is its arc
+ * length on that path (t2d_set_routes' closest point), u_k = max(v_k, v_min).  A yielder is a slot with type_id < n_types,
+ * a position that is not NaN, an IDM controller row and a usable current path p.  It considers the zones of p with
+ * v_i^2 / (2 commit_decel) < d_i = s_in_p - s_i <= the search's max_range.  The partners of a zone are the leader search's
+ * candidates whose path is q, with d_j = s_in_q - s_j and t_j = max(d_j, 0) / u_j; a partner is cleared when
+ * s_j > s_out_q and excluded when its distance to p is <= the search's half_width and its arc length on p is > s_i.  i
+ * must yield to a partner that is neither when d_j <= v_j^2 / (2 commit_decel), or t_j <= critical_gap and priority[q] >
+ * priority[p], or t_j <= critical_gap, priority[q] == priority[p] and (d_j, j) < (d_i, i).  The yield zone is the
+ * considered zone of smallest d_i (then lowest row) with a must-yield partner: yield_to = its lowest such partner slot,
+ * stop_gap = d_i rounded once; -1 and +inf for every other slot.  K5 (t2d_yield_control_kernel) then gives an IDM row with
+ * a finite stop_gap min(IDM on its leader, IDM on the stop point standing at speed 0), the stop point being p's point at
+ * arc length clamp(s_in_p, 0, L).
+ *   t2d_set_yielding binds it: zones HOST [zone_off[n_paths]], zone_off HOST int32 [n_paths + 1], priority HOST int16
+ * [n_paths] or NULL (all 0), all copied; yield_to DEVICE int16 [N][M] and stop_gap DEVICE fp32 [N][M] owned by the caller.
+ * While bound, t2d_control, t2d_step_host_ego and t2d_step_host_agents launch K18 (if bound), K17, K19, then K5.  K19
+ * keeps no state: resets need nothing.  p == NULL unbinds; with nothing bound nothing of this launches and K5 runs its
+ * other instances.  t2d_set_controllers, t2d_set_paths and unbinding the leader search drop the binding.
+ *   t2d_find_yields writes the yields of the bound state into yield_to / stop_gap once (and the stop points K5 reads): one
+ * launch, no allocation, capturable.
+ * Rejected (a rejected call keeps the previous binding whole): critical_gap, commit_decel or v_min not finite and > 0,
+ * NULL zone_off / yield_to / stop_gap (or zones with rows), zone_off[0] != 0 or decreasing, a zone with q outside
+ * [0, n_paths) or q == p, an arc length that is not finite, s_in > s_out, the zones of a path not sorted by s_in_p,
+ * misaligned arrays (T2D_E_INVALID); state, type table, controllers, paths or the leader search not bound, or no yielding
+ * bound for find (T2D_E_STATE). */
+typedef struct t2d_yield_params {
+  double critical_gap; /* (s): a partner this close in time to its zone entry is a gap too small to take */
+  double commit_decel; /* (m/s^2): a car that cannot stop before its zone at this deceleration is committed */
+  double v_min;        /* (m/s): the speed floor of the partners' time to their zone */
+} t2d_yield_params;    /* 24 bytes */
+typedef struct t2d_conflict_zone {
+  int32_t q;           /* the other path */
+  int32_t reserved;    /* 0 */
+  double s_in_p, s_out_p, s_in_q, s_out_q;   /* (m) arc lengths on p and on q */
+} t2d_conflict_zone;   /* 40 bytes */
+int t2d_set_yielding(t2d_ctx* ctx, const t2d_yield_params* p, const t2d_conflict_zone* zones, const int32_t* zone_off,
+                     const int16_t* priority, int16_t* yield_to, float* stop_gap);
+int t2d_find_yields(t2d_ctx* ctx, int16_t* yield_to, float* stop_gap, void* stream);
 
 /* Inputs and memory of the PID rows: DEVICE arrays owned by the caller.  target [N][M][2] fp32 = (target_speed, lateral
  * target: target_heading in rad for HEADING rows, cross_track_error in m for CROSS_TRACK rows; PATH rows ignore it);

@@ -52,6 +52,15 @@ class LaneChangeParamsC(C.Structure):
         ("cooldown", C.c_int32), ("reserved", C.c_int32)]
 
 
+class YieldParamsC(C.Structure):
+    """``t2d_yield_params``: the gap-acceptance parameters of a bound yielding."""
+    _fields_ = [(n, C.c_double) for n in ("critical_gap", "commit_decel", "v_min")]
+
+
+ZONE_DTYPE = [("q", "<i4"), ("reserved", "<i4"), ("s_in_p", "<f8"), ("s_out_p", "<f8"), ("s_in_q", "<f8"),
+              ("s_out_q", "<f8")]   # t2d_conflict_zone
+
+
 class BevStyleC(C.Structure):
     """``t2d_bev_style``: colour, z order and stroke width (points) of one BEV style row."""
     _fields_ = [("r", C.c_uint8), ("g", C.c_uint8), ("b", C.c_uint8), ("z", C.c_int8), ("line_width_pt", C.c_float)]
@@ -131,6 +140,8 @@ SYMBOLS = {
     "t2d_set_leader_search": (C.c_int, [_P, C.c_double, C.c_double, _P, _P]),
     "t2d_find_leaders": (C.c_int, [_P, C.c_double, C.c_double, _P, _P, _P]),
     "t2d_set_lane_change": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
+    "t2d_set_yielding": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
+    "t2d_find_yields": (C.c_int, [_P, _P, _P, _P]),
     "t2d_set_routes": (C.c_int, [_P, _P, C.c_double, C.c_double, C.c_float]),
     "t2d_bind_route_trackers": (C.c_int, [_P, _P, _P, C.c_int32]),
     "t2d_route_observe": (C.c_int, [_P, _P, C.c_int32, C.c_int, C.c_float, _P, _P]),

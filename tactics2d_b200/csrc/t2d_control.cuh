@@ -39,6 +39,8 @@ struct CtrlArgs : WorldArgs {
   const float* pid_target;   // [N][M][2] (target_speed, lateral target) or nullptr; read by the HAS_PID instance only
   double* pid_state;         // [N][M][6] or nullptr; read and written by the HAS_PID instance only
   const float* slot_desired_speed;   // [N][M]: the reactive instance's IDM desired speed of every slot with a path
+  const float* stop_gap;             // [N][M]: the yielding instance's K19 output, +inf where the slot does not yield
+  const double2* stop_xy;            // [N][M]: ... and the stop point where it does
 };
 
 __device__ __forceinline__ double clip_np(double v, double lo, double hi) {   // np.clip: NaN propagates
@@ -203,6 +205,14 @@ __device__ void pid_law(const t2d_controller_params& p, const CtrlArgs& A, size_
   }
 }
 
+// The yielding IDM law of slot i: min(a on the leader, a on the stop point standing at speed 0) while K19 found a stop
+__device__ __forceinline__ double yield_law(const CtrlArgs& A, size_t i, const CtrlLawRow& p, double v, double x, double y,
+                                            double acc) {
+  if (!(A.stop_gap[i] < __int_as_float(0x7f800000))) return acc;   // +inf: no stop
+  const double2 s = A.stop_xy[i];
+  return fmin(acc, idm_law(p, v, x, y, true, 0.0, s.x, s.y));
+}
+
 __device__ __forceinline__ const CtrlLawRow& law_row(const t2d_controller_params* ctab, int cid) {
   return *reinterpret_cast<const CtrlLawRow*>(reinterpret_cast<const char*>(ctab) + (size_t)cid * sizeof(t2d_controller_params));
 }
@@ -210,8 +220,10 @@ __device__ __forceinline__ const CtrlLawRow& law_row(const t2d_controller_params
 // HAS_PID: the instance with the PID law, launched when the bound table holds a PID row or an IDM row with a lateral
 // channel; the other one is the plain K5.  SLOT_SPEED: the reactive-replay instance (t2d_reactive_control_kernel, with
 // the PID law), whose IDM rows take slot_desired_speed in place of the row's desired_speed on every slot whose path_id
-// (there: the replay's drive_path) is >= 0.
-template <bool HAS_PID, bool SLOT_SPEED>
+// (there: the replay's drive_path) is >= 0.  YIELD: the instance launched while yielding is bound (t2d_yield_control_kernel,
+// with the PID law, and the slot desired speeds when slot_desired_speed is not nullptr): an IDM row with a finite stop_gap
+// takes the smaller of its law on the leader and its law on the stop point as a leader standing at speed 0.
+template <bool HAS_PID, bool SLOT_SPEED, bool YIELD = false>
 __device__ __forceinline__ void control_body(const CtrlArgs& A) {
   const int lane = threadIdx.x & 31;
   const int warps = (gridDim.x * blockDim.x) >> 5;
@@ -246,12 +258,14 @@ __device__ __forceinline__ void control_body(const CtrlArgs& A) {
         if (HAS_PID && p.kind == T2D_CTRL_PID) {
           pid_law(A.ctab[cid], A, base + m, x, y, v, (double)A.h[base + m], steer, acc);
         } else if (p.kind == T2D_CTRL_IDM) {
-          if (SLOT_SPEED && A.path_id[base + m] >= 0) {   // a reactive slot: its track's desired speed
+          if (SLOT_SPEED && (!YIELD || A.slot_desired_speed) && A.path_id[base + m] >= 0) {   // a reactive slot: its track's desired speed
             CtrlLawRow q = p;
             q.desired_speed = A.slot_desired_speed[base + m];
             acc = idm_law(q, v, x, y, has, vl, xl, yl);
+            if constexpr (YIELD) acc = yield_law(A, base + m, q, v, x, y, acc);
           } else {
             acc = idm_law(p, v, x, y, has, vl, xl, yl);
+            if constexpr (YIELD) acc = yield_law(A, base + m, p, v, x, y, acc);
           }
           // lane keeping: an IDM row with a lateral channel (only a PATH source passes t2d_set_controllers)
           if (HAS_PID && A.ctab[cid].pid_lateral != T2D_PID_LAT_NONE)
@@ -292,6 +306,10 @@ __global__ void __launch_bounds__(128) t2d_control_kernel(const __grid_constant_
 
 __global__ void __launch_bounds__(128) t2d_reactive_control_kernel(const __grid_constant__ CtrlArgs A) {
   control_body<true, true>(A);
+}
+
+__global__ void __launch_bounds__(128) t2d_yield_control_kernel(const __grid_constant__ CtrlArgs A) {
+  control_body<true, true, true>(A);
 }
 
 }  // namespace t2d

@@ -32,6 +32,8 @@
 // K18 t2d_lane_change_kernel     MOBIL lane changes of the IDM rows with a lateral channel, in front of K17 and K5 while
 //                                a lane change is bound; t2d_lane_reset_kernel restarts the reset scenarios' lanes
 //                                (t2d_lane.cuh).
+// K19 t2d_yield_kernel           whom every path-following IDM car yields to at the conflict zones of its path, and where it
+//                                stops, in front of K5's t2d_yield_control_kernel while yielding is bound (t2d_yield.cuh).
 //     t2d_exchange_allgather_kernel   all-gather of the done masks over NVLink peer memory (t2d_exchange.cuh).
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -63,6 +65,7 @@
 #include "t2d_history.cuh"
 #include "t2d_leader.cuh"
 #include "t2d_lane.cuh"
+#include "t2d_yield.cuh"
 
 // =============================================================================================
 // C ABI
@@ -237,6 +240,18 @@ struct ReactiveReplay {
   float* slot_desired_speed;
 };
 
+// A bound yielding (t2d_set_yielding / K19): the parameters, the zone table and priorities on the device, the stop points
+// K19 writes for K5, and the caller's per-slot outputs
+struct Yielding {
+  t2d_yield_params p;
+  dev_ptr<yield::Zone> zones;
+  dev_ptr<int> zone_off;
+  dev_ptr<int16_t> priority;
+  dev_ptr<double2> stop_xy;            // [N][M]
+  int16_t* yield_to;
+  float* stop_gap;
+};
+
 struct t2d_ctx {
   int device = 0, N = 0, M = 0, G = 0;
   t2d_config cfg{};
@@ -283,6 +298,8 @@ struct t2d_ctx {
   dev_ptr<PathVertex> d_path_v;
   dev_ptr<int> d_path_off;
   int n_paths = 0;
+  std::vector<PathVertex> path_host;   // host copy of the table and its offsets (t2d_set_yielding's stop points)
+  std::vector<int> path_off_host;
   // leader search (t2d_set_leader_search / K17); leader_lead == nullptr: none bound, K5 reads ctrl_lead
   int16_t* leader_lead = nullptr;
   float* leader_gap = nullptr;
@@ -291,6 +308,8 @@ struct t2d_ctx {
   std::unique_ptr<LaneChange> lane;
   // reactive replay (t2d_set_log_reactive); nullptr: none bound, K7 and K5 run their plain instances
   std::unique_ptr<ReactiveReplay> reactive;
+  // yielding (t2d_set_yielding / K19); nullptr: none bound, K5 runs its other instances
+  std::unique_ptr<Yielding> yield;
   // routes (t2d_set_routes / t2d_bind_route_trackers); route_id == nullptr: none bound
   const int16_t* route_id = nullptr;
   double route_threshold = 0.0, route_weight = 0.0;
@@ -1229,6 +1248,22 @@ static int launch_lane_change(t2d_ctx* c, void* stream) {
   return launched();
 }
 
+// K19 on the bound state with the bound yielding and search; the caller has checked the bindings
+static int launch_yields(t2d_ctx* c, int16_t* yield_to, float* stop_gap, void* stream) {
+  const Yielding& Y = *c->yield;
+  CUDA_TRY(cudaSetDevice(c->device));
+  yield::Args A{world_args(c)};
+  A.path_id = current_path(c); A.route_id = c->route_id;
+  A.ctrl_id = c->ctrl_id; A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl;
+  A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.zones = Y.zones.get(); A.zone_off = Y.zone_off.get(); A.priority = Y.priority.get();
+  A.half_width = c->leader_half_width; A.max_range = c->leader_max_range;
+  A.critical_gap = Y.p.critical_gap; A.two_commit_decel = 2.0 * Y.p.commit_decel; A.v_min = Y.p.v_min;
+  A.yield_to = yield_to; A.stop_gap = stop_gap; A.stop_xy = Y.stop_xy.get();
+  yield::t2d_yield_kernel<<<(c->N + yield::WARPS - 1) / yield::WARPS, yield::WARPS * 32, 0, (cudaStream_t)stream>>>(A);
+  return launched();
+}
+
 static int launch_control(t2d_ctx* c, float* action, const float* ego, void* stream) {
   if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
   if (!c->d_ctab) return fail(T2D_E_STATE, "controllers not set: call t2d_set_controllers first");
@@ -1242,6 +1277,9 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
   // a bound search finds the leaders on the state K5 reads next, and K5 follows them instead of the controllers' lead_index
   if (c->leader_lead)
     if (int r = launch_leaders(c, c->leader_half_width, c->leader_max_range, c->leader_lead, c->leader_gap, stream)) return r;
+  // bound yielding (only with a search) finds the stops on the same state, and K5 brakes for them
+  if (c->yield)
+    if (int r = launch_yields(c, c->yield->yield_to, c->yield->stop_gap, stream)) return r;
   CtrlArgs A{world_args(c)};
   A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.path_id = current_path(c);
   A.lead = c->leader_lead ? c->leader_lead : c->ctrl_lead;
@@ -1254,6 +1292,10 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
   if (c->reactive) {   // the reactive slots' own desired speeds (only bound with a PID state)
     A.slot_desired_speed = c->reactive->slot_desired_speed;
     kern = t2d_reactive_control_kernel;
+  }
+  if (c->yield) {   // the stops K19 has just written (slot_desired_speed stays nullptr without a reactive replay)
+    A.stop_gap = c->yield->stop_gap; A.stop_xy = c->yield->stop_xy.get();
+    kern = t2d_yield_control_kernel;
   }
   kern<<<capped_grid(c->N, warps_per_cta, c->sm_count, 16), warps_per_cta * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
@@ -1898,6 +1940,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
     c->ctrl_has_pid = c->ctrl_pid_reads_target = false;
     c->lane.reset();
     c->reactive.reset();
+    c->yield.reset();
     return T2D_OK;
   }
   if (n_rows <= 0 || n_rows > T2D_MAX_CONTROLLERS) return fail(T2D_E_INVALID, "n_rows must be in 1..T2D_MAX_CONTROLLERS");
@@ -1945,6 +1988,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
   c->ctrl_has_pid = has_pid; c->ctrl_pid_reads_target = reads_target;
   c->lane.reset();   // its lane_path was copied from the old path_id
   c->reactive.reset();   // its slots needed the old table's rows
+  c->yield.reset();   // its yielders were the old table's IDM rows
   return T2D_OK;
 }
 
@@ -1965,9 +2009,10 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   CUDA_TRY(cudaSetDevice(c->device));
   if (n_paths == 0 || !xy) {   // unbind
-    c->d_path_v.reset(); c->d_path_off.reset(); c->n_paths = 0;
+    c->d_path_v.reset(); c->d_path_off.reset(); c->n_paths = 0; c->path_host.clear(); c->path_off_host.clear();
     c->lane.reset();
     c->reactive.reset();
+    c->yield.reset();
     return T2D_OK;
   }
   if (n_paths < 0 || !offsets) return fail(T2D_E_INVALID, "t2d_set_paths: bad argument");
@@ -1993,8 +2038,11 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   if (int r = upload(d_v, pv.data(), pv.size())) return r;
   if (int r = upload(d_off, offsets, (size_t)n_paths + 1)) return r;
   c->d_path_v = std::move(d_v); c->d_path_off = std::move(d_off); c->n_paths = n_paths;
+  c->path_host = std::move(pv);
+  c->path_off_host.assign(offsets, offsets + n_paths + 1);
   c->lane.reset();   // its neighbour table named the old paths
   c->reactive.reset();   // its track paths named them too
+  c->yield.reset();   // its zones were built on them
   return T2D_OK;
 }
 
@@ -2052,6 +2100,7 @@ int t2d_set_leader_search(t2d_ctx* c, double half_width, double max_range, int16
     c->leader_lead = nullptr; c->leader_gap = nullptr; c->leader_half_width = c->leader_max_range = 0.0;
     c->lane.reset();   // a lane change reads the search's corridor
     c->reactive.reset();   // reactive slots brake for the search's leaders
+    c->yield.reset();   // yielding reads the search's corridor and range
     return T2D_OK;
   }
   if (int r = check_leader_args("t2d_set_leader_search", half_width, max_range, lead, gap)) return r;
@@ -2112,6 +2161,97 @@ int t2d_set_lane_change(t2d_ctx* c, const t2d_lane_change_params* p, const int16
   if (change) CUDA_TRY(cudaMemset(change, 0, nm));
   c->lane = std::move(L);
   return T2D_OK;
+}
+
+// ---- yielding (t2d_set_yielding / t2d_find_yields; K19)
+// p's point at arc length clamp(s, 0, L): on the first segment of non-zero length that reaches s (the last one past L),
+// x0 + t dx with t = (s - acc) / len and len = sqrt(dx dx + dy dy), the arc lengths of closest_on_path
+static void point_at(const PathVertex* pv, int n_vert, double s, double& x, double& y) {
+  double acc = 0.0;
+  s = std::max(s, 0.0);
+  x = pv[0].x; y = pv[0].y;
+  for (int i = 0; i + 1 < n_vert; ++i) {
+    const double dx = pv[i + 1].x - pv[i].x, dy = pv[i + 1].y - pv[i].y;
+    const double l2 = dx * dx + dy * dy;
+    if (!(l2 > 0.0)) continue;
+    const double len = std::sqrt(l2);
+    const double t = std::min((s - acc) / len, 1.0);
+    x = pv[i].x + t * dx; y = pv[i].y + t * dy;
+    if (s <= acc + len) return;
+    acc = acc + len;
+  }
+}
+
+int t2d_set_yielding(t2d_ctx* c, const t2d_yield_params* p, const t2d_conflict_zone* zones, const int32_t* zone_off,
+                     const int16_t* priority, int16_t* yield_to, float* stop_gap) {
+  const std::string fn = "t2d_set_yielding";
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!p) {   // unbind
+    c->yield.reset();
+    return T2D_OK;
+  }
+  if (!(std::isfinite(p->critical_gap) && p->critical_gap > 0.0))
+    return fail(T2D_E_INVALID, fn + ": critical_gap must be finite and > 0");
+  if (!(std::isfinite(p->commit_decel) && p->commit_decel > 0.0))
+    return fail(T2D_E_INVALID, fn + ": commit_decel must be finite and > 0");
+  if (!(std::isfinite(p->v_min) && p->v_min > 0.0)) return fail(T2D_E_INVALID, fn + ": v_min must be finite and > 0");
+  if (!zone_off || !yield_to || !stop_gap) return fail(T2D_E_INVALID, fn + ": zone_off / yield_to / stop_gap is NULL");
+  if (!aligned2(yield_to) || !aligned4(stop_gap) || !aligned8(zones) || !aligned4(zone_off) || !aligned2(priority))
+    return fail(T2D_E_INVALID, fn + ": yield_to, priority must be 2-byte, stop_gap, zone_off 4-byte and zones 8-byte aligned");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (!c->d_ctab) return fail(T2D_E_STATE, fn + ": controllers not set: call t2d_set_controllers first");
+  if (c->n_paths == 0) return fail(T2D_E_STATE, fn + ": no paths bound: call t2d_set_paths first");
+  if (!c->leader_lead) return fail(T2D_E_STATE, fn + ": no leader search bound: call t2d_set_leader_search first");
+  const int P = c->n_paths;
+  if (zone_off[0] != 0) return fail(T2D_E_INVALID, fn + ": zone_off[0] must be 0");
+  for (int k = 0; k < P; ++k)
+    if (zone_off[k + 1] < zone_off[k]) return fail(T2D_E_INVALID, fn + ": zone_off must not decrease");
+  const int Z = zone_off[P];
+  if (Z > 0 && !zones) return fail(T2D_E_INVALID, fn + ": zones is NULL");
+  for (int k = 0; k < P; ++k) {
+    for (int z = zone_off[k]; z < zone_off[k + 1]; ++z) {
+      const t2d_conflict_zone& r = zones[z];
+      const std::string at = fn + ": zone " + std::to_string(z) + ": ";
+      if (r.q < 0 || r.q >= P) return fail(T2D_E_INVALID, at + "q outside [0, n_paths)");
+      if (r.q == k) return fail(T2D_E_INVALID, at + "q is the zone's own path");
+      if (!(std::isfinite(r.s_in_p) && std::isfinite(r.s_out_p) && std::isfinite(r.s_in_q) && std::isfinite(r.s_out_q)))
+        return fail(T2D_E_INVALID, at + "an arc length is not finite");
+      if (!(r.s_in_p <= r.s_out_p && r.s_in_q <= r.s_out_q)) return fail(T2D_E_INVALID, at + "s_in > s_out");
+      if (z > zone_off[k] && !(zones[z - 1].s_in_p <= r.s_in_p))
+        return fail(T2D_E_INVALID, at + "the zones of a path must be sorted by s_in_p");
+    }
+  }
+  std::vector<yield::Zone> dz((size_t)std::max(Z, 1));   // with the stop points, on the host copy of the table
+  const std::vector<int>& off = c->path_off_host;
+  for (int k = 0; k < P; ++k)
+    for (int z = zone_off[k]; z < zone_off[k + 1]; ++z) {
+      const t2d_conflict_zone& r = zones[z];
+      yield::Zone& d = dz[z];
+      d.s_in_p = r.s_in_p; d.s_in_q = r.s_in_q; d.s_out_q = r.s_out_q; d.q = r.q; d.reserved = 0;
+      point_at(c->path_host.data() + off[k], off[k + 1] - off[k], r.s_in_p, d.stop_x, d.stop_y);
+    }
+  std::vector<int16_t> prio((size_t)P, 0);   // priority == NULL: all 0
+  if (priority) std::copy(priority, priority + P, prio.begin());
+  CUDA_TRY(cudaSetDevice(c->device));
+  auto Y = std::make_unique<Yielding>();
+  Y->p = *p;
+  if (int r = upload(Y->zones, dz.data(), dz.size())) return r;
+  if (int r = upload(Y->zone_off, zone_off, (size_t)P + 1)) return r;
+  if (int r = upload(Y->priority, prio.data(), prio.size())) return r;
+  if (int r = dev_alloc(Y->stop_xy, (size_t)c->N * c->M)) return r;
+  Y->yield_to = yield_to; Y->stop_gap = stop_gap;
+  c->yield = std::move(Y);
+  return T2D_OK;
+}
+
+int t2d_find_yields(t2d_ctx* c, int16_t* yield_to, float* stop_gap, void* stream) {
+  if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
+  if (!yield_to || !stop_gap) return fail(T2D_E_INVALID, "t2d_find_yields: yield_to / stop_gap is NULL");
+  if (!aligned2(yield_to) || !aligned4(stop_gap))
+    return fail(T2D_E_INVALID, "t2d_find_yields: yield_to must be 2-byte and stop_gap 4-byte aligned");
+  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
+  if (!c->yield) return fail(T2D_E_STATE, "t2d_find_yields: no yielding bound: call t2d_set_yielding first");
+  return launch_yields(c, yield_to, stop_gap, stream);
 }
 
 int t2d_set_log_reactive(t2d_ctx* c, const t2d_reactive_replay* r) {

@@ -68,7 +68,7 @@ class ReplayLog:
         (int16 [K]) indexes ``paths``.  ``desired_speed[k]`` (fp32 [K]) is the track's highest logged speed.  A track
         whose path has no segment of non-zero length, or whose highest speed is not > 0 (a parked car), stays plain
         replay: ``track_path[k] = -1``.  A logged stop (at a signal, say) is not reproduced: the IDM only stops behind a
-        leader."""
+        leader, or, with yielding bound (``BatchedWorld.set_yielding``), before a conflict zone of crossing paths."""
         if not tolerance >= 0.0 or not extend >= 0.0:
             raise ValueError("tolerance and extend must be >= 0")
         rec = np.asarray(self.records, np.float32).astype(np.float64)

@@ -52,7 +52,7 @@ class BatchedTrafficEnv:
                  agent_rewards: bool = False, agent_actions: bool = False, lidar: Optional[dict] = None,
                  route: Optional[dict] = None, sampler: Optional[dict] = None, history: Optional[dict] = None,
                  camera: Optional[dict] = None, leaders: Optional[dict] = None, lane_change: Optional[dict] = None,
-                 reactive: Optional[dict] = None):
+                 reactive: Optional[dict] = None, yielding: Optional[dict] = None):
         """``scene``: a :class:`tactics2d_b200.synthetic.Scene` (initial states, types, map tile, bounds);
         ``replay``: optional :class:`tactics2d_b200.dataset_parser.ReplayEpisodes` - one scenario per episode row, the
         ego (participant 0) driven by the policy and the other slots by the recording (``BatchedWorld.set_log``); the
@@ -126,6 +126,13 @@ class BatchedTrafficEnv:
         to the ``route`` paths) with the controller from its first sample on, braking for whatever the leader search finds
         ahead of it, the ego included.  Every slot but the ego's gets the controller row (``world.set_controllers``); the
         reactive replay is bound at ``reset``, and bound again there whenever a later setter dropped it.  It adds
+        ``yielding``: e.g. ``dict(critical_gap=3.0, priority=[...])`` (the keywords of ``BatchedWorld.set_yielding``; needs
+        ``leaders``) makes the path-following IDM traffic yield at the conflict zones of the bound paths (DESIGN.md section 1
+        "Yielding at conflict zones"); with ``reactive`` the zones are those of the track paths and the route paths (the ego
+        routes), so a reactive track also yields to the ego.  It is bound at ``reset``, and bound again there whenever a
+        later setter dropped it.  It adds ``info["yield_to"]`` (int16 [N, M], the slot each car yields to, -1 for none) and
+        ``info["stop_gap"]`` (fp32 [N, M], +inf for none) to ``reset`` and ``step``: the yields of the state after the
+        auto-reset (``BatchedWorld.find_yields``);
         ``info["reactive"]`` (bool [N, M], the slots that show a reactive track, ``BatchedWorld.reactive``) to ``reset``
         and ``step``, after the auto-reset."""
         import torch
@@ -213,6 +220,13 @@ class BatchedTrafficEnv:
                 raise ValueError(f"reactive: unknown keys {sorted(unknown)}")
             if "controller" not in self.reactive:
                 raise ValueError("reactive needs the 'controller' its tracks drive with")
+        self.yielding = None if yielding is None else dict(yielding)
+        if self.yielding is not None:
+            if self.leaders is None:
+                raise ValueError("yielding needs a leader search: pass leaders=dict(...)")
+            unknown = set(self.yielding) - {"priority", "width", "margin", "critical_gap", "commit_decel", "v_min"}
+            if unknown:
+                raise ValueError(f"yielding: unknown keys {sorted(unknown)}")
         self.bev_resolution = (int(bev_resolution[0]), int(bev_resolution[1]))
         self.bev_range = bev_range
 
@@ -352,6 +366,8 @@ class BatchedTrafficEnv:
             info["lane_path"], info["lane_change"] = self.world.lane_path, self.world.lane_change
         if self.reactive is not None:
             info["reactive"] = self.world.reactive
+        if self.yielding is not None:
+            info["yield_to"], info["stop_gap"] = self.world.find_yields()
         return info
 
     # ------------------------------------------------------------------ gym surface
@@ -371,6 +387,8 @@ class BatchedTrafficEnv:
             self.world.set_lane_change(**self.lane_change)
         if self.reactive is not None and self.world.drive_path is None:   # the reset below hands the present tracks over
             self.world.set_reactive_replay(**self._reactive_tracks)
+        if self.yielding is not None and self.world.yield_to is None:   # on the bound paths, controllers and search
+            self.world.set_yielding(**self.yielding)
         if self.agent_rewards:   # every slot takes its pool row's type below; no retired type of the old episodes survives
             self.world.retired_type.fill_(255)
             self.world.reset_agent_trackers()

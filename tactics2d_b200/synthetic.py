@@ -334,3 +334,213 @@ def idm_highway_log(duration_ms: int = 60000, seed: int = 0, lanes: int = 3, lan
                      n_frames=np.asarray([len(r) for r in recs], np.int32), period_ms=np.full(K, period_ms, np.int32),
                      records=np.ascontiguousarray(np.concatenate(recs)), type_row=np.full(K, TYPE_INACTIVE, np.uint8),
                      cls=[Vehicle] * K, length=np.full(K, 4.5), width=np.full(K, 1.9))
+
+
+# ---------------------------------------------------------------------------- scenes with crossing and merging paths
+@dataclass
+class PathScene:
+    """N scenarios of path-following IDM traffic on one ``set_paths`` table: every car is an IDM row that keeps its
+    path (``path_controller``), ``path_id`` [N, M] names its path, ``priority`` [n_paths] the paths' priorities for
+    ``BatchedWorld.set_yielding``.  Slots with ``path_id == -1`` are empty (``type_id`` 255)."""
+    table: TypeTable
+    paths: list
+    priority: np.ndarray   # int16 [n_paths]
+    x: np.ndarray          # fp32 [N, M]
+    y: np.ndarray
+    heading: np.ndarray
+    speed: np.ndarray
+    type_id: np.ndarray    # uint8 [N, M]
+    path_id: np.ndarray    # int16 [N, M]
+    name: str = ""
+
+    @property
+    def shape(self):
+        return self.x.shape
+
+    @property
+    def ctrl_id(self) -> np.ndarray:
+        """uint8 [N, M]: row 0 (``path_controller``) for every car."""
+        return np.where(self.path_id >= 0, 0, 255).astype(np.uint8)
+
+
+def path_table() -> TypeTable:
+    """One kinematic car type (4.8 m x 1.9 m) that cannot reverse: the reference's IDM keeps braking below 0 m/s."""
+    from .types import TypeParams
+
+    return TypeTable([TypeParams(half_len=2.4, half_wid=0.95, lf=1.3, lr=1.3, steer_lo=-0.6, steer_hi=0.6, speed_lo=0.0,
+                                 speed_hi=30.0, accel_lo=-8.0, accel_hi=4.0)])
+
+
+def path_controller():
+    """The IDM every car of a :class:`PathScene` drives, with a PID cross-track channel that keeps it on its path."""
+    from .controller import IDMController, PIDController
+
+    keep = PIDController(dt=0.1, kp_lat=0.3, ki_lat=0.0, kd_lat=0.3, max_steering=0.6, derivative_filter_alpha=1.0,
+                         lateral_error="path_cross_track")
+    # the reference's IDM brakes for a closing speed only through min_spacing (its s* subtracts v (v - v_lead) / (2
+    # sqrt(a b))): a large min_spacing and max_acceleration make it stop short of a stopped car or a stop point
+    return IDMController(desired_speed=10.0, time_headway=1.0, min_spacing=20.0, max_acceleration=8.0,
+                         comfortable_deceleration=8.0, lateral=keep)
+
+
+def _polyline(*pieces):
+    return np.ascontiguousarray(np.concatenate([np.asarray(p, np.float64).reshape(-1, 2) for p in pieces]), np.float32)
+
+
+def _arc(cx, cy, r, a0, a1, n):
+    a = np.linspace(a0, a1, n)
+    return np.stack([cx + r * np.cos(a), cy + r * np.sin(a)], 1)
+
+
+def _bezier(p0, p1, p2, n):
+    t = np.linspace(0.0, 1.0, n)[:, None]
+    p0, p1, p2 = (np.asarray(p, np.float64) for p in (p0, p1, p2))
+    return (1 - t) ** 2 * p0 + 2 * t * (1 - t) * p1 + t ** 2 * p2
+
+
+def _meet(a, u, b, v):
+    """The point where the lines a + s u and b + t v meet."""
+    a, u, b, v = (np.asarray(q, np.float64) for q in (a, u, b, v))
+    cross = lambda p, q: p[0] * q[1] - p[1] * q[0]
+    s = cross(b - a, v) / cross(u, v)
+    return a + s * u
+
+
+def _point_at(path, s):
+    """(x, y, heading) of ``path`` at arc length s (clamped to its ends)."""
+    p = np.asarray(path, np.float64)
+    d = np.diff(p, axis=0)
+    ln = np.hypot(d[:, 0], d[:, 1])
+    cum = np.r_[0.0, np.cumsum(ln)]
+    s = np.clip(s, 0.0, cum[-1])
+    k = np.clip(np.searchsorted(cum, s, side="right") - 1, 0, len(ln) - 1)
+    t = (s - cum[k]) / ln[k]
+    return p[k, 0] + t * d[k, 0], p[k, 1] + t * d[k, 1], np.arctan2(d[k, 1], d[k, 0])
+
+
+def _place(paths, n, m, seed, starts, lane_of, spacing, speed, name, priority):
+    """Cars of rank r = 0, 1, ... on the slots of each start lane (``lane_of[slot]``), the first at arc length
+    ``starts[lane]`` minus a seeded 0-20 m, the others ``spacing`` (+-3 m) behind it, at seeded speeds in ``speed``."""
+    rng = np.random.default_rng(seed)
+    lane_of = np.asarray(lane_of)
+    x, y, h = (np.zeros((n, m)) for _ in range(3))
+    pid = np.full((n, m), -1, np.int16)
+    for i in range(n):
+        s_lane = {l: starts[l] - rng.uniform(0.0, 20.0) for l in set(lane_of.tolist())}
+        for k in range(m):
+            l = int(lane_of[k])
+            s = s_lane[l]
+            s_lane[l] = s - spacing + rng.uniform(-3.0, 3.0)
+            if s < 0.0:
+                continue   # no room left on this lane
+            x[i, k], y[i, k], h[i, k] = _point_at(paths[l], s)
+            pid[i, k] = l
+    v = rng.uniform(speed[0], speed[1], (n, m))
+    tid = np.where(pid >= 0, 0, TYPE_INACTIVE).astype(np.uint8)
+    f = lambda a: np.ascontiguousarray(np.where(pid >= 0, a, 0.0), np.float32)
+    return PathScene(path_table(), paths, np.asarray(priority, np.int16), f(x), f(y), f(h), f(v), tid, pid, name)
+
+
+def intersection(n: int, m: int = 8, seed: int = 0, exit_len: float = 200.0, spacing: float = 25.0,
+                 speed=(6.0, 10.0)) -> PathScene:
+    """A four-arm intersection with one straight-through lane per arm, all four crossing at the centre (right-hand
+    traffic, lanes 1.75 m off the axes): path 0 west to east, 1 south to north, 2 east to west, 3 north to south, each
+    long enough for its cars before the centre and ``exit_len`` after it, equal priority.  Slot k drives path k % 4; the
+    first car of each arm starts 0-20 m further from the centre than 30 m (seeded per scenario and arm), the others
+    ``spacing`` metres behind each other.  Without yielding, cars of crossing arms meet at the centre."""
+    o = 1.75
+    approach = 60.0 + spacing * ((m + 3) // 4)
+    paths = [_polyline([[-approach, -o], [exit_len, -o]]), _polyline([[o, -approach], [o, exit_len]]),
+             _polyline([[approach, o], [-exit_len, o]]), _polyline([[-o, approach], [-o, -exit_len]])]
+    lane_of = [k % 4 for k in range(m)]
+    return _place(paths, n, m, seed, {l: approach - 30.0 for l in range(4)}, lane_of, spacing, speed, "intersection",
+                  [0, 0, 0, 0])
+
+
+def t_junction(n: int, m: int = 8, seed: int = 0, speed=(6.0, 10.0), spacing: float = 25.0) -> PathScene:
+    """A T-junction merge: path 0 is the main road, west to east along y = 0 (priority 1); path 1 comes up from the south
+    along x = 0 and turns right onto it on a 10 m radius (priority 0), sharing its lane from x = 10 m on.  Slot k drives
+    path k % 2."""
+    side = _polyline([[0.0, -100.0], [0.0, -10.0]], _arc(10.0, -10.0, 10.0, np.pi, np.pi / 2, 12)[1:], [[300.0, 0.0]])
+    lane_of = [k % 2 for k in range(m)]
+    main = _polyline([[-120.0 - spacing * (m // 2), 0.0], [300.0, 0.0]])
+    return _place([main, side], n, m, seed, {0: 80.0 + spacing * (m // 2), 1: 60.0}, lane_of, spacing, speed, "t_junction",
+                  [1, 0])
+
+
+def roundabout(n: int, m: int = 11, seed: int = 0, radius: float = 20.0, arm: float = 80.0, speed=(6.0, 9.0),
+               spacing: float = 25.0, ring_cars: int = 3) -> PathScene:
+    """A four-arm roundabout (centre 0, ``radius`` m, anticlockwise, right-hand traffic): path 0 is the ring, three
+    quarters of a turn from 45 degrees and out on the south-east diagonal (priority 1); paths 1-4 enter from the east,
+    north, west and south arms, drive a quarter of the ring and leave by the next arm (priority 0), so that they merge
+    into the ring's traffic and diverge from it but never meet each other.  Entries and exits join the ring tangentially
+    (quadratic Bezier curves), so that a car that keeps its path stays on it, and each arm's two lanes run 3 m either side
+    of its axis.  Slots 0 .. ``ring_cars`` - 1 ride the ring,
+    a quarter turn apart from its start; slot k >= ``ring_cars`` enters by arm (k - ``ring_cars``) % 4."""
+    o = 3.0                                            # lanes 3 m off each arm's axis: a splitter island between them
+    end = 7 * np.pi / 4
+    ring = _polyline(_arc(0.0, 0.0, radius, np.pi / 4, end, 64), [[(radius + arm) * np.cos(end), (radius + arm) * np.sin(end)]])
+    paths = [ring]
+    for a in range(4):
+        th = a * np.pi / 2
+        c, s = np.cos(th), np.sin(th)
+        lane_in = lambda d: (d * c - o * s, d * s + o * c)                    # right of the inbound direction (-c, -s)
+        a_in, out = th + 0.45, th + np.pi / 2
+        a_out = out - 0.45
+        co, so = np.cos(out), np.sin(out)
+        lane_out = lambda d: (d * co + o * so, d * so - o * co)               # right of the outbound direction
+        ring_at = lambda a: (radius * np.cos(a), radius * np.sin(a))
+        tangent = lambda a: (-np.sin(a), np.cos(a))
+        join = _bezier(lane_in(radius + 8.0), _meet(lane_in(radius), (-c, -s), ring_at(a_in), tangent(a_in)), ring_at(a_in), 8)
+        quarter = _arc(0.0, 0.0, radius, a_in, a_out, 10)
+        leave = _bezier(ring_at(a_out), _meet(ring_at(a_out), tangent(a_out), lane_out(radius), (co, so)),
+                        lane_out(radius + 8.0), 8)
+        paths.append(_polyline([lane_in(radius + arm)], join[:-1], quarter, leave[1:], [lane_out(radius + 200.0)]))
+    ring_cars = min(ring_cars, m)
+    lane_of = [0] * ring_cars + [1 + (k - ring_cars) % 4 for k in range(ring_cars, m)]
+    rng = np.random.default_rng(seed + 7)
+    scene = _place(paths, n, m, seed, {0: 0.0, 1: arm - 10.0, 2: arm - 10.0, 3: arm - 10.0, 4: arm - 10.0}, lane_of,
+                   spacing, speed, "roundabout", [1, 0, 0, 0, 0])
+    for k in range(ring_cars):   # the ring's cars, placed by hand a quarter turn apart
+        x, y, h = _point_at(ring, k * radius * np.pi / 2)
+        scene.x[:, k], scene.y[:, k], scene.heading[:, k] = x, y, h
+        scene.path_id[:, k], scene.type_id[:, k] = 0, 0
+        scene.speed[:, k] = rng.uniform(speed[0], speed[1], n)
+    return scene
+
+
+def crossing_log(duration_ms: int = 60000, seed: int = 0, rate_per_s: float = 0.25, speed=(8.0, 12.0),
+                 length_m: float = 200.0, period_ms: int = 100):
+    """A seeded two-stream crossing recording (a :class:`tactics2d_b200.dataset_parser.ReplayLog`, type rows unassigned):
+    one stream drives west to east along y = -1.75, the other south to north along x = 1.75, crossing at the origin, each
+    a Poisson process of ``rate_per_s`` arrivals per second at the start of a ``length_m`` approach, at a constant speed
+    drawn from ``speed`` (m/s), one record every ``period_ms`` until the car leaves.  The recording ignores the other
+    stream: replayed as logged, its cars drive through each other at the crossing.  Cars are 4.5 m x 1.9 m."""
+    from .dataset_parser.replay import ReplayLog
+    from .participant.element import Vehicle
+
+    rng = np.random.default_rng(seed)
+    half = length_m / 2.0
+    tracks = []
+    for stream in range(2):
+        t = rng.exponential(1000.0 / rate_per_s)
+        while t < duration_ms:
+            tracks.append((stream, t, rng.uniform(speed[0], speed[1])))
+            t += max(rng.exponential(1000.0 / rate_per_s), 3000.0)   # at least 3 s apart in a stream
+    tracks.sort(key=lambda r: r[1])
+    recs, first = [], []
+    for stream, t, v in tracks:
+        f0 = int(np.floor(t / period_ms)) * period_ms
+        nfr = int(np.floor(length_m / (v * period_ms / 1000.0))) + 1
+        s = -half + v * np.arange(nfr) * (period_ms / 1000.0)
+        if stream == 0:
+            r = np.stack([s, np.full(nfr, -1.75), np.zeros(nfr), np.full(nfr, v), np.zeros(nfr)], 1)
+        else:
+            r = np.stack([np.full(nfr, 1.75), s, np.full(nfr, np.pi / 2), np.zeros(nfr), np.full(nfr, v)], 1)
+        recs.append(r.astype(np.float32))
+        first.append(f0)
+    K = len(recs)
+    return ReplayLog(ids=np.arange(K, dtype=np.int64), first_ms=np.asarray(first, np.int32),
+                     n_frames=np.asarray([len(r) for r in recs], np.int32), period_ms=np.full(K, period_ms, np.int32),
+                     records=np.ascontiguousarray(np.concatenate(recs)), type_row=np.full(K, TYPE_INACTIVE, np.uint8),
+                     cls=[Vehicle] * K, length=np.full(K, 4.5), width=np.full(K, 1.9))

@@ -180,7 +180,7 @@ class BatchedWorld:
         self._goal = self._ctrl = self._log = self._agents = self._ego_action = self._routes = self._sampler = None
         self._history, self._hist_out = 0, {}
         self._route_out = {}
-        self._leader = self._leader_out = self._lane = self._reactive = None
+        self._leader = self._leader_out = self._lane = self._reactive = self._yield = self._yield_out = None
         self._env = self._npc_action = self._host_out = self._host_agents = self._lidar = self._bev_out = None
         self._agent_lidar, self._obs_out, self._agent_obs_out, self._agent_bev = {}, {}, {}, {}
         self._seg_style_keys = []
@@ -357,7 +357,7 @@ class BatchedWorld:
             off[1:] = np.cumsum([len(p) for p in paths])
             _lib.check(self.lib.t2d_set_paths(self._ctx, C.c_void_p(xy.ctypes.data), C.c_void_p(off.ctypes.data), len(paths)))
         self.paths = paths
-        self._lane = self._reactive = None   # the library dropped a bound lane change and reactive replay
+        self._lane = self._reactive = self._yield = None   # the library dropped a bound lane change, reactive replay and yielding
 
     def set_controllers(self, controllers, ctrl_id, lead_index=None, path_id=None, last_accel=None, pid_target=None,
                         pid_state=None):
@@ -378,7 +378,7 @@ class BatchedWorld:
         if controllers is None:
             _lib.check(self.lib.t2d_set_controllers(self._ctx, _ptr(None), 0, _ptr(None), _ptr(None), _ptr(None), _ptr(None)))
             _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(None), _ptr(None)))
-            self._ctrl = self._lane = self._reactive = None
+            self._ctrl = self._lane = self._reactive = self._yield = None
             return
         rows = [c if isinstance(c, _lib.ControllerParamsC) else c.params() for c in controllers]
         arr = (_lib.ControllerParamsC * len(rows))(*rows)
@@ -403,7 +403,7 @@ class BatchedWorld:
         _lib.check(self.lib.t2d_set_controllers(self._ctx, arr, len(rows), _ptr(cid), _ptr(lead), _ptr(pid), _ptr(la)))
         _lib.check(self.lib.t2d_set_pid(self._ctx, _ptr(tgt), _ptr(st)))
         self._ctrl = dict(rows=arr, ctrl_id=cid, lead_index=lead, path_id=pid, last_accel=la, pid_target=tgt, pid_state=st)
-        self._lane = self._reactive = None   # the library dropped a bound lane change and reactive replay
+        self._lane = self._reactive = self._yield = None   # the library dropped a bound lane change, reactive replay and yielding
 
     @property
     def last_accel(self) -> Optional[torch.Tensor]:
@@ -436,7 +436,8 @@ class BatchedWorld:
         change.  A rejected call keeps the previous search."""
         if half_width is None:
             _lib.check(self.lib.t2d_set_leader_search(self._ctx, 0.0, 0.0, _ptr(None), _ptr(None)))
-            self._leader = self._lane = self._reactive = None   # unbinding the search drops a bound lane change and reactive replay
+            # unbinding the search drops a bound lane change, reactive replay and yielding
+            self._leader = self._lane = self._reactive = self._yield = None
             return
         lead = torch.full((self.N, self.M), -1, dtype=torch.int16, device=self.device)
         gap = torch.full((self.N, self.M), float("inf"), dtype=torch.float32, device=self.device)
@@ -513,6 +514,74 @@ class BatchedWorld:
     def lane_cooldown(self) -> Optional[torch.Tensor]:
         """int16 [N, M] device tensor: the ticks each slot still waits before it may change lanes again."""
         return None if self._lane is None else self._lane["cooldown"]
+
+    # ------------------------------------------------------------------ yielding at conflict zones
+    def set_yielding(self, priority=None, width: float = 2.0, margin: float = 3.0, critical_gap: float = 3.0,
+                     commit_decel: float = 3.0, v_min: float = 0.5):
+        """Yield at crossing and merging paths on the device in front of every ``control`` (``t2d_set_yielding``, K19;
+        DESIGN.md section 1 "Yielding at conflict zones").  The conflict zones of the bound ``set_paths`` table are built
+        once here (:func:`tactics2d_b200.traffic.conflicts.conflict_zones` with ``width`` and ``margin``).
+        Every IDM row on a path then stops ``margin`` metres before a zone, as behind a standing leader, while a car on the
+        other path is inside it or committed to it (it cannot stop at ``commit_decel`` m/s^2), or reaches it within
+        ``critical_gap`` seconds (at its speed, at least ``v_min``) with a higher path ``priority`` (int16 per path,
+        default all 0), or with an equal one and nearer its own zone.  A car already committed itself never yields.  The
+        yields of the last ``control`` are in :attr:`yield_to` (int16 [N, M], the slot yielded to, -1 for none) and
+        :attr:`stop_gap` (fp32 [N, M], the arc length to the stop, +inf for none).  Needs the controllers, the paths and a
+        leader search, whose corridor and range it uses; ``set_paths``, ``set_controllers`` and unbinding the search drop
+        it, and so does :meth:`unset_yielding`.  A rejected call keeps the previous binding."""
+        from .traffic.conflicts import conflict_zones
+
+        n_paths = 0 if self.paths is None else len(self.paths)
+        zones = conflict_zones(self.paths or [], width, margin)
+        rows = np.zeros(len(zones), _lib.ZONE_DTYPE)
+        for k in ("q", "s_in_p", "s_out_p", "s_in_q", "s_out_q"):
+            rows[k] = getattr(zones, k)
+        off = np.ascontiguousarray(zones.zone_off, np.int32)
+        prio = None
+        if priority is not None:
+            prio = np.asarray(priority, np.int64).reshape(-1)
+            if prio.shape != (n_paths,) or (prio < -32768).any() or (prio > 32767).any():
+                raise ValueError(f"priority must hold one int16 per path of set_paths ({n_paths})")
+            prio = np.ascontiguousarray(prio.astype(np.int16))
+        p = _lib.YieldParamsC(critical_gap=float(critical_gap), commit_decel=float(commit_decel), v_min=float(v_min))
+        NM = (self.N, self.M)
+        yield_to = torch.full(NM, -1, dtype=torch.int16, device=self.device)
+        stop_gap = torch.full(NM, float("inf"), dtype=torch.float32, device=self.device)
+        host = lambda a: None if a is None or a.size == 0 else C.c_void_p(a.ctypes.data)
+        _lib.check(self.lib.t2d_set_yielding(self._ctx, C.byref(p), host(rows), host(off), host(prio), _ptr(yield_to),
+                                             _ptr(stop_gap)))
+        self._yield = dict(params=p, zones=zones, priority=prio, yield_to=yield_to, stop_gap=stop_gap)
+
+    def unset_yielding(self):
+        """Unbind yielding: ``control`` launches K19 no more and K5 runs its other instances."""
+        _lib.check(self.lib.t2d_set_yielding(self._ctx, None, None, None, None, None, None))
+        self._yield = None
+
+    @property
+    def conflict_zones(self):
+        """The :class:`~tactics2d_b200.traffic.conflicts.ConflictZones` of the bound yielding (None without one)."""
+        return None if self._yield is None else self._yield["zones"]
+
+    @property
+    def yield_to(self) -> Optional[torch.Tensor]:
+        """int16 [N, M] device tensor: the slot each car yielded to in the last ``control``, -1 for none (None when
+        yielding is not bound)."""
+        return None if self._yield is None else self._yield["yield_to"]
+
+    @property
+    def stop_gap(self) -> Optional[torch.Tensor]:
+        """fp32 [N, M] device tensor: the arc length from each yielding car to its stop, +inf where it does not yield."""
+        return None if self._yield is None else self._yield["stop_gap"]
+
+    def find_yields(self):
+        """The yields of the current state in one launch (``t2d_find_yields``, K19) with the bound yielding:
+        ``(yield_to, stop_gap)`` as :attr:`yield_to` / :attr:`stop_gap`.  The tensors are buffers the next call reuses."""
+        if self._yield_out is None:
+            self._yield_out = (torch.empty((self.N, self.M), dtype=torch.int16, device=self.device),
+                               torch.empty((self.N, self.M), dtype=torch.float32, device=self.device))
+        yt, sg = self._yield_out
+        _lib.check(self.lib.t2d_find_yields(self._ctx, _ptr(yt), _ptr(sg), self._stream()))
+        return yt, sg
 
     # ------------------------------------------------------------------ route following
     def set_routes(self, route_id, threshold: float = None, progress_weight: float = 0.1, off_route_reward: float = -5.0):
