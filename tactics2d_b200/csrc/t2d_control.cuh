@@ -29,9 +29,7 @@ struct CtrlArgs : WorldArgs {
   const uint8_t* ctrl_id;
   const int16_t* lead;
   const int16_t* path_id;
-  const PathVertex* path_v;
-  const int* path_off;
-  int n_paths;
+  PathTable paths;
   float* last_accel;
   float* action;
   const float* ego_action;   // [N][2] or nullptr: participant 0's action (written into its row of `action` as well)
@@ -171,10 +169,10 @@ __device__ __forceinline__ double pid_lateral_law(const t2d_controller_params& p
     } else if (lat == T2D_PID_LAT_CROSS_TRACK) {                                             // :275-279
       e = (double)A.pid_target[2 * i + 1];
     } else {
-      const int pid = A.path_id ? (int)A.path_id[i] : -1;
-      have = pid >= 0 && pid < A.n_paths &&
-             path_lateral_error(A.path_v + A.path_off[pid], A.path_off[pid + 1] - A.path_off[pid], x, y, heading,
-                                lat == T2D_PID_LAT_PATH_CROSS_TRACK, e);
+      const PathVertex* pv;
+      int nv;
+      have = A.paths.vertices(A.path_id ? (int)A.path_id[i] : -1, pv, nv) &&
+             path_lateral_error(pv, nv, x, y, heading, lat == T2D_PID_LAT_PATH_CROSS_TRACK, e);
     }
     if (have) {
       double s[3] = {st[0], st[1], st[2]};
@@ -273,10 +271,10 @@ __device__ __forceinline__ void control_body(const CtrlArgs& A) {
         } else {
           acc = longitudinal_law(p, v, x, y, (double)A.last_accel[base + m], has, vl, xl, yl, al);
           if (p.kind == T2D_CTRL_PURE_PURSUIT) {
-            const int pid = A.path_id ? (int)A.path_id[base + m] : -1;
-            if (pid >= 0 && pid < A.n_paths)
-              steer = pure_pursuit_law(p, A.path_v + A.path_off[pid], A.path_off[pid + 1] - A.path_off[pid], v, x, y,
-                                       (double)A.h[base + m]);
+            const PathVertex* pv;
+            int nv;
+            if (A.paths.vertices(A.path_id ? (int)A.path_id[base + m] : -1, pv, nv))
+              steer = pure_pursuit_law(p, pv, nv, v, x, y, (double)A.h[base + m]);
           }
         }
         out[j] = A.steer_first ? make_float2((float)steer, (float)acc) : make_float2((float)acc, (float)steer);

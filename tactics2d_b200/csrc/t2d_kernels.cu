@@ -337,29 +337,51 @@ struct t2d_ctx {
   std::unique_ptr<DeviceHistory> hist;      // t2d_set_history; nullptr: none bound
 };
 
-enum : unsigned { NEED_STATE = 1, NEED_TABLE = 2, NEED_TICK = 4 };
+enum : unsigned { NEED_STATE = 1, NEED_TABLE = 2, NEED_TICK = 4,
+                  NEED_LOG = 8, NEED_CTRL = 16, NEED_PATHS = 32, NEED_PID = 64, NEED_SEARCH = 128 };
 
-// The call-order preconditions, checked in this order: the bound state, the type table, and what a tick with physics
-// needs besides (a caller that launches other kernels first checks them up front).
-static int require(const t2d_ctx* c, unsigned need) {
-  if ((need & NEED_STATE) && !c->x) return fail(T2D_E_STATE, "state not bound: call t2d_bind_state first");
+// The call-order preconditions, checked in this order: the bound state, the type table, what a tick with physics needs
+// besides (a caller that launches other kernels first checks them up front), then the bindings the traffic stages read:
+// the log, the controllers, the paths, the PID state and the leader search.  fn, when given, prefixes the message.
+static int require(const t2d_ctx* c, unsigned need, const char* fn = nullptr) {
+  const auto missing = [fn](const char* msg) { return fail(T2D_E_STATE, fn ? std::string(fn) + ": " + msg : msg); };
+  if ((need & NEED_STATE) && !c->x) return missing("state not bound: call t2d_bind_state first");
   if ((need & NEED_TABLE) && (!c->d_table || c->n_types == 0))
-    return fail(T2D_E_STATE, "type table not set: call t2d_set_type_table first");
+    return missing("type table not set: call t2d_set_type_table first");
   if (need & NEED_TICK) {
     if (c->has_drift && !(c->wheel_f && c->wheel_r))
-      return fail(T2D_E_STATE, "the type table holds a SingleTrackDrift row: call t2d_bind_wheel_state first");
-    if (c->log && c->log->type_id != c->type_id) return fail(T2D_E_STATE, "state rebound after t2d_set_log: call t2d_set_log again");
+      return missing("the type table holds a SingleTrackDrift row: call t2d_bind_wheel_state first");
+    if (c->log && c->log->type_id != c->type_id) return missing("state rebound after t2d_set_log: call t2d_set_log again");
   }
+  if ((need & NEED_LOG) && !c->log) return missing("no log bound: call t2d_set_log or t2d_set_log_schedule first");
+  if ((need & NEED_CTRL) && !c->d_ctab) return missing("controllers not set: call t2d_set_controllers first");
+  if ((need & NEED_PATHS) && c->n_paths == 0) return missing("no paths bound: call t2d_set_paths first");
+  if ((need & NEED_PID) && !c->pid_state) return missing("no PID state bound: call t2d_set_pid first");
+  if ((need & NEED_SEARCH) && !c->leader_lead) return missing("no leader search bound: call t2d_set_leader_search first");
   return T2D_OK;
+}
+
+// The traffic bindings name what other setters bind.  A lane change and yielding read the controllers' rows and paths,
+// the path table and the search's corridor; a reactive replay reads those too, and the type table's rows and the log's
+// tracks.  A setter that replaces or unbinds one of these (changed: its NEED_ bit) drops every binding that reads it.
+static void drop_traffic(t2d_ctx* c, unsigned changed) {
+  if (changed & (NEED_CTRL | NEED_PATHS | NEED_SEARCH)) {
+    c->lane.reset();
+    c->yield.reset();
+  }
+  if (changed & (NEED_TABLE | NEED_LOG | NEED_CTRL | NEED_PATHS | NEED_SEARCH)) c->reactive.reset();
 }
 
 static WorldArgs world_args(const t2d_ctx* c) {
   return {c->x, c->y, c->h, c->v, c->vx, c->vy, c->type_id, c->step_count, c->d_table.get(), c->n_types, c->N, c->M};
 }
 
+static PathTable path_table(const t2d_ctx* c) {
+  return {c->d_path_v.get(), c->d_path_off.get(), c->n_paths};
+}
+
 static RouteArgs route_args(const t2d_ctx* c) {
-  return {c->route_id, c->d_path_v.get(), c->d_path_off.get(), c->n_paths, c->route_off_reward, c->route_threshold,
-          c->route_weight};
+  return {c->route_id, path_table(c), c->route_off_reward, c->route_threshold, c->route_weight};
 }
 
 // K10 reads its progress tracker by the bound agents' rows: a tracker bound for another Q is a call-order error
@@ -620,7 +642,7 @@ int t2d_set_type_table(t2d_ctx* c, const t2d_type_params* table, int n_types) {
   c->type_model.resize(n_types);
   for (int i = 0; i < n_types; ++i) c->type_model[i] = table[i].model;
   c->type_rows.assign(table, table + n_types);
-  c->reactive.reset();   // its driving rows named the old table
+  drop_traffic(c, NEED_TABLE);
   c->has_pointmass = has_pointmass;
   c->has_drift = has_drift;
   c->rb_max = rb_max;
@@ -992,7 +1014,7 @@ static int set_log(t2d_ctx* c, const t2d_log* L, const char* who, const int32_t*
     c->hist->track = std::move(tracks.track);
   }
   c->log = std::move(g);
-  c->reactive.reset();   // its tables described the old log's tracks
+  drop_traffic(c, NEED_LOG);
   return T2D_OK;
 }
 
@@ -1001,7 +1023,7 @@ int t2d_set_log(t2d_ctx* c, const t2d_log* L) {
   if (!L) {
     CUDA_TRY(cudaSetDevice(c->device));
     c->log.reset();
-    c->reactive.reset();
+    drop_traffic(c, NEED_LOG);
     if (c->hist) c->hist->track.reset();
     return T2D_OK;
   }
@@ -1227,7 +1249,7 @@ static const int16_t* current_path(const t2d_ctx* c) {
 static int launch_leaders(t2d_ctx* c, double half_width, double max_range, int16_t* lead, float* gap, void* stream) {
   CUDA_TRY(cudaSetDevice(c->device));
   leader::Args A{world_args(c)};
-  A.path_id = current_path(c); A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.path_id = current_path(c); A.paths = path_table(c);
   A.half_width = half_width; A.max_range = max_range; A.lead = lead; A.gap = gap;
   leader::t2d_leader_kernel<<<(c->N + leader::WARPS - 1) / leader::WARPS, leader::WARPS * 32, 0, (cudaStream_t)stream>>>(A);
   return launched();
@@ -1237,8 +1259,7 @@ static int launch_leaders(t2d_ctx* c, double half_width, double max_range, int16
 static int launch_lane_change(t2d_ctx* c, void* stream) {
   const LaneChange& L = *c->lane;
   lane::Args A{world_args(c)};
-  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id;
-  A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.paths = path_table(c);
   A.left = L.left.get(); A.right = L.right.get();
   A.half_width = c->leader_half_width; A.max_range = c->leader_max_range;
   A.politeness = L.p.politeness; A.threshold = L.p.threshold; A.b_safe = L.p.b_safe; A.min_gap = L.p.min_gap;
@@ -1254,8 +1275,7 @@ static int launch_yields(t2d_ctx* c, int16_t* yield_to, float* stop_gap, void* s
   CUDA_TRY(cudaSetDevice(c->device));
   yield::Args A{world_args(c)};
   A.path_id = current_path(c); A.route_id = c->route_id;
-  A.ctrl_id = c->ctrl_id; A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl;
-  A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.ctrl_id = c->ctrl_id; A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.paths = path_table(c);
   A.zones = Y.zones.get(); A.zone_off = Y.zone_off.get(); A.priority = Y.priority.get();
   A.half_width = c->leader_half_width; A.max_range = c->leader_max_range;
   A.critical_gap = Y.p.critical_gap; A.two_commit_decel = 2.0 * Y.p.commit_decel; A.v_min = Y.p.v_min;
@@ -1265,8 +1285,7 @@ static int launch_yields(t2d_ctx* c, int16_t* yield_to, float* stop_gap, void* s
 }
 
 static int launch_control(t2d_ctx* c, float* action, const float* ego, void* stream) {
-  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
-  if (!c->d_ctab) return fail(T2D_E_STATE, "controllers not set: call t2d_set_controllers first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE | NEED_CTRL)) return r;
   if (int r = check_pid_binding(c)) return r;
   if (!action) return fail(T2D_E_INVALID, "action is NULL");
   if (!aligned8(action)) return fail(T2D_E_INVALID, "action must be 8-byte aligned");
@@ -1282,8 +1301,7 @@ static int launch_control(t2d_ctx* c, float* action, const float* ego, void* str
     if (int r = launch_yields(c, c->yield->yield_to, c->yield->stop_gap, stream)) return r;
   CtrlArgs A{world_args(c)};
   A.ctab = c->d_ctab.get(); A.n_ctrl = c->n_ctrl; A.ctrl_id = c->ctrl_id; A.path_id = current_path(c);
-  A.lead = c->leader_lead ? c->leader_lead : c->ctrl_lead;
-  A.path_v = c->d_path_v.get(); A.path_off = c->d_path_off.get(); A.n_paths = c->n_paths;
+  A.lead = c->leader_lead ? c->leader_lead : c->ctrl_lead; A.paths = path_table(c);
   A.last_accel = c->ctrl_last_accel; A.action = action; A.ego_action = ego;
   A.steer_first = (c->cfg.flags & T2D_CFG_STEER_FIRST) ? 1 : 0;
   A.pid_target = c->pid_target; A.pid_state = c->pid_state;
@@ -1938,9 +1956,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
     c->n_ctrl = 0; c->ctrl_id = nullptr; c->ctrl_lead = nullptr; c->ctrl_path = nullptr;
     c->ctrl_last_accel = nullptr;
     c->ctrl_has_pid = c->ctrl_pid_reads_target = false;
-    c->lane.reset();
-    c->reactive.reset();
-    c->yield.reset();
+    drop_traffic(c, NEED_CTRL);
     return T2D_OK;
   }
   if (n_rows <= 0 || n_rows > T2D_MAX_CONTROLLERS) return fail(T2D_E_INVALID, "n_rows must be in 1..T2D_MAX_CONTROLLERS");
@@ -1986,9 +2002,7 @@ int t2d_set_controllers(t2d_ctx* c, const t2d_controller_params* table, int n_ro
   if (int r = upload(c->d_ctab, table, (size_t)n_rows)) return r;
   c->n_ctrl = n_rows; c->ctrl_id = ctrl_id; c->ctrl_lead = lead_index; c->ctrl_path = path_id; c->ctrl_last_accel = last_accel;
   c->ctrl_has_pid = has_pid; c->ctrl_pid_reads_target = reads_target;
-  c->lane.reset();   // its lane_path was copied from the old path_id
-  c->reactive.reset();   // its slots needed the old table's rows
-  c->yield.reset();   // its yielders were the old table's IDM rows
+  drop_traffic(c, NEED_CTRL);
   return T2D_OK;
 }
 
@@ -2010,9 +2024,7 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   CUDA_TRY(cudaSetDevice(c->device));
   if (n_paths == 0 || !xy) {   // unbind
     c->d_path_v.reset(); c->d_path_off.reset(); c->n_paths = 0; c->path_host.clear(); c->path_off_host.clear();
-    c->lane.reset();
-    c->reactive.reset();
-    c->yield.reset();
+    drop_traffic(c, NEED_PATHS);
     return T2D_OK;
   }
   if (n_paths < 0 || !offsets) return fail(T2D_E_INVALID, "t2d_set_paths: bad argument");
@@ -2040,9 +2052,7 @@ int t2d_set_paths(t2d_ctx* c, const float* xy, const int32_t* offsets, int n_pat
   c->d_path_v = std::move(d_v); c->d_path_off = std::move(d_off); c->n_paths = n_paths;
   c->path_host = std::move(pv);
   c->path_off_host.assign(offsets, offsets + n_paths + 1);
-  c->lane.reset();   // its neighbour table named the old paths
-  c->reactive.reset();   // its track paths named them too
-  c->yield.reset();   // its zones were built on them
+  drop_traffic(c, NEED_PATHS);
   return T2D_OK;
 }
 
@@ -2098,9 +2108,7 @@ int t2d_set_leader_search(t2d_ctx* c, double half_width, double max_range, int16
   if (!c) return fail(T2D_E_INVALID, "ctx is NULL");
   if (!lead) {   // unbind
     c->leader_lead = nullptr; c->leader_gap = nullptr; c->leader_half_width = c->leader_max_range = 0.0;
-    c->lane.reset();   // a lane change reads the search's corridor
-    c->reactive.reset();   // reactive slots brake for the search's leaders
-    c->yield.reset();   // yielding reads the search's corridor and range
+    drop_traffic(c, NEED_SEARCH);
     return T2D_OK;
   }
   if (int r = check_leader_args("t2d_set_leader_search", half_width, max_range, lead, gap)) return r;
@@ -2136,11 +2144,8 @@ int t2d_set_lane_change(t2d_ctx* c, const t2d_lane_change_params* p, const int16
     return fail(T2D_E_INVALID, "t2d_set_lane_change: left / right / lane_path / cooldown is NULL");
   if (!aligned2(lane_path) || !aligned2(cooldown))
     return fail(T2D_E_INVALID, "t2d_set_lane_change: lane_path and cooldown must be 2-byte aligned");
-  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
-  if (!c->d_ctab) return fail(T2D_E_STATE, "t2d_set_lane_change: controllers not set: call t2d_set_controllers first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE | NEED_CTRL | NEED_PATHS | NEED_SEARCH, "t2d_set_lane_change")) return r;
   if (!c->ctrl_path) return fail(T2D_E_STATE, "t2d_set_lane_change: the controllers have no path_id");
-  if (c->n_paths == 0) return fail(T2D_E_STATE, "t2d_set_lane_change: no paths bound: call t2d_set_paths first");
-  if (!c->leader_lead) return fail(T2D_E_STATE, "t2d_set_lane_change: no leader search bound: call t2d_set_leader_search first");
   if (c->reactive) return fail(T2D_E_STATE, "t2d_set_lane_change: a reactive replay is bound (lane changes on track paths are not supported)");
   if (p->min_gap > c->leader_max_range)
     return fail(T2D_E_INVALID, "t2d_set_lane_change: min_gap must not exceed the search's max_range");
@@ -2198,10 +2203,7 @@ int t2d_set_yielding(t2d_ctx* c, const t2d_yield_params* p, const t2d_conflict_z
   if (!zone_off || !yield_to || !stop_gap) return fail(T2D_E_INVALID, fn + ": zone_off / yield_to / stop_gap is NULL");
   if (!aligned2(yield_to) || !aligned4(stop_gap) || !aligned8(zones) || !aligned4(zone_off) || !aligned2(priority))
     return fail(T2D_E_INVALID, fn + ": yield_to, priority must be 2-byte, stop_gap, zone_off 4-byte and zones 8-byte aligned");
-  if (int r = require(c, NEED_STATE | NEED_TABLE)) return r;
-  if (!c->d_ctab) return fail(T2D_E_STATE, fn + ": controllers not set: call t2d_set_controllers first");
-  if (c->n_paths == 0) return fail(T2D_E_STATE, fn + ": no paths bound: call t2d_set_paths first");
-  if (!c->leader_lead) return fail(T2D_E_STATE, fn + ": no leader search bound: call t2d_set_leader_search first");
+  if (int r = require(c, NEED_STATE | NEED_TABLE | NEED_CTRL | NEED_PATHS | NEED_SEARCH, fn.c_str())) return r;
   const int P = c->n_paths;
   if (zone_off[0] != 0) return fail(T2D_E_INVALID, fn + ": zone_off[0] must be 0");
   for (int k = 0; k < P; ++k)
@@ -2265,12 +2267,8 @@ int t2d_set_log_reactive(t2d_ctx* c, const t2d_reactive_replay* r) {
     return fail(T2D_E_INVALID, fn + ": NULL array");
   if (!aligned2(r->drive_path) || !aligned4(r->slot_desired_speed))
     return fail(T2D_E_INVALID, fn + ": drive_path must be 2-byte and slot_desired_speed 4-byte aligned");
-  if (int e = require(c, NEED_STATE | NEED_TABLE)) return e;
-  if (!c->log) return fail(T2D_E_STATE, fn + ": no log bound: call t2d_set_log or t2d_set_log_schedule first");
-  if (!c->d_ctab) return fail(T2D_E_STATE, fn + ": controllers not set: call t2d_set_controllers first");
-  if (c->n_paths == 0) return fail(T2D_E_STATE, fn + ": no paths bound: call t2d_set_paths first");
-  if (!c->pid_state) return fail(T2D_E_STATE, fn + ": no PID state bound: call t2d_set_pid first");
-  if (!c->leader_lead) return fail(T2D_E_STATE, fn + ": no leader search bound: call t2d_set_leader_search first");
+  const unsigned need = NEED_STATE | NEED_TABLE | NEED_LOG | NEED_CTRL | NEED_PATHS | NEED_PID | NEED_SEARCH;
+  if (int e = require(c, need, fn.c_str())) return e;
   if (c->lane) return fail(T2D_E_STATE, fn + ": a lane change is bound (lane changes on track paths are not supported)");
   if (r->n_tracks != c->log->n_tracks)
     return fail(T2D_E_INVALID, fn + ": n_tracks must be the bound log's (" + std::to_string(c->log->n_tracks) + ")");

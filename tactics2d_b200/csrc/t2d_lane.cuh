@@ -9,7 +9,7 @@
 //   candidate    K17's: type < n_types, a shape, a position that is not NaN; on path r when its distance to r (K17's
 //                closest_on_path<true>) is <= half_width, s^r its arc length there;
 //   changer      an IDM row with a lateral channel, at a position that is not NaN, cooldown 0, its current path p usable
-//                (K17's has_segment), itself on p, and a usable neighbour q in {left[p], right[p]};
+//                (PathTable::usable), itself on p, and a usable neighbour q in {left[p], right[p]};
 //   on q         blocked when a candidate on q has |s^q_j - s^q_c| < min_gap; the new leader l' is the candidate on q of
 //                smallest s^q_j - s^q_c in (0, max_range], the new follower n the same behind (ties: lower slot); the old
 //                leader l and follower o the same on p;
@@ -28,7 +28,6 @@
 #include <stdint.h>
 
 #include "t2d_control.cuh"
-#include "t2d_leader.cuh"
 #include "t2d_route.cuh"
 #include "t2d_world.cuh"
 
@@ -43,9 +42,7 @@ struct Args : WorldArgs {
   const t2d_controller_params* ctab;
   int n_ctrl;
   const uint8_t* ctrl_id;                 // [N][M]
-  const PathVertex* path_v;
-  const int* path_off;
-  int n_paths;
+  PathTable paths;
   const int16_t* left;                    // [n_paths] device: the left / right neighbour of every path, -1 for none
   const int16_t* right;
   double half_width, max_range;           // the bound leader search's
@@ -63,10 +60,6 @@ struct Smem {   // per warp
   uint8_t on[128];                        // ... within half_width of the path being walked
   uint8_t row[128];                       // the slot's IDM row, NONE without one
 };
-
-__device__ __forceinline__ bool usable(const Args& A, int p) {
-  return p >= 0 && p < A.n_paths && leader::has_segment(A.path_v + A.path_off[p], A.path_off[p + 1] - A.path_off[p]);
-}
 
 // a(f | L): idm_law of slot f behind slot L (L == NONE: free flow), with f's IDM row or `own` when f has none
 __device__ __forceinline__ double accel(const Args& A, const Smem& sm, unsigned own, unsigned f, unsigned L) {
@@ -107,9 +100,9 @@ __device__ __forceinline__ void decide_row(const Args& A, Smem& sm, int lane, lo
     sm.v[m] = A.v[base + m];
     const bool finite = !(isnan(x) || isnan(y));
     sm.cand[m] = finite && A.table[t].shape() != SHAPE_NONE;
-    if (!(finite && idm && A.ctab[cid].pid_lateral != T2D_PID_LAT_NONE && c0[k] <= 0 && usable(A, p0[k]))) continue;
+    if (!(finite && idm && A.ctab[cid].pid_lateral != T2D_PID_LAT_NONE && c0[k] <= 0 && A.paths.usable(p0[k]))) continue;
     const int ql = A.left[p0[k]], qr = A.right[p0[k]];
-    const bool hl = usable(A, ql), hr = usable(A, qr);
+    const bool hl = A.paths.usable(ql), hr = A.paths.usable(qr);
     if (!(hl || hr)) continue;
     need[k][0] = p0[k];
     need[k][1] = hl ? ql : NO_PATH;
@@ -128,8 +121,8 @@ __device__ __forceinline__ void decide_row(const Args& A, Smem& sm, int lane, lo
         if (pend[k] & (1u << e)) mine = min(mine, need[k][e]);
     const int r = __reduce_min_sync(0xffffffffu, mine);
     if (r == NO_PATH) break;
-    const PathVertex* pv = A.path_v + A.path_off[r];
-    const int nv = A.path_off[r + 1] - A.path_off[r];
+    const PathVertex* pv = A.paths.v + A.paths.off[r];
+    const int nv = A.paths.off[r + 1] - A.paths.off[r];
     double sc[4];
     bool walk[4];
 #pragma unroll

@@ -31,9 +31,7 @@ constexpr int NO_PATH = 0x7fffffff;       // the follower takes the heading fram
 
 struct Args : WorldArgs {
   const int16_t* path_id;                 // [N][M] the controllers' path of every slot, or nullptr: heading frame for all
-  const PathVertex* path_v;
-  const int* path_off;
-  int n_paths;
+  PathTable paths;
   double half_width, max_range;
   int16_t* lead;                          // [N][M]
   float* gap;                             // [N][M] or nullptr
@@ -45,15 +43,6 @@ struct Smem {   // per warp
   uint8_t cand[128];                      // the slot is a candidate
   uint8_t on[128];                        // ... within half_width of the path being walked
 };
-
-// A path is usable when it has a segment of non-zero length: closest_on_path's test, segment by segment
-__device__ __forceinline__ bool has_segment(const PathVertex* pv, int n_vert) {
-  for (int i = 0; i + 1 < n_vert; ++i) {
-    const double dx = __dsub_rn(pv[i + 1].x, pv[i].x), dy = __dsub_rn(pv[i + 1].y, pv[i].y);
-    if (__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)) > 0.0) return true;
-  }
-  return false;
-}
 
 // The leaders of scenario n, written by one warp
 __device__ __forceinline__ void find_row(const Args& A, Smem& sm, int lane, long long n) {
@@ -82,7 +71,7 @@ __device__ __forceinline__ void find_row(const Args& A, Smem& sm, int lane, long
     if (!fol[k]) continue;
     if (A.path_id) {
       const int p = A.path_id[base + m];
-      if (p >= 0 && p < A.n_paths && has_segment(A.path_v + A.path_off[p], A.path_off[p + 1] - A.path_off[p])) pend[k] = p;
+      if (A.paths.usable(p)) pend[k] = p;
     }
     if (pend[k] == NO_PATH) {
       f[k].x0 = x;
@@ -116,8 +105,8 @@ __device__ __forceinline__ void find_row(const Args& A, Smem& sm, int lane, long
   for (;;) {
     const int p = __reduce_min_sync(0xffffffffu, min(min(pend[0], pend[1]), min(pend[2], pend[3])));
     if (p == NO_PATH) break;
-    const PathVertex* pv = A.path_v + A.path_off[p];
-    const int nv = A.path_off[p + 1] - A.path_off[p];
+    const PathVertex* pv = A.paths.v + A.paths.off[p];
+    const int nv = A.paths.off[p + 1] - A.paths.off[p];
     double si[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {

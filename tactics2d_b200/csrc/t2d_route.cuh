@@ -1,5 +1,5 @@
-// t2d_route.cuh - the path geometry of the polyline table (closest point, OffRoute probe) that K5, the epilogues
-// and K12 read, and K12 t2d_route_obs_kernel (the route of every observer row in its frame).
+// t2d_route.cuh - the polyline table and its path geometry (closest point, OffRoute probe) that K5, K17-K19, the
+// epilogues and K12 read, and K12 t2d_route_obs_kernel (the route of every observer row in its frame).
 #pragma once
 
 #include "t2d_world.cuh"
@@ -7,9 +7,36 @@
 namespace t2d {
 
 // ---------------------------------------------------------------------------- route following
-// DESIGN.md section 1 "Route following": the polyline table (t2d_set_paths) read by K5's PATH sources, the OffRoute
-// detector and route progress of the epilogues, and K12.
+// DESIGN.md section 1 "Route following": the polyline table (t2d_set_paths) read by K5's PATH sources, the traffic
+// stages K17-K19, the OffRoute detector and route progress of the epilogues, and K12.
 struct PathVertex { double x, y, cum, len; };   // vertex, arc length up to it, length of the segment that starts here
+
+// The bound polyline table: path p in [0, n) owns v[off[p] .. off[p + 1]); n == 0 when none is bound
+struct PathTable {
+  const PathVertex* v;
+  const int* off;
+  int n;
+
+  // The polyline of path p into (pv, n_vert); false, with both left alone, when p is not a path of the table
+  __device__ __forceinline__ bool vertices(int p, const PathVertex*& pv, int& n_vert) const {
+    if (p < 0 || p >= n) return false;
+    n_vert = off[p + 1] - off[p];
+    pv = v + off[p];
+    return true;
+  }
+
+  // p is a path of the table with a segment of non-zero length: closest_on_path's test, segment by segment
+  __device__ __forceinline__ bool usable(int p) const {
+    if (p < 0 || p >= n) return false;
+    const PathVertex* pv = v + off[p];
+    const int n_vert = off[p + 1] - off[p];
+    for (int i = 0; i + 1 < n_vert; ++i) {
+      const double dx = __dsub_rn(pv[i + 1].x, pv[i].x), dy = __dsub_rn(pv[i + 1].y, pv[i].y);
+      if (__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)) > 0.0) return true;
+    }
+    return false;
+  }
+};
 
 // The closest point c of a polyline to (x, y): the first strict minimum of |p - c|^2 over the segments of non-zero
 // length, c the clamped projection, and that segment's unit tangent u.  ARC adds d2 = |p - c|^2, the arc length s of c
@@ -54,19 +81,16 @@ __device__ __forceinline__ bool closest_on_path(const PathVertex* pv, int n_vert
 // The bound routes (t2d_set_routes): route_id == nullptr when none are bound
 struct RouteArgs {
   const int16_t* route_id;          // [N][M] path of every slot, -1 (or any id the table does not hold): none
-  const PathVertex* path_v;
-  const int* path_off;
-  int n_paths;
+  PathTable paths;
   float off_reward;                 // the reward of an off-route step
   double threshold, weight;         // OffRoute threshold (m), progress weight (per m)
 };
 
 // The polyline of slot i's route, or nullptr
 __device__ __forceinline__ const PathVertex* route_of(const RouteArgs& R, long long i, int& n_vert) {
-  const int rid = R.route_id[i];
-  if (rid < 0 || rid >= R.n_paths) return nullptr;
-  n_vert = R.path_off[rid + 1] - R.path_off[rid];
-  return R.path_v + R.path_off[rid];
+  const PathVertex* pv = nullptr;
+  R.paths.vertices(R.route_id[i], pv, n_vert);
+  return pv;
 }
 
 enum : int { ROUTE_NONE = 0, ROUTE_ON = 1, ROUTE_OFF = 2 };

@@ -24,7 +24,6 @@
 
 #include <stdint.h>
 
-#include "t2d_leader.cuh"
 #include "t2d_route.cuh"
 #include "t2d_world.cuh"
 
@@ -46,9 +45,7 @@ struct Args : WorldArgs {
   const uint8_t* ctrl_id;
   const t2d_controller_params* ctab;
   int n_ctrl;
-  const PathVertex* path_v;
-  const int* path_off;
-  int n_paths;
+  PathTable paths;
   const Zone* zones;
   const int* zone_off;                    // [n_paths + 1]
   const int16_t* priority;                // [n_paths]
@@ -65,10 +62,6 @@ struct Smem {   // per warp
   float v[128];
   int16_t path[128];                      // the partner's slot path, -1 when the slot is no partner
 };
-
-__device__ __forceinline__ bool usable(const Args& A, int p) {
-  return p >= 0 && p < A.n_paths && leader::has_segment(A.path_v + A.path_off[p], A.path_off[p + 1] - A.path_off[p]);
-}
 
 // v^2 / (2 commit_decel): the distance slot speed v needs to stop at commit_decel
 __device__ __forceinline__ double commit_distance(const Args& A, double v) {
@@ -92,11 +85,11 @@ __device__ __forceinline__ void find_row(const Args& A, Smem& sm, int lane, long
     const float x = A.x[base + m], y = A.y[base + m];
     if (isnan(x) || isnan(y)) continue;
     int p = A.path_id ? (int)A.path_id[base + m] : -1;
-    const bool current = usable(A, p);
-    if (!current) p = A.route_id && usable(A, A.route_id[base + m]) ? (int)A.route_id[base + m] : -1;
+    const bool current = A.paths.usable(p);
+    if (!current) p = A.route_id && A.paths.usable(A.route_id[base + m]) ? (int)A.route_id[base + m] : -1;
     if (p < 0) continue;
     PathPoint c;
-    closest_on_path<true>(A.path_v + A.path_off[p], A.path_off[p + 1] - A.path_off[p], (double)x, (double)y, c);
+    closest_on_path<true>(A.paths.v + A.paths.off[p], A.paths.off[p + 1] - A.paths.off[p], (double)x, (double)y, c);
     const float v = A.v[base + m];
     if (A.table[t].shape() != SHAPE_NONE) {
       sm.path[m] = (int16_t)p;
@@ -130,8 +123,8 @@ __device__ __forceinline__ void find_row(const Args& A, Smem& sm, int lane, long
         if (__dsub_rn(A.zones[mid].s_in_p, si[k]) > cd) hi = mid; else lo = mid + 1;
       }
       const int prio_p = A.priority[p];
-      const PathVertex* pv = A.path_v + A.path_off[p];
-      const int nv = A.path_off[p + 1] - A.path_off[p];
+      const PathVertex* pv = A.paths.v + A.paths.off[p];
+      const int nv = A.paths.off[p + 1] - A.paths.off[p];
       for (int z = lo; z < end && who < 0; ++z) {
         const Zone Z = A.zones[z];
         const double di = __dsub_rn(Z.s_in_p, si[k]);

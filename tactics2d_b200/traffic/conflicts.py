@@ -43,7 +43,7 @@ def _segments(paths):
         l2 = dx * dx + dy * dy
         keep = l2 > 0.0
         if not keep.any():
-            continue   # a degenerate path: K17's has_segment fails, nothing is projected on it
+            continue   # a degenerate path: PathTable::usable fails, nothing is projected on it
         ln = np.sqrt(l2[keep])
         cum = np.zeros(ln.shape[0])
         acc = 0.0
